@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- env-steps/s of the PULSE HumanoidIm hot path on B200 (BASELINE.json metric).
+"""bench.py -- env-steps/s of the PULSE HumanoidIm hot path on H100 (BASELINE.json metric).
 
 One bench "step" = one PPO iteration of BASELINE config C4 (HumanoidIm PPO, 16384 envs total,
 AMASS-shaped synthetic MotionLib, horizon 32): 32 post-physics env steps (fused reward/reset/obs
@@ -9,7 +9,8 @@ normalisation).  Isaac Gym physics is excluded on every arm (not installable her
 reference iteration additionally does that this build does not run yet.
 
 Contract: `python bench.py --gpus N --steps K --warmup W` (torchrun for N > 1), one JSON line on
-rank 0.  `--impl reference` times the CPU port of the reference path (oracle/, kind "port") on the
+rank 0.  `--dump-outputs DIR` writes what the last timed iteration computed as DIR/<name>.npy (seeded inputs: two builds
+run with the same arguments can be compared output for output).  `--impl reference` times the CPU port of the reference path (oracle/, kind "port") on the
 host cores.  Envs shard across ranks (16384 / N each, "strong" scaling); no data-path collective in
 the rollout; NCCL is only used for the timing barrier / max-over-ranks here.
 """
@@ -29,7 +30,7 @@ HORIZON = 32
 MINIBATCH = 16384      # im.yaml:72 (per rank, as under Horovod)
 MINI_EPOCHS = 6        # im.yaml:73
 ALGO_BYTES_PER_ENV_STEP = 9396  # SURVEY.md 8(d): fused step kernel, core total incl. power term
-METRIC = "env-steps/sec at 16384 humanoid envs, 1/2/4/8 B200; obs-kernel HBM GB/s"
+METRIC = "env-steps/sec at 16384 humanoid envs, 1/2/4/8 H100; obs-kernel HBM GB/s"
 
 
 def parse():
@@ -41,6 +42,9 @@ def parse():
     ap.add_argument("--envs", type=int, default=TOTAL_ENVS)
     ap.add_argument("--median-frames", type=int, default=150)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the outputs of the last timed PPO iteration (a fixed sample of the experience rows "
+                         "and the updated policy) to DIR/<name>.npy, float32 / float64, at most 64 MB in all")
     ap.add_argument("--workload", default="ppo", choices=["ppo", "vae", "reach"],
                     help="ppo = the headline (BASELINE configs[3], the default the driver runs); vae = configs[2] PULSE VAE distillation, "
                          "8192 envs; reach = configs[4] latent reach task (1024 envs per GPU): single-GPU records of the secondary workloads")
@@ -229,7 +233,7 @@ def workload_config(a, world, envs_total):
         "mini_epochs": MINI_EPOCHS, "minibatches_per_epoch_per_gpu": mb, "parallelism": f"env-shard x{world}, grad all-reduce per minibatch",
         "phases": ["32x fused env reset of the done envs, no host sync (pulse_reset_ref_state: compaction, start-time draw, MotionLib query, scatter into "
                    "root / dof / rigid-body state, AMP history back-fill) + observation of the reset envs (a13)",
-                   "32x [obs normalise + actor/critic MLP fwd (tcgen05) + in-kernel Gaussian sample, neglogp, value de-normalisation, PD targets, "
+                   "32x [obs normalise + actor/critic MLP fwd (wgmma) + in-kernel Gaussian sample, neglogp, value de-normalisation, PD targets, "
                    "written straight into the experience slices (K7-K9, K22)]",
                    "32x fused progress += 1 + reward + reset + next observation kernel (K1-K5)", "32x AMP observation row written into its experience slice (K6)",
                    "32x critic fwd on the next obs -> next_values * (1 - terminated)", "discriminator fwd + AMP reward over 32xN rows (K10)",
@@ -268,8 +272,8 @@ def mlp_flops_per_env_step():
 
 
 SECONDARY = {
-    "vae": ("env-steps/sec, PULSE VAE distillation (encoder + prior + decoder MLP), 8192 humanoid envs, 1 B200 (BASELINE configs[2])", 8192),
-    "reach": ("env-steps/sec, latent-space reach task with the frozen PULSE decoder, 1024 envs per B200 (BASELINE configs[4]: 8192 envs on 8 GPUs)", 1024),
+    "vae": ("env-steps/sec, PULSE VAE distillation (encoder + prior + decoder MLP), 8192 humanoid envs, 1 H100 (BASELINE configs[2])", 8192),
+    "reach": ("env-steps/sec, latent-space reach task with the frozen PULSE decoder, 1024 envs per H100 (BASELINE configs[4]: 8192 envs on 8 GPUs)", 1024),
 }
 
 
@@ -383,6 +387,31 @@ def run_secondary(a):
     print(json.dumps(line), flush=True)
 
 
+def dump_outputs(out_dir, ps, policy, rows=2048, amp_rows=1024, limit=64 << 20):
+    """What the last timed PPO iteration handed its caller: the experience of the rollout (a fixed sample of `rows` of the n x 32
+    rows; `amp_rows` of the 1960-wide AMP rows) and the policy after the update (weights, log-std, normaliser statistics)."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    n_rows = ps.n * ps.T
+    idx = torch.from_numpy(np.sort(np.random.RandomState(0).choice(n_rows, size=min(rows, n_rows), replace=False))).to(ps.dev)
+    arrays = {}
+    for name in ("obses", "actions", "mus", "neglogp", "values", "next_values", "rewards", "dones", "adv", "ret", "amp_obs"):
+        t = getattr(ps, name).reshape(n_rows, -1)
+        arrays["rollout." + name] = t.index_select(0, idx[:amp_rows] if name == "amp_obs" else idx)
+    arrays.update(policy.state_dict())
+    host = {}
+    for name, t in arrays.items():
+        x = t.detach().cpu().numpy()
+        host[name] = x.astype(np.float64 if x.dtype == np.float64 else np.float32)
+    total = sum(x.nbytes for x in host.values())
+    if total > limit:                          # checked before anything is written: no partial DIR
+        raise SystemExit(f"--dump-outputs: {total >> 20} MB exceeds {limit >> 20} MB")
+    os.makedirs(out_dir, exist_ok=True)
+    for name, x in host.items():
+        np.save(os.path.join(out_dir, name + ".npy"), x)
+
+
 def main():
     a = parse()
     if a.workload != "ppo":
@@ -406,6 +435,9 @@ def main():
     assert world == a.gpus, f"--gpus {a.gpus} but WORLD_SIZE={world} (launch with torch.distributed.run)"
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
+    # every draw without an explicit generator (AMP demo sampling, replay ring, minibatch indices) comes from these seeds: the same
+    # arguments give the same inputs on every run
+    torch.manual_seed(0)
     if world > 1:
         # NCCL prints its version banner on STDOUT when the communicator is created (NCCL_DEBUG >= VERSION in the environment);
         # stdout must carry exactly one JSON line, so fd 1 points at stderr until the communicator exists.
@@ -613,6 +645,8 @@ def main():
     sampler.start()
     ms_dev, launches = timed(False, a.steps, True)
     clocks = sampler.stop()
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, ps, policy)
     ms_e2e, _ = timed(True, max(2, a.steps // 2), False)
 
     torch.cuda.synchronize()
@@ -628,16 +662,10 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_tf = float(peaks.get("bf16_tflops_sustained", 1400.0))
+    # fallbacks: NVIDIA's H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense BF16 at up to 700 W), not reached figures
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_tf = float(peaks.get("bf16_tflops_sustained", 989.0))
     achieved = ALGO_BYTES_PER_ENV_STEP * n / (k_avg * 1e-3) / 1e9
-    traffic = None   # dram__bytes_read.sum + dram__bytes_write.sum of one im_step_kernel launch at 16384 envs (ncu --set full, profiles/)
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "im_step_traffic.json")))
-        if int(tr.get("envs", 0)) == n:
-            traffic = float(tr["dram_bytes_read"]) + float(tr["dram_bytes_write"])
-    except Exception:
-        pass
     env_steps = T * a.envs
     _d = 1960 * 1024 + 1024 * 512 + 512
     _gp = 3 * (512 * 1024 + 1024 * 1960)
@@ -657,21 +685,21 @@ def main():
             "phases_ms": {"rollout_32_steps": rollout_ms, "post_rollout": post_ms, "update": u_ms,
                           "note": "device-resident arm, this rank; rollout = resets + policy + fused step + AMP + next values per step"},
             "resets_per_env_step": resets_per_step,
-            "gemm_switches": {"cta_pairs": os.environ.get("PULSE_GEMM_PAIR", "1") != "0", "pdl": os.environ.get("PULSE_GEMM_PDL", "1") != "0",
+            "gemm_switches": {"pdl": os.environ.get("PULSE_GEMM_PDL", "1") != "0",
                               "grouped_launches": os.environ.get("PULSE_GROUPED", "0") == "1"},
             "update_input_prefetch": bool(prefetching),
             "optimizer_step": ("one peer-memory kernel per rank: reduce-scatter over NVLink + norm clip + sharded Adam + push of masters / bf16 operands"
                                + (" (multimem)" if policy.flat.peer and policy.flat.peer["multicast"] else "")) if (world > 1 and policy.flat.peer)
                               else ("ncclAllReduce(AVG) + sum_squares + adam" if world > 1 else "sum_squares + adam (single GPU)"),
             "roofline": {"kernel": "im_step_kernel", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": traffic, "traffic_unit": "bytes per launch (ncu dram read+write, profiles/im_step_traffic.json)",
+                         "frac": achieved / peak, "traffic": None,
                          "algorithmic_bytes_per_launch": ALGO_BYTES_PER_ENV_STEP * n,
-                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 (of fallback)",
+                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "H100 SXM data sheet 3350",
                          "algorithmic_bytes_per_env_step": ALGO_BYTES_PER_ENV_STEP, "avg_launch_ms": k_avg, "launches_timed": len(k_ms)},
-            "roofline_update": {"kernels": "PPO update phase (tcgen05 GEMMs + loss/Adam/reduction kernels), per rank", "bound": "tensor",
+            "roofline_update": {"kernels": "PPO update phase (wgmma GEMMs + loss/Adam/reduction kernels), per rank", "bound": "tensor",
                                 "achieved": upd_flops / (u_ms * 1e-3) / 1e12, "peak": peak_tf, "unit": "TFLOP/s",
                                 "frac": upd_flops / (u_ms * 1e-3) / 1e12 / peak_tf, "update_ms": u_ms,
-                                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "fallback 1400",
+                                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "H100 SXM data sheet 989 (dense bf16)",
                                 "note": "algorithmic GEMM FLOPs of the update / whole update-phase time (non-GEMM kernels included)"},
             "mlp_mflop_per_env_step": mlp_flops_per_env_step() / 1e6,
         }

@@ -1,5 +1,5 @@
 /*
- * pulse_b200.h -- C ABI of the B200-native PULSE hot path (libpulse_b200.so).
+ * pulse_b200.h -- C ABI of the GPU-native PULSE hot path (libpulse_b200.so, H100 / sm_90a).
  *
  * Boundary rules (SURVEY.md section 8b):
  *   - plain C types only: device pointers, element strides, sizes, a cudaStream_t passed as void*;
@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define PULSE_ABI_VERSION 2
+#define PULSE_ABI_VERSION 3
 
 enum pulse_status {
   PULSE_OK = 0,
@@ -308,7 +308,7 @@ int pulse_normalize_advantages(float* advantages, const double* adv_sum, int64_t
 
 /* ------------------------------------------------------------------------------------------------
  * Dense layers on the tensor cores: D[M,N] = epilogue(alpha * A[M,K] . B[N,K]^T), bf16 operands (both
- * K-major: row-major with the reduction dimension contiguous), fp32 accumulation in TMEM (tcgen05).
+ * K-major: row-major with the reduction dimension contiguous), fp32 accumulation in registers (wgmma).
  * Replaces the nn.Linear + activation stacks of the policy / value / discriminator / VAE networks
  * (phc/learning/network_builder.py:105-124, amp_network_builder.py:58-249, amp_network_z_builder.py:341-467)
  * and their autograd backward: forward (A=X, B=W), dgrad (A=dY, B=W^T), wgrad (A=dY^T, B=X^T).
@@ -363,7 +363,7 @@ int pulse_gemm_num_splits(int64_t k, int32_t split_k);
 
 /* Several GEMMs of the same kind in ONE persistent launch (work items of all problems concatenated): forward groups
  * (flags 0), ReLU-dgrad groups (PULSE_GEMM_B_MN) or weight-gradient groups (PULSE_GEMM_A_MN | PULSE_GEMM_B_MN, fp32 atomic
- * accumulation), at most 4 problems.  EXPERIMENTAL in round 1 (compiled, not yet validated on a device). */
+ * accumulation), at most 4 problems.  Validated against single launches by tests/test_gpu_grouped.py; off by default. */
 typedef struct {
   const void* a; int64_t lda;
   const void* b; int64_t ldb;
@@ -408,9 +408,17 @@ int pulse_head1_forward(const pulse_bf16_t* h, int64_t ldh, int64_t rows, int32_
 
 /* Backward of that head through the ReLU below it, ONE pass over h:  dh[m,j] = dv[m] w[j] (h[m,j] > 0) (bf16, may be
  * NULL);  dw[j] += sum_m dv[m] h[m,j];  db += sum_m dv[m];  dbias_prev[j] += sum_m dh[m,j] (bias gradient of the layer
- * that produced h; may be NULL).  k <= 2048, multiple of 8. */
+ * that produced h; may be NULL).  k <= 2048, multiple of 8.  partials: fp32 scratch of PULSE_HEAD1_MAX_CTAS * (2k + 1) floats
+ * (per-CTA sums, added in CTA order: the result does not depend on scheduling). */
+#define PULSE_HEAD1_MAX_CTAS 264
 int pulse_head1_backward(const pulse_bf16_t* h, int64_t ldh, int64_t rows, int32_t k, const pulse_bf16_t* dv, int64_t ld_dv,
-                         const pulse_bf16_t* w, pulse_bf16_t* dh, int64_t ld_dh, float* dw, float* db, float* dbias_prev, void* stream);
+                         const pulse_bf16_t* w, pulse_bf16_t* dh, int64_t ld_dh, float* dw, float* db, float* dbias_prev, float* partials,
+                         void* stream);
+
+/* out[r, c] += sum_{s < n} x[s * stride_n + r * ld + c], the n terms added in the order s = 0, 1, ... (split-K slabs, partial sums):
+ * a reduction that gives the same bits on every run.  ld / ldo are ignored when rows == 1. */
+int pulse_ordered_sum_add(const float* x, int64_t n, int64_t stride_n, int64_t rows, int64_t cols, int64_t ld, float* out, int64_t ldo,
+                          void* stream);
 
 /* Gaussian policy head (rl_games ModelA2CContinuousLogStd, fixed sigma: im.yaml:21-25):
  * actions = mu + exp(logstd)*eps;  neglogp = 0.5*sum(((a-mu)/sigma)^2) + 0.5*A*log(2*pi) + sum(logstd). */

@@ -8,8 +8,8 @@ where the reference itself is not present, and so `bench.py` has a CPU arm (`cpu
 
 Pinning: `tests/test_oracle_vs_golden.py` checks every routine here against `tests/golden/*.npz`,
 which `tests/golden/make_golden.py` produced by running the reference's own functions (imported
-unmodified from /root/reference under `oracle/refshim`).  When /root/reference is present the
-same test also re-runs the reference live.  Integer outputs (frame indices, reset / terminate
+unmodified from the reference tree under `oracle/refshim`); `make_golden_reference_pins.py` adds the
+reference's outputs on fresh seeded inputs.  Integer outputs (frame indices, reset / terminate
 masks) must be identical; float outputs agree to 1e-6 or better (same op order, same library).
 
 Third-party arithmetic absent from the reference tree and restated here [3P-memory]:

@@ -1,13 +1,12 @@
-"""Import the UNMODIFIED reference (`/root/reference`) in the build container.
+"""Import the UNMODIFIED reference tree (PULSE_REFERENCE_ROOT) for fixture generation.
 
 TEST INFRASTRUCTURE ONLY.  The reference's hot-path functions are plain PyTorch, but the modules
 that hold them import Isaac Gym, rl_games, smpl_sim, ... at module scope.  This loader registers
 (a) the file-based `isaacgym.torch_utils` restatement next to this file and (b) attribute-mocks
 for every other missing third-party module, then imports the reference modules as they are.
 
-Used by `tests/golden/make_golden.py` (fixture generation) and by the `-m "not gpu"` test that
-re-pins `oracle/pulse_oracle.py` against the live reference when `/root/reference` exists.
-`/root/reference` does not exist on the GPU box: nothing on the GPU path calls this.
+Used only by the fixture generators under `tests/golden/` (`make_golden*.py`): the tests compare against the
+fixtures they wrote and never import the reference.  The reference tree's location is PULSE_REFERENCE_ROOT.
 """
 import importlib
 import importlib.abc

@@ -1,4 +1,4 @@
-"""pulse_b200 -- B200-native (sm_100a) implementation of PULSE's per-step rollout / update hot path.
+"""pulse_b200 -- H100-native (sm_90a) implementation of PULSE's per-step rollout / update hot path.
 
 Host code is Python/PyTorch (device memory, streams, torch.distributed) calling hand-written CUDA
 through the C ABI in include/pulse_b200.h (libpulse_b200.so, built in-tree by pulse_b200.build).

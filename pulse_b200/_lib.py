@@ -228,7 +228,8 @@ class PeerAdamArgs(C.Structure):
     ]
 
 
-ABI_VERSION = 2
+ABI_VERSION = 3
+HEAD1_MAX_CTAS = 264        # PULSE_HEAD1_MAX_CTAS: rows of the pulse_head1_backward partial-sum scratch
 ACT_NONE, ACT_RELU, ACT_SILU = 0, 1, 2
 Z_SAMPLE, Z_MEAN, Z_RESIDUAL = 0, 1, 2
 STEP_REWARD, STEP_RESET, STEP_OBS, STEP_ALL, STEP_ADVANCE = 1, 2, 4, 7, 8
@@ -266,7 +267,8 @@ SIGNATURES = {
                                           C.c_void_p, C.c_float, C.c_void_p]),
     "pulse_head1_forward": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_head1_backward": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
-                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pulse_ordered_sum_add": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_column_moments": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
     "pulse_rms_merge": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p,
                                   C.c_void_p]),
@@ -316,7 +318,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise PulseError(f"{LIB_PATH} is missing: build it with `python -m pulse_b200.build` "
-                         "(nvcc, sm_100a). pulse_b200 has no CPU fallback.")
+                         "(nvcc, sm_90a). pulse_b200 has no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the .so does not export a declared symbol

@@ -12,7 +12,8 @@ logging, checkpoint cadence and the experience buffer, Isaac Gym keeps the physi
 These classes only route tensors to `PPOPolicy` / `PulseVAE` / `TeacherPNN` / `ReachTaskB200`; every number is computed by
 the CUDA library (no CPU fallback).  rl_games and Isaac Gym are not installable here (SURVEY.md 8c): tests/test_gpu_boundary.py mixes
 these classes in front of stand-in base classes (tests/standins.py) that carry the reference's attribute / method contract, and
-tests/test_boundary_cpu.py checks that contract against the unmodified reference sources where /root/reference exists.
+tests/test_boundary_cpu.py checks that contract against names recorded from the unmodified reference sources
+(tests/golden/contract_names.json).
 
 Reference methods mirrored:
   CommonAgent.get_action_values   phc/learning/common_agent.py:262-288

@@ -1,4 +1,4 @@
-"""AMP discriminator on the B200: rewards and the training loss with an ANALYTIC gradient penalty.
+"""AMP discriminator on the GPU: rewards and the training loss with an ANALYTIC gradient penalty.
 
 Host-side mirror of `AMPAgent._calc_disc_rewards` (phc/learning/amp_agent.py:1027-1041), `_disc_loss`
 (:895-952) and the `eval_disc` calls of `ModelAMPContinuous.forward` (amp_models.py:33-41) for the ReLU
@@ -7,7 +7,7 @@ discriminator `AMPBuilder._build_disc` builds (amp_network_builder.py:230-249).
 The reference obtains the gradient penalty's parameter gradients by double backward through
 `torch.autograd.grad(..., create_graph=True)`.  For a ReLU MLP D(x) = w3 . relu(W2 relu(W1 x + b1) + b2) + b3 the
 input gradient is  gx = ((m2 * w3) W2 * m1) W1  with the activation masks m1, m2 piecewise constant, so both gx
-and d(mean|gx|^2)/d(W1, W2, w3) are plain GEMM chains -- the same tcgen05 kernel in its dgrad / wgrad / NT forms:
+and d(mean|gx|^2)/d(W1, W2, w3) are plain GEMM chains -- the same wgmma kernel in its dgrad / wgrad / NT forms:
     g2 = m2 * w3            u = g2 W2        g1 = m1 * u        gx = g1 W1
     G  = c * gx  (c = 2 * disc_coef * grad_penalty / B)
     dW1 += g1^T G      du = m1 * (G W1^T)      dW2 += g2^T du      dw3 += colsum(m2 * (du W2^T))
@@ -18,7 +18,7 @@ from typing import Dict, Optional, Sequence
 import torch
 
 from . import _lib
-from .dense import gemm
+from .dense import column_sum_add, gemm
 from .nets import MLP, FlatParams, pad_k, pick_split
 from .ppo import RunningMeanStdB200
 
@@ -60,9 +60,9 @@ class AmpDiscriminator:
                 "dlogit": torch.zeros(3 * B, 8, device=dev, dtype=bf),
                 "g2": torch.zeros(B, L2.Np, device=dev, dtype=bf), "g1": torch.zeros(B, L1.Np, device=dev, dtype=bf),
                 "Gb": torch.zeros(B, self.Kp, device=dev, dtype=bf),
-                "du": torch.zeros(B, L1.Np, device=dev, dtype=bf), "scratch": torch.zeros(B, L2.Np, device=dev, dtype=bf),
-                "split1": pick_split(((L1.N + 127) // 128) * ((L1.Kp + 255) // 256), (B + 63) // 64),
-                "split2": pick_split(((L2.N + 127) // 128) * ((L2.Kp + 255) // 256), (B + 63) // 64),
+                "du": torch.zeros(B, L1.Np, device=dev, dtype=bf), "scratch": torch.zeros(B, L2.Np, device=dev),
+                "split1": pick_split(((L1.N + 127) // 128) * ((L1.Kp + 127) // 128), (B + 63) // 64),
+                "split2": pick_split(((L2.N + 127) // 128) * ((L2.Kp + 127) // 128), (B + 63) // 64),
             }
         return self._bufs[B]
 
@@ -114,7 +114,8 @@ class AmpDiscriminator:
         gemm(b["g1"][:, :L1.N], b["Gb"], a_mn=True, b_mn=True, out_f32=L1.weight_grad, accumulate=True, split_k=b["split1"])  # dW1 += g1^T G (G's bias column is 0)
         gemm(b["Gb"], L1.w_bf16, gate_mask=m1, out=b["du"])                                                # du = m1 * (G W1^T); G's bias / pad columns are 0
         gemm(b["g2"][:, :L2.N], b["du"][:, :L1.N], a_mn=True, b_mn=True, out_f32=L2.weight_grad, accumulate=True, split_k=b["split2"])  # dW2 += g2^T du
-        gemm(b["du"][:, :L1.N], W2, gate_mask=m2, out=b["scratch"], colsum=L3.weight_grad.view(-1))        # dw3 += colsum(m2 * (du W2^T))
+        gemm(b["du"][:, :L1.N], W2, gate_mask=m2, out_f32=b["scratch"])                                    # m2 * (du W2^T), fp32
+        column_sum_add(b["scratch"][:, :L2.N], L3.weight_grad.view(-1))                                    # dw3 += its column sums, fixed order
         # ---- logit regulariser and weight decay (amp_agent.py:905-908, :932-937): d/dw coef*sum(w^2) = 2*coef*w, weights only ------
         reg = _lib.WeightReg()
         reg.count = 3

@@ -1,4 +1,4 @@
-// Element-wise and reduction kernels around the tcgen05 GEMMs: observation normalisation, Gaussian
+// Element-wise and reduction kernels around the wgmma GEMMs: observation normalisation, Gaussian
 // policy head, PPO losses + output gradients, bias-gradient column sums, split-K slab reduction,
 // gradient-norm clip + Adam, bf16 operand refresh.  All HBM-bound streaming kernels: 16-byte accesses
 // where the layout allows, grid-stride loops sized to a multiple of the SM count.
@@ -9,7 +9,7 @@
 namespace pulse {
 namespace {
 
-constexpr int kSMs = 148;
+constexpr int kSMs = kNumSMs;
 
 __device__ __forceinline__ double warp_sum_d(double v) {
 #pragma unroll
@@ -162,8 +162,7 @@ __global__ void __launch_bounds__(128) gaussian_sample_kernel(const float* __res
 // ---- PPO losses + gradients w.r.t. mu / value ---------------------------------------------------------------------
 __global__ void __launch_bounds__(256) ppo_loss_kernel(const pulse_ppo_loss_args_t a, long long rows) {
   // Warps stride over the rows (a few rows each on a one-wave grid): the per-action constants are computed once per lane, the loss
-  // statistics stay in registers until ONE set of fp64 atomics per block (round 1 issued six per 128-thread block: 24 k serialised
-  // atomics on six addresses were most of this kernel's 19 us).
+  // statistics stay in registers until ONE set of fp64 atomics per block (six per 128-thread block serialise on six addresses).
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
   __shared__ double s_stats[8][6];
@@ -516,7 +515,7 @@ __global__ void __launch_bounds__(256) refresh_weight_kernel(const float* __rest
 }
 
 // ---- single-output head (critic value, discriminator logit): GEMV forward and ONE fused backward pass ---------------
-// A [M,K] x [K,1] product has no tensor-core shape: the 128 x 256 MMA tile would be 255/256 padding and the three
+// A [M,K] x [K,1] product has no tensor-core shape: a 128 x 128 MMA tile would be 127/128 padding and the three
 // backward GEMMs (K = 1 dgrad, M = 1 wgrad) are pure epilogue / pure reduction.  Both directions are HBM streams
 // over the last hidden activation h [M,K] bf16: forward reads it once; backward reads it once and writes dh once.
 __global__ void __launch_bounds__(256) head1_forward_kernel(const __nv_bfloat16* __restrict__ h, long long ldh, long long rows, int K,
@@ -556,11 +555,12 @@ __global__ void __launch_bounds__(256) head1_forward_kernel(const __nv_bfloat16*
 
 
 // dh[m,k] = dv[m] * w[k] * (h[m,k] > 0);  dw[k] += sum_m dv[m] h[m,k];  db += sum_m dv[m];  dbias_prev[k] += sum_m dh[m,k].
-// Thread = 8 columns (one 16-byte load / store); blockDim.x / (K/8) row lanes per CTA; fp32 atomics once per CTA.
+// Thread = 8 columns (one 16-byte load / store); blockDim.x / (K/8) row lanes per CTA.  Each CTA writes its column sums to its own
+// row of `partials` [gridDim.x][2K + 1]; ordered_sum_kernel then adds the rows in CTA order, so the sums do not depend on scheduling.
 __global__ void __launch_bounds__(256) head1_backward_kernel(const __nv_bfloat16* __restrict__ h, long long ldh, long long rows, int K,
                                                              const __nv_bfloat16* __restrict__ dv, long long ld_dv,
                                                              const __nv_bfloat16* __restrict__ w, __nv_bfloat16* __restrict__ dh, long long ld_dh,
-                                                             float* __restrict__ dw, float* __restrict__ db, float* __restrict__ dbias_prev) {
+                                                             float* __restrict__ partials) {
   extern __shared__ float red[];  // [row lanes][2 * K + 1]
   const int groups = K >> 3;                     // column groups of 8
   const int lanes = blockDim.x / groups;         // row lanes per CTA (host guarantees >= 1)
@@ -633,13 +633,22 @@ __global__ void __launch_bounds__(256) head1_backward_kernel(const __nv_bfloat16
   for (int i = threadIdx.x; i < 2 * K + 1; i += blockDim.x) {
     float t = 0.0f;
     for (int l = 0; l < lanes; ++l) t += red[(long long)l * (2 * K + 1) + i];
-    if (i < K) {
-      atomicAdd(dw + i, t);
-    } else if (i < 2 * K) {
-      if (dbias_prev != nullptr) atomicAdd(dbias_prev + (i - K), t);
-    } else if (db != nullptr) {
-      atomicAdd(db, t);
-    }
+    partials[(long long)blockIdx.x * (2 * K + 1) + i] = t;
+  }
+}
+
+// out[r, c] += sum_{s < n} x[s * stride_n + r * ld + c], the n terms added in the order s = 0, 1, ...: a reduction whose result does not
+// depend on how the producing CTAs were scheduled (split-K slabs, per-CTA partial sums), so repeated runs compute identical bits.
+__global__ void __launch_bounds__(256) ordered_sum_kernel(const float* __restrict__ x, long long n, long long stride_n, long long rows,
+                                                          long long cols, long long ld, float* __restrict__ out, long long ldo) {
+  const long long total = rows * cols;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long r = i / cols, c = i - r * cols;
+    const float* p = x + r * ld + c;
+    float s = 0.0f;
+#pragma unroll 8
+    for (long long k = 0; k < n; ++k) s += __ldg(p + k * stride_n);
+    out[r * ldo + c] += s;
   }
 }
 
@@ -725,20 +734,40 @@ extern "C" int pulse_head1_forward(const pulse_bf16_t* h, int64_t ldh, int64_t r
 
 extern "C" int pulse_head1_backward(const pulse_bf16_t* h, int64_t ldh, int64_t rows, int32_t k, const pulse_bf16_t* dv, int64_t ld_dv,
                                     const pulse_bf16_t* w, pulse_bf16_t* dh, int64_t ld_dh, float* dw, float* db, float* dbias_prev,
-                                    void* stream) {
-  PULSE_REQUIRE(h && dv && w && dw && rows > 0 && k > 0 && ld_dv >= 1, "pulse_head1_backward: bad argument");
+                                    float* partials, void* stream) {
+  PULSE_REQUIRE(h && dv && w && dw && partials && rows > 0 && k > 0 && ld_dv >= 1, "pulse_head1_backward: bad argument");
   PULSE_REQUIRE(k % 8 == 0 && k <= 2048 && ldh % 8 == 0 && (dh == nullptr || ld_dh % 8 == 0), "pulse_head1_backward: K <= 2048, K and lds multiples of 8");
   PULSE_REQUIRE(reinterpret_cast<uintptr_t>(h) % 16 == 0 && reinterpret_cast<uintptr_t>(w) % 16 == 0 && reinterpret_cast<uintptr_t>(dh) % 16 == 0,
                 "pulse_head1_backward: 16-byte aligned operands required");
   const int groups = k / 8, lanes = 256 / groups;
   const size_t smem = static_cast<size_t>(lanes) * (2 * k + 1) * sizeof(float);
   long long blocks = (rows + 8LL * lanes - 1) / (8LL * lanes);  // >= 8 rows per row lane
-  if (blocks > 2 * kSMs) blocks = 2 * kSMs;
+  if (blocks > PULSE_HEAD1_MAX_CTAS) blocks = PULSE_HEAD1_MAX_CTAS;
   if (blocks < 1) blocks = 1;
-  head1_backward_kernel<<<static_cast<unsigned>(blocks), 256, smem, static_cast<cudaStream_t>(stream)>>>(
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  head1_backward_kernel<<<static_cast<unsigned>(blocks), 256, smem, st>>>(
       reinterpret_cast<const __nv_bfloat16*>(h), ldh, rows, k, reinterpret_cast<const __nv_bfloat16*>(dv), ld_dv,
-      reinterpret_cast<const __nv_bfloat16*>(w), reinterpret_cast<__nv_bfloat16*>(dh), ld_dh, dw, db, dbias_prev);
+      reinterpret_cast<const __nv_bfloat16*>(w), reinterpret_cast<__nv_bfloat16*>(dh), ld_dh, partials);
   PULSE_LAUNCH_OK("head1_backward_kernel");
+  const long long row = 2LL * k + 1;
+  ordered_sum_kernel<<<static_cast<unsigned>((k + 255) / 256), 256, 0, st>>>(partials, blocks, row, 1, k, 0, dw, 0);
+  PULSE_LAUNCH_OK("ordered_sum_kernel");
+  if (dbias_prev != nullptr) {
+    ordered_sum_kernel<<<static_cast<unsigned>((k + 255) / 256), 256, 0, st>>>(partials + k, blocks, row, 1, k, 0, dbias_prev, 0);
+    PULSE_LAUNCH_OK("ordered_sum_kernel");
+  }
+  if (db != nullptr) {
+    ordered_sum_kernel<<<1, 32, 0, st>>>(partials + 2 * k, blocks, row, 1, 1, 0, db, 0);
+    PULSE_LAUNCH_OK("ordered_sum_kernel");
+  }
+  return PULSE_OK;
+}
+
+extern "C" int pulse_ordered_sum_add(const float* x, int64_t n, int64_t stride_n, int64_t rows, int64_t cols, int64_t ld, float* out, int64_t ldo,
+                                     void* stream) {
+  PULSE_REQUIRE(x && out && n > 0 && rows > 0 && cols > 0 && (rows == 1 || (ld >= cols && ldo >= cols)), "pulse_ordered_sum_add: bad argument");
+  ordered_sum_kernel<<<grid_for(rows * cols, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, n, stride_n, rows, cols, ld, out, ldo);
+  PULSE_LAUNCH_OK("ordered_sum_kernel");
   return PULSE_OK;
 }
 

@@ -8,7 +8,7 @@
 // Precision follows the reference stage by stage (oracle.pulse_oracle.loader_clip): heading rotation, local rotations and
 // the consecutive-frame rotation differences in float64; forward kinematics, linear and dof velocities in float32.
 //
-// STATUS (round 1): parity green against the reference's tables on a B200 (tests/test_gpu_loader.py); not yet timed, and the
+// STATUS: parity against the reference's tables is checked by tests/test_gpu_loader.py; not yet timed, and the
 // bench still builds its synthetic tables directly.
 #include "pulse_common.cuh"
 #include "quat_math.cuh"

@@ -138,7 +138,7 @@ extern "C" int pulse_motionlib_create(const pulse_motionlib_desc_t* desc, void* 
   const long long total = d.total_frames * (PULSE_FRAME_REC + PULSE_AUX_REC);
   const int threads = 256;
   long long blocks = (total + threads - 1) / threads;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
   pack_tables_kernel<<<static_cast<unsigned>(blocks), threads, 0, static_cast<cudaStream_t>(stream)>>>(d);
   PULSE_LAUNCH_OK("pack_tables_kernel");
   pulse_motionlib* h = static_cast<pulse_motionlib*>(malloc(sizeof(pulse_motionlib)));

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libpulse_b200.so (sm_100a only).
+// Shared host/device helpers for libpulse_b200.so (sm_90a, H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -42,6 +42,9 @@ void count_launch(int n = 1);
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 constexpr int kWarp = 32;
+// SM count of the H100 SXM: sizes the grid caps of the grid-stride element-wise / reduction kernels (the persistent GEMM
+// queries the device instead).
+constexpr int kNumSMs = 132;
 constexpr unsigned kFull = 0xffffffffu;
 
 }  // namespace pulse

@@ -1,5 +1,5 @@
 // Row-wise kernels of the PULSE VAE distillation path (SURVEY K17-K19), the Z-task action decode (K20), the reach task
-// (K21) and the PD-target map (K22).  The dense layers between them run on the tcgen05 GEMM; everything here is
+// (K21) and the PD-target map (K22).  The dense layers between them run on the wgmma GEMM; everything here is
 // HBM-bound streaming work: one warp per row (lane = latent dimension / body), fp64 atomics for the scalar statistics.
 #include <cuda_bf16.h>
 
@@ -9,7 +9,7 @@
 namespace pulse {
 namespace {
 
-constexpr int kSMs = 148;
+constexpr int kSMs = kNumSMs;
 
 inline unsigned warp_grid(long long rows, int warps_per_block, int waves = 8) {
   long long blocks = (rows + warps_per_block - 1) / warps_per_block;

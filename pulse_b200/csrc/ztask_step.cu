@@ -150,7 +150,7 @@ extern "C" int pulse_ztask_step(const pulse_ztask_step_args_t* args, int64_t num
     PULSE_REQUIRE(a.obs_stride >= PULSE_STRIKE_OBS, "pulse_ztask_step: obs_stride %lld < %d", (long long)a.obs_stride, PULSE_STRIKE_OBS);
   }
   long long ctas = (num_envs + 7) / 8;
-  if (ctas > 148ll * 8) ctas = 148ll * 8;
+  if (ctas > kNumSMs * 8ll) ctas = kNumSMs * 8ll;
   ztask_step_kernel<<<static_cast<unsigned>(ctas), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, (long long)num_envs);
   PULSE_LAUNCH_OK("ztask_step_kernel");
   return PULSE_OK;

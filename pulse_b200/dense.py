@@ -1,4 +1,4 @@
-"""Dense layers on the B200 tensor cores: thin host wrapper over `pulse_gemm_bf16_nt` (tcgen05 / TMEM / TMA).
+"""Dense layers on the H100 tensor cores: thin host wrapper over `pulse_gemm_bf16_nt` (wgmma / TMA).
 
 `gemm_nt(a, b)` computes a @ b.T for bf16 row-major a [M,K], b [N,K] with fp32 accumulation and a fused
 epilogue (bias, ReLU / SiLU, activation-derivative gating, transposed copy, fp32 output, split-K slabs).
@@ -22,6 +22,28 @@ def num_splits(k: int, split_k: int) -> int:
     return int(_lib.load().pulse_gemm_num_splits(k, split_k))
 
 
+def ordered_sum_add(x: torch.Tensor, out: torch.Tensor) -> None:
+    """out += x.sum(0) for fp32 x [n, rows, cols] (rows with contiguous columns), the n terms added in order: same bits on every run."""
+    if x.dtype != torch.float32 or out.dtype != torch.float32 or x.stride(-1) != 1 or out.stride(-1) != 1 or x.shape[1:] != out.shape:
+        raise _lib.PulseError("ordered_sum_add: fp32 x [n, rows, cols] and out [rows, cols] with contiguous columns")
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.load().pulse_ordered_sum_add(x.data_ptr(), x.shape[0], x.stride(0), x.shape[1], x.shape[2], x.stride(1), out.data_ptr(),
+                                                     out.stride(0), _lib.current_stream(x.device)), "pulse_ordered_sum_add")
+
+
+def column_sum_add(y: torch.Tensor, out: torch.Tensor, chunk: int = 64) -> None:
+    """out[c] += sum_r y[r, c] for fp32 y [rows, cols], in a fixed order (rows in chunks of `chunk`, then the chunk sums in order)."""
+    rows, cols = y.shape
+    n = -(-rows // chunk)
+    part = torch.zeros(n, cols, device=y.device)
+    full = rows // chunk
+    if full:
+        ordered_sum_add(y[:full * chunk].as_strided((chunk, full, cols), (y.stride(0), chunk * y.stride(0), 1)), part[:full])
+    if rows > full * chunk:
+        ordered_sum_add(y[full * chunk:].unsqueeze(1), part[full:])
+    ordered_sum_add(part.unsqueeze(1), out.view(1, -1)[:, :cols])
+
+
 def gemm_nt(a, b, **kw) -> None:
     """a [M,K] . b [N,K]^T (both K-major)."""
     gemm(a, b, **kw)
@@ -33,11 +55,24 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
          colsum: Optional[torch.Tensor] = None, accumulate: bool = False, split_k: int = 1, sumsq: Optional[torch.Tensor] = None,
          relu_mask: Optional[torch.Tensor] = None, gate_mask: Optional[torch.Tensor] = None) -> None:
     """D[M,N] = epilogue(sum_k A(m,k) B(n,k)).  a is [M,K] (K-major) or, with a_mn, [K,M] (MN-major: the reduction index
-    is the row); likewise b is [N,K] or, with b_mn, [K,N].  No operand is ever transposed in memory."""
+    is the row); likewise b is [N,K] or, with b_mn, [K,N].  No operand is ever transposed in memory.
+    accumulate=True with several split-K slices: every slice writes its own fp32 slab and the slabs are added to out_f32 in slice
+    order, so repeated runs give identical bits (atomic adds from concurrently running slices would not)."""
     lib = _lib.load()
     _check_bf16(a, "a")
     _check_bf16(b, "b")
     (K, M) = a.shape if a_mn else (a.shape[1], a.shape[0])
+    if accumulate and out_f32 is not None and out_f32.dim() == 2 and split_k > 1 and num_splits(K, split_k) > 1:
+        if (bias, gate, gate_mode, out, out_t, preact, colsum, sumsq, relu_mask, gate_mask) != (None,) * 10 or act not in (None, "none") \
+                or alpha != 1.0:
+            raise _lib.PulseError("split-K accumulation takes a plain fp32 output only (no alpha, activation, gate or extra outputs)")
+        N = b.shape[1] if b_mn else b.shape[0]
+        slabs = torch.empty(num_splits(K, split_k), M, (N + 3) // 4 * 4, device=a.device)[:, :, :N]
+        gemm(a, b, a_mn=a_mn, b_mn=b_mn, out_f32=slabs, split_k=split_k)
+        if out_f32.stride(-1) != 1:
+            raise _lib.PulseError("out_f32 must be fp32 with contiguous rows")
+        ordered_sum_add(slabs, out_f32[:M, :N])
+        return
     (Kb, N) = b.shape if b_mn else (b.shape[1], b.shape[0])
     if K != Kb:
         raise _lib.PulseError(f"K mismatch: a {tuple(a.shape)} (mn={a_mn}) vs b {tuple(b.shape)} (mn={b_mn})")
@@ -171,8 +206,8 @@ def _prepare(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool
 
 
 def grouped_enabled() -> bool:
-    """PULSE_GROUPED=1 routes the actor + critic layers of a PPO minibatch through grouped launches (EXPERIMENTAL in round 1:
-    the grouped kernel is compiled but has not run on a device yet; default off)."""
+    """PULSE_GROUPED=1 routes the actor + critic layers of a PPO minibatch through grouped launches (default off: validated by
+    tests/test_gpu_grouped.py, not faster than the three-stream path)."""
     import os
     return os.environ.get("PULSE_GROUPED", "0") == "1"
 

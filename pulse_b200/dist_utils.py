@@ -1,4 +1,4 @@
-"""Multi-GPU plumbing: one process per GPU, `torch.distributed` (NCCL over NVLink 5 / NVSwitch).
+"""Multi-GPU plumbing: one process per GPU, `torch.distributed` (NCCL over NVLink / NVSwitch).
 
 Replaces the Horovod calls the reference reaches through rl_games (SURVEY.md section 5):
   hvd.DistributedOptimizer gradient averaging (amp_agent.py:735-742)   -> average_gradients (one all-reduce on the flat bucket)
@@ -65,8 +65,7 @@ class ChainReducer:
     back to back, and each network's backward chain runs on its own CUDA stream (ppo.PPOPolicy.train_minibatch) -- so each slice is
     all-reduced on ITS stream as soon as that chain has produced it, through its own communicator (one NCCL communicator serialises its
     collectives; three let the critic's and the discriminator's reductions run under the remaining GEMMs).  Only the reduction of the chain
-    that finishes last is exposed.  Replaces the single 22 MB all-reduce after all chains joined (round 1: 24 x 136 us per iteration at
-    8 GPUs, none of it overlapped) -- Horovod's DistributedOptimizer also reduces gradients as they become ready (amp_agent.py:735-742)."""
+    that finishes last is exposed.  Replaces the single 22 MB all-reduce after all chains joined (none of it overlapped) -- Horovod's DistributedOptimizer also reduces gradients as they become ready (amp_agent.py:735-742)."""
 
     def __init__(self, world: int, num_chains: int = 3):
         self.world = world

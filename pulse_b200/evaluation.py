@@ -1,7 +1,7 @@
 """Evaluation over all clips of a MotionLib with the metrics on the device (SURVEY 8f-2).
 
 Host-side mirror of `IMAmpAgent.eval` / `_post_step_eval` (phc/learning/im_amp.py:136-363) and of
-`update_training_data` (:126-132), B200-first:
+`update_training_data` (:126-132), GPU-first:
 
   * the reference copies every env's 24 body positions (simulated and reference) to the host EVERY evaluation step
     (`extras['body_pos'] = body_pos.cpu().numpy()`, humanoid_im.py:664-673), keeps Python lists of frames and runs

@@ -1,4 +1,4 @@
-"""HumanoidIm per-step compute on the B200: host-side mirror of the reference task's
+"""HumanoidIm per-step compute on the GPU: host-side mirror of the reference task's
 `_compute_reward` / `_compute_reset` / `_compute_observations` / `_compute_amp_observations`
 (phc/env/tasks/humanoid_im.py, humanoid.py, humanoid_amp.py), backed by the fused CUDA kernels.
 

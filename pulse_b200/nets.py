@@ -1,8 +1,8 @@
-"""MLP stacks of the PULSE / PHC agents on the B200 tensor cores.
+"""MLP stacks of the PULSE / PHC agents on the H100 tensor cores.
 
 Mirrors what `phc.learning.network_builder.NetworkBuilder._build_mlp` + `AMPBuilder.Network`
 (network_builder.py:105-124, amp_network_builder.py:20-249) build -- Linear+activation stacks with a
-linear head -- but stores them for the tcgen05 GEMM: fp32 master weights in ONE flat buffer (so the
+linear head -- but stores them for the wgmma GEMM: fp32 master weights in ONE flat buffer (so the
 gradient all-reduce, the norm clip and Adam are single launches) with a bf16 mirror in the same
 layout that the Adam kernel writes -- the GEMM operands.  Nothing is ever transposed in memory: the
 GEMM reads K-major or MN-major operands as they sit (forward: X, W K-major; dgrad: dY K-major, W
@@ -30,12 +30,11 @@ def pad8(n: int) -> int:
 
 def pad_k(n: int) -> int:
     """Leading dimension of a GEMM operand with n useful columns: a multiple of 64 bf16 (128 bytes) once n > 64, so every
-    64-column TMA box row starts on a 128-byte line (a 936-wide row makes each box row straddle an extra 32-byte sector:
-    measured 54.7 -> 39.7 us on the 16384 x 1024 x 934 layer)."""
+    64-column TMA box row starts on a 128-byte line (a 936-wide row makes each box row straddle an extra 32-byte sector)."""
     return pad8(n) if n <= 64 else (n + 63) // 64 * 64
 
 
-def pick_split(tiles: int, num_kb: int, sms: int = 148, epilogue_kb: int = 24) -> int:
+def pick_split(tiles: int, num_kb: int, sms: int = 132, epilogue_kb: int = 24) -> int:
     """Split-K factor for a weight-gradient GEMM on the persistent kernel: minimise rounds x (k-blocks per item +
     epilogue cost in k-block equivalents), where rounds = ceil(tiles * splits / SMs)."""
     best, best_cost = 1, None
@@ -126,8 +125,8 @@ class FlatParams:
             a.grads[p], a.params[p], a.params_bf16[p], a.signals[p] = int(hg.buffer_ptrs[p]), int(hp.buffer_ptrs[p]), int(hb.buffer_ptrs[p]), int(hs.buffer_ptrs[p])
         if int(a.grads[rank]) != grads.data_ptr() or int(a.params[rank]) != params.data_ptr():
             raise RuntimeError("symmetric-memory handle does not describe the local tensors")
-        # multimem (NVLS) variant: measured 107 vs 112 us per step at 8 GPUs but 112 vs 75 us at 2 (profiles/r02_peer_adam_probe_n*.json):
-        # the switch-side reduction pays once the peer count makes the pull / push fan-out the bound
+        # multimem (NVLS) variant by default at 8 ranks: the switch-side reduction pays once the peer count makes the pull / push
+        # fan-out the bound
         mc_env = os.environ.get("PULSE_PEER_MC", "auto")
         use_mc = mc_env == "1" or (mc_env == "auto" and world >= 8)
         mc = [int(getattr(h, "multicast_ptr", 0) or 0) for h in (hg, hp, hb)]
@@ -232,7 +231,7 @@ class Dense:
     Bias-augmented (`aug`): ONE slot W [N, Kp] with Kp = pad_k(K + 1) whose column K holds the bias; the operand it multiplies carries
     1.0 in its column K (written by the normalise kernels / set once in the activation buffers), so the bias add of the forward pass
     and the bias gradient of the backward pass (column K of dW = dY^T [X | 1]) are done by the tensor cores -- no bias loads in the
-    forward epilogue, no column sums in the dgrad epilogue (both ran on the shared-memory pipe the UMMA operand reads saturate)."""
+    forward epilogue, no column sums in the dgrad epilogue."""
 
     def __init__(self, flat: FlatParams, in_features: int, out_features: int, act: Optional[str], aug: bool = False):
         self.K, self.N, self.act, self.aug = in_features, out_features, act, aug
@@ -350,7 +349,7 @@ class MLP:
                     ws["pre"].append(bf(M, l.Np) if (l.act == "silu") else None)
                     ws["dact"].append(None if last else bf(M, l.Np))      # gradient w.r.t. this layer's OUTPUT
                     ws["mask"].append(torch.zeros((l.N + 31) // 32, M, device=dev, dtype=torch.int32) if (l.act == "relu" and not last) else None)
-                    tiles = ((l.N + 127) // 128) * ((l.Kp + 255) // 256)   # 128 x 256 output tiles
+                    tiles = ((l.N + 127) // 128) * ((l.Kp + 127) // 128)   # 128 x 128 output tiles
                     ws["split"].append(pick_split(tiles, (M + 63) // 64))
             hn = self.layers[-1].N     # fp32 head output: rows padded to a multiple of 4 floats so the epilogue's 16-byte stores apply (N = 69)
             ws["out"] = torch.zeros(M, (hn + 3) // 4 * 4, device=dev)[:, :hn]
@@ -442,9 +441,11 @@ class MLP:
             else:
                 hb, pb = head.bias_grad, self.flat.view_padded(prev.b_idx, "grads", prev.Np)
             with torch.cuda.device(dev):
+                if "head1_partials" not in ws:
+                    ws["head1_partials"] = torch.empty(_lib.HEAD1_MAX_CTAS * (2 * head.Kp + 1), device=dev)
                 _lib.check(lib.pulse_head1_backward(h.data_ptr(), h.stride(0), M, head.Kp, dout.data_ptr(), dout.stride(0), head.w_bf16.data_ptr(),
                                                     dh.data_ptr(), dh.stride(0), head.weight_grad.data_ptr(), hb.data_ptr(), pb.data_ptr(),
-                                                    _lib.current_stream(dev)), "pulse_head1_backward")
+                                                    ws["head1_partials"].data_ptr(), _lib.current_stream(dev)), "pulse_head1_backward")
             return dh, top - 1
         if not self.aug:
             with torch.cuda.device(dev):  # bias gradient of the head: column sums of dout
@@ -518,8 +519,8 @@ def normalize_to_bf16(x: torch.Tensor, mean: Optional[torch.Tensor], rstd: Optio
 
 # ---------------------------------------------------------------------------------------------------------------------------
 # Lock-step execution of several MLPs of the same depth through GROUPED launches (pulse_gemm_bf16_grouped): the hidden layers of
-# all nets in one persistent launch per layer, likewise their weight-gradient and their dgrad GEMMs.  EXPERIMENTAL in round 1
-# (compiled, not yet run on a device); used only when PULSE_GROUPED=1 (dense.grouped_enabled()).  MLP.forward / MLP.backward
+# all nets in one persistent launch per layer, likewise their weight-gradient and their dgrad GEMMs.  Validated against the
+# three-stream path by tests/test_gpu_grouped.py; used only when PULSE_GROUPED=1 (dense.grouped_enabled()).  MLP.forward / MLP.backward
 # above remain the validated path and are not touched by this code.
 # ---------------------------------------------------------------------------------------------------------------------------
 def forward_lockstep(mlps: Sequence["MLP"], xs: Sequence[torch.Tensor], train: bool = False) -> List[torch.Tensor]:

@@ -1,4 +1,4 @@
-"""PPO actor / critic on the B200: host-side mirror of the agent-side arithmetic of
+"""PPO actor / critic on the GPU: host-side mirror of the agent-side arithmetic of
 `phc.learning.common_agent.CommonAgent` / `amp_agent.AMPAgent` for the continuous-action 'amp' network
 (separate actor and critic MLPs, fixed log-std; im.yaml:13-42):
 
@@ -296,10 +296,9 @@ class PPOPolicy:
 
         self.flat.begin_backward()                                # weight / bias gradients are accumulated by bulk reductions / atomics
         reducer = self._reducer(world_size)                  # multi-GPU: every chain averages ITS gradient slice on its own stream
-        # Measured at 2 GPUs (profiles/r02_grad_reduce_ab.txt): reducing every chain's slice on its own stream ("chain") is SLOWER than one
-        # all-reduce after the join (72.2 vs 69.8 ms update phase): the persistent GEMMs own all 148 SMs and walk a static tile schedule,
-        # so NCCL's CTAs either wait for a GEMM to drain or delay the CTAs of the next one -- the collective is not hidden, it is
-        # interleaved.  Default: one all-reduce; PULSE_GRAD_REDUCE=chain keeps the per-chain variant for experiments.
+        # Reducing every chain's slice on its own stream ("chain") does not hide the collective: the persistent GEMMs own every SM and
+        # walk a static tile schedule, so NCCL's CTAs either wait for a GEMM to drain or delay the CTAs of the next one -- the collective
+        # is interleaved, not overlapped.  Default: one all-reduce; PULSE_GRAD_REDUCE=chain keeps the per-chain variant for experiments.
         single = reducer is not None and os.environ.get("PULSE_GRAD_REDUCE", "single") != "chain"
         if single:
             reducer = None

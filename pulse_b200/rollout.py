@@ -82,7 +82,7 @@ class PlayStepsB200:
         self.physics = None
         # Independent pieces of a step run on a second stream (fork / join inside the captured segment): the AMP row beside the
         # next-value critic, the critic beside the actor.  At 2048 envs per rank (8 GPUs) every kernel of the step is latency-bound
-        # (7-17 us each, profiles/r02_rollout_step_2048envs_launches.txt), so the step time is the length of the dependency chain.
+        # so the step time is the length of the dependency chain.
         self.fork = os.environ.get("PULSE_ROLLOUT_FORK", "1") != "0"
         self.overlap = os.environ.get("PULSE_ROLLOUT_OVERLAP", "1") != "0"   # next values of step t beside reset / actor of step t+1 (_whole_overlapped)
         self._side = None
@@ -185,7 +185,7 @@ class PlayStepsB200:
            that B's normalise reads (main waits for the event B records after it); the step kernel(t+1) rewrites `terminate_buf` that
            B's value_post reads (main waits for B).  The reset does not clear `terminate_buf` here (the step kernel rewrites it for
            every env each step; nothing else reads it in between).  At 2048 envs per rank the step is a chain of latency-bound
-           launches: 142 -> ~110 us per step."""
+           launches."""
         s, pol, T = self.sim, self.policy, self.T
         main = torch.cuda.current_stream(self.dev)
         A = self._side_stream()

@@ -1,4 +1,4 @@
-"""PULSE VAE distillation on the B200 (SURVEY K17-K20): host-side mirror of
+"""PULSE VAE distillation on the GPU (SURVEY K17-K20): host-side mirror of
 
   AMPZBuilder.Network            phc/learning/amp_network_z_builder.py:24-557   -> PulseVAE (encoder / prior / decoder / critic stacks)
     eval_actor(return_extra)     :341-467, form_embedding :79-121               -> PulseVAE.eval_actor
@@ -9,7 +9,7 @@
   HumanoidZ.compute_z_actions    phc/env/tasks/humanoid_z.py:81-155             -> PulseVAE.compute_z_actions
   Humanoid._action_to_pd_targets phc/env/tasks/humanoid.py:1222-1247,1392-1394  -> pd_targets
 
-Every dense layer is a tcgen05 GEMM (`pulse_gemm_bf16`), forward and explicit backward; the row-wise pieces between them are
+Every dense layer is a wgmma GEMM (`pulse_gemm_bf16`), forward and explicit backward; the row-wise pieces between them are
 the kernels of csrc/vae_ops.cu.  Layout notes:
   * the decoder input is stored as [z (E) | self_obs (S) | 0-pad], i.e. the reference's `cat([self_obs, z])` with the two
     blocks swapped, so the latent window starts on a 16-byte boundary (its input gradient is one small GEMM on W0[:, :E]);

@@ -3,8 +3,8 @@
 Isaac Gym and rl_games are not installable (SURVEY.md 8c), so `HumanoidImB200Mixin` / `AMPAgentB200Mixin` cannot be mixed in front of
 the real `phc.env.tasks.humanoid_im.HumanoidIm` / `phc.learning.im_amp.IMAmpAgent` here.  These classes carry exactly the part of the
 reference's attribute / method contract the mixins touch -- names, shapes, dtypes and call order as in the cited reference lines -- and
-nothing else.  tests/test_boundary_cpu.py checks, where /root/reference exists, that every name used here occurs in the unmodified
-reference sources it is cited from.
+nothing else.  tests/test_boundary_cpu.py checks that every name used here occurs in the unmodified reference sources it is cited from,
+against the pairs recorded from those sources (tests/golden/contract_names.json, make_golden_contract.py).
 """
 import types
 

@@ -30,7 +30,7 @@ def test_header_symbols_exported(lib):
     for n in names:
         assert hasattr(lib, n), f"{n} declared in include/pulse_b200.h but not exported"
         assert n in _lib.SIGNATURES, f"{n} has no ctypes signature in pulse_b200/_lib.py"
-    assert lib.pulse_abi_version() == 2
+    assert lib.pulse_abi_version() == 3
 
 
 def test_struct_sizes_match_header(lib):

@@ -1,27 +1,21 @@
 """CPU checks of the drop-in layer's CONTRACT: (1) every reference attribute / method name the stand-ins carry (tests/standins.CONTRACT)
-occurs in the unmodified reference file it is cited from -- run where /root/reference exists; (2) every attribute the mixins read from
-`self` is either defined by the mixin, listed in the contract, or private to the mixin (`_pulse*`) -- so the stand-ins cannot silently
-drift from what the mixins need."""
+occurs in the unmodified reference file it is cited from -- against the pairs recorded from those files (tests/golden/contract_names.json,
+make_golden_contract.py); (2) every attribute the mixins read from `self` is either defined by the mixin, listed in the contract, or
+private to the mixin (`_pulse*`) -- so the stand-ins cannot silently drift from what the mixins need."""
 import ast
+import json
 import os
-import re
 
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get("PULSE_REFERENCE_ROOT", "/root/reference")
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree only exists in the build container")
 def test_contract_names_exist_in_the_reference_sources():
     from tests.standins import CONTRACT
-    missing = []
-    for side in CONTRACT.values():
-        for rel, names in side.items():
-            src = open(os.path.join(REF, rel)).read()
-            for n in names:
-                if not re.search(r"\b" + re.escape(n) + r"\b", src):
-                    missing.append((rel, n))
+    with open(os.path.join(ROOT, "tests", "golden", "contract_names.json")) as f:
+        recorded = {rel: set(names) for rel, names in json.load(f).items()}
+    missing = [(rel, n) for side in CONTRACT.values() for rel, names in side.items() for n in names if n not in recorded.get(rel, ())]
     assert not missing, missing
 
 

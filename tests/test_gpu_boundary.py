@@ -1,5 +1,6 @@
 """The drop-in layer EXECUTED: `HumanoidImB200Mixin` and `AMPAgentB200Mixin` mixed in front of stand-in base classes that carry the
-reference's attribute / method contract (tests/standins.py; checked against the reference sources by tests/test_boundary_cpu.py).
+reference's attribute / method contract (tests/standins.py; checked against names recorded from the reference sources by
+tests/test_boundary_cpu.py).
 
   task  : Humanoid.post_physics_step -> _compute_reward -> _compute_reset -> _compute_observations -> AMP history + observation
           (humanoid.py:1315-1346, humanoid_amp.py:194-210) against the oracle; the getup recovery masking (humanoid_im_getup.py:203-210)

@@ -1,4 +1,4 @@
-"""tcgen05 bf16 GEMM vs a plain PyTorch fp32 reference of the same op (bf16-rounded inputs)."""
+"""wgmma bf16 GEMM vs a plain PyTorch fp32 reference of the same op (bf16-rounded inputs)."""
 import pytest
 import torch
 

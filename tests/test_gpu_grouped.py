@@ -1,6 +1,5 @@
-"""EXPERIMENTAL grouped GEMM launches (several problems per persistent launch) and the lock-step actor + critic update built
-on them.  Opt-in: the grouped kernel was written after round 1's GPU budget was spent and has not run on a device yet; set
-PULSE_GROUPED_TEST=1 to run these tests (the product path does not use grouped launches unless PULSE_GROUPED=1)."""
+"""Grouped GEMM launches (several problems per persistent launch) and the lock-step actor + critic update built on them (the
+product path does not use grouped launches unless PULSE_GROUPED=1)."""
 import pytest
 import torch
 
@@ -58,8 +57,11 @@ def test_ppo_minibatch_grouped_matches_three_stream_path(monkeypatch):
     g = torch.Generator(device=DEV).manual_seed(3)
     M = 2048
     obs = torch.randn(M, 934, device=DEV, generator=g)
-    act = torch.randn(M, 69, device=DEV, generator=g) * 0.1
-    nlp = torch.randn(M, device=DEV, generator=g) + 60
+    # a PPO minibatch as a rollout hands it over: actions drawn by the same policy, old neglogp close to the current one (ratios
+    # around 1, some clipped).  Far-off old neglogp overflows exp(old - new) in fp32 and makes both paths' gradients NaN.
+    drawn = PPOPolicy(device=DEV, seed=5).act(obs, eps=torch.randn(M, 69, device=DEV, generator=g))
+    act = drawn["actions"].clone()
+    nlp = drawn["neglogpacs"].clone() + 0.3 * torch.randn(M, device=DEV, generator=g)
     adv, ret = torch.randn(M, device=DEV, generator=g), torch.randn(M, device=DEV, generator=g)
     results = []
     for flag in ("0", "1"):

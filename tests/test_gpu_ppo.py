@@ -236,8 +236,9 @@ def test_single_output_head_kernels(rows, k):
     torch.testing.assert_close(out[:, 0], ref, atol=1e-4, rtol=1e-4)
     dh = torch.full((rows, k), 3.0, device=DEV, dtype=torch.bfloat16)
     dw, db, dbp = torch.ones(k, device=DEV), torch.ones(1, device=DEV), torch.ones(k, device=DEV)
+    part = torch.empty(_lib.HEAD1_MAX_CTAS * (2 * k + 1), device=DEV)
     _lib.check(lib.pulse_head1_backward(h.data_ptr(), h.stride(0), rows, k, dv.data_ptr(), dv.stride(0), w.data_ptr(), dh.data_ptr(), dh.stride(0),
-                                        dw.data_ptr(), db.data_ptr(), dbp.data_ptr(), st), "bwd")
+                                        dw.data_ptr(), db.data_ptr(), dbp.data_ptr(), part.data_ptr(), st), "bwd")
     d = dv[:, 0].float()
     dh_ref = d[:, None] * w.float()[None, :] * (h.float() > 0)
     assert torch.equal(dh, dh_ref.bfloat16())                          # single products: exact up to the bf16 rounding

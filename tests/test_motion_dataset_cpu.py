@@ -1,10 +1,6 @@
 """Host-side MotionLib dataset logic (pulse_b200/motion_dataset.py) without a GPU: clip selection, heading draws and the PMCP
-sampling-weight updates against the reference's own methods (live, when /root/reference exists) and the committed fixtures."""
-import os
-import types
-
+sampling-weight updates against fixtures written by the reference's own methods."""
 import numpy as np
-import pytest
 import torch
 
 from tests.helpers import load_npz
@@ -44,23 +40,14 @@ def test_selection_and_sampling_weights():
     assert ds.crop(ds._motion_data_list[0], max_len=-1) is ds._motion_data_list[0]
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="reference tree only exists in the build container")
-def test_sampling_weights_against_live_reference():
-    import sys
-    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "refshim"))
-    from load_reference import load_reference
-    ref = load_reference()
-    Base = ref.motion_lib_base.MotionLibBase
-    keys = np.array([f"clip_{i:02d}" for i in range(6)])
-    fake = types.SimpleNamespace(_motion_data_keys=keys, _num_unique_motions=6, _device="cpu", _sampling_prob=torch.ones(6) / 6,
-                                 _termination_history=torch.zeros(6))
-    fake.update_sampling_prob = types.MethodType(Base.update_sampling_prob, fake)
+def test_sampling_weights_against_reference_pins():
+    """PMCP soft / hard sampling-weight updates against what the reference's MotionLibBase methods computed for the same
+    sequence of failed clips (tests/golden/reference_pins.npz, make_golden_reference_pins.py)."""
+    g = load_npz("reference_pins.npz")
     ds = _dataset()
-    for failed in (["clip_02"], ["clip_02", "clip_05"], [], ["clip_00", "clip_01", "clip_04"]):
-        Base.update_soft_sampling_weight(fake, failed)
+    for i, failed in enumerate((["clip_02"], ["clip_02", "clip_05"], [], ["clip_00", "clip_01", "clip_04"])):
         ds.update_soft_sampling_weight(failed)
-        assert torch.allclose(ds._sampling_prob, fake._sampling_prob.float())
-    for failed in (["clip_03"], [], ["clip_01", "clip_05"]):
-        Base.update_hard_sampling_weight(fake, failed)
+        assert torch.allclose(ds._sampling_prob, g[f"soft_prob_{i}"].float())
+    for i, failed in enumerate((["clip_03"], [], ["clip_01", "clip_05"])):
         ds.update_hard_sampling_weight(failed)
-        assert torch.allclose(ds._sampling_prob, fake._sampling_prob.float())
+        assert torch.allclose(ds._sampling_prob, g[f"hard_prob_{i}"].float())

@@ -143,31 +143,23 @@ def test_agent_arithmetic():
     assert float(rms.count) == float(z["rms_count"])
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="reference tree only exists in the build container")
-def test_oracle_against_live_reference():
-    """Re-pin against the reference itself on fresh random inputs (container only)."""
-    import sys
-    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "refshim"))
-    from load_reference import load_reference
-    ref = load_reference()
-    g = torch.Generator().manual_seed(123)
-    n = 500
-    unit = lambda x: torch.nn.functional.normalize(x, dim=-1)
-    pos, vel, ang = (torch.randn(n, 24, 3, generator=g) for _ in range(3))
-    rot = unit(torch.randn(n, 24, 4, generator=g))
-    rpos, rvel, rang = (torch.randn(n, 24, 3, generator=g) for _ in range(3))
-    rrot = unit(torch.randn(n, 24, 4, generator=g))
-    empty = torch.zeros(n, 0)
-    a = ref.humanoid.compute_humanoid_observations_smpl_max(pos, rot, vel, ang, empty, empty, True, True, True, False, False)
-    close(po.self_obs_smpl_max(pos, rot, vel, ang), a)
-    b = ref.humanoid_im.compute_imitation_observations_v6(pos[:, 0], rot[:, 0], pos, rot, vel, ang, rpos, rrot, rvel, rang, 1, True)
-    close(po.imitation_obs_v6(pos[:, 0], rot[:, 0], pos, rot, vel, ang, rpos, rrot, rvel, rang), b)
-    r, raw = ref.humanoid_im.compute_imitation_reward(pos[:, 0], rot[:, 0], pos, rot, vel, ang, rpos, rrot, rvel, rang, dict(po.REWARD_SPECS))
+def test_oracle_against_reference_pins():
+    """The oracle against the reference's own functions on fresh seeded inputs (tests/golden/reference_pins.npz,
+    make_golden_reference_pins.py: every 8th observation / reward row, every 4th slerp row)."""
+    import importlib.util
+    spec = importlib.util.spec_from_file_location("make_golden_reference_pins", os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden",
+                                                                                              "make_golden_reference_pins.py"))
+    m = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(m)
+    g = load_npz("reference_pins.npz")
+    z, chk = m.pin_inputs()
+    assert abs(chk - float(g["checksum"])) < 1e-9 * abs(chk)
+    pos, rot, vel, ang, rpos, rrot, rvel, rang = (z[k] for k in ("pos", "rot", "vel", "ang", "rpos", "rrot", "rvel", "rang"))
+    close(po.self_obs_smpl_max(pos, rot, vel, ang)[m.ROWS], g["self_obs"])
+    close(po.imitation_obs_v6(pos[:, 0], rot[:, 0], pos, rot, vel, ang, rpos, rrot, rvel, rang)[m.ROWS], g["imitation_obs_v6"])
     r2, raw2 = po.imitation_reward(pos, rot, vel, ang, rpos, rrot, rvel, rang)
-    close(r2, r); close(raw2, raw)
-    q0, q1 = unit(torch.randn(4000, 4, generator=g)), unit(torch.randn(4000, 4, generator=g))
-    t = torch.rand(4000, 1, generator=g)
-    close(po.slerp(q0, q1, t), ref.torch_utils.slerp(q0, q1, t))
+    close(r2[m.ROWS], g["reward"]); close(raw2[m.ROWS], g["reward_raw"])
+    close(po.slerp(z["q0"], z["q1"], z["t"])[m.SLERP_ROWS], g["slerp"])
 
 
 def test_vae_distillation_teacher_zdecode_reach_pd():

@@ -1,4 +1,4 @@
-"""GEMM micro-benchmark: tcgen05 kernel vs torch.matmul (cuBLAS) at the MLP shapes."""
+"""GEMM micro-benchmark: wgmma kernel vs torch.matmul (cuBLAS) at the MLP shapes."""
 import json
 import os
 import sys

@@ -164,7 +164,7 @@ def bench_vae(a, dev):
     teach = 3 * macs([960, 1024, 512, 69]) + macs([960, 1024, 512, 3])
     roll = enc + dec + critic + teach
     peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-    peak_tf = float(peaks.get("bf16_tflops_sustained", 1400.0))
+    peak_tf = float(peaks.get("bf16_tflops_sustained", 989.0))   # fallback: H100 SXM data sheet, dense bf16
     L = vae.losses(MINIBATCH)
     return {
         "workload": "PULSE VAE distillation (BASELINE configs[2]): %d envs, horizon 32, im_z_fit.yaml nets, minibatch 16384, 6 mini-epochs" % n,
@@ -282,7 +282,7 @@ def bench_reach(a, dev):
     zdec = macs([384, 1536, 1024, 512, 64]) + macs([448, 3096, 2048, 1024, 69])
     upd = 3 * (pol + crit) - 2 * 384 * 2048
     peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-    peak_tf = float(peaks.get("bf16_tflops_sustained", 1400.0))
+    peak_tf = float(peaks.get("bf16_tflops_sustained", 989.0))   # fallback: H100 SXM data sheet, dense bf16
     upd_flops = 2.0 * MINI_EPOCHS * upd * T * n
     return {
         "workload": "latent-space reach task (BASELINE configs[4]): %d envs on this GPU, frozen PULSE prior + decoder, pulse_z_task.yaml policy" % n,

@@ -38,11 +38,11 @@ def main():
     ap.add_argument("--vae", action="store_true", help="the SiLU stacks of the PULSE VAE (im_z_fit.yaml) instead of the PPO nets")
     a = ap.parse_args()
     dev = torch.device("cuda:0")
-    peaks = {"bf16": 1514.7, "hbm": 6481.8}
+    peaks = {"bf16": 989.0, "hbm": 3350.0}   # fallback: H100 SXM data sheet (dense bf16 TFLOP/s, HBM3 GB/s)
     p = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        peaks = {"bf16": d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1514.7)), "hbm": d.get("hbm_gbs", 6481.8)}
+        peaks = {"bf16": d.get("bf16_tflops_sustained", d.get("bf16_tflops", peaks["bf16"])), "hbm": d.get("hbm_gbs", peaks["hbm"])}
     bf = lambda r, c: (torch.randn(r, c, device=dev) * 0.1).bfloat16()
     rows = []
 
@@ -65,7 +65,7 @@ def main():
             kw.update(a_mn=True, b_mn=True)
         byt = av.numel() * 2 + bv.numel() * 2
         if kind == "wgrad":
-            tiles = ((M + 127) // 128) * ((N + 255) // 256)
+            tiles = ((M + 127) // 128) * ((N + 127) // 128)
             kw.update(out_f32=torch.zeros(M, Np, device=dev), accumulate=True, split_k=pick_split(tiles, (K + 63) // 64))
             byt += M * N * 4 * 2
         else:

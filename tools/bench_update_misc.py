@@ -41,7 +41,7 @@ def main():
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
     dev = torch.device("cuda:0")
-    hbm = 6481.8
+    hbm = 3350.0   # fallback: H100 SXM data sheet HBM3 bandwidth
     p = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")
     if os.path.exists(p):
         hbm = json.load(open(p)).get("hbm_gbs", hbm)

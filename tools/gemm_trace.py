@@ -1,5 +1,5 @@
 """Development tool: per-phase clock trace of CTA 0 of one GEMM launch.  Needs the trace build:
-    tools/build_variant.sh trace gemm_tcgen05.cu -DPULSE_GEMM_VARIANT=3
+    tools/build_variant.sh trace gemm_wgmma.cu -DPULSE_GEMM_VARIANT=3
     PULSE_ALT_LIB=$PWD/pulse_b200/build/libpulse_trace.so python tools/gemm_trace.py"""
 import ctypes as C
 import os
@@ -12,10 +12,9 @@ from pulse_b200 import _lib  # noqa: E402
 _lib.LIB_PATH = os.environ["PULSE_ALT_LIB"]
 from pulse_b200.dense import gemm  # noqa: E402
 
-NAMES = {0: "start", 1: "setup done", 2: "producer past griddep wait", 3: "first stage landed", 12: "item0 last kb landed", 4: "item0 MMAs committed",
-         16: "epi item0 tmem_full", 17: "epi item0 done", 13: "item1 last kb landed", 5: "item1 MMAs committed", 18: "epi item1 tmem_full",
-         19: "epi item1 done", 22: "  i1 c0 top", 23: "  i1 c0 tmem data ready", 24: "  i1 c0 math done", 25: "  i1 c0 stored",
-         26: "  i1 c1 top", 27: "  i1 c1 tmem data ready", 28: "  i1 c1 math done", 29: "  i1 c1 stored", 14: "item2 last kb landed", 6: "item2 committed", 20: "epi item2 tmem_full", 21: "epi item2 done", 10: "teardown"}
+NAMES = {0: "start", 1: "setup done", 2: "producer past griddep wait", 3: "first stage landed", 4: "item0 MMAs retired", 16: "epi item0 staged",
+         17: "epi item0 done", 5: "item1 MMAs retired", 18: "epi item1 staged", 19: "epi item1 done", 6: "item2 MMAs retired",
+         20: "epi item2 staged", 21: "epi item2 done", 10: "teardown"}
 
 
 def main():
@@ -40,7 +39,7 @@ def main():
             buf = (C.c_longlong * 32)()
             lib.pulse_debug_gemm_trace(buf)
             t0 = buf[0]
-            print(f"--- {name}  PULSE_GEMM_PAIR={os.environ.get('PULSE_GEMM_PAIR', '1')}")
+            print(f"--- {name}")
             for slot, t in sorted(((s, buf[s]) for s in NAMES if buf[s] >= t0), key=lambda x: x[1]):
                 print(f"   {t - t0:8d} cyc  {NAMES[slot]}")
             break

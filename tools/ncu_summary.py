@@ -1,4 +1,4 @@
-"""Summarise an .ncu-rep (raw page) into the handful of numbers DESIGN.md / profiles/ quote."""
+"""Summarise an .ncu-rep (raw page) into a handful of numbers (time, DRAM bytes, pipe use)."""
 import csv
 import subprocess
 import sys

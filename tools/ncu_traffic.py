@@ -1,5 +1,5 @@
-"""Extract the DRAM traffic of one kernel launch from an .ncu-rep (`ncu --set full`) into the JSON bench.py reads for
-`roofline.traffic` (profiles/im_step_traffic.json).  usage: ncu_traffic.py <report.ncu-rep> <kernel substring> <envs> <out.json>"""
+"""Extract the DRAM traffic of one kernel launch from an .ncu-rep (`ncu --set full`) into a JSON
+file.  usage: ncu_traffic.py <report.ncu-rep> <kernel substring> <envs> <out.json>"""
 import csv
 import json
 import subprocess

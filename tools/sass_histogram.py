@@ -1,7 +1,7 @@
 """SASS opcode histogram per kernel of libpulse_b200.so (cuobjdump -sass): evidence of WHICH hardware paths each kernel uses
-(UTCHMMA = tcgen05.mma, LDTM = tcgen05.ld, UTMALDG / UTMAREDG = TMA tensor load / reduction, UBLKCP = bulk async copy, ...).
+(HGMMA = wgmma.mma_async, UTMALDG / UTMAREDG = TMA tensor load / reduction, UBLKCP = bulk async copy, ...).
 
-    python tools/sass_histogram.py > profiles/r02_sass_histogram.txt
+    python tools/sass_histogram.py > sass_histogram.txt
 """
 import collections
 import os
