@@ -654,6 +654,80 @@ typedef struct {
 int pulse_ztask_step(const pulse_ztask_step_args_t* args, int64_t num_envs, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Pedestrian terrain task HumanoidPedestrianTerrain(Z) (phc/env/tasks/humanoid_pedestrian_terrain.py): post_physics_step in one launch,
+ * one warp per env, selected by PULSE_STEP_REWARD / RESET / OBS:
+ *   reward  _compute_reward :871-896: exp(-2 |tar - actor root|^2_xy) at tar = calc_pos(progress * dt) (fuzzy: errors < 0.0025 -> 0,
+ *           :1633-1646); power = -coef * sum |dof_force * dof_vel| always in reward_raw[:, 1], added to rew only with power_reward.
+ *   reset   compute_humanoid_reset :1477-1531: |sum of the contact forces of the non-contact bodies| > 50 and progress > 1, or the
+ *           rigid-body root farther than fail_dist from tar (xy); no_collision_check clears both; progress >= max_len - 1 resets.
+ *   obs     [self 358 | trajectory 2T | heights P]: the self observation with the mean center height around the rigid-body root
+ *           subtracted from every body's z (:195-223); trajectory samples at progress * dt + k * traj_sample_timestep in the actor
+ *           root's heading frame (:385-440, :1588-1616); heights at the head pose (:296-311, :718-772), clip(ref - h, -3, 3) * 5 with
+ *           ref = the mean center height around the actor root (use_center_height) or the actor root's z.
+ * Heights: Terrain.world_points_to_map / sample_height_points (:1191-1198, :1261-1267) on the int16 heightfield [rows, cols]
+ * (row = x cell), or 0 everywhere for a plane (heightfield NULL).  Trajectories: TrajGenerator.calc_pos (phc/utils/traj_generator.py:
+ * 148-165) on traj_verts [N, PULSE_TRAJ_VERTS, 3]; traj_dur = num_verts * the generator's dt (the reference's divisor).
+ * env_ids (+ optional device-side env_count) restricts an OBS-only call to the listed envs (_compute_observations(env_ids)).
+ * Not covered: group observations, the velocity map, mesh terrain, shape observations.
+ * ---------------------------------------------------------------------------------------------- */
+#define PULSE_TRAJ_VERTS 101
+#define PULSE_TRAJ_DRAWS (4 * (PULSE_TRAJ_VERTS - 1) + 2)
+#define PULSE_TERRAIN_OBS 1402      /* 358 + 2 * 10 + 32 * 32 (env_pulse_terrain.yaml) */
+typedef struct {
+  uint32_t flags;                                            /* PULSE_STEP_REWARD | PULSE_STEP_RESET | PULSE_STEP_OBS */
+  int32_t upright;                                           /* _has_upright_start (else remove_base_rot) */
+  const float* body_state; int64_t body_env_stride;          /* rigid bodies [N, >=24, 13] */
+  const float* root_states; int64_t root_env_stride;         /* actor root state [N, 13] view (_humanoid_root_states) */
+  const int64_t* progress_buf; int64_t max_episode_length;
+  const float* contact_forces; int64_t contact_env_stride;   /* [N, >=24, 3] */
+  uint32_t contact_body_mask;                                /* _contact_body_ids */
+  int32_t enable_early_termination, no_collision_check, fuzzy_target, power_reward;
+  int32_t num_traj_samples, num_height_points, num_center_points, head_body_id, use_center_height;
+  float dt, traj_dur, traj_sample_timestep, fail_dist, power_coefficient;
+  const float* traj_verts;                                   /* [N, PULSE_TRAJ_VERTS, 3] */
+  const int16_t* heightfield; int64_t hf_rows, hf_cols;      /* NULL = plane */
+  float horizontal_scale, vertical_scale;
+  const float* height_points;                                /* [num_height_points, 3] sensor offsets (square / fov / square_fov) */
+  const float* center_points;                                /* [num_center_points, 3] (the 3 x 3 grid of init_center_height_points) */
+  const float* dof_force; int64_t dof_force_stride;          /* [N, 69]: the power term; required with power_reward or reward_raw */
+  const float* dof_vel; int64_t dof_env_stride, dof_elem_stride;
+  const int64_t* env_ids; const int32_t* env_count;          /* optional, OBS only */
+  float* obs_buf; int64_t obs_stride;
+  float* rew_buf; float* reward_raw; int64_t raw_stride;     /* reward_raw [N, 2] or NULL */
+  int64_t* reset_buf; int64_t* terminate_buf;
+} pulse_terrain_step_args_t;
+int pulse_terrain_step(const pulse_terrain_step_args_t* args, int64_t num_envs, void* stream);
+
+/* TrajGenerator.reset (phc/utils/traj_generator.py:57-112) for num_ids envs, one thread each: random turns (sharp turns with
+ * probability sharp_turn_prob), the clipped speed recurrence, waypoints from init_pos's xy (row i belongs to env_ids[i]).  rand
+ * [num_ids, PULSE_TRAJ_DRAWS] injects the uniform draws (layout in terrain.cu); NULL draws them with Philox4x32-10 keyed by
+ * (seed, env, offset + *offset_dev + k), k < PULSE_TRAJ_VERTS -- a different stream from torch's generator, the same distribution.
+ * dtheta_scale = dtheta_max * dt, dspeed_scale = accel_max * dt, seg_dt = dt, with dt = episode_dur / (num_verts - 1). */
+typedef struct {
+  const int64_t* env_ids; int64_t num_ids;
+  const float* init_pos; int64_t init_stride;
+  const float* rand;
+  uint64_t seed, offset; const uint64_t* offset_dev;
+  float dtheta_scale, dspeed_scale, seg_dt, speed_min, speed_max, sharp_turn_prob;
+  float* verts;                                              /* [N, PULSE_TRAJ_VERTS, 3] */
+} pulse_traj_reset_args_t;
+int pulse_traj_reset(const pulse_traj_reset_args_t* args, void* stream);
+
+/* get_center_heights (PULSE_HEIGHTS_CENTER: points rotated by the yaw of the root, quat_apply_yaw :1571-1576) or get_heights
+ * (PULSE_HEIGHTS_GRID: by calc_heading_quat) for num_rows root states [pos 3 | quat 4], heights [num_rows, num_points]. */
+#define PULSE_HEIGHTS_CENTER 1
+#define PULSE_HEIGHTS_GRID 2
+typedef struct {
+  int32_t mode, upright;
+  const float* root_states; int64_t root_stride; int64_t num_rows;
+  const float* points; int64_t num_points;
+  const int16_t* heightfield; int64_t hf_rows, hf_cols;
+  float horizontal_scale, vertical_scale;
+  float* heights; int64_t heights_stride;
+} pulse_terrain_heights_args_t;
+int pulse_terrain_heights(const pulse_terrain_heights_args_t* args, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Task observation for every observation version / tracked-body subset / number of future samples (SURVEY 8f-4): replaces the
  * dispatch of HumanoidIm._compute_task_obs (phc/env/tasks/humanoid_im.py:757-833) over compute_imitation_observations (:1222-1258,
  * obs_v 1), _v2 (:1261-1301), _v3 (:1304-1326), _v6 (:1328-1378, obs_v 4 / 6), _v7 (:1381-1413), _v8 (:1415-1479, time_steps 1) and

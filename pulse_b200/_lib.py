@@ -192,6 +192,44 @@ class ZTaskStepArgs(C.Structure):
 ZTASK_SPEED, ZTASK_STRIKE = 1, 2
 
 
+class TerrainStepArgs(C.Structure):
+    _fields_ = [
+        ("flags", C.c_uint32), ("upright", C.c_int32), ("body_state", C.c_void_p), ("body_env_stride", C.c_int64),
+        ("root_states", C.c_void_p), ("root_env_stride", C.c_int64), ("progress_buf", C.c_void_p), ("max_episode_length", C.c_int64),
+        ("contact_forces", C.c_void_p), ("contact_env_stride", C.c_int64), ("contact_body_mask", C.c_uint32),
+        ("enable_early_termination", C.c_int32), ("no_collision_check", C.c_int32), ("fuzzy_target", C.c_int32), ("power_reward", C.c_int32),
+        ("num_traj_samples", C.c_int32), ("num_height_points", C.c_int32), ("num_center_points", C.c_int32), ("head_body_id", C.c_int32),
+        ("use_center_height", C.c_int32), ("dt", C.c_float), ("traj_dur", C.c_float), ("traj_sample_timestep", C.c_float),
+        ("fail_dist", C.c_float), ("power_coefficient", C.c_float), ("traj_verts", C.c_void_p),
+        ("heightfield", C.c_void_p), ("hf_rows", C.c_int64), ("hf_cols", C.c_int64), ("horizontal_scale", C.c_float), ("vertical_scale", C.c_float),
+        ("height_points", C.c_void_p), ("center_points", C.c_void_p), ("dof_force", C.c_void_p), ("dof_force_stride", C.c_int64),
+        ("dof_vel", C.c_void_p), ("dof_env_stride", C.c_int64), ("dof_elem_stride", C.c_int64), ("env_ids", C.c_void_p), ("env_count", C.c_void_p),
+        ("obs_buf", C.c_void_p), ("obs_stride", C.c_int64), ("rew_buf", C.c_void_p), ("reward_raw", C.c_void_p), ("raw_stride", C.c_int64),
+        ("reset_buf", C.c_void_p), ("terminate_buf", C.c_void_p),
+    ]
+
+
+class TrajResetArgs(C.Structure):
+    _fields_ = [
+        ("env_ids", C.c_void_p), ("num_ids", C.c_int64), ("init_pos", C.c_void_p), ("init_stride", C.c_int64), ("rand", C.c_void_p),
+        ("seed", C.c_uint64), ("offset", C.c_uint64), ("offset_dev", C.c_void_p), ("dtheta_scale", C.c_float), ("dspeed_scale", C.c_float),
+        ("seg_dt", C.c_float), ("speed_min", C.c_float), ("speed_max", C.c_float), ("sharp_turn_prob", C.c_float), ("verts", C.c_void_p),
+    ]
+
+
+class TerrainHeightsArgs(C.Structure):
+    _fields_ = [
+        ("mode", C.c_int32), ("upright", C.c_int32), ("root_states", C.c_void_p), ("root_stride", C.c_int64), ("num_rows", C.c_int64),
+        ("points", C.c_void_p), ("num_points", C.c_int64), ("heightfield", C.c_void_p), ("hf_rows", C.c_int64), ("hf_cols", C.c_int64),
+        ("horizontal_scale", C.c_float), ("vertical_scale", C.c_float), ("heights", C.c_void_p), ("heights_stride", C.c_int64),
+    ]
+
+
+TRAJ_VERTS = 101
+TRAJ_DRAWS = 4 * (TRAJ_VERTS - 1) + 2
+HEIGHTS_CENTER, HEIGHTS_GRID = 1, 2
+
+
 class TaskObsArgs(C.Structure):
     _fields_ = [
         ("body_state", C.c_void_p), ("body_env_stride", C.c_int64), ("track_ids", C.c_void_p),
@@ -302,6 +340,9 @@ SIGNATURES = {
                                           C.c_int64, C.c_void_p]),
     "pulse_reach_step": (C.c_int, [C.POINTER(ReachStepArgs), C.c_int64, C.c_void_p]),
     "pulse_ztask_step": (C.c_int, [C.POINTER(ZTaskStepArgs), C.c_int64, C.c_void_p]),
+    "pulse_terrain_step": (C.c_int, [C.POINTER(TerrainStepArgs), C.c_int64, C.c_void_p]),
+    "pulse_traj_reset": (C.c_int, [C.POINTER(TrajResetArgs), C.c_void_p]),
+    "pulse_terrain_heights": (C.c_int, [C.POINTER(TerrainHeightsArgs), C.c_void_p]),
     "pulse_task_obs_size": (C.c_int, [C.c_int32, C.c_int32, C.c_int32]),
     "pulse_im_task_obs": (C.c_int, [C.POINTER(TaskObsArgs), C.c_void_p]),
     "pulse_eval_step": (C.c_int, [C.POINTER(EvalArgs), C.c_void_p]),

@@ -1,0 +1,400 @@
+// HumanoidPedestrianTerrain(Z) (phc/env/tasks/humanoid_pedestrian_terrain.py) on the device:
+//   terrain_step_kernel   reward, reset and observation of post_physics_step in one launch, one warp per env (lane = body):
+//                         _compute_reward :871-896, _compute_reset :849-869 -> compute_humanoid_reset :1477-1531,
+//                         _compute_humanoid_obs :195-223, _compute_task_obs :385-440 (compute_location_observations :1588-1616,
+//                         get_heights :718-772 at the head pose :296-311, get_center_heights :690-716).
+//   traj_reset_kernel     TrajGenerator.reset (phc/utils/traj_generator.py:57-112), one thread per reset env.
+//   terrain_heights_kernel get_center_heights / get_heights alone (the spawn lift of _reset_ref_state_init :527-584).
+// Height sampling is Terrain.world_points_to_map / sample_height_points (:1191-1198, :1261-1267); trajectory lookups are
+// TrajGenerator.calc_pos (traj_generator.py:148-165).
+//
+// Cell indices, the reset mask and the trajectory segment indices are integers decided by fp32 arithmetic, so the operations that
+// feed them keep the reference's order with round-to-nearest intrinsics (no FMA contraction), as in im_step.cu.  Everything else
+// is under the 1e-4 float tolerance of the observations and rewards.
+#include "philox.cuh"
+#include "pulse_common.cuh"
+#include "quat_math.cuh"
+
+namespace pulse {
+namespace {
+
+constexpr int kTB = PULSE_NUM_BODIES;
+constexpr int kVerts = PULSE_TRAJ_VERTS;
+
+__device__ __forceinline__ float wsum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
+  return v;
+}
+
+// isaacgym.torch_utils.quat_apply [3P-memory]: t = 2 (xyz x b); b + w t + xyz x t, in this order.
+__device__ __forceinline__ Vec3 cross_rn(Vec3 a, Vec3 b) {
+  return {__fsub_rn(__fmul_rn(a.y, b.z), __fmul_rn(a.z, b.y)), __fsub_rn(__fmul_rn(a.z, b.x), __fmul_rn(a.x, b.z)),
+          __fsub_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x))};
+}
+__device__ __forceinline__ Vec3 quat_apply_rn(Quat q, Vec3 b) {
+  const Vec3 u = {q.x, q.y, q.z};
+  Vec3 t = cross_rn(u, b);
+  t = {__fmul_rn(t.x, 2.0f), __fmul_rn(t.y, 2.0f), __fmul_rn(t.z, 2.0f)};
+  const Vec3 c = cross_rn(u, t);
+  return {__fadd_rn(__fadd_rn(b.x, __fmul_rn(q.w, t.x)), c.x), __fadd_rn(__fadd_rn(b.y, __fmul_rn(q.w, t.y)), c.y),
+          __fadd_rn(__fadd_rn(b.z, __fmul_rn(q.w, t.z)), c.z)};
+}
+
+// humanoid.py:1617-1620 (remove_base_rot): q (x) conj(0.5, 0.5, 0.5, 0.5)
+__device__ __forceinline__ Quat base_rot_removed(Quat q, bool upright) {
+  return upright ? q : qmul(q, Quat{-0.5f, -0.5f, -0.5f, 0.5f});
+}
+
+// calc_heading_quat / calc_heading_quat_inv (phc/utils/torch_utils.py:200-240) in the angle form the reference computes: heading =
+// atan2 of the rotated x axis, quat_from_angle_axis(+-heading, z) incl. its final quat_unit.  The height-map points rotate by it, so
+// their cell indices follow it; heading_half() would move them by ~2e-7.
+__device__ __forceinline__ Quat heading_quat_ref(Quat q, bool inverse) {
+  const float s = __fsub_rn(__fmul_rn(2.0f, __fmul_rn(q.w, q.w)), 1.0f);
+  const float rx = __fadd_rn(s, __fmul_rn(__fmul_rn(q.x, q.x), 2.0f));
+  const float ry = __fadd_rn(__fmul_rn(__fmul_rn(q.z, q.w), 2.0f), __fmul_rn(__fmul_rn(q.y, q.x), 2.0f));
+  float h = atan2f(ry, rx);
+  if (inverse) h = -h;
+  float sn, cs;
+  sincosf(__fmul_rn(h, 0.5f), &sn, &cs);
+  const float n = fmaxf(__fsqrt_rn(__fadd_rn(__fmul_rn(sn, sn), __fmul_rn(cs, cs))), 1e-9f);
+  return {0.0f, 0.0f, __fdiv_rn(sn, n), __fdiv_rn(cs, n)};
+}
+
+// quat_apply_yaw (:1571-1576): x = y = 0, normalize, quat_apply
+__device__ __forceinline__ Quat yaw_only(Quat q) {
+  const float n = fmaxf(__fsqrt_rn(__fadd_rn(__fmul_rn(q.z, q.z), __fmul_rn(q.w, q.w))), 1e-9f);
+  return {0.0f, 0.0f, __fdiv_rn(q.z, n), __fdiv_rn(q.w, n)};
+}
+
+struct HeightField {
+  const int16_t* hf;
+  long long rows, cols;
+  float hscale, vscale;
+};
+
+// Terrain.world_points_to_map + sample_height_points (:1191-1198, :1261-1267): long(x / horizontal_scale) truncates toward zero,
+// the indices clip to [0, dim - 2], height = min(hf[px, py], hf[px + 1, py + 1]) * vertical_scale.  A plane (hf == NULL) is flat 0.
+__device__ __forceinline__ float sample_height(const HeightField& t, float x, float y) {
+  if (t.hf == nullptr) return 0.0f;
+  long long px = static_cast<long long>(__fdiv_rn(x, t.hscale));
+  long long py = static_cast<long long>(__fdiv_rn(y, t.hscale));
+  px = min(max(px, 0ll), t.rows - 2);
+  py = min(max(py, 0ll), t.cols - 2);
+  const int h1 = __ldg(t.hf + px * t.cols + py), h2 = __ldg(t.hf + (px + 1) * t.cols + py + 1);
+  return __fmul_rn(static_cast<float>(min(h1, h2)), t.vscale);
+}
+
+// world point = quat_apply(q, offset) + origin (get_heights :734-742, get_center_heights :703-711)
+__device__ __forceinline__ float height_at(const HeightField& t, Quat q, const float* off, Vec3 origin) {
+  const Vec3 r = quat_apply_rn(q, Vec3{off[0], off[1], off[2]});
+  return sample_height(t, __fadd_rn(r.x, origin.x), __fadd_rn(r.y, origin.y));
+}
+
+// mean of get_center_heights over the points (lanes < count hold one point each); the result is in every lane
+__device__ __forceinline__ float center_height(const HeightField& t, const float* pts, int count, Quat q_root, Vec3 p_root, bool upright,
+                                               int lane) {
+  const Quat qy = yaw_only(base_rot_removed(q_root, upright));
+  float h = 0.0f;
+  for (int i = lane; i < count; i += 32) h += height_at(t, qy, pts + 3 * i, p_root);
+  return wsum(h) / static_cast<float>(count);
+}
+
+// TrajGenerator.calc_pos (traj_generator.py:148-165): phase = clip(t / (num_verts * dt), 0, 1) -- num_verts, not num_segs, as in the
+// reference -- then the floor / ceil waypoints and their lerp, each operation rounded as the reference rounds it.
+__device__ __forceinline__ Vec3 traj_pos(const float* verts, float t, float traj_dur) {
+  const float phase = fminf(fmaxf(__fdiv_rn(t, traj_dur), 0.0f), 1.0f);
+  const float seg = __fmul_rn(phase, static_cast<float>(kVerts - 1));
+  const int i0 = static_cast<int>(floorf(seg)), i1 = static_cast<int>(ceilf(seg));
+  const float b = __fsub_rn(seg, static_cast<float>(i0));
+  const float* p0 = verts + 3 * i0;
+  const float* p1 = verts + 3 * i1;
+  return {lerp_rn(p0[0], p1[0], b), lerp_rn(p0[1], p1[1], b), lerp_rn(p0[2], p1[2], b)};
+}
+
+__global__ void __launch_bounds__(256) terrain_step_kernel(const pulse_terrain_step_args_t a, long long n) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const HeightField hfield = {a.heightfield, a.hf_rows, a.hf_cols, a.horizontal_scale, a.vertical_scale};
+  const bool upright = a.upright != 0;
+  long long rows = n;
+  if (a.env_ids != nullptr && a.env_count != nullptr) rows = min(rows, static_cast<long long>(*a.env_count));
+  for (long long r = blockIdx.x * 8ll + warp; r < rows; r += 8ll * gridDim.x) {
+    const long long e = a.env_ids != nullptr ? a.env_ids[r] : r;
+    const int j = lane;
+    const bool body = j < kTB;
+    const float* bs = a.body_state + e * a.body_env_stride + (body ? j : 0) * 13;
+    const Vec3 p = {bs[0], bs[1], bs[2]};
+    const Vec3 p_root = {__shfl_sync(kFull, p.x, 0), __shfl_sync(kFull, p.y, 0), __shfl_sync(kFull, p.z, 0)};
+    const float* rs = a.root_states + e * a.root_env_stride;
+    const Vec3 a_pos = {rs[0], rs[1], rs[2]};
+    const long long prog = a.progress_buf[e];
+    const float t_now = __fmul_rn(__ll2float_rn(prog), a.dt);   // progress_buf * dt
+    const float* verts = a.traj_verts + e * (kVerts * 3);
+
+    if (a.flags & PULSE_STEP_REWARD) {
+      // _compute_reward (:871-896): location reward against the ACTOR root state; the power term is always reported in reward_raw[:, 1]
+      float power = 0.0f;
+      if (a.dof_force != nullptr) {
+        const float* fr = a.dof_force + e * a.dof_force_stride;
+        const float* dv = a.dof_vel + e * a.dof_env_stride;
+        for (int d = lane; d < PULSE_NUM_DOF; d += 32) power += fabsf(fr[d] * dv[d * a.dof_elem_stride]);
+        power = -a.power_coefficient * wsum(power);
+      }
+      if (lane == 0) {
+        const Vec3 tar = traj_pos(verts, t_now, a.traj_dur);
+        const float dx = tar.x - a_pos.x, dy = tar.y - a_pos.y;
+        float err = dx * dx + dy * dy;
+        if (a.fuzzy_target && err < 0.0025f) err = 0.0f;   // compute_location_reward_fuzzy (:1633-1646)
+        const float loc = expf(-2.0f * err);                // compute_location_reward (:1620-1630)
+        a.rew_buf[e] = a.power_reward ? loc + power : loc;
+        if (a.reward_raw != nullptr) {
+          a.reward_raw[e * a.raw_stride] = loc;
+          a.reward_raw[e * a.raw_stride + 1] = power;
+        }
+      }
+    }
+
+    if (a.flags & PULSE_STEP_RESET) {
+      // compute_humanoid_reset (:1477-1531): the contact force summed over the non-contact bodies, in body order, has norm > 50
+      // (after progress 1), or the RIGID-BODY root is more than fail_dist from the trajectory point.  center_height and the
+      // termination heights are unused by the reference.
+      Vec3 f = {0.0f, 0.0f, 0.0f};
+      if (a.enable_early_termination && body && !((a.contact_body_mask >> j) & 1u)) {
+        const float* cf = a.contact_forces + e * a.contact_env_stride + j * 3;
+        f = {cf[0], cf[1], cf[2]};
+      }
+      Vec3 s = {0.0f, 0.0f, 0.0f};
+      for (int b = 0; b < kTB; ++b) {
+        s.x = __fadd_rn(s.x, __shfl_sync(kFull, f.x, b));
+        s.y = __fadd_rn(s.y, __shfl_sync(kFull, f.y, b));
+        s.z = __fadd_rn(s.z, __shfl_sync(kFull, f.z, b));
+      }
+      if (lane == 0) {
+        long long term = 0;
+        if (a.enable_early_termination) {
+          const float nrm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(s.x, s.x), __fmul_rn(s.y, s.y)), __fmul_rn(s.z, s.z)));
+          const bool fallen = nrm > 50.0f && prog > 1;
+          const Vec3 tar = traj_pos(verts, t_now, a.traj_dur);
+          const float dx = __fsub_rn(tar.x, p_root.x), dy = __fsub_rn(tar.y, p_root.y);
+          const bool far = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)) > __fmul_rn(a.fail_dist, a.fail_dist);
+          term = (!a.no_collision_check && (fallen || far)) ? 1 : 0;
+        }
+        a.terminate_buf[e] = term;
+        a.reset_buf[e] = prog >= a.max_episode_length - 1 ? 1 : term;
+      }
+    }
+
+    if (a.flags & PULSE_STEP_OBS) {
+      const Quat q = {bs[3], bs[4], bs[5], bs[6]};
+      const Vec3 v = {bs[7], bs[8], bs[9]}, w = {bs[10], bs[11], bs[12]};
+      const Quat q_root = {__shfl_sync(kFull, q.x, 0), __shfl_sync(kFull, q.y, 0), __shfl_sync(kFull, q.z, 0), __shfl_sync(kFull, q.w, 0)};
+      float* o = a.obs_buf + e * a.obs_stride;
+      // _compute_humanoid_obs (:195-223): every body's z minus the mean center height around the rigid-body root, then
+      // compute_humanoid_observations_smpl_max (humanoid.py:1675-1731) with local root obs and the root height
+      const float c_self = center_height(hfield, a.center_points, a.num_center_points, q_root, p_root, upright, lane);
+      float hs, hc;
+      heading_half(base_rot_removed(q_root, upright), hs, hc);
+      const Yaw yr = make_yaw(Quat{0.0f, 0.0f, -hs, hc});
+      if (body) {
+        if (j == 0) o[0] = p_root.z - c_self;
+        else {
+          const Vec3 lp = yaw_rot(yr, Vec3{p.x - p_root.x, p.y - p_root.y, (p.z - c_self) - (p_root.z - c_self)});
+          o[1 + 3 * (j - 1)] = lp.x; o[2 + 3 * (j - 1)] = lp.y; o[3 + 3 * (j - 1)] = lp.z;
+        }
+        float six[6];
+        qsix(yaw_mul_left(-hs, hc, q), six);
+#pragma unroll
+        for (int i = 0; i < 6; ++i) o[70 + 6 * j + i] = six[i];
+        const Vec3 lv = yaw_rot(yr, v), lw = yaw_rot(yr, w);
+        o[214 + 3 * j] = lv.x; o[215 + 3 * j] = lv.y; o[216 + 3 * j] = lv.z;
+        o[286 + 3 * j] = lw.x; o[287 + 3 * j] = lw.y; o[288 + 3 * j] = lw.z;
+      }
+      // _compute_task_obs (:385-440).  Trajectory samples at progress * dt + k * trajSampleTimestep (humanoid_traj.py:196-211) in the
+      // heading frame of the actor root (compute_location_observations :1588-1616), xy only.
+      const Quat a_rot = {rs[3], rs[4], rs[5], rs[6]};
+      float* t = o + PULSE_SELF_OBS;
+      if (lane < a.num_traj_samples) {
+        const float tk = __fadd_rn(t_now, __fmul_rn(static_cast<float>(lane), a.traj_sample_timestep));
+        const Vec3 tp = traj_pos(verts, tk, a.traj_dur);
+        const Vec3 d = qrot(heading_quat_ref(base_rot_removed(a_rot, upright), true), tp - a_pos);
+        t[2 * lane] = d.x;
+        t[2 * lane + 1] = d.y;
+      }
+      // height map at the head pose (get_head_pose :296-311, get_heights :718-772), relative to the mean center height around the
+      // actor root (use_center_height) or to the actor root's z, clipped to +-3 m and scaled by 5
+      const float ref_h = a.use_center_height ? center_height(hfield, a.center_points, a.num_center_points, a_rot, a_pos, upright, lane)
+                                              : a_pos.z;
+      const Vec3 head_p = {__shfl_sync(kFull, p.x, a.head_body_id), __shfl_sync(kFull, p.y, a.head_body_id),
+                           __shfl_sync(kFull, p.z, a.head_body_id)};
+      const Quat head_q = {__shfl_sync(kFull, q.x, a.head_body_id), __shfl_sync(kFull, q.y, a.head_body_id),
+                           __shfl_sync(kFull, q.z, a.head_body_id), __shfl_sync(kFull, q.w, a.head_body_id)};
+      const Quat hq = heading_quat_ref(base_rot_removed(head_q, upright), false);
+      float* hobs = t + 2 * a.num_traj_samples;
+      for (int i = lane; i < a.num_height_points; i += 32) {
+        const float m = height_at(hfield, hq, a.height_points + 3 * i, head_p);
+        hobs[i] = fminf(fmaxf(ref_h - m, -3.0f), 3.0f) * 5.0f;
+      }
+    }
+  }
+}
+
+// TrajGenerator.reset (traj_generator.py:57-112) for one env.  Injected draws per env (PULSE_TRAJ_DRAWS = 4 * S + 2, S = num_verts - 1):
+// [0, S) turn angles, [S, 2S) sharp-turn angles, [2S, 3S) sharp-turn coins (sharp where u < sharp_turn_prob, the bernoulli draw),
+// [3S, 4S) speed changes, 4S initial heading, 4S + 1 initial speed.  Column 0 of the first four rows is overwritten, as in the
+// reference.  Without injected draws, Philox block (seed, env, offset + k) supplies the four draws of segment k and block
+// (seed, env, offset + S) the initial heading and speed: a different stream from torch's generator, the same distribution.
+// torch.cumsum on the CPU accumulates fp32 in double; so do the two running sums here.
+__global__ void __launch_bounds__(128) traj_reset_kernel(const pulse_traj_reset_args_t a) {
+  constexpr int S = kVerts - 1;
+  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  if (i >= a.num_ids) return;
+  const long long e = a.env_ids[i];
+  const float* rin = a.rand != nullptr ? a.rand + i * PULSE_TRAJ_DRAWS : nullptr;
+  const unsigned long long off = a.offset + (a.offset_dev != nullptr ? *a.offset_dev : 0ull);
+  float u_head, u_v0;
+  if (rin != nullptr) {
+    u_head = rin[4 * S];
+    u_v0 = rin[4 * S + 1];
+  } else {
+    const Philox4 b = philox4x32_10(a.seed, static_cast<unsigned long long>(e), off + S);
+    u_head = u01(b.x);
+    u_v0 = u01(b.y);
+  }
+  const float pi = 3.14159265358979f;
+  const float x0 = a.init_pos[i * a.init_stride], y0 = a.init_pos[i * a.init_stride + 1];
+  float* vt = a.verts + e * (kVerts * 3);
+  vt[0] = x0;
+  vt[1] = y0;
+  double ang = 0.0, px = 0.0, py = 0.0;
+  float speed = 0.0f;
+  for (int k = 0; k < S; ++k) {
+    float u_turn, u_sharp, coin, u_speed;
+    if (rin != nullptr) {
+      u_turn = rin[k];
+      u_sharp = rin[S + k];
+      coin = rin[2 * S + k];
+      u_speed = rin[3 * S + k];
+    } else {
+      const Philox4 b = philox4x32_10(a.seed, static_cast<unsigned long long>(e), off + k);
+      u_turn = u01(b.x);
+      u_sharp = u01(b.y);
+      coin = u01(b.z);
+      u_speed = u01(b.w);
+    }
+    float dth;
+    if (k == 0) dth = __fmul_rn(pi, __fsub_rn(__fmul_rn(2.0f, u_head), 1.0f));
+    else if (coin < a.sharp_turn_prob) dth = __fmul_rn(pi, __fsub_rn(__fmul_rn(2.0f, u_sharp), 1.0f));
+    else dth = __fmul_rn(__fsub_rn(__fmul_rn(2.0f, u_turn), 1.0f), a.dtheta_scale);
+    if (k == 0) speed = __fadd_rn(__fmul_rn(__fsub_rn(a.speed_max, a.speed_min), u_v0), a.speed_min);
+    else speed = fminf(fmaxf(__fadd_rn(speed, __fmul_rn(__fsub_rn(__fmul_rn(2.0f, u_speed), 1.0f), a.dspeed_scale)), a.speed_min), a.speed_max);
+    ang += static_cast<double>(dth);
+    const float th = static_cast<float>(ang);
+    float sn, cs;
+    sincosf(th, &sn, &cs);
+    const float seg = __fmul_rn(speed, a.seg_dt);
+    float dx = __fmul_rn(cs, seg), dy = __fmul_rn(-sn, seg);
+    if (k == 0) {
+      dx = __fadd_rn(dx, x0);
+      dy = __fadd_rn(dy, y0);
+    }
+    px += static_cast<double>(dx);
+    py += static_cast<double>(dy);
+    vt[3 * (k + 1)] = static_cast<float>(px);
+    vt[3 * (k + 1) + 1] = static_cast<float>(py);
+    vt[3 * (k + 1) + 2] = 0.0f;
+  }
+}
+
+__global__ void __launch_bounds__(256) terrain_heights_kernel(const pulse_terrain_heights_args_t a) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const HeightField hfield = {a.heightfield, a.hf_rows, a.hf_cols, a.horizontal_scale, a.vertical_scale};
+  for (long long r = blockIdx.x * 8ll + warp; r < a.num_rows; r += 8ll * gridDim.x) {
+    const float* rs = a.root_states + r * a.root_stride;
+    const Vec3 org = {rs[0], rs[1], rs[2]};
+    Quat q = base_rot_removed(Quat{rs[3], rs[4], rs[5], rs[6]}, a.upright != 0);
+    q = a.mode == PULSE_HEIGHTS_CENTER ? yaw_only(q) : heading_quat_ref(q, false);
+    for (int i = lane; i < a.num_points; i += 32) a.heights[r * a.heights_stride + i] = height_at(hfield, q, a.points + 3 * i, org);
+  }
+}
+
+int check_heightfield(const char* who, const int16_t* hf, int64_t rows, int64_t cols, float hscale) {
+  PULSE_REQUIRE(hf == nullptr || (rows >= 2 && cols >= 2), "%s: heightfield needs at least 2 x 2 cells", who);
+  PULSE_REQUIRE(hf == nullptr || hscale > 0.0f, "%s: horizontal_scale must be positive", who);
+  return PULSE_OK;
+}
+
+long long warp_grid(long long rows) {
+  long long ctas = (rows + 7) / 8;
+  if (ctas > kNumSMs * 8ll) ctas = kNumSMs * 8ll;
+  return ctas < 1 ? 1 : ctas;
+}
+
+}  // namespace
+}  // namespace pulse
+
+extern "C" int pulse_terrain_step(const pulse_terrain_step_args_t* args, int64_t num_envs, void* stream) {
+  using namespace pulse;
+  PULSE_REQUIRE(args != nullptr, "pulse_terrain_step: null args");
+  const pulse_terrain_step_args_t& a = *args;
+  PULSE_REQUIRE(num_envs > 0, "pulse_terrain_step: num_envs must be positive");
+  PULSE_REQUIRE((a.flags & ~PULSE_STEP_ALL) == 0 && a.flags != 0, "pulse_terrain_step: flags must be a non-empty set of REWARD / RESET / OBS");
+  PULSE_REQUIRE(a.body_state && a.root_states && a.progress_buf && a.traj_verts, "pulse_terrain_step: null input buffer");
+  PULSE_REQUIRE(a.body_env_stride >= 24 * 13 && a.root_env_stride >= 13, "pulse_terrain_step: body / root strides too small");
+  PULSE_REQUIRE(a.dt > 0.0f && a.traj_dur > 0.0f, "pulse_terrain_step: dt and traj_dur must be positive");
+  PULSE_REQUIRE(a.env_ids == nullptr || a.flags == PULSE_STEP_OBS, "pulse_terrain_step: env_ids only with PULSE_STEP_OBS");
+  if (a.flags & PULSE_STEP_REWARD) {
+    PULSE_REQUIRE(a.rew_buf != nullptr, "pulse_terrain_step: reward needs rew_buf");
+    PULSE_REQUIRE(!(a.power_reward || a.reward_raw) || (a.dof_force && a.dof_vel && a.dof_elem_stride >= 1),
+                  "pulse_terrain_step: the power term (power_reward / reward_raw) needs dof_force and dof_vel");
+    PULSE_REQUIRE(a.reward_raw == nullptr || a.raw_stride >= 2, "pulse_terrain_step: raw_stride < 2");
+  }
+  if (a.flags & PULSE_STEP_RESET) {
+    PULSE_REQUIRE(a.reset_buf && a.terminate_buf, "pulse_terrain_step: reset needs reset_buf and terminate_buf");
+    PULSE_REQUIRE(!a.enable_early_termination || (a.contact_forces && a.contact_env_stride >= 24 * 3),
+                  "pulse_terrain_step: early termination needs contact_forces with env stride >= 72");
+  }
+  if (a.flags & PULSE_STEP_OBS) {
+    PULSE_REQUIRE(a.obs_buf && a.height_points && a.center_points, "pulse_terrain_step: observation needs obs_buf, height_points, center_points");
+    PULSE_REQUIRE(a.num_traj_samples >= 1 && a.num_traj_samples <= 32, "pulse_terrain_step: num_traj_samples %d not in [1, 32]", a.num_traj_samples);
+    PULSE_REQUIRE(a.num_height_points >= 1 && a.num_center_points >= 1, "pulse_terrain_step: empty point set");
+    PULSE_REQUIRE(a.head_body_id >= 0 && a.head_body_id < 24, "pulse_terrain_step: head_body_id %d out of range", a.head_body_id);
+    PULSE_REQUIRE(a.obs_stride >= PULSE_SELF_OBS + 2 * a.num_traj_samples + a.num_height_points, "pulse_terrain_step: obs_stride %lld too small",
+                  (long long)a.obs_stride);
+    const int st = check_heightfield("pulse_terrain_step", a.heightfield, a.hf_rows, a.hf_cols, a.horizontal_scale);
+    if (st != PULSE_OK) return st;
+  }
+  terrain_step_kernel<<<static_cast<unsigned>(warp_grid(num_envs)), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, (long long)num_envs);
+  PULSE_LAUNCH_OK("terrain_step_kernel");
+  return PULSE_OK;
+}
+
+extern "C" int pulse_traj_reset(const pulse_traj_reset_args_t* args, void* stream) {
+  using namespace pulse;
+  PULSE_REQUIRE(args != nullptr, "pulse_traj_reset: null args");
+  const pulse_traj_reset_args_t& a = *args;
+  PULSE_REQUIRE(a.num_ids >= 0, "pulse_traj_reset: negative num_ids");
+  if (a.num_ids == 0) return PULSE_OK;
+  PULSE_REQUIRE(a.env_ids && a.init_pos && a.verts, "pulse_traj_reset: null buffer");
+  PULSE_REQUIRE(a.init_stride >= 2, "pulse_traj_reset: init_stride < 2");
+  PULSE_REQUIRE(a.seg_dt > 0.0f && a.speed_max >= a.speed_min, "pulse_traj_reset: bad trajectory parameters");
+  const long long blocks = (a.num_ids + 127) / 128;
+  traj_reset_kernel<<<static_cast<unsigned>(blocks), 128, 0, static_cast<cudaStream_t>(stream)>>>(a);
+  PULSE_LAUNCH_OK("traj_reset_kernel");
+  return PULSE_OK;
+}
+
+extern "C" int pulse_terrain_heights(const pulse_terrain_heights_args_t* args, void* stream) {
+  using namespace pulse;
+  PULSE_REQUIRE(args != nullptr, "pulse_terrain_heights: null args");
+  const pulse_terrain_heights_args_t& a = *args;
+  PULSE_REQUIRE(a.mode == PULSE_HEIGHTS_CENTER || a.mode == PULSE_HEIGHTS_GRID, "pulse_terrain_heights: unknown mode %d", a.mode);
+  PULSE_REQUIRE(a.num_rows >= 0 && a.num_points >= 1, "pulse_terrain_heights: bad sizes");
+  if (a.num_rows == 0) return PULSE_OK;
+  PULSE_REQUIRE(a.root_states && a.points && a.heights, "pulse_terrain_heights: null buffer");
+  PULSE_REQUIRE(a.root_stride >= 7 && a.heights_stride >= a.num_points, "pulse_terrain_heights: strides too small");
+  const int st = check_heightfield("pulse_terrain_heights", a.heightfield, a.hf_rows, a.hf_cols, a.horizontal_scale);
+  if (st != PULSE_OK) return st;
+  terrain_heights_kernel<<<static_cast<unsigned>(warp_grid(a.num_rows)), 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
+  PULSE_LAUNCH_OK("terrain_heights_kernel");
+  return PULSE_OK;
+}
