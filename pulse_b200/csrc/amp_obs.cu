@@ -5,17 +5,13 @@
 // One warp per env.  The shift reads the (steps-1) older rows into registers before any store, so
 // the in-place move is safe; lanes 0..18 then convert the 19 kept joints' exponential maps to 6-D
 // rotations.  Layout of one step: [h | six(hinv*q0) | R v0 | R w0 | 19x six(dof) | 57 dof_vel | 4x R(key-p0)].
-#include "pulse_common.cuh"
-#include "quat_math.cuh"
+#include "humanoid_obs.cuh"
 
 namespace pulse {
 namespace {
 
 constexpr int kAmp = PULSE_AMP_OBS;
 constexpr int kMaxHist = 16;  // numAMPObsSteps - 1 <= 15
-// kept joints (joint = body - 1), dropping L_Toe(3) R_Toe(7) L_Hand(17) R_Hand(22): humanoid.py:397,417-421
-__constant__ int c_kept_joint[19] = {0, 1, 2, 4, 5, 6, 8, 9, 10, 11, 12, 13, 14, 15, 16, 18, 19, 20, 21};
-__constant__ int c_key_body[4] = {7, 3, 22, 17};  // R_Ankle, L_Ankle, R_Wrist, L_Wrist (env_im.yaml:36)
 
 __global__ void __launch_bounds__(128) amp_obs_kernel(const pulse_amp_obs_args_t a, long long n) {
   const long long e = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -42,44 +38,7 @@ __global__ void __launch_bounds__(128) amp_obs_kernel(const pulse_amp_obs_args_t
     }
   }
   // ---- current observation -------------------------------------------------------------------
-  const float* bs = a.body_state + e * a.body_env_stride;
-  const Vec3 p0 = {bs[0], bs[1], bs[2]};
-  const Quat q0 = {bs[3], bs[4], bs[5], bs[6]};
-  float hs, hc;
-  heading_half(q0, hs, hc);
-  const Quat h_inv = {0.0f, 0.0f, -hs, hc};
-  const Yaw yr = make_yaw(h_inv);
-  float* o = buf;
-  if (lane == 0) {
-    o[0] = p0.z;
-    float six[6];
-    qsix(qmul(h_inv, q0), six);
-#pragma unroll
-    for (int i = 0; i < 6; ++i) o[1 + i] = six[i];
-    Vec3 lv = yaw_rot(yr, {bs[7], bs[8], bs[9]});
-    Vec3 lw = yaw_rot(yr, {bs[10], bs[11], bs[12]});
-    o[7] = lv.x; o[8] = lv.y; o[9] = lv.z;
-    o[10] = lw.x; o[11] = lw.y; o[12] = lw.z;
-  }
-  const float* dp = a.dof_pos + e * a.dof_env_stride;
-  const float* dv = a.dof_vel + e * a.dof_env_stride;
-  if (lane < 19) {
-    const int jt = c_kept_joint[lane];
-    Vec3 em = {dp[(3 * jt + 0) * a.dof_elem_stride], dp[(3 * jt + 1) * a.dof_elem_stride], dp[(3 * jt + 2) * a.dof_elem_stride]};
-    float six[6];
-    qsix(exp_map_quat(em), six);
-#pragma unroll
-    for (int i = 0; i < 6; ++i) o[13 + 6 * lane + i] = six[i];
-#pragma unroll
-    for (int i = 0; i < 3; ++i) o[127 + 3 * lane + i] = dv[(3 * jt + i) * a.dof_elem_stride];
-  } else if (lane < 23) {
-    const int kb = c_key_body[lane - 19];
-    const float* bk = bs + kb * PULSE_BODY_STATE_W;
-    Vec3 lp = yaw_rot(yr, Vec3{bk[0], bk[1], bk[2]} - p0);
-    o[184 + 3 * (lane - 19) + 0] = lp.x;
-    o[184 + 3 * (lane - 19) + 1] = lp.y;
-    o[184 + 3 * (lane - 19) + 2] = lp.z;
-  }
+  store_amp_obs_sim(buf, lane, a, e);
 }
 
 }  // namespace

@@ -17,12 +17,6 @@ namespace {
 
 constexpr int kEvalBodies = PULSE_NUM_BODIES;
 
-__device__ __forceinline__ float wsum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
-
 // Largest eigenvalue / eigenvector of a symmetric 4x4 matrix by cyclic Jacobi rotations (every lane runs the same scalars).
 __device__ __forceinline__ void jacobi4_max(float A[4][4], float q[4], float& lambda) {
   float V[4][4] = {{1, 0, 0, 0}, {0, 1, 0, 0}, {0, 0, 1, 0}, {0, 0, 0, 1}};
@@ -98,7 +92,7 @@ __global__ void __launch_bounds__(128) eval_accumulate_kernel(const pulse_eval_a
   }
   const float dx = px - gx, dy = py - gy, dz = pz - gz;
   const float inv_j = 1.0f / kEvalBodies;
-  const float mg = wsum(body ? sqrtf(dx * dx + dy * dy + dz * dz) : 0.0f) * inv_j;     // extras['mpjpe'] (humanoid_im.py:671)
+  const float mg = warp_sum(body ? sqrtf(dx * dx + dy * dy + dz * dz) : 0.0f) * inv_j;     // extras['mpjpe'] (humanoid_im.py:671)
   if (a.mpjpe_out != nullptr && lane == 0) a.mpjpe_out[e] = mg;
   // history of (pred - gt): velocity / acceleration errors are finite differences of it
   float* h = a.hist + (long long)e * (2 * kEvalBodies * 3);
@@ -116,18 +110,18 @@ __global__ void __launch_bounds__(128) eval_accumulate_kernel(const pulse_eval_a
     const float yx = px - prx, yy = py - pry, yz = pz - prz;   // predicted, root-relative
     const float xx = gx - grx, xy = gy - gry, xz = gz - grz;   // target, root-relative
     const float lx = yx - xx, ly = yy - xy, lz = yz - xz;
-    const float ml = wsum(body ? sqrtf(lx * lx + ly * ly + lz * lz) : 0.0f) * inv_j;
+    const float ml = warp_sum(body ? sqrtf(lx * lx + ly * ly + lz * lz) : 0.0f) * inv_j;
     // Procrustes alignment of the root-relative sets
-    const float mxx = wsum(body ? xx : 0.0f) * inv_j, mxy = wsum(body ? xy : 0.0f) * inv_j, mxz = wsum(body ? xz : 0.0f) * inv_j;
-    const float myx = wsum(body ? yx : 0.0f) * inv_j, myy = wsum(body ? yy : 0.0f) * inv_j, myz = wsum(body ? yz : 0.0f) * inv_j;
+    const float mxx = warp_sum(body ? xx : 0.0f) * inv_j, mxy = warp_sum(body ? xy : 0.0f) * inv_j, mxz = warp_sum(body ? xz : 0.0f) * inv_j;
+    const float myx = warp_sum(body ? yx : 0.0f) * inv_j, myy = warp_sum(body ? yy : 0.0f) * inv_j, myz = warp_sum(body ? yz : 0.0f) * inv_j;
     const float X[3] = {body ? xx - mxx : 0.0f, body ? xy - mxy : 0.0f, body ? xz - mxz : 0.0f};
     const float Y[3] = {body ? yx - myx : 0.0f, body ? yy - myy : 0.0f, body ? yz - myz : 0.0f};
-    const float ny2 = wsum(Y[0] * Y[0] + Y[1] * Y[1] + Y[2] * Y[2]);
+    const float ny2 = warp_sum(Y[0] * Y[0] + Y[1] * Y[1] + Y[2] * Y[2]);
     float S[3][3];   // S[a][b] = sum_j Y_a X_b: the correlation of Horn's method for the rotation taking Y onto X
 #pragma unroll
     for (int r = 0; r < 3; ++r)
 #pragma unroll
-      for (int c = 0; c < 3; ++c) S[r][c] = wsum(Y[r] * X[c]);
+      for (int c = 0; c < 3; ++c) S[r][c] = warp_sum(Y[r] * X[c]);
     float Nm[4][4];
     Nm[0][0] = S[0][0] + S[1][1] + S[2][2];
     Nm[1][1] = S[0][0] - S[1][1] - S[2][2];
@@ -151,11 +145,11 @@ __global__ void __launch_bounds__(128) eval_accumulate_kernel(const pulse_eval_a
     const float ax = scale * (r00 * Y[0] + r01 * Y[1] + r02 * Y[2]) - X[0];
     const float ay = scale * (r10 * Y[0] + r11 * Y[1] + r12 * Y[2]) - X[1];
     const float az = scale * (r20 * Y[0] + r21 * Y[1] + r22 * Y[2]) - X[2];
-    const float mpa = wsum(body ? sqrtf(ax * ax + ay * ay + az * az) : 0.0f) * inv_j;
+    const float mpa = warp_sum(body ? sqrtf(ax * ax + ay * ay + az * az) : 0.0f) * inv_j;
     const float vx = dx - d1x, vy = dy - d1y, vz = dz - d1z;
-    const float mv = wsum(body ? sqrtf(vx * vx + vy * vy + vz * vz) : 0.0f) * inv_j;
+    const float mv = warp_sum(body ? sqrtf(vx * vx + vy * vy + vz * vz) : 0.0f) * inv_j;
     const float cx = dx - 2.0f * d1x + d2x, cy = dy - 2.0f * d1y + d2y, cz = dz - 2.0f * d1z + d2z;
-    const float ma = wsum(body ? sqrtf(cx * cx + cy * cy + cz * cz) : 0.0f) * inv_j;
+    const float ma = warp_sum(body ? sqrtf(cx * cx + cy * cy + cz * cz) : 0.0f) * inv_j;
     if (lane == 0) {
       double* s = a.sums + (long long)e * 5;
       int* c = a.counts + (long long)e * 3;

@@ -87,9 +87,7 @@ extern "C" int pulse_normalize_advantages(float* advantages, const double* adv_s
   using namespace pulse;
   PULSE_REQUIRE(advantages && adv_sum, "pulse_normalize_advantages: null buffer");
   PULSE_REQUIRE(count >= 2, "pulse_normalize_advantages: need at least 2 samples");
-  long long blocks = (count + 255) / 256;
-  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
-  normalize_adv_kernel<<<static_cast<unsigned>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(advantages, adv_sum, (long long)count);
+  normalize_adv_kernel<<<grid_for(count, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(advantages, adv_sum, (long long)count);
   PULSE_LAUNCH_OK("normalize_adv_kernel");
   return PULSE_OK;
 }

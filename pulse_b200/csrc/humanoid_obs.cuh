@@ -1,0 +1,102 @@
+// Humanoid observation layouts and per-env terms shared by the task step kernels (one warp per env, lane = body).
+#pragma once
+#include "pulse_common.cuh"
+#include "quat_math.cuh"
+
+namespace pulse {
+
+// compute_humanoid_observations_smpl_max (humanoid.py:1675-1731) with local root obs and the root height: body j's slice of the
+// 358-float self observation [root height | 23 x position | 24 x six-D rotation | 24 x velocity | 24 x angular velocity], all in
+// the heading frame.  The heights p.z and p_root.z are taken from the task's reference (the ground, or the terrain's center
+// height); (hs, hc) is the heading's half-angle sine / cosine and yr = make_yaw of the inverse heading.  The imitation and reach
+// step kernels write the same layout inline (see im_step.cu).
+__device__ __forceinline__ void store_self_obs(float* o, int j, Vec3 p, Vec3 p_root, Quat q, Vec3 v, Vec3 w, float hs, float hc, Yaw yr) {
+  if (j == 0) o[0] = p_root.z;
+  else stv(o + 1 + 3 * (j - 1), yaw_rot(yr, p - p_root));
+  qsix(yaw_mul_left(-hs, hc, q), o + 70 + 6 * j);
+  stv(o + 214 + 3 * j, yaw_rot(yr, v));
+  stv(o + 286 + 3 * j, yaw_rot(yr, w));
+}
+
+namespace {  // __constant__ tables are per module; one copy in every translation unit that builds AMP rows
+// kept joints (joint = body - 1), dropping L_Toe(3) R_Toe(7) L_Hand(17) R_Hand(22): humanoid.py:397,417-421
+__constant__ int c_kept_joint[19] = {0, 1, 2, 4, 5, 6, 8, 9, 10, 11, 12, 13, 14, 15, 16, 18, 19, 20, 21};
+__constant__ int c_key_body[4] = {7, 3, 22, 17};  // R_Ankle, L_Ankle, R_Wrist, L_Wrist (env_im.yaml:36)
+}  // namespace
+
+struct AmpJoint {
+  Vec3 exp_map;  // the joint's local rotation
+  Vec3 vel;      // its three dof velocities
+};
+
+// build_amp_observations_smpl (humanoid_amp.py:924-969) with dof_to_obs_smpl (humanoid.py:1436-1446): one warp writes the 196-float
+// AMP observation [h | six(hinv q0) | R v0 | R w0 | 19 x six(dof) | 57 dof velocities | 4 x R(key - p0)] of the root state
+// (p0, q0, v0, w0).  Lane 0 writes the root features, lanes 0..18 the kept joints, lanes 19..22 the key bodies.  joint(jt) returns
+// joint jt's AmpJoint, key_pos(kb) key body kb's world position.
+template <class JointFn, class KeyPosFn>
+__device__ __forceinline__ void store_amp_obs(float* o, int lane, Vec3 p0, Quat q0, Vec3 v0, Vec3 w0, JointFn joint, KeyPosFn key_pos) {
+  float hs, hc;
+  heading_half(q0, hs, hc);
+  const Quat h_inv = {0.0f, 0.0f, -hs, hc};
+  const Yaw yr = make_yaw(h_inv);
+  if (lane == 0) {
+    o[0] = p0.z;
+    qsix(qmul(h_inv, q0), o + 1);
+    stv(o + 7, yaw_rot(yr, v0));
+    stv(o + 10, yaw_rot(yr, w0));
+  }
+  if (lane < 19) {
+    const AmpJoint jt = joint(c_kept_joint[lane]);
+    qsix(exp_map_quat(jt.exp_map), o + 13 + 6 * lane);
+    stv(o + 127 + 3 * lane, jt.vel);
+  } else if (lane < 23) {
+    stv(o + 184 + 3 * (lane - 19), yaw_rot(yr, key_pos(c_key_body[lane - 19]) - p0));
+  }
+}
+
+// store_amp_obs from the simulator state of env e: the root and key bodies from body_state ([pos | quat | vel | ang vel] per body),
+// the joints from the dof position / velocity views.
+template <class Args>
+__device__ __forceinline__ void store_amp_obs_sim(float* o, int lane, const Args& a, long long e) {
+  const float* bs = a.body_state + e * a.body_env_stride;
+  const float* dp = a.dof_pos + e * a.dof_env_stride;
+  const float* dv = a.dof_vel + e * a.dof_env_stride;
+  const long long ds = a.dof_elem_stride;
+  const auto joint = [&](int jt) {
+    return AmpJoint{{dp[(3 * jt + 0) * ds], dp[(3 * jt + 1) * ds], dp[(3 * jt + 2) * ds]},
+                    {dv[(3 * jt + 0) * ds], dv[(3 * jt + 1) * ds], dv[(3 * jt + 2) * ds]}};
+  };
+  const auto key_pos = [&](int kb) { return ldv(bs + kb * PULSE_BODY_STATE_W); };
+  store_amp_obs(o, lane, ldv(bs), ldq(bs + 3), ldv(bs + 7), ldv(bs + 10), joint, key_pos);
+}
+
+// The fall test of compute_humanoid_reset (humanoid.py:1573-1608) for body lane j of env e: `contact` when a body that may not
+// touch the ground has a contact force component above 0.1 N, `height` when such a body is below its termination height.  The env
+// has fallen when some lane has `contact` and some lane has `height`.
+struct FallFlags {
+  bool contact, height;
+};
+template <class Args>
+__device__ __forceinline__ FallFlags fall_flags(const Args& a, long long e, int j, bool body, float z) {
+  FallFlags f = {false, false};
+  if (a.enable_early_termination && body && !((a.contact_body_mask >> j) & 1u)) {
+    if (a.contact_forces != nullptr) {
+      const float* cf = a.contact_forces + e * a.contact_env_stride + j * 3;
+      f.contact = fabsf(cf[0]) > 0.1f || fabsf(cf[1]) > 0.1f || fabsf(cf[2]) > 0.1f;
+    }
+    f.height = z < a.termination_heights[j];
+  }
+  return f;
+}
+
+// sum |tau * qdot| over the 69 dofs of env e, in every lane: the power term (humanoid_speed.py:215-222)
+template <class Args>
+__device__ __forceinline__ float dof_power(const Args& a, long long e, int lane) {
+  const float* fr = a.dof_force + e * a.dof_force_stride;
+  const float* dv = a.dof_vel + e * a.dof_env_stride;
+  float power = 0.0f;
+  for (int d = lane; d < PULSE_NUM_DOF; d += 32) power += fabsf(fr[d] * dv[d * a.dof_elem_stride]);
+  return warp_sum(power);
+}
+
+}  // namespace pulse

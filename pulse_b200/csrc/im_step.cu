@@ -21,8 +21,7 @@
 // HBM-bound by design: algorithmic traffic is 9 396 B per env-step (SURVEY.md 8d), nothing is
 // re-read from DRAM.  References: humanoid_im.py:853-919, :1119-1192, :677-851, :1328-1378,
 // :1543-1628; humanoid.py:1675-1731; motion_lib_base.py:434-517, :546-556.
-#include "pulse_common.cuh"
-#include "quat_math.cuh"
+#include "humanoid_obs.cuh"
 
 namespace pulse {
 namespace {
@@ -141,11 +140,6 @@ __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.comm
 __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
-__device__ __forceinline__ Quat ld4(const float* p) {
-  float4 v = *reinterpret_cast<const float4*>(p);
-  return {v.x, v.y, v.z, v.w};
-}
-
 // Reference pose of body j blended between two frame records.
 struct RefPose {
   Vec3 p, v, w;
@@ -157,7 +151,7 @@ __device__ __forceinline__ RefPose blend_pose(const float* f0, const float* f1, 
   r.p.x = __fadd_rn(lerp_rn(f0[3 * j + 0], f1[3 * j + 0], b), gx);
   r.p.y = __fadd_rn(lerp_rn(f0[3 * j + 1], f1[3 * j + 1], b), gy);
   r.p.z = __fadd_rn(lerp_rn(f0[3 * j + 2], f1[3 * j + 2], b), gz);
-  r.q = slerp(ld4(f0 + 72 + 4 * j), ld4(f1 + 72 + 4 * j), b);
+  r.q = slerp(ldq4(f0 + 72 + 4 * j), ldq4(f1 + 72 + 4 * j), b);
   const float a = 1.0f - b;
   const float* v0 = f0 + 168 + 3 * j;
   const float* v1 = f1 + 168 + 3 * j;
@@ -166,12 +160,6 @@ __device__ __forceinline__ RefPose blend_pose(const float* f0, const float* f1, 
   const float* w1 = f1 + 240 + 3 * j;
   r.w = {a * w0[0] + b * w1[0], a * w0[1] + b * w1[1], a * w0[2] + b * w1[2]};
   return r;
-}
-
-__device__ __forceinline__ void st3(float* o, Vec3 v) {
-  o[0] = v.x;
-  o[1] = v.y;
-  o[2] = v.z;
 }
 
 // ---- planner: one pass plans kBatch groups (lane = group-in-batch * 8 + env slot) ----------------------
@@ -461,23 +449,24 @@ __global__ void __launch_bounds__(kThreads, 1) im_step_kernel(const pulse_motion
       // global 16-byte boundaries coincide with shared ones; a row starting 3 floats past a boundary would need 937 staging floats:
       // it is written straight to global memory instead (never the case for [N, 934]-strided buffers: 934 k = 0 or 2 mod 4)
       float* o = ophase == 3 ? orow : blk + ophase;
-      // self observation (humanoid.py:1675-1731)
+      // self observation, store_self_obs's layout written out: through the helper ptxas fuses the other product of yaw_rot's
+      // a * b - c * d, which moves the result by an ulp
       if (j == 0) o[0] = p_root.z;
-      else st3(o + 1 + 3 * (j - 1), yaw_rot(yr, p - p_root));
+      else stv(o + 1 + 3 * (j - 1), yaw_rot(yr, p - p_root));
       qsix(yaw_mul_left(-hs, hc, q), o + 70 + 6 * j);
-      st3(o + 214 + 3 * j, yaw_rot(yr, v));
-      st3(o + 286 + 3 * j, yaw_rot(yr, w));
+      stv(o + 214 + 3 * j, yaw_rot(yr, v));
+      stv(o + 286 + 3 * j, yaw_rot(yr, w));
       // task observation v6 (humanoid_im.py:1328-1378), block-major
       float* t = o + PULSE_SELF_OBS;
-      st3(t + 3 * j, yaw_rot(yr, r2.p - p));
+      stv(t + 3 * j, yaw_rot(yr, r2.p - p));
       qsix(yaw_mul_right(yaw_mul_left(-hs, hc, qmul(r2.q, qconj(q))), hs, hc), t + 72 + 6 * j);
-      st3(t + 216 + 3 * j, yaw_rot(yr, r2.v - v));
-      st3(t + 288 + 3 * j, yaw_rot(yr, r2.w - w));
-      st3(t + 360 + 3 * j, yaw_rot(yr, r2.p - p_root));
+      stv(t + 216 + 3 * j, yaw_rot(yr, r2.v - v));
+      stv(t + 288 + 3 * j, yaw_rot(yr, r2.w - w));
+      stv(t + 360 + 3 * j, yaw_rot(yr, r2.p - p_root));
       qsix(yaw_mul_left(-hs, hc, r2.q), t + 432 + 6 * j);
       // reference-pose side buffers (humanoid_im.py:835-848)
-      if (a.ref_body_pos != nullptr) st3(a.ref_body_pos + P.env * (kNB * 3) + 3 * j, r2.p);
-      if (a.ref_body_vel != nullptr) st3(a.ref_body_vel + P.env * (kNB * 3) + 3 * j, r2.v);
+      if (a.ref_body_pos != nullptr) stv(a.ref_body_pos + P.env * (kNB * 3) + 3 * j, r2.p);
+      if (a.ref_body_vel != nullptr) stv(a.ref_body_vel + P.env * (kNB * 3) + 3 * j, r2.v);
       if (a.ref_body_rot != nullptr) {
         float* d = a.ref_body_rot + P.env * (kNB * 4) + 4 * j;
         d[0] = r2.q.x; d[1] = r2.q.y; d[2] = r2.q.z; d[3] = r2.q.w;
@@ -486,7 +475,7 @@ __global__ void __launch_bounds__(kThreads, 1) im_step_kernel(const pulse_motion
         // dof_pos = exp_map(slerp(lrs[f0, j], lrs[f1, j], blend)), joints 1..23 (motion_lib_base.py:489-490)
         const float* x0 = lib.aux_rec + P.aux0 * PULSE_AUX_REC + 4 * j;
         const float* x1 = lib.aux_rec + P.aux1 * PULSE_AUX_REC + 4 * j;
-        st3(a.ref_dof_pos + P.env * PULSE_NUM_DOF + 3 * (j - 1), quat_exp_map(slerp(ld4(x0), ld4(x1), P.b_obs)));
+        stv(a.ref_dof_pos + P.env * PULSE_NUM_DOF + 3 * (j - 1), quat_exp_map(slerp(ldq4(x0), ldq4(x1), P.b_obs)));
       }
     }
     // column sums of the partials: thread (kk, c) adds 24 values; fallen flags OR-ed per env

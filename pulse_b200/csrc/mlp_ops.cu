@@ -11,17 +11,6 @@ namespace {
 
 constexpr int kSMs = kNumSMs;
 
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
-__device__ __forceinline__ float warp_sum_f(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
-
 // ---- RunningMeanStd normalise + clamp -> bf16 (and transposed bf16) -------------------------------------------
 // One CTA handles a 32-row x 32-col tile so the transposed copy can go through a padded shared tile.
 __global__ void __launch_bounds__(256) normalize_kernel(const float* __restrict__ x, long long ldx, long long rows, long long cols,
@@ -154,8 +143,8 @@ __global__ void __launch_bounds__(128) gaussian_sample_kernel(const float* __res
     acc += z * z;
     ls += l;
   }
-  acc = warp_sum_f(acc);
-  ls = warp_sum_f(ls);
+  acc = warp_sum(acc);
+  ls = warp_sum(ls);
   if (lane == 0) neglogp[row] = 0.5f * acc + 0.5f * 1.8378770664093453f * A + ls;  // log(2*pi)
 }
 
@@ -177,7 +166,7 @@ __global__ void __launch_bounds__(256) ppo_loss_kernel(const pulse_ppo_loss_args
     inv_sg2[q] = 1.0f / (sg[q] * sg[q]);
     lsum += k < A ? l : 0.0f;
   }
-  lsum = warp_sum_f(lsum);
+  lsum = warp_sum(lsum);
   const float inv_rows = 1.0f / static_cast<float>(rows);
   double st[6] = {0, 0, 0, 0, 0, 0};
   for (long long row = warp0; row < rows; row += nwarps) {
@@ -201,9 +190,9 @@ __global__ void __launch_bounds__(256) ppo_loss_kernel(const pulse_ppo_loss_args
         }
       }
     }
-    z2 = warp_sum_f(z2);
-    bl = warp_sum_f(bl);
-    kl = warp_sum_f(kl);
+    z2 = warp_sum(z2);
+    bl = warp_sum(bl);
+    kl = warp_sum(kl);
     const float nlp = 0.5f * z2 + 0.5f * 1.8378770664093453f * A + lsum;
     const float ratio = expf(old_nlp - nlp);
     const float rc = fminf(fmaxf(ratio, 1.0f - a.e_clip), 1.0f + a.e_clip);
@@ -340,7 +329,7 @@ __global__ void __launch_bounds__(256) sum_squares_kernel(const float* __restric
     s += static_cast<double>(fmaf(a.x, a.x, fmaf(a.y, a.y, fmaf(a.z, a.z, a.w * a.w))));
   }
   for (long long k = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; k < count; k += stride) s += static_cast<double>(x[k] * x[k]);
-  s = warp_sum_d(s);
+  s = warp_sum(s);
   __shared__ double ws[8];
   if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = s;
   __syncthreads();
@@ -442,7 +431,7 @@ __global__ void __launch_bounds__(256) disc_loss_kernel(const float* __restrict_
   }
   __shared__ double ws[8][4];
 #pragma unroll
-  for (int k = 0; k < 4; ++k) st[k] = warp_sum_d(st[k]);
+  for (int k = 0; k < 4; ++k) st[k] = warp_sum(st[k]);
   if ((threadIdx.x & 31) == 0)
     for (int k = 0; k < 4; ++k) ws[threadIdx.x >> 5][k] = st[k];
   __syncthreads();
@@ -547,7 +536,7 @@ __global__ void __launch_bounds__(256) head1_forward_kernel(const __nv_bfloat16*
     }
 #pragma unroll
     for (int i = 0; i < R; ++i) {
-      const float t = warp_sum_f(acc[i]);
+      const float t = warp_sum(acc[i]);
       if (lane == 0 && r0 + i < rows) out[(r0 + i) * ldo] = t + b;
     }
   }
@@ -650,14 +639,6 @@ __global__ void __launch_bounds__(256) ordered_sum_kernel(const float* __restric
     for (long long k = 0; k < n; ++k) s += __ldg(p + k * stride_n);
     out[r * ldo + c] += s;
   }
-}
-
-inline unsigned grid_for(long long work_items, int per_block, int waves = 8) {
-  long long b = (work_items + per_block - 1) / per_block;
-  const long long cap = static_cast<long long>(kSMs) * waves;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return static_cast<unsigned>(b);
 }
 
 }  // namespace
@@ -785,9 +766,8 @@ extern "C" int pulse_ppo_loss(const pulse_ppo_loss_args_t* args, int64_t rows, v
   const pulse_ppo_loss_args_t& a = *args;
   PULSE_REQUIRE(a.mu && a.value && a.actions && a.old_neglogp && a.advantages && a.returns && a.logstd, "pulse_ppo_loss: null input");
   PULSE_REQUIRE(a.num_actions > 0 && a.num_actions <= 128, "pulse_ppo_loss: num_actions outside [1,128]");
-  long long blocks = (rows + 7) / 8;            // 8 warps per block, one row per warp at a time
-  if (blocks > 8LL * kSMs) blocks = 8LL * kSMs; // all resident: 2048 threads per SM
-  ppo_loss_kernel<<<static_cast<unsigned>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, rows);
+  // 8 warps per block, one row per warp at a time; 8 blocks per SM are all resident (2048 threads per SM)
+  ppo_loss_kernel<<<grid_for(rows, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, rows);
   PULSE_LAUNCH_OK("ppo_loss_kernel");
   return PULSE_OK;
 }
@@ -896,8 +876,7 @@ __global__ void __launch_bounds__(256) weight_reg_kernel(const pulse_weight_reg_
       sq += static_cast<double>(w * w);
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(kFull, sq, o);
+  sq = warp_sum(sq);
   __shared__ double part_s[8];
   if ((threadIdx.x & 31) == 0) part_s[threadIdx.x >> 5] = sq;
   __syncthreads();

@@ -47,11 +47,6 @@ __global__ void pack_tables_kernel(pulse_motionlib_desc_t d) {
   }
 }
 
-__device__ __forceinline__ Quat ldq(const float* p) {
-  float4 v = *reinterpret_cast<const float4*>(p);
-  return {v.x, v.y, v.z, v.w};
-}
-
 // One warp per query, lane j = body j.  Everything is read straight from the packed records (L2).
 __global__ void __launch_bounds__(128) motion_state_kernel(const pulse_motionlib_desc_t lib, const pulse_motion_query_t q,
                                                            long long n) {
@@ -88,7 +83,7 @@ __global__ void __launch_bounds__(128) motion_state_kernel(const pulse_motionlib
     w.x = lerp_rn(r0[240 + 3 * j], r1[240 + 3 * j], b);
     w.y = lerp_rn(r0[241 + 3 * j], r1[241 + 3 * j], b);
     w.z = lerp_rn(r0[242 + 3 * j], r1[242 + 3 * j], b);
-    const Quat rq = slerp(ldq(r0 + 72 + 4 * j), ldq(r1 + 72 + 4 * j), b);
+    const Quat rq = slerp(ldq4(r0 + 72 + 4 * j), ldq4(r1 + 72 + 4 * j), b);
     if (q.rg_pos) { float* d = q.rg_pos + i * 72 + 3 * j; d[0] = p.x; d[1] = p.y; d[2] = p.z; }
     if (q.body_vel) { float* d = q.body_vel + i * 72 + 3 * j; d[0] = v.x; d[1] = v.y; d[2] = v.z; }
     if (q.body_ang_vel) { float* d = q.body_ang_vel + i * 72 + 3 * j; d[0] = w.x; d[1] = w.y; d[2] = w.z; }
@@ -104,7 +99,7 @@ __global__ void __launch_bounds__(128) motion_state_kernel(const pulse_motionlib
     const float* x0 = lib.aux_rec + f0 * PULSE_AUX_REC;
     const float* x1 = lib.aux_rec + f1 * PULSE_AUX_REC;
     if (q.dof_pos && lane >= 1 && lane < PULSE_NUM_BODIES) {
-      Vec3 em = quat_exp_map(slerp(ldq(x0 + 4 * lane), ldq(x1 + 4 * lane), b));
+      Vec3 em = quat_exp_map(slerp(ldq4(x0 + 4 * lane), ldq4(x1 + 4 * lane), b));
       float* d = q.dof_pos + i * PULSE_NUM_DOF + 3 * (lane - 1);
       d[0] = em.x; d[1] = em.y; d[2] = em.z;
     }
@@ -136,10 +131,7 @@ extern "C" int pulse_motionlib_create(const pulse_motionlib_desc_t* desc, void* 
   PULSE_REQUIRE(d.aux_rec == nullptr || (aligned16(d.aux_rec) && d.lrs && d.dvs),
                 "pulse_motionlib_create: aux_rec needs 16-byte alignment and the lrs/dvs tables");
   const long long total = d.total_frames * (PULSE_FRAME_REC + PULSE_AUX_REC);
-  const int threads = 256;
-  long long blocks = (total + threads - 1) / threads;
-  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
-  pack_tables_kernel<<<static_cast<unsigned>(blocks), threads, 0, static_cast<cudaStream_t>(stream)>>>(d);
+  pack_tables_kernel<<<grid_for(total, 256, 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(d);
   PULSE_LAUNCH_OK("pack_tables_kernel");
   pulse_motionlib* h = static_cast<pulse_motionlib*>(malloc(sizeof(pulse_motionlib)));
   PULSE_REQUIRE(h != nullptr, "pulse_motionlib_create: host allocation failed");

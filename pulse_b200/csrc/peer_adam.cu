@@ -137,8 +137,7 @@ __global__ void __launch_bounds__(kPeerThreads, 1) peer_reduce_adam_kernel(const
     sq += static_cast<double>(fmaf(acc.x, acc.x, fmaf(acc.y, acc.y, fmaf(acc.z, acc.z, acc.w * acc.w))));
   }
   __shared__ double red[kPeerThreads / 32];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(kFull, sq, o);
+  sq = warp_sum(sq);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = sq;
   __syncthreads();
   if (threadIdx.x == 0) {

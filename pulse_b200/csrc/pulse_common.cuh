@@ -47,6 +47,23 @@ constexpr int kWarp = 32;
 constexpr int kNumSMs = 132;
 constexpr unsigned kFull = 0xffffffffu;
 
+// Blocks for `items` work items at `per_block` per block, capped at `waves` blocks per SM: the kernels grid-stride over the rest.
+inline unsigned grid_for(long long items, int per_block, int waves = 8) {
+  long long b = (items + per_block - 1) / per_block;
+  const long long cap = static_cast<long long>(kNumSMs) * waves;
+  if (b > cap) b = cap;
+  if (b < 1) b = 1;
+  return static_cast<unsigned>(b);
+}
+
+// Sum over the 32 lanes of a full warp (float or double), the result in every lane.
+template <typename T>
+__device__ __forceinline__ T warp_sum(T v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
+  return v;
+}
+
 }  // namespace pulse
 
 struct pulse_motionlib {

@@ -22,6 +22,19 @@ __device__ __forceinline__ Vec3 operator+(Vec3 a, Vec3 b) { return {a.x + b.x, a
 __device__ __forceinline__ float dot3(Vec3 a, Vec3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
 __device__ __forceinline__ float sq3(Vec3 a) { return a.x * a.x + a.y * a.y + a.z * a.z; }
 
+__device__ __forceinline__ Vec3 ldv(const float* p) { return {p[0], p[1], p[2]}; }
+__device__ __forceinline__ Quat ldq(const float* p) { return {p[0], p[1], p[2], p[3]}; }
+// one 16-byte load: p must be 16-byte aligned
+__device__ __forceinline__ Quat ldq4(const float* p) {
+  const float4 v = *reinterpret_cast<const float4*>(p);
+  return {v.x, v.y, v.z, v.w};
+}
+__device__ __forceinline__ void stv(float* o, Vec3 v) {
+  o[0] = v.x;
+  o[1] = v.y;
+  o[2] = v.z;
+}
+
 // isaacgym.torch_utils.quat_mul [3P-memory]: 8-multiplication Hamilton product.
 __device__ __forceinline__ Quat qmul(Quat a, Quat b) {
   float ww = (a.z + a.x) * (b.x + b.y);
@@ -38,6 +51,11 @@ __device__ __forceinline__ Quat qmul(Quat a, Quat b) {
 }
 
 __device__ __forceinline__ Quat qconj(Quat a) { return {-a.x, -a.y, -a.z, a.w}; }
+
+// humanoid.py:1617-1620 (remove_base_rot): q (x) conj(0.5, 0.5, 0.5, 0.5), skipped for an upright start
+__device__ __forceinline__ Quat base_rot_removed(Quat q, bool upright) {
+  return upright ? q : qmul(q, Quat{-0.5f, -0.5f, -0.5f, 0.5f});
+}
 
 // phc/utils/torch_utils.py:45-55 (my_quat_rotate)
 __device__ __forceinline__ Vec3 qrot(Quat q, Vec3 v) {

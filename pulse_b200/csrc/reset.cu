@@ -9,15 +9,12 @@
 //                           humanoid.py:589-609); every k writes its AMP observation row (_init_amp_obs, humanoid_amp.py:519-563).
 // HBM-bound gather / scatter: ~44 KB of packed frame records per reset env (20 rows x 2 208 B), ~11 KB written.
 #include "philox.cuh"
-#include "pulse_common.cuh"
-#include "quat_math.cuh"
+#include "humanoid_obs.cuh"
 
 namespace pulse {
 namespace {
 
 constexpr int kCompactThreads = 1024;
-__constant__ int r_kept_joint[19] = {0, 1, 2, 4, 5, 6, 8, 9, 10, 11, 12, 13, 14, 15, 16, 18, 19, 20, 21};   // amp_obs.cu
-__constant__ int r_key_body[4] = {7, 3, 22, 17};
 
 __global__ void __launch_bounds__(kCompactThreads) reset_compact_kernel(const pulse_reset_args_t a, long long num_envs) {
   __shared__ int warp_cnt[kCompactThreads / 32];
@@ -53,11 +50,6 @@ __global__ void __launch_bounds__(kCompactThreads) reset_compact_kernel(const pu
     __syncthreads();
   }
   if (tid == 0) *a.count = base;
-}
-
-__device__ __forceinline__ Quat ldq4(const float* p) {
-  const float4 v = *reinterpret_cast<const float4*>(p);
-  return {v.x, v.y, v.z, v.w};
 }
 
 __global__ void __launch_bounds__(256) reset_ref_state_kernel(const pulse_motionlib_desc_t lib, const pulse_reset_args_t a) {
@@ -142,36 +134,16 @@ __global__ void __launch_bounds__(256) reset_ref_state_kernel(const pulse_motion
     }
     if (a.amp_obs_buf == nullptr) continue;
     // ---- AMP observation of the reference motion at t (build_amp_observations_smpl, humanoid_amp.py:924-969) --------------------------
-    float* o = a.amp_obs_buf + (e * a.num_amp_steps + k) * PULSE_AMP_OBS;
-    float hs, hc;
-    heading_half(q0, hs, hc);
-    const Quat h_inv = {0.0f, 0.0f, -hs, hc};
-    const Yaw yr = make_yaw(h_inv);
-    if (lane == 0) {
-      o[0] = p0.z;
-      float six[6];
-      qsix(qmul(h_inv, q0), six);
-#pragma unroll
-      for (int c = 0; c < 6; ++c) o[1 + c] = six[c];
-      const Vec3 lv = yaw_rot(yr, v0), lw = yaw_rot(yr, w0);
-      o[7] = lv.x; o[8] = lv.y; o[9] = lv.z; o[10] = lw.x; o[11] = lw.y; o[12] = lw.z;
-    }
-    if (lane < 19) {
-      const int jt = r_kept_joint[lane];            // joint jt = body jt + 1
-      const Vec3 em = quat_exp_map(slerp(ldq4(x0 + 4 * (jt + 1)), ldq4(x1 + 4 * (jt + 1)), b));
-      float six[6];
-      qsix(exp_map_quat(em), six);                  // dof_to_obs_smpl (humanoid.py:1436-1446)
-#pragma unroll
-      for (int c = 0; c < 6; ++c) o[13 + 6 * lane + c] = six[c];
-#pragma unroll
-      for (int c = 0; c < 3; ++c) o[127 + 3 * lane + c] = lerp_rn(x0[96 + 3 * jt + c], x1[96 + 3 * jt + c], b);
-    } else if (lane < 23) {
-      const int kb = r_key_body[lane - 19];
-      Vec3 pk;
-      pk.x = lerp_rn(r0[3 * kb], r1[3 * kb], b); pk.y = lerp_rn(r0[3 * kb + 1], r1[3 * kb + 1], b); pk.z = lerp_rn(r0[3 * kb + 2], r1[3 * kb + 2], b);
-      const Vec3 lp = yaw_rot(yr, pk - p0);
-      o[184 + 3 * (lane - 19)] = lp.x; o[185 + 3 * (lane - 19)] = lp.y; o[186 + 3 * (lane - 19)] = lp.z;
-    }
+    // joint jt = body jt + 1: dof_pos = exp_map(slerp(local rotations)), dof_vel blended
+    const auto joint = [&](int jt) {
+      return AmpJoint{quat_exp_map(slerp(ldq4(x0 + 4 * (jt + 1)), ldq4(x1 + 4 * (jt + 1)), b)),
+                      {lerp_rn(x0[96 + 3 * jt], x1[96 + 3 * jt], b), lerp_rn(x0[97 + 3 * jt], x1[97 + 3 * jt], b),
+                       lerp_rn(x0[98 + 3 * jt], x1[98 + 3 * jt], b)}};
+    };
+    const auto key_pos = [&](int kb) {
+      return Vec3{lerp_rn(r0[3 * kb], r1[3 * kb], b), lerp_rn(r0[3 * kb + 1], r1[3 * kb + 1], b), lerp_rn(r0[3 * kb + 2], r1[3 * kb + 2], b)};
+    };
+    store_amp_obs(a.amp_obs_buf + (e * a.num_amp_steps + k) * PULSE_AMP_OBS, lane, p0, q0, v0, w0, joint, key_pos);
   }
 }
 

@@ -10,17 +10,10 @@
 //                       of the in-place shift (7 056 + 7 840) followed by a 7 840 + 7 840 B copy.  Envs reset since the last step take
 //                       their previous row from the rows `pulse_reset_ref_state` back-filled (`fresh` flags, cleared here).
 #include "philox.cuh"
-#include "pulse_common.cuh"
-#include "quat_math.cuh"
+#include "humanoid_obs.cuh"
 
 namespace pulse {
 namespace {
-
-__device__ __forceinline__ float wsum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
 
 // RunningMeanStd.forward(unnorm=True): clamp(y, -5, 5) * sqrt(var.float() + eps) + mean.float()
 __device__ __forceinline__ float value_unnorm(float y, const double* mean, const double* var, float eps) {
@@ -66,8 +59,8 @@ __global__ void __launch_bounds__(128) policy_post_kernel(const pulse_policy_pos
       ls += l;
     }
   }
-  acc = wsum(acc);
-  ls = wsum(ls);
+  acc = warp_sum(acc);
+  ls = warp_sum(ls);
   if (lane == 0) {
     a.neglogp[row * a.ld_neglogp] = 0.5f * acc + 0.5f * 1.8378770664093453f * A + ls;   // log(2*pi)
     if (a.values_out != nullptr) a.values_out[row * a.ld_values] = value_unnorm(a.value[row * a.ld_value], a.value_mean, a.value_var, a.value_eps);
@@ -84,8 +77,6 @@ __global__ void __launch_bounds__(256) value_post_kernel(const float* __restrict
   out[r * ld_out] = v;
 }
 
-__constant__ int a_kept_joint[19] = {0, 1, 2, 4, 5, 6, 8, 9, 10, 11, 12, 13, 14, 15, 16, 18, 19, 20, 21};
-__constant__ int a_key_body[4] = {7, 3, 22, 17};
 constexpr int kAmp = PULSE_AMP_OBS;
 
 __global__ void __launch_bounds__(128) amp_row_kernel(const pulse_amp_row_args_t a, long long n) {
@@ -116,45 +107,8 @@ __global__ void __launch_bounds__(128) amp_row_kernel(const pulse_amp_row_args_t
     for (int c = lane + 512; c < nvec; c += 32) dst[c] = src[c];   // more than 11 history steps
   }
   if (fresh && lane == 0) a.fresh[e] = 0;
-  // ---- current observation (same arithmetic as amp_obs_kernel) ---------------------------------------------------------------
-  const float* bs = a.body_state + e * a.body_env_stride;
-  const Vec3 p0 = {bs[0], bs[1], bs[2]};
-  const Quat q0 = {bs[3], bs[4], bs[5], bs[6]};
-  float hs, hc;
-  heading_half(q0, hs, hc);
-  const Quat h_inv = {0.0f, 0.0f, -hs, hc};
-  const Yaw yr = make_yaw(h_inv);
-  float* o = out;
-  if (lane == 0) {
-    o[0] = p0.z;
-    float six[6];
-    qsix(qmul(h_inv, q0), six);
-#pragma unroll
-    for (int i = 0; i < 6; ++i) o[1 + i] = six[i];
-    const Vec3 lv = yaw_rot(yr, {bs[7], bs[8], bs[9]});
-    const Vec3 lw = yaw_rot(yr, {bs[10], bs[11], bs[12]});
-    o[7] = lv.x; o[8] = lv.y; o[9] = lv.z;
-    o[10] = lw.x; o[11] = lw.y; o[12] = lw.z;
-  }
-  const float* dp = a.dof_pos + e * a.dof_env_stride;
-  const float* dv = a.dof_vel + e * a.dof_env_stride;
-  if (lane < 19) {
-    const int jt = a_kept_joint[lane];
-    const Vec3 em = {dp[(3 * jt + 0) * a.dof_elem_stride], dp[(3 * jt + 1) * a.dof_elem_stride], dp[(3 * jt + 2) * a.dof_elem_stride]};
-    float six[6];
-    qsix(exp_map_quat(em), six);
-#pragma unroll
-    for (int i = 0; i < 6; ++i) o[13 + 6 * lane + i] = six[i];
-#pragma unroll
-    for (int i = 0; i < 3; ++i) o[127 + 3 * lane + i] = dv[(3 * jt + i) * a.dof_elem_stride];
-  } else if (lane < 23) {
-    const int kb = a_key_body[lane - 19];
-    const float* bk = bs + kb * PULSE_BODY_STATE_W;
-    const Vec3 lp = yaw_rot(yr, Vec3{bk[0], bk[1], bk[2]} - p0);
-    o[184 + 3 * (lane - 19) + 0] = lp.x;
-    o[184 + 3 * (lane - 19) + 1] = lp.y;
-    o[184 + 3 * (lane - 19) + 2] = lp.z;
-  }
+  // ---- current observation -------------------------------------------------------------------------------------------------------
+  store_amp_obs_sim(out, lane, a, e);
 }
 
 __global__ void bump_counter_kernel(unsigned long long* c, unsigned long long by) { *c += by; }

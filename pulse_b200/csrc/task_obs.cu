@@ -11,10 +11,6 @@
 namespace pulse {
 namespace {
 
-__device__ __forceinline__ Quat ldq(const float* p) { return {p[0], p[1], p[2], p[3]}; }
-__device__ __forceinline__ Vec3 ldv(const float* p) { return {p[0], p[1], p[2]}; }
-__device__ __forceinline__ void stv(float* o, Vec3 v) { o[0] = v.x; o[1] = v.y; o[2] = v.z; }
-
 __global__ void __launch_bounds__(128) task_obs_kernel(const pulse_task_obs_args_t a) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= a.num_envs) return;
@@ -23,8 +19,7 @@ __global__ void __launch_bounds__(128) task_obs_kernel(const pulse_task_obs_args
   const float* bs = a.body_state + e * a.body_env_stride;
   // heading of the ROOT body (body 0 of the env, not of the subset): humanoid_im.py:746-747
   const Vec3 p_root = ldv(bs);
-  Quat q_root = ldq(bs + 3);
-  if (!a.upright) q_root = qmul(q_root, Quat{-0.5f, -0.5f, -0.5f, 0.5f});   // remove_base_rot (humanoid.py:1617-1620)
+  const Quat q_root = base_rot_removed(ldq(bs + 3), a.upright != 0);
   float hs, hc;
   heading_half(q_root, hs, hc);
   const Yaw yr = make_yaw(Quat{0.0f, 0.0f, -hs, hc});

@@ -11,21 +11,14 @@
 // Cell indices, the reset mask and the trajectory segment indices are integers decided by fp32 arithmetic, so the operations that
 // feed them keep the reference's order with round-to-nearest intrinsics (no FMA contraction), as in im_step.cu.  Everything else
 // is under the 1e-4 float tolerance of the observations and rewards.
+#include "humanoid_obs.cuh"
 #include "philox.cuh"
-#include "pulse_common.cuh"
-#include "quat_math.cuh"
 
 namespace pulse {
 namespace {
 
 constexpr int kTB = PULSE_NUM_BODIES;
 constexpr int kVerts = PULSE_TRAJ_VERTS;
-
-__device__ __forceinline__ float wsum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
 
 // isaacgym.torch_utils.quat_apply [3P-memory]: t = 2 (xyz x b); b + w t + xyz x t, in this order.
 __device__ __forceinline__ Vec3 cross_rn(Vec3 a, Vec3 b) {
@@ -39,11 +32,6 @@ __device__ __forceinline__ Vec3 quat_apply_rn(Quat q, Vec3 b) {
   const Vec3 c = cross_rn(u, t);
   return {__fadd_rn(__fadd_rn(b.x, __fmul_rn(q.w, t.x)), c.x), __fadd_rn(__fadd_rn(b.y, __fmul_rn(q.w, t.y)), c.y),
           __fadd_rn(__fadd_rn(b.z, __fmul_rn(q.w, t.z)), c.z)};
-}
-
-// humanoid.py:1617-1620 (remove_base_rot): q (x) conj(0.5, 0.5, 0.5, 0.5)
-__device__ __forceinline__ Quat base_rot_removed(Quat q, bool upright) {
-  return upright ? q : qmul(q, Quat{-0.5f, -0.5f, -0.5f, 0.5f});
 }
 
 // calc_heading_quat / calc_heading_quat_inv (phc/utils/torch_utils.py:200-240) in the angle form the reference computes: heading =
@@ -97,7 +85,7 @@ __device__ __forceinline__ float center_height(const HeightField& t, const float
   const Quat qy = yaw_only(base_rot_removed(q_root, upright));
   float h = 0.0f;
   for (int i = lane; i < count; i += 32) h += height_at(t, qy, pts + 3 * i, p_root);
-  return wsum(h) / static_cast<float>(count);
+  return warp_sum(h) / static_cast<float>(count);
 }
 
 // TrajGenerator.calc_pos (traj_generator.py:148-165): phase = clip(t / (num_verts * dt), 0, 1) -- num_verts, not num_segs, as in the
@@ -133,13 +121,7 @@ __global__ void __launch_bounds__(256) terrain_step_kernel(const pulse_terrain_s
 
     if (a.flags & PULSE_STEP_REWARD) {
       // _compute_reward (:871-896): location reward against the ACTOR root state; the power term is always reported in reward_raw[:, 1]
-      float power = 0.0f;
-      if (a.dof_force != nullptr) {
-        const float* fr = a.dof_force + e * a.dof_force_stride;
-        const float* dv = a.dof_vel + e * a.dof_env_stride;
-        for (int d = lane; d < PULSE_NUM_DOF; d += 32) power += fabsf(fr[d] * dv[d * a.dof_elem_stride]);
-        power = -a.power_coefficient * wsum(power);
-      }
+      const float power = a.dof_force != nullptr ? -a.power_coefficient * dof_power(a, e, lane) : 0.0f;
       if (lane == 0) {
         const Vec3 tar = traj_pos(verts, t_now, a.traj_dur);
         const float dx = tar.x - a_pos.x, dy = tar.y - a_pos.y;
@@ -195,20 +177,6 @@ __global__ void __launch_bounds__(256) terrain_step_kernel(const pulse_terrain_s
       float hs, hc;
       heading_half(base_rot_removed(q_root, upright), hs, hc);
       const Yaw yr = make_yaw(Quat{0.0f, 0.0f, -hs, hc});
-      if (body) {
-        if (j == 0) o[0] = p_root.z - c_self;
-        else {
-          const Vec3 lp = yaw_rot(yr, Vec3{p.x - p_root.x, p.y - p_root.y, (p.z - c_self) - (p_root.z - c_self)});
-          o[1 + 3 * (j - 1)] = lp.x; o[2 + 3 * (j - 1)] = lp.y; o[3 + 3 * (j - 1)] = lp.z;
-        }
-        float six[6];
-        qsix(yaw_mul_left(-hs, hc, q), six);
-#pragma unroll
-        for (int i = 0; i < 6; ++i) o[70 + 6 * j + i] = six[i];
-        const Vec3 lv = yaw_rot(yr, v), lw = yaw_rot(yr, w);
-        o[214 + 3 * j] = lv.x; o[215 + 3 * j] = lv.y; o[216 + 3 * j] = lv.z;
-        o[286 + 3 * j] = lw.x; o[287 + 3 * j] = lw.y; o[288 + 3 * j] = lw.z;
-      }
       // _compute_task_obs (:385-440).  Trajectory samples at progress * dt + k * trajSampleTimestep (humanoid_traj.py:196-211) in the
       // heading frame of the actor root (compute_location_observations :1588-1616), xy only.
       const Quat a_rot = {rs[3], rs[4], rs[5], rs[6]};
@@ -220,6 +188,9 @@ __global__ void __launch_bounds__(256) terrain_step_kernel(const pulse_terrain_s
         t[2 * lane] = d.x;
         t[2 * lane + 1] = d.y;
       }
+      // the self observation is stored after the trajectory samples: in the other order ptxas spills a register
+      const Vec3 pc = {p.x, p.y, p.z - c_self}, rc = {p_root.x, p_root.y, p_root.z - c_self};
+      if (body) store_self_obs(o, j, pc, rc, q, v, w, hs, hc, yr);
       // height map at the head pose (get_head_pose :296-311, get_heights :718-772), relative to the mean center height around the
       // actor root (use_center_height) or to the actor root's z, clipped to +-3 m and scaled by 5
       const float ref_h = a.use_center_height ? center_height(hfield, a.center_points, a.num_center_points, a_rot, a_pos, upright, lane)
@@ -323,12 +294,6 @@ int check_heightfield(const char* who, const int16_t* hf, int64_t rows, int64_t 
   return PULSE_OK;
 }
 
-long long warp_grid(long long rows) {
-  long long ctas = (rows + 7) / 8;
-  if (ctas > kNumSMs * 8ll) ctas = kNumSMs * 8ll;
-  return ctas < 1 ? 1 : ctas;
-}
-
 }  // namespace
 }  // namespace pulse
 
@@ -363,7 +328,7 @@ extern "C" int pulse_terrain_step(const pulse_terrain_step_args_t* args, int64_t
     const int st = check_heightfield("pulse_terrain_step", a.heightfield, a.hf_rows, a.hf_cols, a.horizontal_scale);
     if (st != PULSE_OK) return st;
   }
-  terrain_step_kernel<<<static_cast<unsigned>(warp_grid(num_envs)), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, (long long)num_envs);
+  terrain_step_kernel<<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, (long long)num_envs);
   PULSE_LAUNCH_OK("terrain_step_kernel");
   return PULSE_OK;
 }
@@ -394,7 +359,7 @@ extern "C" int pulse_terrain_heights(const pulse_terrain_heights_args_t* args, v
   PULSE_REQUIRE(a.root_stride >= 7 && a.heights_stride >= a.num_points, "pulse_terrain_heights: strides too small");
   const int st = check_heightfield("pulse_terrain_heights", a.heightfield, a.hf_rows, a.hf_cols, a.horizontal_scale);
   if (st != PULSE_OK) return st;
-  terrain_heights_kernel<<<static_cast<unsigned>(warp_grid(a.num_rows)), 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
+  terrain_heights_kernel<<<grid_for(a.num_rows, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
   PULSE_LAUNCH_OK("terrain_heights_kernel");
   return PULSE_OK;
 }

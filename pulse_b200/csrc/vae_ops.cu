@@ -1,29 +1,12 @@
-// Row-wise kernels of the PULSE VAE distillation path (SURVEY K17-K19), the Z-task action decode (K20), the reach task
-// (K21) and the PD-target map (K22).  The dense layers between them run on the wgmma GEMM; everything here is
-// HBM-bound streaming work: one warp per row (lane = latent dimension / body), fp64 atomics for the scalar statistics.
+// Row-wise kernels of the PULSE VAE distillation path (SURVEY K17-K19), the Z-task action decode (K20) and the PD-target map
+// (K22).  The dense layers between them run on the wgmma GEMM; everything here is HBM-bound streaming work: element-wise
+// grid-stride loops, or one warp per row (lane = action / latent dimension) with fp64 atomics for the scalar statistics.
 #include <cuda_bf16.h>
 
 #include "pulse_common.cuh"
-#include "quat_math.cuh"
 
 namespace pulse {
 namespace {
-
-constexpr int kSMs = kNumSMs;
-
-inline unsigned warp_grid(long long rows, int warps_per_block, int waves = 8) {
-  long long blocks = (rows + warps_per_block - 1) / warps_per_block;
-  const long long cap = static_cast<long long>(kSMs) * waves;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return static_cast<unsigned>(blocks);
-}
-
-__device__ __forceinline__ float wsum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
 
 // ---- normalise a column window -------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) normalize_cols_kernel(const float* __restrict__ x, long long ldx, long long rows, long long cols,
@@ -95,7 +78,7 @@ __global__ void __launch_bounds__(256) vae_action_loss_kernel(const float* __res
       d[q] = c < A ? pred[r * ld_pred + c] - gt[r * ld_gt + c] : 0.0f;
       ss = fmaf(d[q], d[q], ss);
     }
-    ss = wsum(ss);
+    ss = warp_sum(ss);
     const float nrm = sqrtf(ss);
     const float scale = nrm > 0.0f ? inv_rows / nrm : 0.0f;  // torch.norm backward: 0 at the origin
 #pragma unroll
@@ -161,7 +144,7 @@ __global__ void __launch_bounds__(256) vae_latent_kernel(const pulse_vae_latent_
         if (keep) {
           const float prev = on ? a.enc_head[(r - 1) * a.ld_enc + lane] : 0.0f;
           const float e = on ? qm - a.phi * prev : 0.0f;
-          const float nrm = sqrtf(wsum(e * e));
+          const float nrm = sqrtf(warp_sum(e * e));
           if (nrm > 0.0f) g_qm += a.ar1_coef * inv_pairs * e / nrm;
           ar_row = nrm;  // each pair is counted once, by its "next" row
         }
@@ -172,7 +155,7 @@ __global__ void __launch_bounds__(256) vae_latent_kernel(const pulse_vae_latent_
         if (keep) {
           const float nxt = on ? a.enc_head[(r + 1) * a.ld_enc + lane] : 0.0f;
           const float e = on ? nxt - a.phi * qm : 0.0f;
-          const float nrm = sqrtf(wsum(e * e));
+          const float nrm = sqrtf(warp_sum(e * e));
           if (nrm > 0.0f) g_qm -= a.ar1_coef * inv_pairs * a.phi * e / nrm;
         }
       }
@@ -191,13 +174,13 @@ __global__ void __launch_bounds__(256) vae_latent_kernel(const pulse_vae_latent_
       d_pri[r * a.ld_dp + lane] = __float2bfloat16(g_pm);
       d_pri[r * a.ld_dp + E + lane] = __float2bfloat16(g_pv);
     }
-    s_kl += static_cast<double>(wsum(kl));
+    s_kl += static_cast<double>(warp_sum(kl));
     s_ar += static_cast<double>(ar_row);
     if (a.regu_coef != 0.0f) {
-      s_pm += static_cast<double>(wsum(on ? pm * pm : 0.0f));
-      s_qm += static_cast<double>(wsum(on ? qm * qm : 0.0f));
-      s_pv += static_cast<double>(wsum(on ? pv * pv : 0.0f));
-      s_qv += static_cast<double>(wsum(on ? qv * qv : 0.0f));
+      s_pm += static_cast<double>(warp_sum(on ? pm * pm : 0.0f));
+      s_qm += static_cast<double>(warp_sum(on ? qm * qm : 0.0f));
+      s_pv += static_cast<double>(warp_sum(on ? pv * pv : 0.0f));
+      s_qv += static_cast<double>(warp_sum(on ? qv * qv : 0.0f));
     }
   }
   if (lane == 0) {
@@ -243,86 +226,6 @@ __global__ void __launch_bounds__(256) pd_targets_kernel(const float* __restrict
   }
 }
 
-// ---- reach task --------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) reach_update_task_kernel(const long long* __restrict__ progress, long long* __restrict__ change,
-                                                                float* __restrict__ tar, const float* __restrict__ u,
-                                                                const long long* __restrict__ steps, float dist_max, float h_min, float h_max,
-                                                                long long n) {
-  for (long long e = blockIdx.x * 256ll + threadIdx.x; e < n; e += 256ll * gridDim.x) {
-    if (progress[e] >= change[e]) {
-      tar[3 * e + 0] = dist_max * (2.0f * u[3 * e + 0] - 1.0f);
-      tar[3 * e + 1] = dist_max * (2.0f * u[3 * e + 1] - 1.0f);
-      tar[3 * e + 2] = (h_max - h_min) * u[3 * e + 2] + h_min;
-      change[e] = progress[e] + steps[e];
-    }
-  }
-}
-
-constexpr int kNB = 24;
-
-__global__ void __launch_bounds__(256) reach_step_kernel(const pulse_reach_step_args_t a, long long n) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (long long e = blockIdx.x * 8ll + warp; e < n; e += 8ll * gridDim.x) {
-    const int j = lane;
-    const bool body = j < kNB;
-    const float* bs = a.body_state + e * a.body_env_stride + (body ? j : 0) * 13;
-    Vec3 p = {bs[0], bs[1], bs[2]}, v = {bs[7], bs[8], bs[9]}, w = {bs[10], bs[11], bs[12]};
-    Quat q = {bs[3], bs[4], bs[5], bs[6]};
-    const Vec3 p_root = {__shfl_sync(kFull, p.x, 0), __shfl_sync(kFull, p.y, 0), __shfl_sync(kFull, p.z, 0)};
-    const Quat q_root = {__shfl_sync(kFull, q.x, 0), __shfl_sync(kFull, q.y, 0), __shfl_sync(kFull, q.z, 0), __shfl_sync(kFull, q.w, 0)};
-    float hs, hc;
-    heading_half(q_root, hs, hc);
-    const Yaw yr = make_yaw(Quat{0.0f, 0.0f, -hs, hc});
-    float* o = a.obs_buf + e * a.obs_stride;
-    if (body) {  // compute_humanoid_observations_smpl_max (humanoid.py:1675-1731), same layout as the imitation step kernel
-      if (j == 0) o[0] = p_root.z;
-      else {
-        const Vec3 lp = yaw_rot(yr, p - p_root);
-        o[1 + 3 * (j - 1)] = lp.x; o[2 + 3 * (j - 1)] = lp.y; o[3 + 3 * (j - 1)] = lp.z;
-      }
-      float six[6];
-      qsix(yaw_mul_left(-hs, hc, q), six);
-#pragma unroll
-      for (int i = 0; i < 6; ++i) o[70 + 6 * j + i] = six[i];
-      const Vec3 lv = yaw_rot(yr, v), lw = yaw_rot(yr, w);
-      o[214 + 3 * j] = lv.x; o[215 + 3 * j] = lv.y; o[216 + 3 * j] = lv.z;
-      o[286 + 3 * j] = lw.x; o[287 + 3 * j] = lw.y; o[288 + 3 * j] = lw.z;
-    }
-    const Vec3 tar = {a.tar_pos[3 * e], a.tar_pos[3 * e + 1], a.tar_pos[3 * e + 2]};
-    // early termination (humanoid.py:1573-1608)
-    bool fall_contact = false, fall_height = false;
-    if (a.enable_early_termination && body && !((a.contact_body_mask >> j) & 1u)) {
-      if (a.contact_forces != nullptr) {
-        const float* cf = a.contact_forces + e * a.contact_env_stride + j * 3;
-        fall_contact = fabsf(cf[0]) > 0.1f || fabsf(cf[1]) > 0.1f || fabsf(cf[2]) > 0.1f;
-      }
-      fall_height = p.z < a.termination_heights[j];
-    }
-    const bool any_contact = __any_sync(kFull, fall_contact), any_height = __any_sync(kFull, fall_height);
-    // the reach body's position, broadcast
-    const int rb = a.reach_body_id;
-    const Vec3 pr = {__shfl_sync(kFull, p.x, rb), __shfl_sync(kFull, p.y, rb), __shfl_sync(kFull, p.z, rb)};
-    if (lane == 0) {
-      const Vec3 lt = yaw_rot(yr, tar - p_root);  // compute_location_observations (humanoid_reach.py:224-236)
-      o[PULSE_SELF_OBS + 0] = lt.x; o[PULSE_SELF_OBS + 1] = lt.y; o[PULSE_SELF_OBS + 2] = lt.z;
-      const Vec3 d = tar - pr;                    // compute_reach_reward (:238-250)
-      a.rew_buf[e] = expf(-4.0f * (d.x * d.x + d.y * d.y + d.z * d.z));
-      const long long prog = a.progress_buf[e];
-      const long long term = (any_contact && any_height && prog > 1) ? 1 : 0;
-      a.terminate_buf[e] = term;
-      a.reset_buf[e] = prog >= a.max_episode_length - 1 ? 1 : term;
-    }
-  }
-}
-
-inline unsigned elem_grid(long long total) {
-  long long b = (total + 255) / 256;
-  const long long cap = static_cast<long long>(kSMs) * 8;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return static_cast<unsigned>(b);
-}
-
 }  // namespace
 }  // namespace pulse
 
@@ -334,7 +237,7 @@ extern "C" int pulse_normalize_cols(const float* x, int64_t ldx, int64_t rows, i
   PULSE_REQUIRE(rows > 0 && cols > 0 && ldx >= cols && ld_out >= cols && zero_to <= ld_out, "pulse_normalize_cols: bad shape");
   PULSE_REQUIRE((mean == nullptr) == (rstd == nullptr), "pulse_normalize_cols: mean and rstd go together");
   const long long width = zero_to > cols ? zero_to : cols;
-  normalize_cols_kernel<<<elem_grid(rows * width), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  normalize_cols_kernel<<<grid_for(rows * width, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       x, ldx, rows, cols, mean, rstd, clamp, reinterpret_cast<__nv_bfloat16*>(out), ld_out, zero_to);
   PULSE_LAUNCH_OK("normalize_cols_kernel");
   return PULSE_OK;
@@ -347,7 +250,7 @@ extern "C" int pulse_copy_cols_bf16(const pulse_bf16_t* src, int64_t ld_src, int
                 "pulse_copy_cols_bf16: cols and leading dimensions must be even");
   PULSE_REQUIRE((reinterpret_cast<uintptr_t>(src) & 3) == 0 && (reinterpret_cast<uintptr_t>(dst1) & 3) == 0 &&
                     (reinterpret_cast<uintptr_t>(dst2) & 3) == 0, "pulse_copy_cols_bf16: 4-byte alignment required");
-  copy_cols_kernel<<<elem_grid(rows * (cols / 2)), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  copy_cols_kernel<<<grid_for(rows * (cols / 2), 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __nv_bfloat16*>(src), ld_src, rows, cols, reinterpret_cast<__nv_bfloat16*>(dst1), ld1,
       reinterpret_cast<__nv_bfloat16*>(dst2), ld2);
   PULSE_LAUNCH_OK("copy_cols_kernel");
@@ -362,7 +265,7 @@ extern "C" int pulse_vae_reparam(const float* head, int64_t ld_head, const float
   PULSE_REQUIRE(mode == PULSE_Z_MEAN || noise != nullptr, "pulse_vae_reparam: noise required unless mode is PULSE_Z_MEAN");
   PULSE_REQUIRE(mode == PULSE_Z_SAMPLE || mode == PULSE_Z_MEAN || mode == PULSE_Z_RESIDUAL, "pulse_vae_reparam: unknown mode %d", mode);
   PULSE_REQUIRE(ld_head >= (mode == PULSE_Z_SAMPLE ? 2 * latent : latent), "pulse_vae_reparam: head too narrow");
-  vae_reparam_kernel<<<elem_grid(rows * latent), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  vae_reparam_kernel<<<grid_for(rows * latent, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       head, ld_head, noise, ld_noise, rows, latent, mode, clamp, clamp_lo, clamp_hi, reinterpret_cast<__nv_bfloat16*>(z_bf16), ld_z, z_f32, ld_zf);
   PULSE_LAUNCH_OK("vae_reparam_kernel");
   return PULSE_OK;
@@ -373,7 +276,7 @@ extern "C" int pulse_vae_action_loss(const float* pred, int64_t ld_pred, const f
   PULSE_REQUIRE(pred && gt && dpred && stats, "pulse_vae_action_loss: null buffer");
   PULSE_REQUIRE(rows > 0 && num_actions > 0 && num_actions <= 128 && zero_to <= 128 && zero_to <= ld_d && ld_d >= num_actions,
                 "pulse_vae_action_loss: bad shape (num_actions <= 128)");
-  vae_action_loss_kernel<<<warp_grid(rows, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  vae_action_loss_kernel<<<grid_for(rows, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       pred, ld_pred, gt, ld_gt, rows, num_actions, reinterpret_cast<__nv_bfloat16*>(dpred), ld_d, zero_to, stats);
   PULSE_LAUNCH_OK("vae_action_loss_kernel");
   return PULSE_OK;
@@ -388,7 +291,7 @@ extern "C" int pulse_vae_latent_loss(const pulse_vae_latent_args_t* args, int64_
                 "pulse_vae_latent_loss: head buffers narrower than 2*latent");
   PULSE_REQUIRE(a.progress == nullptr || a.ar1_coef == 0.0f || (a.horizon > 0 && rows % a.horizon == 0),
                 "pulse_vae_latent_loss: rows must be a multiple of horizon for the AR(1) term");
-  vae_latent_kernel<<<warp_grid(rows, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, rows);
+  vae_latent_kernel<<<grid_for(rows, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, rows);
   PULSE_LAUNCH_OK("vae_latent_kernel");
   return PULSE_OK;
 }
@@ -398,7 +301,7 @@ extern "C" int pulse_pnn_compose(const float* acts, int64_t prim_stride, int64_t
   PULSE_REQUIRE(acts && w && out, "pulse_pnn_compose: null buffer");
   PULSE_REQUIRE(rows > 0 && num_actions > 0 && num_prim > 0 && ld_a >= num_actions && ld_w >= num_prim && ld_out >= num_actions,
                 "pulse_pnn_compose: bad shape");
-  pnn_compose_kernel<<<elem_grid(rows * num_actions), 256, 0, static_cast<cudaStream_t>(stream)>>>(acts, prim_stride, ld_a, w, ld_w, act, rows,
+  pnn_compose_kernel<<<grid_for(rows * num_actions, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(acts, prim_stride, ld_a, w, ld_w, act, rows,
                                                                                                     num_actions, num_prim, out, ld_out);
   PULSE_LAUNCH_OK("pnn_compose_kernel");
   return PULSE_OK;
@@ -408,33 +311,8 @@ extern "C" int pulse_pd_targets(const float* action, int64_t ld_a, const float* 
                                 int32_t dofs, float* out, int64_t ld_out, void* stream) {
   PULSE_REQUIRE(action && offset && scale && out, "pulse_pd_targets: null buffer");
   PULSE_REQUIRE(rows > 0 && dofs > 0 && ld_a >= dofs && ld_out >= dofs, "pulse_pd_targets: bad shape");
-  pd_targets_kernel<<<elem_grid(rows * dofs), 256, 0, static_cast<cudaStream_t>(stream)>>>(action, ld_a, offset, scale, freeze, rows, dofs, out,
+  pd_targets_kernel<<<grid_for(rows * dofs, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(action, ld_a, offset, scale, freeze, rows, dofs, out,
                                                                                            ld_out);
   PULSE_LAUNCH_OK("pd_targets_kernel");
-  return PULSE_OK;
-}
-
-extern "C" int pulse_reach_update_task(const int64_t* progress, int64_t* tar_change_steps, float* tar_pos, const float* rand01,
-                                       const int64_t* steps, float dist_max, float h_min, float h_max, int64_t num_envs, void* stream) {
-  PULSE_REQUIRE(progress && tar_change_steps && tar_pos && rand01 && steps, "pulse_reach_update_task: null buffer");
-  PULSE_REQUIRE(num_envs > 0, "pulse_reach_update_task: num_envs <= 0");
-  reach_update_task_kernel<<<elem_grid(num_envs), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const long long*>(progress), reinterpret_cast<long long*>(tar_change_steps), tar_pos, rand01,
-      reinterpret_cast<const long long*>(steps), dist_max, h_min, h_max, num_envs);
-  PULSE_LAUNCH_OK("reach_update_task_kernel");
-  return PULSE_OK;
-}
-
-extern "C" int pulse_reach_step(const pulse_reach_step_args_t* args, int64_t num_envs, void* stream) {
-  PULSE_REQUIRE(args, "pulse_reach_step: null args");
-  const pulse_reach_step_args_t& a = *args;
-  PULSE_REQUIRE(a.body_state && a.tar_pos && a.progress_buf && a.obs_buf && a.rew_buf && a.reset_buf && a.terminate_buf,
-                "pulse_reach_step: null buffer");
-  PULSE_REQUIRE(num_envs > 0 && a.body_env_stride >= 24 * 13 && a.obs_stride >= PULSE_REACH_OBS, "pulse_reach_step: bad strides");
-  PULSE_REQUIRE(a.reach_body_id >= 0 && a.reach_body_id < 24, "pulse_reach_step: reach_body_id out of range");
-  PULSE_REQUIRE(!a.enable_early_termination || a.termination_heights != nullptr, "pulse_reach_step: termination_heights required");
-  PULSE_REQUIRE(a.contact_forces == nullptr || a.contact_env_stride >= 24 * 3, "pulse_reach_step: bad contact stride");
-  reach_step_kernel<<<warp_grid(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, num_envs);
-  PULSE_LAUNCH_OK("reach_step_kernel");
   return PULSE_OK;
 }

@@ -1,22 +1,77 @@
-// Post-physics step of the downstream latent-space tasks HumanoidSpeedZ and HumanoidStrikeZ (SURVEY 8f-4), the siblings of the reach
-// task (vae_ops.cu: reach_step_kernel): one warp per env, lane = body -- self observation (humanoid.py:1675-1731), task observation,
-// reward and reset in one launch.
+// Post-physics step of the downstream latent-space tasks HumanoidReach (SURVEY K21), HumanoidSpeedZ and HumanoidStrikeZ (SURVEY 8f-4):
+// one warp per env, lane = body -- self observation (humanoid.py:1675-1731), task observation, reward and reset in one launch.
+//   reach   compute_location_observations / compute_reach_reward  phc/env/tasks/humanoid_reach.py:224-250, target resampling
+//           (_update_task :126-147) in reach_update_task_kernel, reset = compute_humanoid_reset  humanoid.py:1573-1608
 //   speed   compute_speed_observations / compute_speed_reward   phc/env/tasks/humanoid_speed.py:310-343, power term :215-222,
-//           reset = compute_humanoid_reset                        humanoid.py:1573-1608
+//           reset = compute_humanoid_reset
 //   strike  compute_strike_observations / compute_strike_reward  phc/env/tasks/humanoid_strike.py:270-328,
 //           reset = the strike variant of compute_humanoid_reset  :330-375
-#include "pulse_common.cuh"
-#include "quat_math.cuh"
+#include "humanoid_obs.cuh"
 
 namespace pulse {
 namespace {
 
 constexpr int kZB = PULSE_NUM_BODIES;
 
-__device__ __forceinline__ float wsumf(float v) {
+__global__ void __launch_bounds__(256) reach_update_task_kernel(const long long* __restrict__ progress, long long* __restrict__ change,
+                                                                float* __restrict__ tar, const float* __restrict__ u,
+                                                                const long long* __restrict__ steps, float dist_max, float h_min, float h_max,
+                                                                long long n) {
+  for (long long e = blockIdx.x * 256ll + threadIdx.x; e < n; e += 256ll * gridDim.x) {
+    if (progress[e] >= change[e]) {
+      tar[3 * e + 0] = dist_max * (2.0f * u[3 * e + 0] - 1.0f);
+      tar[3 * e + 1] = dist_max * (2.0f * u[3 * e + 1] - 1.0f);
+      tar[3 * e + 2] = (h_max - h_min) * u[3 * e + 2] + h_min;
+      change[e] = progress[e] + steps[e];
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) reach_step_kernel(const pulse_reach_step_args_t a, long long n) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (long long e = blockIdx.x * 8ll + warp; e < n; e += 8ll * gridDim.x) {
+    const int j = lane;
+    const bool body = j < kZB;
+    const float* bs = a.body_state + e * a.body_env_stride + (body ? j : 0) * 13;
+    Vec3 p = {bs[0], bs[1], bs[2]}, v = {bs[7], bs[8], bs[9]}, w = {bs[10], bs[11], bs[12]};
+    Quat q = {bs[3], bs[4], bs[5], bs[6]};
+    const Vec3 p_root = {__shfl_sync(kFull, p.x, 0), __shfl_sync(kFull, p.y, 0), __shfl_sync(kFull, p.z, 0)};
+    const Quat q_root = {__shfl_sync(kFull, q.x, 0), __shfl_sync(kFull, q.y, 0), __shfl_sync(kFull, q.z, 0), __shfl_sync(kFull, q.w, 0)};
+    float hs, hc;
+    heading_half(q_root, hs, hc);
+    const Yaw yr = make_yaw(Quat{0.0f, 0.0f, -hs, hc});
+    float* o = a.obs_buf + e * a.obs_stride;
+    if (body) {  // store_self_obs's layout written out, for the reason given in im_step.cu
+      if (j == 0) o[0] = p_root.z;
+      else {
+        const Vec3 lp = yaw_rot(yr, p - p_root);
+        o[1 + 3 * (j - 1)] = lp.x; o[2 + 3 * (j - 1)] = lp.y; o[3 + 3 * (j - 1)] = lp.z;
+      }
+      float six[6];
+      qsix(yaw_mul_left(-hs, hc, q), six);
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
+      for (int i = 0; i < 6; ++i) o[70 + 6 * j + i] = six[i];
+      const Vec3 lv = yaw_rot(yr, v), lw = yaw_rot(yr, w);
+      o[214 + 3 * j] = lv.x; o[215 + 3 * j] = lv.y; o[216 + 3 * j] = lv.z;
+      o[286 + 3 * j] = lw.x; o[287 + 3 * j] = lw.y; o[288 + 3 * j] = lw.z;
+    }
+    const Vec3 tar = {a.tar_pos[3 * e], a.tar_pos[3 * e + 1], a.tar_pos[3 * e + 2]};
+    const FallFlags fall = fall_flags(a, e, j, body, p.z);
+    const bool any_contact = __any_sync(kFull, fall.contact), any_height = __any_sync(kFull, fall.height);
+    // the reach body's position, broadcast
+    const int rb = a.reach_body_id;
+    const Vec3 pr = {__shfl_sync(kFull, p.x, rb), __shfl_sync(kFull, p.y, rb), __shfl_sync(kFull, p.z, rb)};
+    if (lane == 0) {
+      const Vec3 lt = yaw_rot(yr, tar - p_root);  // compute_location_observations (humanoid_reach.py:224-236)
+      o[PULSE_SELF_OBS + 0] = lt.x; o[PULSE_SELF_OBS + 1] = lt.y; o[PULSE_SELF_OBS + 2] = lt.z;
+      const Vec3 d = tar - pr;                    // compute_reach_reward (:238-250)
+      a.rew_buf[e] = expf(-4.0f * (d.x * d.x + d.y * d.y + d.z * d.z));
+      const long long prog = a.progress_buf[e];
+      const long long term = (any_contact && any_height && prog > 1) ? 1 : 0;
+      a.terminate_buf[e] = term;
+      a.reset_buf[e] = prog >= a.max_episode_length - 1 ? 1 : term;
+    }
+  }
 }
 
 __global__ void __launch_bounds__(256) ztask_step_kernel(const pulse_ztask_step_args_t a, long long n) {
@@ -33,42 +88,18 @@ __global__ void __launch_bounds__(256) ztask_step_kernel(const pulse_ztask_step_
     heading_half(q_root, hs, hc);
     const Yaw yr = make_yaw(Quat{0.0f, 0.0f, -hs, hc});
     float* o = a.obs_buf + e * a.obs_stride;
-    if (body) {  // compute_humanoid_observations_smpl_max (humanoid.py:1675-1731): the layout of the imitation and reach kernels
-      if (j == 0) o[0] = p_root.z;
-      else {
-        const Vec3 lp = yaw_rot(yr, p - p_root);
-        o[1 + 3 * (j - 1)] = lp.x; o[2 + 3 * (j - 1)] = lp.y; o[3 + 3 * (j - 1)] = lp.z;
-      }
-      float six[6];
-      qsix(yaw_mul_left(-hs, hc, q), six);
-#pragma unroll
-      for (int i = 0; i < 6; ++i) o[70 + 6 * j + i] = six[i];
-      const Vec3 lv = yaw_rot(yr, v), lw = yaw_rot(yr, w);
-      o[214 + 3 * j] = lv.x; o[215 + 3 * j] = lv.y; o[216 + 3 * j] = lv.z;
-      o[286 + 3 * j] = lw.x; o[287 + 3 * j] = lw.y; o[288 + 3 * j] = lw.z;
+    if (body) store_self_obs(o, j, p, p_root, q, v, w, hs, hc, yr);
+    const FallFlags fall = fall_flags(a, e, j, body, p.z);
+    // strike: a body that is neither a ground-contact body nor a strike body pressing harder than 50 N (humanoid_strike.py:356-364)
+    bool hard_contact = false;
+    if (a.enable_early_termination && body && a.contact_forces != nullptr && !(((a.contact_body_mask | a.strike_body_mask) >> j) & 1u)) {
+      const float* cf = a.contact_forces + e * a.contact_env_stride + j * 3;
+      hard_contact = fabsf(cf[0]) > 50.0f || fabsf(cf[1]) > 50.0f || fabsf(cf[2]) > 50.0f;
     }
-    // ---- early termination: fall = (contact on a non-contact body) and (a non-contact body below its height) ------------------------
-    bool fall_contact = false, fall_height = false, hard_contact = false;
-    if (a.enable_early_termination && body && !((a.contact_body_mask >> j) & 1u)) {
-      if (a.contact_forces != nullptr) {
-        const float* cf = a.contact_forces + e * a.contact_env_stride + j * 3;
-        const float fx = fabsf(cf[0]), fy = fabsf(cf[1]), fz = fabsf(cf[2]);
-        fall_contact = fx > 0.1f || fy > 0.1f || fz > 0.1f;
-        // strike: a body that is neither a ground-contact body nor a strike body pressing harder than 50 N (humanoid_strike.py:356-364)
-        if (!((a.strike_body_mask >> j) & 1u)) hard_contact = fx > 50.0f || fy > 50.0f || fz > 50.0f;
-      }
-      fall_height = p.z < a.termination_heights[j];
-    }
-    const bool any_contact = __any_sync(kFull, fall_contact), any_height = __any_sync(kFull, fall_height);
+    const bool any_contact = __any_sync(kFull, fall.contact), any_height = __any_sync(kFull, fall.height);
     const bool any_hard = __any_sync(kFull, hard_contact);
-    // ---- power term of the speed task: -c * sum |tau * qdot|, zero for progress <= 3 (humanoid_speed.py:215-222) ----------------------
-    float power = 0.0f;
-    if (a.kind == PULSE_ZTASK_SPEED && a.dof_force != nullptr) {
-      const float* fr = a.dof_force + e * a.dof_force_stride;
-      const float* dv = a.dof_vel + e * a.dof_env_stride;
-      for (int d = lane; d < PULSE_NUM_DOF; d += 32) power += fabsf(fr[d] * dv[d * a.dof_elem_stride]);
-      power = wsumf(power);
-    }
+    // power term of the speed task: -c * sum |tau * qdot|, zero for progress <= 3 (humanoid_speed.py:215-222)
+    const float power = a.kind == PULSE_ZTASK_SPEED && a.dof_force != nullptr ? dof_power(a, e, lane) : 0.0f;
     if (lane == 0) {
       const long long prog = a.progress_buf[e];
       const float* pr = a.prev_root_pos + 3 * e;
@@ -149,9 +180,34 @@ extern "C" int pulse_ztask_step(const pulse_ztask_step_args_t* args, int64_t num
     PULSE_REQUIRE(a.target_states && a.tar_contact_forces, "pulse_ztask_step: strike task needs target_states and tar_contact_forces");
     PULSE_REQUIRE(a.obs_stride >= PULSE_STRIKE_OBS, "pulse_ztask_step: obs_stride %lld < %d", (long long)a.obs_stride, PULSE_STRIKE_OBS);
   }
-  long long ctas = (num_envs + 7) / 8;
-  if (ctas > kNumSMs * 8ll) ctas = kNumSMs * 8ll;
-  ztask_step_kernel<<<static_cast<unsigned>(ctas), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, (long long)num_envs);
+  ztask_step_kernel<<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, (long long)num_envs);
   PULSE_LAUNCH_OK("ztask_step_kernel");
+  return PULSE_OK;
+}
+
+extern "C" int pulse_reach_update_task(const int64_t* progress, int64_t* tar_change_steps, float* tar_pos, const float* rand01,
+                                       const int64_t* steps, float dist_max, float h_min, float h_max, int64_t num_envs, void* stream) {
+  using namespace pulse;
+  PULSE_REQUIRE(progress && tar_change_steps && tar_pos && rand01 && steps, "pulse_reach_update_task: null buffer");
+  PULSE_REQUIRE(num_envs > 0, "pulse_reach_update_task: num_envs <= 0");
+  reach_update_task_kernel<<<grid_for(num_envs, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const long long*>(progress), reinterpret_cast<long long*>(tar_change_steps), tar_pos, rand01,
+      reinterpret_cast<const long long*>(steps), dist_max, h_min, h_max, num_envs);
+  PULSE_LAUNCH_OK("reach_update_task_kernel");
+  return PULSE_OK;
+}
+
+extern "C" int pulse_reach_step(const pulse_reach_step_args_t* args, int64_t num_envs, void* stream) {
+  using namespace pulse;
+  PULSE_REQUIRE(args, "pulse_reach_step: null args");
+  const pulse_reach_step_args_t& a = *args;
+  PULSE_REQUIRE(a.body_state && a.tar_pos && a.progress_buf && a.obs_buf && a.rew_buf && a.reset_buf && a.terminate_buf,
+                "pulse_reach_step: null buffer");
+  PULSE_REQUIRE(num_envs > 0 && a.body_env_stride >= 24 * 13 && a.obs_stride >= PULSE_REACH_OBS, "pulse_reach_step: bad strides");
+  PULSE_REQUIRE(a.reach_body_id >= 0 && a.reach_body_id < 24, "pulse_reach_step: reach_body_id out of range");
+  PULSE_REQUIRE(!a.enable_early_termination || a.termination_heights != nullptr, "pulse_reach_step: termination_heights required");
+  PULSE_REQUIRE(a.contact_forces == nullptr || a.contact_env_stride >= 24 * 3, "pulse_reach_step: bad contact stride");
+  reach_step_kernel<<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, num_envs);
+  PULSE_LAUNCH_OK("reach_step_kernel");
   return PULSE_OK;
 }
