@@ -395,6 +395,15 @@ int pulse_column_moments(const float* x, int64_t ldx, int64_t rows, int64_t cols
 int pulse_normalize_moments(const float* x, int64_t ldx, int64_t rows, int64_t cols, const float* mean, const float* rstd,
                             pulse_bf16_t* out, int64_t ld_out, double* sums, float pad_one, void* stream);
 
+/* The same normalisation for an observation [self | task] that feeds two bias-augmented first layers (the amp_sept network:
+ * a task encoder whose output joins the self observation), in ONE pass over x [rows, cols]:
+ *   p [rows, ldp] = [columns 0..p_off-1 untouched (the encoder output goes there) | self (self_cols) | 1 | 0 ...]
+ *   t [rows, ldt] = [task (cols - self_cols) | 1 | 0 ...]
+ * sums[2*cols] += the batch moments of all cols columns when sums != NULL (training mode); NULL = normalise only.
+ * cols, self_cols, p_off, ldp, ldt and ldx even; x, mean, rstd 8-byte and p, t 4-byte aligned. */
+int pulse_normalize_split(const float* x, int64_t ldx, int64_t rows, int64_t cols, int64_t self_cols, const float* mean, const float* rstd,
+                          pulse_bf16_t* p, int64_t ldp, int64_t p_off, pulse_bf16_t* t, int64_t ldt, double* sums, void* stream);
+
 /* RunningMeanStd._update_mean_var_count_from_moments (:54-66) on the device: merges the batch sums of
  * pulse_column_moments (n rows) into the fp64 running mean / var / count and refreshes the fp32 mean / rstd
  * vectors pulse_normalize_to_bf16 reads, then zeroes `sums` for the next batch.  One launch, no host round trip. */

@@ -303,6 +303,8 @@ SIGNATURES = {
                                           C.c_void_p, C.c_int64, C.c_float, C.c_void_p]),
     "pulse_normalize_moments": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                           C.c_void_p, C.c_float, C.c_void_p]),
+    "pulse_normalize_split": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                        C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "pulse_head1_forward": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_head1_backward": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -22,6 +22,7 @@ Reference methods mirrored:
   AMPAgent.calc_gradients         phc/learning/amp_agent.py:605-760
   AMPAgent._optimize_kin          :771-849
   AMPAgent._calc_amp_rewards      :1011-1041
+  AMPSeptBuilder.Network          phc/learning/amp_network_sept_builder.py (pulse_z_terrain.yaml's policy)  -> SeptPolicy
   HumanoidImDistill.step (teacher) phc/env/tasks/humanoid_im_distill.py:143-205
   HumanoidZ.compute_z_actions     phc/env/tasks/humanoid_z.py:81-155
   Humanoid._action_to_pd_targets  phc/env/tasks/humanoid.py:1392-1394
@@ -35,6 +36,7 @@ from . import _lib
 from .ppo import PPOPolicy
 from .reach import ReachTaskB200
 from .rollout import discount_values
+from .sept import SeptPolicy
 from .vae import PulseVAE, TeacherPNN, pd_targets
 
 
@@ -72,6 +74,21 @@ class AMPAgentB200Mixin:
                                        kld_coefficient_min=float(task.kld_coefficient_min), kld_anneal=bool(task.kld_anneal),
                                        ar1_coefficient=float(task.ar1_coefficient), use_ar1_prior=bool(task.use_ar1_prior),
                                        use_vae_prior_regu=bool(task.use_vae_prior_regu), horizon=int(self.horizon_length))
+            elif hasattr(net, "_task_mlp"):                                             # amp_sept (pulse_z_terrain.yaml): shared task encoder
+                detail = dict(task.get_task_obs_size_detail())
+                if set(detail) != {"traj", "heightmap"}:
+                    extra = sorted(set(detail) - {"traj", "heightmap"})
+                    raise _lib.PulseError(f"the amp_sept policy covers the trajectory + height-map task observation only; task_obs_size_detail "
+                                          f"has {extra or sorted(detail)} (the 'people' PointNet branch / 'heightmap_velocity' are not built)")
+                units, act = _mlp_shape(net.actor_mlp)
+                task_units, task_act = _mlp_shape(net._task_mlp)
+                disc_units, _ = _mlp_shape(net._disc_mlp)
+                self._pulse = SeptPolicy(self_obs_size=task.get_self_obs_size(), task_obs_size_detail=detail, task_units=task_units, units=units,
+                                         act=act, task_act=task_act, num_actions=self.actions_num, with_disc=True, device=dev,
+                                         lr=float(self.last_lr), e_clip=float(self.e_clip), critic_coef=float(self.critic_coef),
+                                         bounds_coef=float(self.bounds_loss_coef), grad_norm=float(self.grad_norm),
+                                         normalize_value=bool(self.normalize_value), amp_obs_size=int(self._amp_observation_space.shape[0]),
+                                         disc_units=disc_units)
             else:
                 units, act = _mlp_shape(net.actor_mlp)                                   # im.yaml / pulse_z_task.yaml / im_big.yaml alike
                 disc_units, _ = _mlp_shape(net._disc_mlp)

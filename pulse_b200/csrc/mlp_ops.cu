@@ -75,20 +75,11 @@ __global__ void __launch_bounds__(256) column_moments_kernel(const float* __rest
 // PHC's RunningMeanStd normalises with the statistics from BEFORE the batch and merges the batch moments afterwards
 // (running_mean_std.py:91-107), so both consume the same fp32 rows: each thread owns a column PAIR (8-byte load,
 // 4-byte bf16x2 store), walks a row chunk with 8 rows in flight, and finishes with four fp64 atomics.
-__global__ void __launch_bounds__(256) normalize_moments_kernel(const float* __restrict__ x, long long ldx, long long rows, long long cols,
-                                                                const float* __restrict__ mean, const float* __restrict__ rstd,
-                                                                __nv_bfloat16* __restrict__ out, long long ld_out,
-                                                                double* __restrict__ sums, float pad_one) {
-  const long long c = 2 * ((long long)blockIdx.x * blockDim.x + threadIdx.x);
-  if (c >= ld_out) return;
-  const bool live = c < cols;  // cols is even on this path: a pair is either fully inside or fully padding
-  const long long chunk = (rows + gridDim.y - 1) / gridDim.y;
-  const long long r0 = blockIdx.y * chunk, r1 = min(rows, r0 + chunk);
-  if (!live) {
-    const __nv_bfloat162 fill = __floats2bfloat162_rn(c == cols ? pad_one : 0.0f, 0.0f);   // (ones column | 0) on the first pad pair
-    for (long long r = r0; r < r1; ++r) *reinterpret_cast<__nv_bfloat162*>(out + r * ld_out + c) = fill;
-    return;
-  }
+// Rows [r0, r1) of source columns (c, c+1) of x -> destination columns (oc, oc+1) of out; sums[2*cols] += their moments.
+__device__ __forceinline__ void normalize_pair_rows(const float* __restrict__ x, long long ldx, long long cols, long long c, long long r0,
+                                                    long long r1, const float* __restrict__ mean, const float* __restrict__ rstd,
+                                                    __nv_bfloat16* __restrict__ out, long long ld_out, long long oc,
+                                                    double* __restrict__ sums) {
   const float2 m = *reinterpret_cast<const float2*>(mean + c), rs = *reinterpret_cast<const float2*>(rstd + c);
   double s0 = 0.0, s1 = 0.0, q0 = 0.0, q1 = 0.0;
   long long r = r0;
@@ -99,7 +90,7 @@ __global__ void __launch_bounds__(256) normalize_moments_kernel(const float* __r
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const float y0 = fminf(fmaxf((v[i].x - m.x) * rs.x, -5.0f), 5.0f), y1 = fminf(fmaxf((v[i].y - m.y) * rs.y, -5.0f), 5.0f);
-      *reinterpret_cast<__nv_bfloat162*>(out + (r + i) * ld_out + c) = __floats2bfloat162_rn(y0, y1);
+      *reinterpret_cast<__nv_bfloat162*>(out + (r + i) * ld_out + oc) = __floats2bfloat162_rn(y0, y1);
       const double d0 = v[i].x, d1 = v[i].y;
       s0 += d0;
       s1 += d1;
@@ -110,7 +101,7 @@ __global__ void __launch_bounds__(256) normalize_moments_kernel(const float* __r
   for (; r < r1; ++r) {
     const float2 v = *reinterpret_cast<const float2*>(x + r * ldx + c);
     const float y0 = fminf(fmaxf((v.x - m.x) * rs.x, -5.0f), 5.0f), y1 = fminf(fmaxf((v.y - m.y) * rs.y, -5.0f), 5.0f);
-    *reinterpret_cast<__nv_bfloat162*>(out + r * ld_out + c) = __floats2bfloat162_rn(y0, y1);
+    *reinterpret_cast<__nv_bfloat162*>(out + r * ld_out + oc) = __floats2bfloat162_rn(y0, y1);
     const double d0 = v.x, d1 = v.y;
     s0 += d0;
     s1 += d1;
@@ -122,6 +113,54 @@ __global__ void __launch_bounds__(256) normalize_moments_kernel(const float* __r
   atomicAdd(sums + c + 1, s1);
   atomicAdd(sums + cols + c, q0);
   atomicAdd(sums + cols + c + 1, q1);
+}
+
+// (first, 0) into destination columns (oc, oc+1) of rows [r0, r1): zero padding, or the ones column of a bias-augmented operand
+__device__ __forceinline__ void fill_pair_rows(__nv_bfloat16* __restrict__ out, long long ld_out, long long oc, long long r0, long long r1,
+                                               float first) {
+  const __nv_bfloat162 fill = __floats2bfloat162_rn(first, 0.0f);
+  for (long long r = r0; r < r1; ++r) *reinterpret_cast<__nv_bfloat162*>(out + r * ld_out + oc) = fill;
+}
+
+__global__ void __launch_bounds__(256) normalize_moments_kernel(const float* __restrict__ x, long long ldx, long long rows, long long cols,
+                                                                const float* __restrict__ mean, const float* __restrict__ rstd,
+                                                                __nv_bfloat16* __restrict__ out, long long ld_out,
+                                                                double* __restrict__ sums, float pad_one) {
+  const long long c = 2 * ((long long)blockIdx.x * blockDim.x + threadIdx.x);
+  if (c >= ld_out) return;
+  const long long chunk = (rows + gridDim.y - 1) / gridDim.y;
+  const long long r0 = blockIdx.y * chunk, r1 = min(rows, r0 + chunk);
+  if (c < cols)  // cols is even on this path: a pair is either fully inside or fully padding
+    normalize_pair_rows(x, ldx, cols, c, r0, r1, mean, rstd, out, ld_out, c, sums);
+  else
+    fill_pair_rows(out, ld_out, c, r0, r1, c == cols ? pad_one : 0.0f);   // (ones column | 0) on the first pad pair
+}
+
+// ---- split normalise for the task network of amp_sept (pulse_b200/sept.py) --------------------------------------------
+// The observation [self | task] (self_cols even) feeds two bias-augmented first layers: the policy operand
+// P = [embedding (p_off columns, written by the task network's top GEMM, not touched here) | self | 1 | 0...] and the task
+// operand T = [task | 1 | 0...].  Thread j owns destination pair j of the concatenation P[:, p_off:ldp) ++ T[:, 0:ldt); every live pair
+// maps to ONE source pair (the split is even), so this is normalize_moments_kernel with a remapped store and the same fp64 moments.
+__global__ void __launch_bounds__(256) normalize_split_kernel(const float* __restrict__ x, long long ldx, long long rows, long long cols,
+                                                              long long self_cols, const float* __restrict__ mean,
+                                                              const float* __restrict__ rstd, __nv_bfloat16* __restrict__ p, long long ldp,
+                                                              long long p_off, __nv_bfloat16* __restrict__ t, long long ldt,
+                                                              double* __restrict__ sums) {
+  const long long j = 2 * ((long long)blockIdx.x * blockDim.x + threadIdx.x);
+  const long long pw = ldp - p_off;
+  if (j >= pw + ldt) return;
+  const long long chunk = (rows + gridDim.y - 1) / gridDim.y;
+  const long long r0 = blockIdx.y * chunk, r1 = min(rows, r0 + chunk);
+  const bool in_p = j < pw;
+  __nv_bfloat16* out = in_p ? p : t;
+  const long long ld = in_p ? ldp : ldt;
+  const long long oc = in_p ? p_off + j : j - pw;
+  const long long width = in_p ? self_cols : cols - self_cols;   // live columns of this operand
+  const long long k = in_p ? j : j - pw;                         // column within this operand's live block
+  if (k < width)
+    normalize_pair_rows(x, ldx, cols, in_p ? k : self_cols + k, r0, r1, mean, rstd, out, ld, oc, sums);
+  else
+    fill_pair_rows(out, ld, oc, r0, r1, k == width ? 1.0f : 0.0f);
 }
 
 // ---- Gaussian head ------------------------------------------------------------------------------------------------
@@ -699,6 +738,27 @@ extern "C" int pulse_normalize_moments(const float* x, int64_t ldx, int64_t rows
   if (gy < 1) gy = 1;
   normalize_moments_kernel<<<dim3(gx, gy), 256, 0, st>>>(x, ldx, rows, cols, mean, rstd, reinterpret_cast<__nv_bfloat16*>(out), ld_out, sums, pad_one);
   PULSE_LAUNCH_OK("normalize_moments_kernel");
+  return PULSE_OK;
+}
+
+extern "C" int pulse_normalize_split(const float* x, int64_t ldx, int64_t rows, int64_t cols, int64_t self_cols, const float* mean,
+                                     const float* rstd, pulse_bf16_t* p, int64_t ldp, int64_t p_off, pulse_bf16_t* t, int64_t ldt, double* sums,
+                                     void* stream) {
+  PULSE_REQUIRE(x && mean && rstd && p && t, "pulse_normalize_split: null buffer");
+  PULSE_REQUIRE(rows > 0 && self_cols > 0 && cols > self_cols && ldx >= cols, "pulse_normalize_split: bad shape");
+  PULSE_REQUIRE(p_off >= 0 && ldp > p_off + self_cols && ldt > cols - self_cols, "pulse_normalize_split: operands too narrow for the ones column");
+  PULSE_REQUIRE(cols % 2 == 0 && self_cols % 2 == 0 && p_off % 2 == 0 && ldp % 2 == 0 && ldt % 2 == 0 && ldx % 2 == 0,
+                "pulse_normalize_split: cols, self_cols, p_off, ldp, ldt and ldx must be even");
+  PULSE_REQUIRE(reinterpret_cast<uintptr_t>(x) % 8 == 0 && reinterpret_cast<uintptr_t>(mean) % 8 == 0 && reinterpret_cast<uintptr_t>(rstd) % 8 == 0 &&
+                    reinterpret_cast<uintptr_t>(p) % 4 == 0 && reinterpret_cast<uintptr_t>(t) % 4 == 0,
+                "pulse_normalize_split: x / mean / rstd need 8-byte, p / t 4-byte alignment");
+  const unsigned gx = static_cast<unsigned>(((ldp - p_off + ldt) / 2 + 255) / 256);
+  unsigned gy = (2 * kSMs + gx - 1) / gx;  // as pulse_normalize_moments: two 256-thread CTAs per SM, 8 rows in flight per thread
+  if (gy > rows / 8) gy = static_cast<unsigned>(rows / 8);
+  if (gy < 1) gy = 1;
+  normalize_split_kernel<<<dim3(gx, gy), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      x, ldx, rows, cols, self_cols, mean, rstd, reinterpret_cast<__nv_bfloat16*>(p), ldp, p_off, reinterpret_cast<__nv_bfloat16*>(t), ldt, sums);
+  PULSE_LAUNCH_OK("normalize_split_kernel");
   return PULSE_OK;
 }
 

@@ -188,6 +188,10 @@ class FlatParams:
         off, _ = self._shapes[idx]
         return getattr(self, what)[off:off + n]
 
+    def offset(self, idx: int) -> int:
+        """first element of slot idx in the flat buffers"""
+        return self._shapes[idx][0]
+
     @property
     def numel(self):
         return self._numel
@@ -240,6 +244,7 @@ class Dense:
         self.flat = flat
         self.w_idx = flat.reserve(out_features, self.Kp)
         self.b_idx = None if aug else flat.reserve(out_features)
+        self.ref_cols = None   # LongTensor [K]: reference input column j sits in internal column ref_cols[j] (None: the same order)
 
     # views (valid after flat.finalize())
     @property
@@ -274,9 +279,23 @@ class Dense:
         b = (torch.rand(self.N, device=self.flat.device, generator=gen) * 2 - 1) * bound
         self.set_weights(w, b)
 
+    def ref_weight(self, what: str = "params") -> torch.Tensor:
+        """Copy of the weight block [N, K] of a weight-shaped slot (parameters, gradients or an Adam moment) in the reference's
+        input-column order."""
+        m = self.flat.view(self.w_idx, what)
+        return m[:, :self.K].clone() if self.ref_cols is None else m[:, self.ref_cols.to(m.device)]
+
+    def set_ref_weight(self, what: str, w: torch.Tensor) -> None:
+        """Inverse of ref_weight: writes a reference-ordered [N, K] block into the slot."""
+        m = self.flat.view(self.w_idx, what)
+        if self.ref_cols is None:
+            m[:, :self.K].copy_(w)
+        else:
+            m[:, self.ref_cols.to(m.device)] = w.to(m.device, m.dtype)
+
     def set_weights(self, w: torch.Tensor, b: torch.Tensor):
         self.weight.zero_()
-        self.weight[:, :self.K].copy_(w)
+        self.set_ref_weight("params", w)
         self.bias.copy_(b)
         self.refresh()
 
@@ -286,31 +305,39 @@ class Dense:
 
 
 class MLP:
-    """units: hidden sizes; `head` linear output layer size (or None).  Activation 'relu' | 'silu'.
+    """units: hidden sizes; `head` linear output layer size, or None for a headless net whose last layer keeps its activation and
+    writes bf16 (forward(out=) may give it a window of a caller's operand, e.g. the task encoder writing into the policy input).
+    Activation 'relu' | 'silu'.
     hidden_acts: per-hidden-layer override (None = a Linear with no activation, e.g. the last Linear of `z_mlp` that feeds the
     `z_mu` / `z_logvar` heads, amp_network_z_builder.py:492-497).  input_grad_cols > 0: backward() also returns the gradient
     w.r.t. the first `input_grad_cols` input columns (the latent window of the PULSE decoder input).
     in_perm: internal input column i holds reference input column in_perm[i] (checkpoint import / export of layer 0).
     aug: bias-augmented layers (see Dense) -- the caller's input operand must carry 1.0 in column `in_features`.
-    ReLU layers save their activation masks as bit words in the forward epilogue (train=True) and the backward pass gates with those."""
+    ReLU layers save their activation masks as bit words in the forward epilogue (train=True) and the backward pass gates with those.
+    first: layer 0, reserved by the caller (so that two nets' first layers can sit back to back in the flat buffers)."""
 
     def __init__(self, flat: FlatParams, in_features: int, units: Sequence[int], head: Optional[int], act: str = "relu",
                  hidden_acts: Optional[Sequence[Optional[str]]] = None, input_grad_cols: int = 0, in_perm: Optional[torch.Tensor] = None,
-                 aug: bool = False):
+                 aug: bool = False, first: Optional[Dense] = None):
         self.flat = flat
         self.act = act
         self.aug = aug
+        self.headless = head is None
         sizes = [in_features] + list(units)
         acts = list(hidden_acts) if hidden_acts is not None else [act] * len(units)
         if len(acts) != len(units):
             raise _lib.PulseError("hidden_acts must have one entry per hidden layer")
-        self.layers: List[Dense] = [Dense(flat, sizes[i], sizes[i + 1], acts[i], aug) for i in range(len(units))]
+        if first is not None and (first.K, first.N, first.act, first.aug) != (in_features, sizes[1], acts[0], aug):
+            raise _lib.PulseError("the caller-reserved first layer does not match the net's input size, width, activation or bias layout")
+        self.layers: List[Dense] = [first if (i == 0 and first is not None) else Dense(flat, sizes[i], sizes[i + 1], acts[i], aug)
+                                    for i in range(len(units))]
         if head is not None:
             self.layers.append(Dense(flat, sizes[-1], head, None, aug))
         self.in_features, self.Kp0 = in_features, self.layers[0].Kp
         self.input_grad_cols = input_grad_cols
         self.in_perm = in_perm
         self._ws: Dict[int, dict] = {}
+        self._dact0: Dict[int, torch.Tensor] = {}
         self._scratch = None
         self._zero = None
 
@@ -341,14 +368,18 @@ class MLP:
             ws = {"act": [], "pre": [], "dact": [], "split": [], "mask": []}
             for i, l in enumerate(self.layers):
                 last = i == len(self.layers) - 1
-                a = None if last else bf(M, l.Np)
+                fp32_head = last and not self.headless
+                a = None if fp32_head else bf(M, l.Np)
                 if a is not None and self.aug:
                     a[:, l.N] = 1.0                    # the ones column the next (bias-augmented) layer multiplies its bias column with
                 ws["act"].append(a)
                 if train:
                     ws["pre"].append(bf(M, l.Np) if (l.act == "silu") else None)
-                    ws["dact"].append(None if last else bf(M, l.Np))      # gradient w.r.t. this layer's OUTPUT
-                    ws["mask"].append(torch.zeros((l.N + 31) // 32, M, device=dev, dtype=torch.int32) if (l.act == "relu" and not last) else None)
+                    if i == 0 and not last and M in self._dact0:
+                        ws["dact"].append(self._dact0[M])
+                    else:
+                        ws["dact"].append(None if last else bf(M, l.Np))      # gradient w.r.t. this layer's OUTPUT
+                    ws["mask"].append(torch.zeros((l.N + 31) // 32, M, device=dev, dtype=torch.int32) if (l.act == "relu" and not fp32_head) else None)
                     tiles = ((l.N + 127) // 128) * ((l.Kp + 127) // 128)   # 128 x 128 output tiles
                     ws["split"].append(pick_split(tiles, (M + 63) // 64))
             hn = self.layers[-1].N     # fp32 head output: rows padded to a multiple of 4 floats so the epilogue's 16-byte stores apply (N = 69)
@@ -357,6 +388,20 @@ class MLP:
                 ws["dx"] = torch.zeros(M, self.input_grad_cols, device=dev)
             self._ws[key] = ws
         return self._ws[key]
+
+    def provide_dact0(self, M: int, buf: torch.Tensor) -> None:
+        """Training at batch size M writes the gradient w.r.t. layer 0's pre-activation into `buf` (bf16 [M, >= N0], any row stride)
+        instead of a buffer of its own: two nets can then fill the two column halves of ONE operand."""
+        if buf.dtype != torch.bfloat16 or buf.shape[0] != M or buf.shape[1] < self.layers[0].N or buf.stride(1) != 1:
+            raise _lib.PulseError("provide_dact0: bf16 [M, >= N0] with contiguous rows")
+        self._dact0[M] = buf
+        if (M, True) in self._ws:
+            self._ws[(M, True)]["dact"][0] = buf
+
+    def top_preact(self, M: int) -> torch.Tensor:
+        """SiLU pre-activation of a headless net's last layer from the last training forward pass at batch size M (the gate of the
+        gradient a caller hands to backward())."""
+        return self._ws[(M, True)]["pre"][-1]
 
     def _dummy(self, n: int) -> torch.Tensor:
         """fp32 scratch the fused single-output-head kernels may add bias gradients into when the layers are bias-augmented (the weight
@@ -368,7 +413,7 @@ class MLP:
     def _head1(self, i: int) -> bool:
         """Layer i is a single-output head on top of a ReLU layer narrow enough for the fused GEMV kernels."""
         l = self.layers[i]
-        return i == len(self.layers) - 1 and i > 0 and l.N == 1 and self.layers[i - 1].act == "relu" and l.Kp <= 2048
+        return not self.headless and i == len(self.layers) - 1 and i > 0 and l.N == 1 and self.layers[i - 1].act == "relu" and l.Kp <= 2048
 
     # ---- per-layer GEMM arguments, shared by the single-problem path below and the grouped (lock-step) path ----------------------
     def _fwd_problem(self, i: int, h: torch.Tensor, ws: dict, train: bool):
@@ -400,15 +445,23 @@ class MLP:
     # ------------------------------------------------------------------ forward
     def forward(self, x: torch.Tensor, train: bool = False, out: Optional[torch.Tensor] = None, slot: int = 0) -> torch.Tensor:
         """x: bf16 [M, Kp0] (normalised, zero padded; column `in_features` = 1.0 for augmented nets).  Returns fp32 [M, head] (view of a
-        reused workspace buffer, or `out`).  With train=True the activations / ReLU masks / SiLU pre-activations backward() needs are kept."""
+        reused workspace buffer, or `out`).  With train=True the activations / ReLU masks / SiLU pre-activations backward() needs are kept.
+        Headless nets return the bf16 activation of the last layer: columns [0, N) of `out` when given (any row stride), else of a
+        workspace buffer."""
         M = x.shape[0]
         ws = self._workspace(M, train, slot)
-        if out is not None:
+        if out is not None and not self.headless:
             ws = dict(ws, out=out)
         h = x
         for i, l in enumerate(self.layers):
             last = i == len(self.layers) - 1
-            if last and self._head1(i):
+            if last and self.headless:
+                a, b, kw = self._fwd_problem(i, h, ws, train)
+                if out is not None:
+                    kw["out"] = out
+                gemm_nt(a, b, **kw)
+                h = kw["out"]
+            elif last and self._head1(i):
                 # [M,K] x [K,1]: no tensor-core shape -- one HBM pass over h (pulse_head1_forward); augmented: the bias is w[K] * h[:, K]
                 bias = self._zero_bias() if self.aug else l.bias
                 with torch.cuda.device(self.flat.device):
@@ -423,7 +476,7 @@ class MLP:
                 h = ws["act"][i]
         if train:
             self._ws[(M, True)]["x"] = x
-        return ws["out"]
+        return h[:, :self.layers[-1].N] if self.headless else ws["out"]
 
     # ------------------------------------------------------------------ backward
     def _backward_head(self, ws: dict, dout: torch.Tensor, M: int):
@@ -454,8 +507,9 @@ class MLP:
         return dout, top
 
     def backward(self, dout: torch.Tensor, M: int) -> None:
-        """dout bf16 [M, pad8(head)]: gradient of the loss w.r.t. the head output.  ADDS dW, db of every layer into the
-        flat gradient buffer (the caller zeroes it once per minibatch with flat.zero_grad())."""
+        """dout bf16 [M, pad8(head)]: gradient of the loss w.r.t. the head output (headless nets: w.r.t. the last layer's
+        PRE-activation, i.e. already gated by its activation's derivative).  ADDS dW, db of every layer into the flat gradient buffer
+        (the caller zeroes it once per minibatch with flat.zero_grad())."""
         ws = self._ws[(M, True)]
         dy, top = self._backward_head(ws, dout, M)
         for i in reversed(range(top + 1)):

@@ -73,6 +73,21 @@ class RunningMeanStdB200:
     def normalize_into(self, x: torch.Tensor, out: torch.Tensor, out_t: Optional[torch.Tensor] = None) -> None:
         normalize_to_bf16(x, self.mean_f32, self.rstd_f32, out, out_t, pad_one=self.pad_one)
 
+    def normalize_split(self, x: torch.Tensor, self_cols: int, p: torch.Tensor, p_off: int, t: torch.Tensor, update: bool) -> None:
+        """forward() of an observation [self | task] into two bias-augmented operands in one pass (pulse_normalize_split):
+        p[:, p_off:] = [self | 1 | 0...], t = [task | 1 | 0...].  update=True (training mode, unless frozen) merges the batch afterwards."""
+        if x.dtype != torch.float32 or x.stride(1) != 1 or x.shape[1] != self.size:
+            raise _lib.PulseError("normalize_split: x must be fp32 [rows, size] with contiguous rows")
+        lib = _lib.load()
+        upd = update and not self.frozen
+        with torch.cuda.device(self.device):
+            _lib.check(lib.pulse_normalize_split(x.data_ptr(), x.stride(0), x.shape[0], self.size, self_cols, self.mean_f32.data_ptr(),
+                                                 self.rstd_f32.data_ptr(), p.data_ptr(), p.stride(0), p_off, t.data_ptr(), t.stride(0),
+                                                 self._sums.data_ptr() if upd else None, _lib.current_stream(self.device)),
+                       "pulse_normalize_split")
+            if upd:
+                self._merge(lib, x.shape[0])
+
     def unnormalize(self, y: torch.Tensor) -> torch.Tensor:
         """forward(unnorm=True) (:84-87): clamp to +-5 then scale back (value de-normalisation)."""
         return torch.clamp(y, -5.0, 5.0) * torch.sqrt(self.running_var.float() + self.eps) + self.running_mean.float()
@@ -82,6 +97,8 @@ class RunningMeanStdB200:
 
 
 class PPOPolicy:
+    grouped_ok = True    # PULSE_GROUPED may run actor + critic in lock step (subclasses whose nets do not fit it set False)
+
     def __init__(self, obs_size: int = 934, num_actions: int = 69, units: Sequence[int] = (1024, 512), act: str = "relu",
                  logstd: float = -2.9, device="cuda:0", seed: int = 0, lr: float = 2e-5, e_clip: float = 0.2, critic_coef: float = 5.0,
                  bounds_coef: float = 10.0, grad_norm: float = 50.0, normalize_value: bool = True, with_disc: bool = False,
@@ -90,17 +107,15 @@ class PPOPolicy:
         self.obs_size, self.A = obs_size, num_actions
         self.lr, self.e_clip, self.critic_coef, self.bounds_coef, self.grad_norm = lr, e_clip, critic_coef, bounds_coef, grad_norm
         self.flat = FlatParams(self.device)
-        # bias-augmented layers (nets.Dense): bias add and bias gradients are done by the tensor cores, the epilogues carry neither
-        self.actor = MLP(self.flat, obs_size, units, num_actions, act, aug=True)
-        self.critic = MLP(self.flat, obs_size, units, 1, act, aug=True)
+        self._build_nets(obs_size, units, act)
         self.disc = None
         if with_disc:  # one optimizer / one grad-norm clip over actor + critic + discriminator, as in the reference
             from .amp import AmpDiscriminator
             self.disc = AmpDiscriminator(self.flat, amp_obs_size, disc_units)
         self.flat.finalize()
         gen = torch.Generator(device=self.device).manual_seed(seed)
-        self.actor.init_default(gen)
-        self.critic.init_default(gen)
+        for net in self._policy_nets():
+            net.init_default(gen)
         if self.disc is not None:
             self.disc.mlp.init_default(gen)
         self.logstd = torch.full((num_actions,), logstd, device=self.device)  # fixed_sigma, const_initializer (im.yaml:21-25)
@@ -114,6 +129,15 @@ class PPOPolicy:
         self._side = None
         self.rng_seed = (int(seed) * 0x9E3779B97F4A7C15 + 0x243F6A8885A308D3) & (2 ** 64 - 1)
         self.rng_offset = torch.zeros(1, dtype=torch.int64, device=self.device)    # uint64 counter read by the sampling kernel
+
+    def _build_nets(self, obs_size: int, units: Sequence[int], act: str) -> None:
+        # bias-augmented layers (nets.Dense): bias add and bias gradients are done by the tensor cores, the epilogues carry neither
+        self.actor = MLP(self.flat, obs_size, units, self.A, act, aug=True)
+        self.critic = MLP(self.flat, obs_size, units, 1, act, aug=True)
+
+    def _policy_nets(self):
+        """The nets besides the discriminator, in initialisation order."""
+        return (self.actor, self.critic)
 
     # ------------------------------------------------------------------ buffers
     def _buf(self, M: int, train: bool):
@@ -131,15 +155,19 @@ class PPOPolicy:
             self._bufs[key] = b
         return self._bufs[key]
 
+    def _normalize_eval(self, obs: torch.Tensor, b: dict) -> None:
+        """Evaluation-mode input of the actor / critic: b['x'] <- normalised obs."""
+        self.obs_rms.normalize_into(obs, b["x"])
+
     # ------------------------------------------------------------------ rollout side
     def act(self, obs: torch.Tensor, eps: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
         """get_action_values (common_agent.py:262-288): normalise obs, actor + critic forward, sample, neglogp.
         `eps` lets a test inject the standard-normal draw."""
         M = obs.shape[0]
         b = self._buf(M, False)
-        self.obs_rms.normalize_into(obs, b["x"])
+        self._normalize_eval(obs, b)
         from .dense import grouped_enabled
-        if grouped_enabled():   # experimental (default off): actor + critic hidden layers in one grouped launch per layer
+        if self.grouped_ok and grouped_enabled():   # experimental (default off): actor + critic hidden layers in one grouped launch per layer
             from .nets import forward_lockstep
             mu, value = forward_lockstep((self.actor, self.critic), (b["x"], b["x"]))
         else:
@@ -246,7 +274,7 @@ class PPOPolicy:
         """_eval_critic (common_agent.py:552-562)."""
         M = obs.shape[0]
         b = self._buf(M, False)
-        self.obs_rms.normalize_into(obs, b["x"])
+        self._normalize_eval(obs, b)
         value = self.critic.forward(b["x"])
         return self.value_rms.unnormalize(value) if self.value_rms is not None else value
 
@@ -276,14 +304,13 @@ class PPOPolicy:
         stream (same order of running-statistics updates as the reference: batch i+1 after batch i)."""
         M = obs.shape[0]
         b = self._buf(M, True)
-        x = b["x2"][slot]
         # Three independent chains -- actor, critic, discriminator -- run on three streams (fork/join with events, so
         # the whole minibatch still captures into ONE CUDA graph): the persistent GEMMs of one chain fill the partial
         # last wave of another, and the HBM-bound normalise / moments / loss kernels overlap with tensor-core work.
         main = torch.cuda.current_stream(self.device)
         if self._side is None:
             self._side = (torch.cuda.Stream(self.device), torch.cuda.Stream(self.device), torch.cuda.Stream(self.device))
-        s_critic, s_disc, s_pref = self._side
+        _, s_disc, s_pref = self._side
         # where the next minibatch's input preparation is forked: under the NCCL all-reduce when there is one (it leaves most SMs idle);
         # at the start, under the GEMMs, on one GPU and with the peer-memory optimizer kernel (which occupies every SM while it runs)
         peer_step = self.flat.peer is not None and world_size > 1 and not keep_grads
@@ -314,16 +341,8 @@ class PPOPolicy:
                     d0, d1 = self.disc.mlp.param_span()
                     reducer.reduce(self.flat.grads[d0:d1], 2)
         from .dense import grouped_enabled
-        grouped = grouped_enabled()    # PULSE_GROUPED=1: actor + critic in lock step through grouped launches (experimental, default off)
-        if grouped:
-            from .nets import backward_lockstep, forward_lockstep
-            mu, value = forward_lockstep((self.actor, self.critic), (x, x), train=True)
-        else:
-            s_critic.wait_stream(main)
-            with torch.cuda.stream(s_critic):
-                value = self.critic.forward(x, train=True)
-            mu = self.actor.forward(x, train=True)
-            main.wait_stream(s_critic)
+        grouped = self.grouped_ok and grouped_enabled()    # PULSE_GROUPED=1: actor + critic in lock step through grouped launches (experimental, default off)
+        mu, value = self._forward_train(b, slot, grouped)
         a = _lib.PpoLossArgs(
             mu=mu.data_ptr(), ld_mu=mu.stride(0), value=value.data_ptr(), ld_value=value.stride(0), actions=actions.data_ptr(),
             old_neglogp=old_neglogp.data_ptr(), advantages=advantages.data_ptr(), returns=returns.data_ptr(),
@@ -335,24 +354,7 @@ class PPOPolicy:
             _lib.check(self.lib.pulse_ppo_loss(C.byref(a), M, _lib.current_stream(self.device)), "pulse_ppo_loss")
         if pref_at == "loss":
             fork_prefetch()
-        if grouped:
-            backward_lockstep((self.actor, self.critic), (b["dmu"], b["dv"]), M)
-        else:
-            s_critic.wait_stream(main)
-            with torch.cuda.stream(s_critic):
-                self.critic.backward(b["dv"], M)
-                if reducer is not None:
-                    c0, c1 = self.critic.param_span()
-                    reducer.reduce(self.flat.grads[c0:c1], 1)
-            self.actor.backward(b["dmu"], M)
-            if reducer is not None:
-                a0, a1 = self.actor.param_span()
-                reducer.reduce(self.flat.grads[a0:a1], 0)
-            main.wait_stream(s_critic)
-        if grouped and reducer is not None:                  # lock-step path: actor + critic slices are adjacent, one reduction
-            a0, _ = self.actor.param_span()
-            _, c1 = self.critic.param_span()
-            reducer.reduce(self.flat.grads[a0:c1], 0)
+        self._backward_train(b, M, grouped, reducer)
         if amp is not None:
             main.wait_stream(s_disc)
         if pref_at == "reduce":
@@ -369,6 +371,44 @@ class PPOPolicy:
         if pref_at is not None:
             main.wait_stream(s_pref)
         return self.stats
+
+    def _forward_train(self, b: dict, slot: int, grouped: bool):
+        """Training forward pass of the policy nets on operand slot `slot` of the minibatch buffers: (mu, value), fp32."""
+        x = b["x2"][slot]
+        if grouped:
+            from .nets import forward_lockstep
+            return forward_lockstep((self.actor, self.critic), (x, x), train=True)
+        main, s_critic = torch.cuda.current_stream(self.device), self._side[0]
+        s_critic.wait_stream(main)
+        with torch.cuda.stream(s_critic):
+            value = self.critic.forward(x, train=True)
+        mu = self.actor.forward(x, train=True)
+        main.wait_stream(s_critic)
+        return mu, value
+
+    def _backward_train(self, b: dict, M: int, grouped: bool, reducer) -> None:
+        """Backward pass of the policy nets from the loss kernel's output gradients b['dmu'] / b['dv']; `reducer` (multi-GPU, per-chain
+        gradient exchange) averages each net's gradient slice once it is complete."""
+        if grouped:
+            from .nets import backward_lockstep
+            backward_lockstep((self.actor, self.critic), (b["dmu"], b["dv"]), M)
+            if reducer is not None:                      # lock-step path: actor + critic slices are adjacent, one reduction
+                a0, _ = self.actor.param_span()
+                _, c1 = self.critic.param_span()
+                reducer.reduce(self.flat.grads[a0:c1], 0)
+            return
+        main, s_critic = torch.cuda.current_stream(self.device), self._side[0]
+        s_critic.wait_stream(main)
+        with torch.cuda.stream(s_critic):
+            self.critic.backward(b["dv"], M)
+            if reducer is not None:
+                c0, c1 = self.critic.param_span()
+                reducer.reduce(self.flat.grads[c0:c1], 1)
+        self.actor.backward(b["dmu"], M)
+        if reducer is not None:
+            a0, a1 = self.actor.param_span()
+            reducer.reduce(self.flat.grads[a0:a1], 0)
+        main.wait_stream(s_critic)
 
     # ------------------------------------------------------------------ checkpoint keys (rl_games layout)
     def _rms_pairs(self):
@@ -398,7 +438,7 @@ class PPOPolicy:
         `<section>.running_mean|running_var|count`."""
         sd = {}
         for name, l in self._named_layers():
-            sd[name + ".weight"] = l.weight[:, :l.K].clone()
+            sd[name + ".weight"] = l.ref_weight()
             sd[name + ".bias"] = l.bias.clone()
         sd["a2c_network.sigma"] = self.logstd.clone()
         for sec, rms in self._rms_pairs():
@@ -428,7 +468,7 @@ class PPOPolicy:
         step = self.flat.step.clone().float().reshape(())
         for name, l in self._named_layers():
             m, v = self.flat.view(l.w_idx, "exp_avg"), self.flat.view(l.w_idx, "exp_avg_sq")
-            out[name + ".weight"] = {"exp_avg": m[:, :l.K].clone(), "exp_avg_sq": v[:, :l.K].clone(), "step": step.clone()}
+            out[name + ".weight"] = {"exp_avg": l.ref_weight("exp_avg"), "exp_avg_sq": l.ref_weight("exp_avg_sq"), "step": step.clone()}
             if l.aug:
                 out[name + ".bias"] = {"exp_avg": m[:, l.K].clone(), "exp_avg_sq": v[:, l.K].clone(), "step": step.clone()}
             else:
@@ -445,8 +485,8 @@ class PPOPolicy:
                     continue
                 m, v = self.flat.view(l.w_idx, "exp_avg"), self.flat.view(l.w_idx, "exp_avg_sq")
                 if kind == "weight":
-                    m[:, :l.K].copy_(st["exp_avg"].to(self.device))
-                    v[:, :l.K].copy_(st["exp_avg_sq"].to(self.device))
+                    l.set_ref_weight("exp_avg", st["exp_avg"].to(self.device))
+                    l.set_ref_weight("exp_avg_sq", st["exp_avg_sq"].to(self.device))
                 elif l.aug:
                     m[:, l.K].copy_(st["exp_avg"].to(self.device))
                     v[:, l.K].copy_(st["exp_avg_sq"].to(self.device))
