@@ -12,10 +12,14 @@
 //                continuously across work items, completion on "full" mbarriers;
 //   warps 4..11  two consumer warpgroups, 64 rows of the tile each: wgmma.mma_async m64n128k16 (fp32 accumulators in registers),
 //                one wgmma group in flight, each stage handed back to the producer ("empty") as soon as the group that read it
-//                retires.  After the last k-block the accumulator goes to a per-warpgroup shared tile (32 x 32 fp32 blocks,
-//                128-byte swizzle) and the same warps run the epilogue from it: bias / activation / activation-derivative gate /
-//                column sums -> bf16 and/or fp32 outputs, or bulk tensor reductions of the staged blocks into the
-//                weight-gradient buffer (split-K).  The producer keeps filling the ring for the next item meanwhile.
+//                retires.  After the last k-block the same warps run the epilogue while the producer keeps filling the ring for the
+//                next item:
+//                  forward / input-gradient GEMMs with bf16 outputs only: straight from the accumulator registers -- bias /
+//                  activation / ReLU mask words / mask-word gate -> bf16 pairs -> stmatrix into the warpgroup's shared area ->
+//                  bulk tensor stores of 64 x 64 boxes;
+//                  everything else: the accumulator goes to a per-warpgroup shared tile (32 x 32 fp32 blocks, 128-byte swizzle)
+//                  and the epilogue runs from it: bias / activation / activation-derivative gate / column sums -> bf16 and/or fp32
+//                  outputs, or bulk tensor reductions of the staged blocks into the weight-gradient buffer (split-K).
 #include <cuda.h>
 #include <stdlib.h>
 #include <string.h>
@@ -42,9 +46,10 @@ constexpr unsigned kStageBytesB = BN * BK * 2;
 struct __align__(1024) GemmSmem {
   unsigned char a[kStages][kStageBytesA];
   unsigned char b[kStages][kStageBytesB];
-  float acc[2][64 * BN];                   // per consumer warpgroup: 2 x 4 blocks of 32 x 32 fp32, 128-byte swizzled (4 KB each)
+  float acc[2][64 * BN];                   // per consumer warpgroup: 2 x 4 blocks of 32 x 32 fp32, 128-byte swizzled (4 KB each), or
+                                           // (register-resident epilogue) 2 + 2 bf16 boxes of 64 x 64 for the output / pre-activation stores
   float red[kConsumerWarps][16 * 33];      // per-warp tile: bf16 store staging / fp32 transpose for atomics
-  float bias[kConsumerWarps][kCols];       // per-warp copy of the bias of its columns (broadcast reads in the forward epilogue)
+  float bias[2][BN];                       // per-warpgroup copy of the tile's bias (register-resident forward epilogue)
   unsigned long long full[kStages];
   unsigned long long empty[kStages];
 };
@@ -80,6 +85,24 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
                    s_u32(smem_dst)),
                "l"(map), "r"(s_u32(bar)), "r"(c0), "r"(c1)
                : "memory");
+}
+// bulk tensor store of one box from shared memory (128-byte swizzled, as the map says); completion through the bulk async-group
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, unsigned smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];\n" ::"l"(map), "r"(smem_src), "r"(c0), "r"(c1)
+               : "memory");
+}
+// four 8 x 8 bf16 matrices to shared memory; r[m] holds this thread's pair (row lane / 4, columns 2 (lane % 4) + {0, 1}) of matrix m, and
+// lane l gives the 16-byte row address of row l % 8 of matrix l / 8
+__device__ __forceinline__ void stmatrix_x4(unsigned addr, const unsigned (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};\n" ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+__device__ __forceinline__ unsigned bf16x2_bits(__nv_bfloat162 h) { return *reinterpret_cast<unsigned*>(&h); }
+// a warp's share of sum(v^2) into the fp64 accumulator: all 32 lanes call it
+__device__ __forceinline__ void add_sumsq(double* sumsq, float sq) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+  if ((threadIdx.x & 31) == 0) atomicAdd(sumsq, static_cast<double>(sq));
 }
 // named barrier of one consumer warpgroup (id 0 is __syncthreads)
 __device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;\n" ::"r"(1 + wg) : "memory"); }
@@ -196,6 +219,37 @@ __device__ __forceinline__ __nv_bfloat162 silu_bf16x2(__nv_bfloat162 z) {
   return __floats2bfloat162_rn(f.x, f.y);
 }
 
+// Register-resident epilogue: the warpgroup's 64 x 128 fp32 fragment -> bf16 pairs -> stmatrix into the output boxes at `stage`
+// ([0, 16 KB): two 64 x 64 boxes, 128-byte swizzle, row r = 8 16-byte units, unit u at u ^ (r & 7)) and, when `pre`, the rounded
+// pre-activation into the same layout at +16 KB.  ACT runs on the rounded pair (exact for ReLU, which commutes with the rounding); a
+// SiLU column group that reaches past N applies it in fp32 before the one rounding, as the staged epilogue does.
+// stmatrix x4 at even j: matrices (j, rows r0), (j, r0 + 8), (j + 1, r0), (j + 1, r0 + 8); lane l gives the address of row l % 8 of
+// matrix l / 8.
+template <int ACT>
+__device__ __forceinline__ void stage_tile_bf16(const float (&d)[64], unsigned stage, bool pre, int n0, int N) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned srow = stage + ((warp & 3) * 16 + ((lane >> 3) & 1) * 8 + (lane & 7)) * 128;
+  const int sj = lane >> 4;
+  const __nv_bfloat162 zero2 = __float2bfloat162_rn(0.0f);
+#pragma unroll
+  for (int j = 0; j < BN / 8; j += 2) {
+    const bool full_half = n0 + 64 * (j >> 3) + 64 <= N;
+    unsigned o[4], p[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int i = 4 * (j + (k >> 1)) + 2 * (k & 1);
+      __nv_bfloat162 h = __floats2bfloat162_rn(d[i], d[i + 1]);
+      p[k] = bf16x2_bits(h);
+      if (ACT == PULSE_ACT_RELU) h = __hmax2(h, zero2);
+      if (ACT == PULSE_ACT_SILU) h = full_half ? silu_bf16x2(h) : __floats2bfloat162_rn(act_apply(d[i], ACT), act_apply(d[i + 1], ACT));
+      o[k] = bf16x2_bits(h);
+    }
+    const unsigned addr = srow + (j >> 3) * 8192 + ((((j & 7) + sj) ^ (lane & 7)) << 4);
+    stmatrix_x4(addr, o);
+    if (pre) stmatrix_x4(addr + 16384, p);
+  }
+}
+
 // A_MN / B_MN: operand is MN-major in global memory ([reduction rows, non-reduction cols] row-major) instead of K-major.
 // MODE selects which epilogue features are COMPILED IN: the fully general epilogue is several thousand SASS instructions per
 // instance, so each specialisation carries only what its caller can ask for (instruction-cache footprint); the host picks the
@@ -205,11 +259,11 @@ enum : int { kModeGeneric = 0, kModeFwd = 1, kModeDgrad = 2, kModeWgrad = 3, kMo
 // ---- grouped launch: several problems of the same operand majors / epilogue mode in ONE persistent launch ------------------
 constexpr int kMaxGroup = 4;
 struct GemmProblem {
-  CUtensorMap map_a, map_b, map_c;
+  CUtensorMap map_a, map_b, map_c, map_p;
   pulse_gemm_epilogue_t ep;
   int M, N, K, kb_per_split;
   int item_end;   // cumulative work items (tiles x split-K slices) up to and including this problem
-  int use_tma_red;
+  int tma_out;
   int pad[2];
 };
 struct GemmGroup {
@@ -268,6 +322,37 @@ bool make_map_c(CUtensorMap* map, const float* base, long long rows, long long c
 bool tma_reduce_ok(const pulse_gemm_epilogue_t& ep) {
   return ep.out_f32 != nullptr && ep.accumulate && (ep.ldf % 4) == 0 && (reinterpret_cast<uintptr_t>(ep.out_f32) % 16) == 0;
 }
+bool tma_rows_ok(const void* base, long long ld) { return (ld % 8) == 0 && (reinterpret_cast<uintptr_t>(base) % 16) == 0; }
+
+// Tensor maps of the epilogue and whether the kernel uses them (tma_out):
+//   wgrad: map_c = the fp32 gradient, target of the bulk tensor reductions;
+//   forward / input gradient with bf16 outputs only (no fp32 or transposed copy, bf16 gate or column sums): the register-resident
+//   epilogue, map_c = out, map_p = preact, [M, N] bf16 with 64 x 64 boxes, so the hardware clips the row and column tails.  It clips
+//   columns in whole 16-byte units, so N must be a multiple of 8 (an N = 69 store would overwrite columns 69..71).
+// Anything else, or rows that are not 16-byte aligned, runs the staged epilogue.
+int epilogue_maps(int mode, const pulse_gemm_epilogue_t& ep, long long m, long long n, CUtensorMap* map_c, CUtensorMap* map_p, int* tma_out) {
+  memset(map_c, 0, sizeof(*map_c));
+  memset(map_p, 0, sizeof(*map_p));
+  *tma_out = 0;
+  if (mode == kModeWgrad) {
+    if (!tma_reduce_ok(ep)) return PULSE_OK;
+    if (!make_map_c(map_c, ep.out_f32, m, n, ep.ldf)) {
+      set_error("pulse_gemm_bf16: cuTensorMapEncodeTiled failed for the fp32 output");
+      return PULSE_ERR_CUDA;
+    }
+    *tma_out = 1;
+    return PULSE_OK;
+  }
+  if ((mode != kModeFwd && mode != kModeDgrad) || (n % 8) != 0 || ep.out == nullptr || ep.out_f32 != nullptr || ep.out_t != nullptr || ep.gate != nullptr ||
+      ep.colsum != nullptr || !tma_rows_ok(ep.out, ep.ldo) || (ep.preact != nullptr && !tma_rows_ok(ep.preact, ep.ldp)))
+    return PULSE_OK;
+  if (!make_map(map_c, ep.out, m, n, ep.ldo, 64) || (ep.preact != nullptr && !make_map(map_p, ep.preact, m, n, ep.ldp, 64))) {
+    set_error("pulse_gemm_bf16: cuTensorMapEncodeTiled failed for the bf16 output");
+    return PULSE_ERR_CUDA;
+  }
+  *tma_out = 1;
+  return PULSE_OK;
+}
 
 constexpr size_t kSmemBytes = sizeof(GemmSmem) + 1024;  // slack so the kernel can align the ring to 1024 B
 
@@ -288,16 +373,10 @@ template <bool A_MN, bool B_MN, int MODE>
 int launch_gemm(const CUtensorMap& map_a, const CUtensorMap& map_b, const pulse_gemm_epilogue_t& ep, int m, int n, int k, int splits,
                 int kb_per_split, cudaStream_t stream) {
   static bool attr_set = false;
-  CUtensorMap map_c;
-  memset(&map_c, 0, sizeof(map_c));
-  int use_tma_red = 0;
-  if (MODE == kModeWgrad && tma_reduce_ok(ep)) {
-    if (!make_map_c(&map_c, ep.out_f32, m, n, ep.ldf)) {
-      set_error("pulse_gemm_bf16: cuTensorMapEncodeTiled failed for the fp32 output");
-      return PULSE_ERR_CUDA;
-    }
-    use_tma_red = 1;
-  }
+  CUtensorMap map_c, map_p;
+  int tma_out = 0;
+  const int rc = epilogue_maps(MODE, ep, m, n, &map_c, &map_p, &tma_out);
+  if (rc != PULSE_OK) return rc;
   if (!attr_set) {
     PULSE_CUDA_OK(cudaFuncSetAttribute(gemm_bf16_kernel<A_MN, B_MN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
     attr_set = true;
@@ -326,7 +405,7 @@ int launch_gemm(const CUtensorMap& map_a, const CUtensorMap& map_b, const pulse_
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
-  PULSE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_kernel<A_MN, B_MN, MODE>, map_a, map_b, map_c, ep, m, n, k, kb_per_split, splits, use_tma_red));
+  PULSE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_kernel<A_MN, B_MN, MODE>, map_a, map_b, map_c, map_p, ep, m, n, k, kb_per_split, splits, tma_out));
   PULSE_LAUNCH_OK("gemm_bf16_kernel");
   return PULSE_OK;
 }
@@ -480,14 +559,8 @@ extern "C" int pulse_gemm_bf16_grouped(const pulse_gemm_problem_t* problems, int
       return PULSE_ERR_CUDA;
     }
     g.ep = q.ep;
-    g.use_tma_red = 0;
-    if (mode == kModeWgrad && tma_reduce_ok(q.ep)) {
-      if (!make_map_c(&g.map_c, q.ep.out_f32, q.m, q.n, q.ep.ldf)) {
-        set_error("pulse_gemm_bf16_grouped: cuTensorMapEncodeTiled failed for the fp32 output of problem %d", i);
-        return PULSE_ERR_CUDA;
-      }
-      g.use_tma_red = 1;
-    }
+    const int rc = epilogue_maps(mode, q.ep, q.m, q.n, &g.map_c, &g.map_p, &g.tma_out);
+    if (rc != PULSE_OK) return rc;
     g.M = static_cast<int>(q.m);
     g.N = static_cast<int>(q.n);
     g.K = static_cast<int>(q.k);

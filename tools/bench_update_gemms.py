@@ -1,4 +1,6 @@
 """Every GEMM of one PPO + discriminator minibatch update, timed alone (CUDA events, warm L2), with its tensor / HBM floor.
+The epilogue arguments are the ones the update passes: the nets are bias-augmented (no bias vector, no column sums), the forward
+layers write ReLU mask words and the input-gradient GEMMs are gated by them.
 
     python tools/bench_update_gemms.py [--json out.json]
 floor_us = max(flops / bf16 peak, compulsory bytes / HBM peak) from MEASURED_PEAKS.json (sustained figures).
@@ -46,8 +48,10 @@ def main():
     bf = lambda r, c: (torch.randn(r, c, device=dev) * 0.1).bfloat16()
     rows = []
 
-    def case(name, M, N, K, kind, gate=False, colsum=False, f32=False, bf16_out=True, alpha=1.0, act="relu", preact=False):
-        """kind: 'nt' (A [M,K], B [N,K]), 'dgrad' (A [M,K], B [K,N] MN-major), 'wgrad' (A [K,M], B [K,N], atomics into fp32)."""
+    def case(name, M, N, K, kind, gate=None, colsum=False, f32=False, bf16_out=True, alpha=1.0, act="relu", preact=False, bias=False,
+             relu_mask=False, sumsq=False):
+        """kind: 'nt' (A [M,K], B [N,K]), 'dgrad' (A [M,K], B [K,N] MN-major), 'wgrad' (A [K,M], B [K,N], atomics into fp32).
+        gate: None, 'act' (bf16 saved tensor, act') or 'mask' (ReLU mask words); relu_mask: a forward case writes the mask words."""
         if a.only and a.only not in name:
             return
         Mp, Np, Kp = pad_k(M), pad_k(N), pad_k(K)
@@ -75,14 +79,24 @@ def main():
             if f32:
                 kw.update(out_f32=torch.zeros(M, Np, device=dev))
                 byt += M * N * 4
-            if kind == "nt" and not gate:
-                kw.update(bias=torch.zeros(N, device=dev), act=act if bf16_out and not f32 else None)
+            if kind == "nt" and gate is None:
+                kw.update(act=act if bf16_out and not f32 else None)
+                if bias:
+                    kw.update(bias=torch.zeros(N, device=dev))
                 if preact:
                     kw.update(preact=torch.zeros(M, Np, device=dev, dtype=torch.bfloat16))
                     byt += M * N * 2
-        if gate:
+                if relu_mask:
+                    kw.update(relu_mask=torch.zeros((N + 31) // 32, M, device=dev, dtype=torch.int32))
+                    byt += M * N // 8
+        if gate == "act":
             kw.update(gate=bf(M, Np), gate_mode=act)
             byt += M * N * 2
+        elif gate == "mask":
+            kw.update(gate_mask=torch.randint(-2 ** 31, 2 ** 31 - 1, ((N + 31) // 32, M), device=dev, dtype=torch.int32))
+            byt += M * N // 8
+        if sumsq:
+            kw.update(sumsq=torch.zeros(1, device=dev, dtype=torch.float64))
         if colsum:
             kw.update(colsum=torch.zeros(Np, device=dev))
         if alpha != 1.0:
@@ -98,36 +112,36 @@ def main():
         for net, sizes in (("enc", [934, 1536, 1024, 512, 160]), ("prior", [358, 1536, 1024, 512]), ("dec", [390, 3096, 2048, 1024])):
             for i in range(len(sizes) - 1):
                 k, n = sizes[i], sizes[i + 1]
-                case(f"{net}.fwd{i}", B, n, k, "nt", act="silu", preact=True)
+                case(f"{net}.fwd{i}", B, n, k, "nt", act="silu", preact=True, bias=True)
                 case(f"{net}.wgrad{i}", n, k, B, "wgrad")
                 if i > 0:
-                    case(f"{net}.dgrad{i}", B, k, n, "dgrad", gate=True, colsum=True, act="silu")
+                    case(f"{net}.dgrad{i}", B, k, n, "dgrad", gate="act", colsum=True, act="silu")
     for net, head in (() if a.vae else (("actor", 69), ("critic", 1))):
-        case(f"{net}.fwd1", B, 1024, 934, "nt")
-        case(f"{net}.fwd2", B, 512, 1024, "nt")
+        case(f"{net}.fwd1", B, 1024, 934, "nt", relu_mask=True)
+        case(f"{net}.fwd2", B, 512, 1024, "nt", relu_mask=True)
         case(f"{net}.head", B, head, 512, "nt", f32=True, bf16_out=False)
         case(f"{net}.wgrad_head", head, 512, B, "wgrad")
-        case(f"{net}.dgrad_head", B, 512, head, "dgrad", gate=True, colsum=True)
+        case(f"{net}.dgrad_head", B, 512, head, "dgrad", gate="mask")
         case(f"{net}.wgrad2", 512, 1024, B, "wgrad")
-        case(f"{net}.dgrad2", B, 1024, 512, "dgrad", gate=True, colsum=True)
+        case(f"{net}.dgrad2", B, 1024, 512, "dgrad", gate="mask")
         case(f"{net}.wgrad1", 1024, 934, B, "wgrad")
     if a.vae:
         Bd = Bg = 0
     nonvae = lambda *args, **kw2: None if a.vae else case(*args, **kw2)
-    nonvae("disc.fwd1", Bd, 1024, 1960, "nt")
-    nonvae("disc.fwd2", Bd, 512, 1024, "nt")
+    nonvae("disc.fwd1", Bd, 1024, 1960, "nt", relu_mask=True)
+    nonvae("disc.fwd2", Bd, 512, 1024, "nt", relu_mask=True)
     nonvae("disc.head", Bd, 1, 512, "nt", f32=True, bf16_out=False)
     nonvae("disc.wgrad_head", 1, 512, Bd, "wgrad")
-    nonvae("disc.dgrad_head", Bd, 512, 1, "dgrad", gate=True, colsum=True)
+    nonvae("disc.dgrad_head", Bd, 512, 1, "dgrad", gate="mask")
     nonvae("disc.wgrad2", 512, 1024, Bd, "wgrad")
-    nonvae("disc.dgrad2", Bd, 1024, 512, "dgrad", gate=True, colsum=True)
+    nonvae("disc.dgrad2", Bd, 1024, 512, "dgrad", gate="mask")
     nonvae("disc.wgrad1", 1024, 1960, Bd, "wgrad")
-    nonvae("gp.g1", Bg, 1024, 512, "dgrad", gate=True)
-    nonvae("gp.G", Bg, 1960, 1024, "dgrad", f32=True, alpha=0.01)
+    nonvae("gp.g1", Bg, 1024, 512, "dgrad", gate="mask")
+    nonvae("gp.G", Bg, 1960, 1024, "dgrad", alpha=0.01, sumsq=True)
     nonvae("gp.dW1", 1024, 1960, Bg, "wgrad")
-    nonvae("gp.du", Bg, 1024, 1960, "nt", gate=True)
+    nonvae("gp.du", Bg, 1024, 1960, "nt", gate="mask")
     nonvae("gp.dW2", 512, 1024, Bg, "wgrad")
-    nonvae("gp.dw3", Bg, 512, 1024, "nt", gate=True, colsum=True)
+    nonvae("gp.dw3", Bg, 512, 1024, "nt", gate="mask", f32=True, bf16_out=False)
     tot, fl = sum(r["us"] for r in rows), sum(r["floor_us"] for r in rows)
     for r in rows:
         print(f"{r['name']:18s} {r['kind']:5s} M={r['M']:6d} N={r['N']:5d} K={r['K']:6d}  {r['us']:8.2f} us  {r['tflops']:7.1f} TF  "
