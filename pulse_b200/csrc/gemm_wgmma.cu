@@ -8,8 +8,9 @@
 // Operands are read as they sit in memory: the wgmma transpose bits select K-major or MN-major, nothing is transposed.
 //
 // Structure (persistent: one CTA per SM loops over 128 x 128 output tiles x split-K slices):
-//   warp 0       TMA producer: cp.async.bulk.tensor 2D loads (128B swizzle) into a 4-stage shared-memory ring that runs
-//                continuously across work items, completion on "full" mbarriers;
+//   warp 0       TMA producer: cp.async.bulk.tensor 2D loads (128B swizzle) into a shared-memory ring that runs continuously
+//                across work items, completion on "full" mbarriers (4 stages; 6, or 5 with a pre-activation, where the epilogue is
+//                register-resident: see GemmSmem);
 //   warps 4..11  two consumer warpgroups, 64 rows of the tile each: wgmma.mma_async m64n128k16 (fp32 accumulators in registers),
 //                one wgmma group in flight, each stage handed back to the producer ("empty") as soon as the group that read it
 //                retires.  After the last k-block the same warps run the epilogue while the producer keeps filling the ring for the
@@ -39,20 +40,45 @@ constexpr int kThreads = 128 + 32 * kConsumerWarps;   // producer warpgroup (one
 // Each consumer warp drains 32 rows x kCols columns of its warpgroup's 64 x 128 accumulator in 32-column chunks.
 constexpr int kCols = 64;
 constexpr int kChunks = kCols / 32;
-constexpr int kStages = 4;
+constexpr int kStages = 4;   // ring depth of the instantiations that can take the staged epilogue
+constexpr int kTmaOutF32 = 2;   // tma_out of a plain fp32 output through the register-resident epilogue (deep-ring kernels only)
 constexpr unsigned kStageBytesA = BM * BK * 2;
 constexpr unsigned kStageBytesB = BN * BK * 2;
 
+// Shared memory of an instantiation with an S-stage operand ring.  The consumers hold up to two stages, so a 4-stage ring gives the
+// producer two stages of lead; the update's short-K items (8-16 k-blocks) wait on operand loads for a quarter of their main loop,
+// and two more stages cut the 8-k-block input-gradient items by about a quarter (DESIGN.md section 3.3).  Only the
+// register-resident epilogue can afford more stages: it needs 16 KB of bf16 output boxes per consumer warpgroup
+// (32 KB with the pre-activation), not the staged path's fp32 tile and per-warp tiles.  So the instantiations that may take the
+// staged path keep kStages (the specialisation below), and the register-epilogue-only ones give that room to the ring: 6 stages,
+// or 5 when the pre-activation boxes need the second 16 KB.
+template <int S>
 struct __align__(1024) GemmSmem {
+  unsigned char a[S][kStageBytesA];
+  unsigned char b[S][kStageBytesB];
+  unsigned char epi[2][S >= 6 ? 16384 : 32768];   // per consumer warpgroup: output boxes [0, 16 KB), pre-activation boxes [16, 32 KB);
+                                                 // or one 64-column half of a plain fp32 output at a time
+  float bias[2][BN];                             // per-warpgroup copy of the tile's bias
+  unsigned long long full[S];
+  unsigned long long empty[S];
+};
+template <>
+struct __align__(1024) GemmSmem<kStages> {
   unsigned char a[kStages][kStageBytesA];
   unsigned char b[kStages][kStageBytesB];
-  float acc[2][64 * BN];                   // per consumer warpgroup: 2 x 4 blocks of 32 x 32 fp32, 128-byte swizzled (4 KB each), or
+  float epi[2][64 * BN];                   // per consumer warpgroup: 2 x 4 blocks of 32 x 32 fp32, 128-byte swizzled (4 KB each), or
                                            // (register-resident epilogue) 2 + 2 bf16 boxes of 64 x 64 for the output / pre-activation stores
   float red[kConsumerWarps][16 * 33];      // per-warp tile: bf16 store staging / fp32 transpose for atomics
   float bias[2][BN];                       // per-warpgroup copy of the tile's bias (register-resident forward epilogue)
   unsigned long long full[kStages];
   unsigned long long empty[kStages];
 };
+// dynamic shared memory of a launch: 1 KB of slack so the kernel can align the ring to 1024 B
+template <int S>
+constexpr size_t smem_bytes() { return sizeof(GemmSmem<S>) + 1024; }
+constexpr size_t kSmemOptin = 232448;   // sm_90 opt-in limit of dynamic shared memory per block (227 KB)
+static_assert(smem_bytes<kStages>() <= kSmemOptin && smem_bytes<5>() <= kSmemOptin && smem_bytes<6>() <= kSmemOptin,
+              "GEMM shared-memory layout exceeds the per-block opt-in limit");
 
 __device__ __forceinline__ unsigned s_u32(const void* p) { return static_cast<unsigned>(__cvta_generic_to_shared(p)); }
 __device__ __forceinline__ void g_mbar_init(unsigned long long* bar, unsigned count) {
@@ -89,6 +115,12 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
 // bulk tensor store of one box from shared memory (128-byte swizzled, as the map says); completion through the bulk async-group
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, unsigned smem_src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];\n" ::"l"(map), "r"(smem_src), "r"(c0), "r"(c1)
+               : "memory");
+}
+// the same for a 3-D map ({column, row, split-K slab})
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, unsigned smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];\n" ::"l"(map), "r"(smem_src), "r"(c0), "r"(c1),
+               "r"(c2)
                : "memory");
 }
 // four 8 x 8 bf16 matrices to shared memory; r[m] holds this thread's pair (row lane / 4, columns 2 (lane % 4) + {0, 1}) of matrix m, and
@@ -203,10 +235,36 @@ __device__ long long g_gemm_trace[32];
   do {                                                             \
     if (blockIdx.x == 0) g_gemm_trace[slot] = clock64();           \
   } while (0)
+#define PULSE_TRACE_SET(slot, v)                                   \
+  do {                                                             \
+    if (blockIdx.x == 0) g_gemm_trace[slot] = (v);                 \
+  } while (0)
+// launch start: the slots of an earlier launch (possibly clocks of another SM) are cleared first
+#define PULSE_TRACE_START()                                        \
+  do {                                                             \
+    if (blockIdx.x == 0) {                                         \
+      for (int i_ = 1; i_ < 32; ++i_) g_gemm_trace[i_] = 0;        \
+      g_gemm_trace[0] = clock64();                                 \
+    }                                                              \
+  } while (0)
+// a ring-barrier wait that adds the clocks it spent to `clk` (stall counters of the trace)
+#define PULSE_RING_WAIT(bar, parity, clk)                          \
+  do {                                                             \
+    const long long t_ = clock64();                                \
+    g_mbar_wait(bar, parity);                                      \
+    clk += clock64() - t_;                                         \
+  } while (0)
 #else
 #define PULSE_TRACE(slot) \
   do {                    \
   } while (0)
+#define PULSE_TRACE_SET(slot, v) \
+  do {                           \
+  } while (0)
+#define PULSE_TRACE_START() \
+  do {                      \
+  } while (0)
+#define PULSE_RING_WAIT(bar, parity, clk) g_mbar_wait(bar, parity)
 #endif
 
 // silu(z) = z / (1 + e^-z) on a bf16 pair, evaluated in fp32 (ex2.approx + rcp.approx per element) and rounded ONCE to bf16.
@@ -318,6 +376,18 @@ bool make_map_c(CUtensorMap* map, const float* base, long long rows, long long c
   return fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
+// fp32 split-K slabs [splits][rows, cols] (slab z at base + z * split_stride floats, row stride ld floats) as a 3-D tensor map with 32 x 32 x 1
+// boxes, 128-byte swizzle: the target of the register-resident epilogue's fp32 stores (rows / columns beyond the slab are clipped).
+bool make_map_slabs(CUtensorMap* map, const float* base, long long splits, long long rows, long long cols, long long ld, long long split_stride) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (fn == nullptr) return false;
+  cuuint64_t dims[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows), static_cast<cuuint64_t>(splits)};
+  cuuint64_t strides[2] = {static_cast<cuuint64_t>(ld) * 4, static_cast<cuuint64_t>(splits > 1 ? split_stride : rows * ld) * 4};
+  cuuint32_t box[3] = {32, 32, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  return fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
 // the reduction path needs 16-byte aligned rows; otherwise the kernel falls back to fp32 atomics
 bool tma_reduce_ok(const pulse_gemm_epilogue_t& ep) {
   return ep.out_f32 != nullptr && ep.accumulate && (ep.ldf % 4) == 0 && (reinterpret_cast<uintptr_t>(ep.out_f32) % 16) == 0;
@@ -329,8 +399,12 @@ bool tma_rows_ok(const void* base, long long ld) { return (ld % 8) == 0 && (rein
 //   forward / input gradient with bf16 outputs only (no fp32 or transposed copy, bf16 gate or column sums): the register-resident
 //   epilogue, map_c = out, map_p = preact, [M, N] bf16 with 64 x 64 boxes, so the hardware clips the row and column tails.  It clips
 //   columns in whole 16-byte units, so N must be a multiple of 8 (an N = 69 store would overwrite columns 69..71).
+//   forward with a plain fp32 output only (split-K slabs of the weight gradients: no alpha, bias, activation or other output), N a
+//   multiple of 4: the register-resident epilogue of the deep-ring kernel, map_c = the slabs (tma_out = kTmaOutF32).  The 4-stage kernel
+//   has no such path: the launch clears tma_out when it runs that one.
 // Anything else, or rows that are not 16-byte aligned, runs the staged epilogue.
-int epilogue_maps(int mode, const pulse_gemm_epilogue_t& ep, long long m, long long n, CUtensorMap* map_c, CUtensorMap* map_p, int* tma_out) {
+int epilogue_maps(int mode, const pulse_gemm_epilogue_t& ep, long long m, long long n, int splits, CUtensorMap* map_c, CUtensorMap* map_p,
+                  int* tma_out) {
   memset(map_c, 0, sizeof(*map_c));
   memset(map_p, 0, sizeof(*map_p));
   *tma_out = 0;
@@ -343,6 +417,16 @@ int epilogue_maps(int mode, const pulse_gemm_epilogue_t& ep, long long m, long l
     *tma_out = 1;
     return PULSE_OK;
   }
+  if (mode == kModeFwd && ep.out_f32 != nullptr && ep.out == nullptr && ep.out_t == nullptr && ep.preact == nullptr && ep.relu_mask == nullptr &&
+      ep.bias == nullptr && ep.act == PULSE_ACT_NONE && ep.alpha == 1.0f && !ep.accumulate && (n % 4) == 0 && (ep.ldf % 4) == 0 &&
+      (reinterpret_cast<uintptr_t>(ep.out_f32) % 16) == 0 && (splits == 1 || (ep.split_stride % 4) == 0)) {
+    if (!make_map_slabs(map_c, ep.out_f32, splits, m, n, ep.ldf, ep.split_stride)) {
+      set_error("pulse_gemm_bf16: cuTensorMapEncodeTiled failed for the fp32 output");
+      return PULSE_ERR_CUDA;
+    }
+    *tma_out = kTmaOutF32;
+    return PULSE_OK;
+  }
   if ((mode != kModeFwd && mode != kModeDgrad) || (n % 8) != 0 || ep.out == nullptr || ep.out_f32 != nullptr || ep.out_t != nullptr || ep.gate != nullptr ||
       ep.colsum != nullptr || !tma_rows_ok(ep.out, ep.ldo) || (ep.preact != nullptr && !tma_rows_ok(ep.preact, ep.ldp)))
     return PULSE_OK;
@@ -353,8 +437,6 @@ int epilogue_maps(int mode, const pulse_gemm_epilogue_t& ep, long long m, long l
   *tma_out = 1;
   return PULSE_OK;
 }
-
-constexpr size_t kSmemBytes = sizeof(GemmSmem) + 1024;  // slack so the kernel can align the ring to 1024 B
 
 int gemm_num_sms(bool honour_limit) {
   static int num_sms = 0, limited = 0;
@@ -369,18 +451,34 @@ int gemm_num_sms(bool honour_limit) {
   return honour_limit ? limited : num_sms;
 }
 
-template <bool A_MN, bool B_MN, int MODE>
-int launch_gemm(const CUtensorMap& map_a, const CUtensorMap& map_b, const pulse_gemm_epilogue_t& ep, int m, int n, int k, int splits,
-                int kb_per_split, cudaStream_t stream) {
+// Ring depth of a launch whose epilogue is register-resident (reg_epi) or not: see GemmSmem.  PULSE_GEMM_STAGES=4 keeps every launch
+// on the 4-stage kernel; it is read at every launch, so one process can compare both kernels.
+int ring_stages(bool reg_epi, bool preact) {
+  const char* e = getenv("PULSE_GEMM_STAGES");
+  const bool force4 = e != nullptr && atoi(e) == kStages;
+  return (!reg_epi || force4) ? kStages : preact ? 5 : 6;
+}
+
+// sets the kernel's dynamic shared-memory size once per instantiation and checks it against the device's opt-in limit
+template <typename Kernel>
+int set_smem_once(Kernel kernel, size_t bytes, bool* done) {
+  if (*done) return PULSE_OK;
+  int dev = 0, optin = 0;
+  PULSE_CUDA_OK(cudaGetDevice(&dev));
+  PULSE_CUDA_OK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  PULSE_REQUIRE(bytes <= static_cast<size_t>(optin), "pulse_gemm_bf16: the GEMM needs %zu bytes of shared memory per block, the device allows %d",
+                bytes, optin);
+  PULSE_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes)));
+  *done = true;
+  return PULSE_OK;
+}
+
+template <bool A_MN, bool B_MN, int MODE, int S>
+int launch_gemm_ring(const CUtensorMap& map_a, const CUtensorMap& map_b, const CUtensorMap& map_c, const CUtensorMap& map_p,
+                     const pulse_gemm_epilogue_t& ep, int m, int n, int k, int splits, int kb_per_split, int tma_out, cudaStream_t stream) {
   static bool attr_set = false;
-  CUtensorMap map_c, map_p;
-  int tma_out = 0;
-  const int rc = epilogue_maps(MODE, ep, m, n, &map_c, &map_p, &tma_out);
+  const int rc = set_smem_once(gemm_bf16_kernel<A_MN, B_MN, MODE, S>, smem_bytes<S>(), &attr_set);
   if (rc != PULSE_OK) return rc;
-  if (!attr_set) {
-    PULSE_CUDA_OK(cudaFuncSetAttribute(gemm_bf16_kernel<A_MN, B_MN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
-    attr_set = true;
-  }
   const int num_sms = gemm_num_sms(true);
   PULSE_REQUIRE(num_sms > 0, "pulse_gemm_bf16: cannot query the device's SM count");
   // persistent: one CTA per SM loops over the work items
@@ -394,7 +492,7 @@ int launch_gemm(const CUtensorMap& map_a, const CUtensorMap& map_b, const pulse_
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid, 1, 1);
   cfg.blockDim = dim3(kThreads, 1, 1);
-  cfg.dynamicSmemBytes = kSmemBytes;
+  cfg.dynamicSmemBytes = smem_bytes<S>();
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   int na = 0;
@@ -405,32 +503,48 @@ int launch_gemm(const CUtensorMap& map_a, const CUtensorMap& map_b, const pulse_
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
-  PULSE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_kernel<A_MN, B_MN, MODE>, map_a, map_b, map_c, map_p, ep, m, n, k, kb_per_split, splits, tma_out));
+  PULSE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_kernel<A_MN, B_MN, MODE, S>, map_a, map_b, map_c, map_p, ep, m, n, k, kb_per_split, splits, tma_out));
   PULSE_LAUNCH_OK("gemm_bf16_kernel");
   return PULSE_OK;
 }
 
 template <bool A_MN, bool B_MN, int MODE>
+int launch_gemm(const CUtensorMap& map_a, const CUtensorMap& map_b, const pulse_gemm_epilogue_t& ep, int m, int n, int k, int splits,
+                int kb_per_split, cudaStream_t stream) {
+  CUtensorMap map_c, map_p;
+  int tma_out = 0;
+  const int rc = epilogue_maps(MODE, ep, m, n, splits, &map_c, &map_p, &tma_out);
+  if (rc != PULSE_OK) return rc;
+  if constexpr (MODE == kModeFwd || MODE == kModeDgrad) {
+    const int s = ring_stages(tma_out != 0, ep.preact != nullptr);
+    if (s == kStages && tma_out == kTmaOutF32) tma_out = 0;
+    if (s == 6) return launch_gemm_ring<A_MN, B_MN, MODE, 6>(map_a, map_b, map_c, map_p, ep, m, n, k, splits, kb_per_split, tma_out, stream);
+    if constexpr (MODE == kModeFwd) {   // only the forward epilogue writes a pre-activation
+      if (s == 5) return launch_gemm_ring<A_MN, B_MN, MODE, 5>(map_a, map_b, map_c, map_p, ep, m, n, k, splits, kb_per_split, tma_out, stream);
+    }
+  }
+  return launch_gemm_ring<A_MN, B_MN, MODE, kStages>(map_a, map_b, map_c, map_p, ep, m, n, k, splits, kb_per_split, tma_out, stream);
+}
+
+template <bool A_MN, bool B_MN, int MODE, int S>
 int launch_gemm_grouped(const GemmGroup& grp, cudaStream_t stream) {
   static bool attr_set = false;
-  if (!attr_set) {
-    PULSE_CUDA_OK(cudaFuncSetAttribute(gemm_bf16_grouped_kernel<A_MN, B_MN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
-    attr_set = true;
-  }
+  const int rc = set_smem_once(gemm_bf16_grouped_kernel<A_MN, B_MN, MODE, S>, smem_bytes<S>(), &attr_set);
+  if (rc != PULSE_OK) return rc;
   const int num_sms = gemm_num_sms(false);
   PULSE_REQUIRE(num_sms > 0, "pulse_gemm_bf16_grouped: cannot query the device's SM count");
   const unsigned grid = static_cast<unsigned>(grp.total_items < num_sms ? grp.total_items : num_sms);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid, 1, 1);
   cfg.blockDim = dim3(kThreads, 1, 1);
-  cfg.dynamicSmemBytes = kSmemBytes;
+  cfg.dynamicSmemBytes = smem_bytes<S>();
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  PULSE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_grouped_kernel<A_MN, B_MN, MODE>, grp));
+  PULSE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_grouped_kernel<A_MN, B_MN, MODE, S>, grp));
   PULSE_LAUNCH_OK("gemm_bf16_grouped_kernel");
   return PULSE_OK;
 }
@@ -559,7 +673,7 @@ extern "C" int pulse_gemm_bf16_grouped(const pulse_gemm_problem_t* problems, int
       return PULSE_ERR_CUDA;
     }
     g.ep = q.ep;
-    const int rc = epilogue_maps(mode, q.ep, q.m, q.n, &g.map_c, &g.map_p, &g.tma_out);
+    const int rc = epilogue_maps(mode, q.ep, q.m, q.n, 1, &g.map_c, &g.map_p, &g.tma_out);
     if (rc != PULSE_OK) return rc;
     g.M = static_cast<int>(q.m);
     g.N = static_cast<int>(q.n);
@@ -573,7 +687,23 @@ extern "C" int pulse_gemm_bf16_grouped(const pulse_gemm_problem_t* problems, int
   }
   grp.total_items = static_cast<int>(items);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (mode == kModeFwd) return launch_gemm_grouped<false, false, kModeFwd>(grp, st);
-  if (mode == kModeDgrad) return launch_gemm_grouped<false, true, kModeDgrad>(grp, st);
-  return launch_gemm_grouped<true, true, kModeWgrad>(grp, st);
+  // the deep ring only when every problem takes the register-resident epilogue
+  bool reg_epi = true, preact = false;
+  for (int i = 0; i < count; ++i) {
+    reg_epi = reg_epi && grp.p[i].tma_out;
+    preact = preact || problems[i].ep.preact != nullptr;
+  }
+  const int s = ring_stages(mode != kModeWgrad && reg_epi, preact);
+  for (int i = 0; i < count; ++i)
+    if (s == kStages && grp.p[i].tma_out == kTmaOutF32) grp.p[i].tma_out = 0;
+  if (mode == kModeFwd) {
+    if (s == 6) return launch_gemm_grouped<false, false, kModeFwd, 6>(grp, st);
+    if (s == 5) return launch_gemm_grouped<false, false, kModeFwd, 5>(grp, st);
+    return launch_gemm_grouped<false, false, kModeFwd, kStages>(grp, st);
+  }
+  if (mode == kModeDgrad) {
+    if (s == 6) return launch_gemm_grouped<false, true, kModeDgrad, 6>(grp, st);
+    return launch_gemm_grouped<false, true, kModeDgrad, kStages>(grp, st);
+  }
+  return launch_gemm_grouped<true, true, kModeWgrad, kStages>(grp, st);
 }
