@@ -360,6 +360,11 @@ int pulse_gemm_bf16_nt(const void* a, int64_t lda, const void* b, int64_t ldb, i
 int pulse_gemm_bf16(const void* a, int64_t lda, const void* b, int64_t ldb, int64_t m, int64_t n, int64_t k,
                     const pulse_gemm_epilogue_t* ep, int32_t split_k, uint32_t flags, void* stream);
 int pulse_gemm_num_splits(int64_t k, int32_t split_k);
+/* The GEMM's shape rule alone: the output tile width (128 or 256) it picks for an m x n x k GEMM with split_k on `sms` SMs.  A launch
+ * takes the wide tile only for forward / ReLU-dgrad GEMMs with a K-major A and bf16-only outputs without a pre-activation, and never
+ * under PULSE_GEMM_BN=128 or PULSE_GEMM_STAGES=4.  pulse_gemm_last_tile_n: the width the last GEMM launch took (0 before the first). */
+int pulse_gemm_tile_n(int64_t m, int64_t n, int64_t k, int32_t split_k, int32_t sms);
+int pulse_gemm_last_tile_n(void);
 
 /* Several GEMMs of the same kind in ONE persistent launch (work items of all problems concatenated): forward groups
  * (flags 0), ReLU-dgrad groups (PULSE_GEMM_B_MN) or weight-gradient groups (PULSE_GEMM_A_MN | PULSE_GEMM_B_MN, fp32 atomic

@@ -298,6 +298,8 @@ SIGNATURES = {
     "pulse_gemm_bf16": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                                   C.POINTER(GemmEpilogue), C.c_int32, C.c_uint32, C.c_void_p]),
     "pulse_gemm_num_splits": (C.c_int, [C.c_int64, C.c_int32]),
+    "pulse_gemm_tile_n": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32]),
+    "pulse_gemm_last_tile_n": (C.c_int, []),
     "pulse_gemm_bf16_grouped": (C.c_int, [C.POINTER(GemmProblem), C.c_int32, C.c_uint32, C.c_void_p]),
     "pulse_normalize_to_bf16": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                           C.c_void_p, C.c_int64, C.c_float, C.c_void_p]),

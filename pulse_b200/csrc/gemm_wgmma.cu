@@ -7,7 +7,8 @@
 //   wgrad     dW = dY^T X                    A = dY [M,N] MN-major,  B = X  [M,K] MN-major   (reduction over the batch rows)
 // Operands are read as they sit in memory: the wgmma transpose bits select K-major or MN-major, nothing is transposed.
 //
-// Structure (persistent: one CTA per SM loops over 128 x 128 output tiles x split-K slices):
+// Structure (persistent: one CTA per SM loops over 128 x 128 output tiles x split-K slices; 128 x 256 tiles with m64n256k16 where
+// gemm_tile_n picks them):
 //   warp 0       TMA producer: cp.async.bulk.tensor 2D loads (128B swizzle) into a shared-memory ring that runs continuously
 //                across work items, completion on "full" mbarriers (4 stages; 6, or 5 with a pre-activation, where the epilogue is
 //                register-resident: see GemmSmem);
@@ -34,16 +35,19 @@ namespace {
 #ifndef PULSE_GEMM_VARIANT
 #define PULSE_GEMM_VARIANT 0   // 0 = product; 3 = phase-trace build for tools/gemm_trace.py (tools/build_variant.sh trace gemm_wgmma.cu -DPULSE_GEMM_VARIANT=3)
 #endif
-constexpr int BM = 128, BN = 128, BK = 64, MMA_K = 16;
+constexpr int BM = 128, BK = 64, MMA_K = 16;
+constexpr int kNarrowBN = 128, kWideBN = 256;   // output tile widths (BN, a template parameter of the kernels); see gemm_tile_n
 constexpr int kConsumerWarps = 8;                 // two warpgroups
 constexpr int kThreads = 128 + 32 * kConsumerWarps;   // producer warpgroup (one warp issues, three idle) + consumers
 // Each consumer warp drains 32 rows x kCols columns of its warpgroup's 64 x 128 accumulator in 32-column chunks.
 constexpr int kCols = 64;
 constexpr int kChunks = kCols / 32;
-constexpr int kStages = 4;   // ring depth of the instantiations that can take the staged epilogue
+constexpr int kStages = 4;   // ring depth of the instantiations that can take the staged epilogue, and of the wide ones
 constexpr int kTmaOutF32 = 2;   // tma_out of a plain fp32 output through the register-resident epilogue (deep-ring kernels only)
 constexpr unsigned kStageBytesA = BM * BK * 2;
-constexpr unsigned kStageBytesB = BN * BK * 2;
+// registers per thread of the wide kernels after setmaxnreg: the producer warpgroup gives up what the consumers' 64 x 256 fp32
+// fragments (128 registers) need; 128 x (40 + 2 x 232) = 64 512 = 384 threads x 168, the launch's allocation
+constexpr int kWideProducerRegs = 40, kWideConsumerRegs = 232;
 
 // Shared memory of an instantiation with an S-stage operand ring.  The consumers hold up to two stages, so a 4-stage ring gives the
 // producer two stages of lead; the update's short-K items (8-16 k-blocks) wait on operand loads for a quarter of their main loop,
@@ -52,10 +56,10 @@ constexpr unsigned kStageBytesB = BN * BK * 2;
 // (32 KB with the pre-activation), not the staged path's fp32 tile and per-warp tiles.  So the instantiations that may take the
 // staged path keep kStages (the specialisation below), and the register-epilogue-only ones give that room to the ring: 6 stages,
 // or 5 when the pre-activation boxes need the second 16 KB.
-template <int S>
+template <int S, int BN>
 struct __align__(1024) GemmSmem {
   unsigned char a[S][kStageBytesA];
-  unsigned char b[S][kStageBytesB];
+  unsigned char b[S][BN * BK * 2];
   unsigned char epi[2][S >= 6 ? 16384 : 32768];   // per consumer warpgroup: output boxes [0, 16 KB), pre-activation boxes [16, 32 KB);
                                                  // or one 64-column half of a plain fp32 output at a time
   float bias[2][BN];                             // per-warpgroup copy of the tile's bias
@@ -63,21 +67,34 @@ struct __align__(1024) GemmSmem {
   unsigned long long empty[S];
 };
 template <>
-struct __align__(1024) GemmSmem<kStages> {
+struct __align__(1024) GemmSmem<kStages, kNarrowBN> {
   unsigned char a[kStages][kStageBytesA];
-  unsigned char b[kStages][kStageBytesB];
-  float epi[2][64 * BN];                   // per consumer warpgroup: 2 x 4 blocks of 32 x 32 fp32, 128-byte swizzled (4 KB each), or
+  unsigned char b[kStages][kNarrowBN * BK * 2];
+  float epi[2][64 * kNarrowBN];            // per consumer warpgroup: 2 x 4 blocks of 32 x 32 fp32, 128-byte swizzled (4 KB each), or
                                            // (register-resident epilogue) 2 + 2 bf16 boxes of 64 x 64 for the output / pre-activation stores
   float red[kConsumerWarps][16 * 33];      // per-warp tile: bf16 store staging / fp32 transpose for atomics
-  float bias[2][BN];                       // per-warpgroup copy of the tile's bias (register-resident forward epilogue)
+  float bias[2][kNarrowBN];                // per-warpgroup copy of the tile's bias (register-resident forward epilogue)
+  unsigned long long full[kStages];
+  unsigned long long empty[kStages];
+};
+// 128 x 256 tiles (register-resident bf16 epilogue without a pre-activation): 4 stages of 16 KB A + 32 KB B (4 x 1024 clocks of
+// tensor-core work in flight, as many clocks as the narrow 6-stage ring).  Each warpgroup drains its 64 x 256 fragment in two
+// 128-column halves through its 16 KB area, as the narrow kernels drain their one.  No room is left for a shared bias copy: the
+// wide epilogue reads the bias from global memory.
+template <>
+struct __align__(1024) GemmSmem<kStages, kWideBN> {
+  unsigned char a[kStages][kStageBytesA];
+  unsigned char b[kStages][kWideBN * BK * 2];
+  unsigned char epi[2][16384];
   unsigned long long full[kStages];
   unsigned long long empty[kStages];
 };
 // dynamic shared memory of a launch: 1 KB of slack so the kernel can align the ring to 1024 B
-template <int S>
-constexpr size_t smem_bytes() { return sizeof(GemmSmem<S>) + 1024; }
+template <int S, int BN>
+constexpr size_t smem_bytes() { return sizeof(GemmSmem<S, BN>) + 1024; }
 constexpr size_t kSmemOptin = 232448;   // sm_90 opt-in limit of dynamic shared memory per block (227 KB)
-static_assert(smem_bytes<kStages>() <= kSmemOptin && smem_bytes<5>() <= kSmemOptin && smem_bytes<6>() <= kSmemOptin,
+static_assert(smem_bytes<kStages, kNarrowBN>() <= kSmemOptin && smem_bytes<5, kNarrowBN>() <= kSmemOptin && smem_bytes<6, kNarrowBN>() <= kSmemOptin &&
+                  smem_bytes<kStages, kWideBN>() <= kSmemOptin,
               "GEMM shared-memory layout exceeds the per-block opt-in limit");
 
 __device__ __forceinline__ unsigned s_u32(const void* p) { return static_cast<unsigned>(__cvta_generic_to_shared(p)); }
@@ -156,9 +173,10 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
 // keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
-__device__ __forceinline__ void acc_fence(float (&d)[64]) {
+template <int NF>
+__device__ __forceinline__ void acc_fence(float (&d)[NF]) {
 #pragma unroll
-  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+  for (int i = 0; i < NF; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 // D[64 x 128] (+)= A[64 x 16] B[16 x 128]; TA / TB = 1: operand is MN-major in shared memory
 template <int TA, int TB>
@@ -179,6 +197,39 @@ __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], unsigned long long
         "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
         "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
         "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB)
+      : "memory");
+}
+// D[64 x 256] (+)= A[64 x 16] B[16 x 256]: the wide tile's MMA (the fragment's columns 0..127 are d[0..63], 128..255 are d[64..127])
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n256(float (&d)[128], unsigned long long da, unsigned long long db, unsigned accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, "
+      "%27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, "
+      "%52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, "
+      "%77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, "
+      "%101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, "
+      "%121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, %131, %132;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
       : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB)
       : "memory");
 }
@@ -277,20 +328,21 @@ __device__ __forceinline__ __nv_bfloat162 silu_bf16x2(__nv_bfloat162 z) {
   return __floats2bfloat162_rn(f.x, f.y);
 }
 
-// Register-resident epilogue: the warpgroup's 64 x 128 fp32 fragment -> bf16 pairs -> stmatrix into the output boxes at `stage`
-// ([0, 16 KB): two 64 x 64 boxes, 128-byte swizzle, row r = 8 16-byte units, unit u at u ^ (r & 7)) and, when `pre`, the rounded
-// pre-activation into the same layout at +16 KB.  ACT runs on the rounded pair (exact for ReLU, which commutes with the rounding); a
-// SiLU column group that reaches past N applies it in fp32 before the one rounding, as the staged epilogue does.
+// Register-resident epilogue: 128 columns of the warpgroup's fp32 fragment (d[0..63], columns n0 + 8 j + 2 (lane & 3) + {0, 1}) -> bf16
+// pairs -> stmatrix into the output boxes at `stage` ([0, 16 KB): two 64 x 64 boxes, 128-byte swizzle, row r = 8 16-byte units, unit u
+// at u ^ (r & 7)) and, when `pre`, the rounded pre-activation into the same layout at +16 KB.  ACT runs on the rounded pair (exact for
+// ReLU, which commutes with the rounding); a SiLU column group that reaches past N applies it in fp32 before the one rounding, as the
+// staged epilogue does.
 // stmatrix x4 at even j: matrices (j, rows r0), (j, r0 + 8), (j + 1, r0), (j + 1, r0 + 8); lane l gives the address of row l % 8 of
 // matrix l / 8.
 template <int ACT>
-__device__ __forceinline__ void stage_tile_bf16(const float (&d)[64], unsigned stage, bool pre, int n0, int N) {
+__device__ __forceinline__ void stage_tile_bf16(const float* d, unsigned stage, bool pre, int n0, int N) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const unsigned srow = stage + ((warp & 3) * 16 + ((lane >> 3) & 1) * 8 + (lane & 7)) * 128;
   const int sj = lane >> 4;
   const __nv_bfloat162 zero2 = __float2bfloat162_rn(0.0f);
 #pragma unroll
-  for (int j = 0; j < BN / 8; j += 2) {
+  for (int j = 0; j < kNarrowBN / 8; j += 2) {
     const bool full_half = n0 + 64 * (j >> 3) + 64 <= N;
     unsigned o[4], p[4];
 #pragma unroll
@@ -459,6 +511,29 @@ int ring_stages(bool reg_epi, bool preact) {
   return (!reg_epi || force4) ? kStages : preact ? 5 : 6;
 }
 
+// Output tile width of an m x n GEMM whose work items run kb_per_item k-blocks, split-K `splits`, on `sms` persistent CTAs.  A
+// 128 x 256 k-block moves 48 KB into shared memory for 1024 tensor-core clocks, a quarter fewer bytes per MMA clock than the 32 KB /
+// 512 clocks of a 128 x 128 one, and the narrow main loops are bound by that operand stream (DESIGN.md section 3.3).  The wide tile is
+// taken where it does not cost a round: twice the work per item, so 2 x its rounds must not exceed the narrow rounds (an M = 12288,
+// N = 512 GEMM has 192 wide items, 2 rounds, against 384 narrow ones, 3 rounds).  Items of fewer than kWideMinKb k-blocks are mostly
+// epilogue and ring fill, which the wide tile does not shorten.
+constexpr int kWideMinKb = 4;
+int gemm_tile_n(long long m, long long n, int kb_per_item, int splits, int sms) {
+  if (n < kWideBN || kb_per_item < kWideMinKb || sms < 1) return kNarrowBN;
+  const long long tm = (m + BM - 1) / BM;
+  const long long rounds_narrow = (tm * ((n + kNarrowBN - 1) / kNarrowBN) * splits + sms - 1) / sms;
+  const long long rounds_wide = (tm * ((n + kWideBN - 1) / kWideBN) * splits + sms - 1) / sms;
+  return 2 * rounds_wide <= rounds_narrow ? kWideBN : kNarrowBN;
+}
+
+// PULSE_GEMM_BN=128 keeps every launch on the 128 x 128 tile (to compare both widths in one process; read at every launch).  The
+// default is always the shape rule above.
+bool narrow_forced() {
+  const char* e = getenv("PULSE_GEMM_BN");
+  return e != nullptr && atoi(e) == kNarrowBN;
+}
+int g_last_tile_n = 0;   // tile width of the last GEMM launch issued from the host (pulse_gemm_last_tile_n)
+
 // sets the kernel's dynamic shared-memory size once per instantiation and checks it against the device's opt-in limit
 template <typename Kernel>
 int set_smem_once(Kernel kernel, size_t bytes, bool* done) {
@@ -473,11 +548,11 @@ int set_smem_once(Kernel kernel, size_t bytes, bool* done) {
   return PULSE_OK;
 }
 
-template <bool A_MN, bool B_MN, int MODE, int S>
+template <bool A_MN, bool B_MN, int MODE, int S, int BN>
 int launch_gemm_ring(const CUtensorMap& map_a, const CUtensorMap& map_b, const CUtensorMap& map_c, const CUtensorMap& map_p,
                      const pulse_gemm_epilogue_t& ep, int m, int n, int k, int splits, int kb_per_split, int tma_out, cudaStream_t stream) {
   static bool attr_set = false;
-  const int rc = set_smem_once(gemm_bf16_kernel<A_MN, B_MN, MODE, S>, smem_bytes<S>(), &attr_set);
+  const int rc = set_smem_once(gemm_bf16_kernel<A_MN, B_MN, MODE, S, BN>, smem_bytes<S, BN>(), &attr_set);
   if (rc != PULSE_OK) return rc;
   const int num_sms = gemm_num_sms(true);
   PULSE_REQUIRE(num_sms > 0, "pulse_gemm_bf16: cannot query the device's SM count");
@@ -492,7 +567,7 @@ int launch_gemm_ring(const CUtensorMap& map_a, const CUtensorMap& map_b, const C
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid, 1, 1);
   cfg.blockDim = dim3(kThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem_bytes<S>();
+  cfg.dynamicSmemBytes = smem_bytes<S, BN>();
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   int na = 0;
@@ -503,14 +578,16 @@ int launch_gemm_ring(const CUtensorMap& map_a, const CUtensorMap& map_b, const C
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
-  PULSE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_kernel<A_MN, B_MN, MODE, S>, map_a, map_b, map_c, map_p, ep, m, n, k, kb_per_split, splits, tma_out));
+  PULSE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_kernel<A_MN, B_MN, MODE, S, BN>, map_a, map_b, map_c, map_p, ep, m, n, k, kb_per_split, splits, tma_out));
   PULSE_LAUNCH_OK("gemm_bf16_kernel");
+  g_last_tile_n = BN;
   return PULSE_OK;
 }
 
+// b / ldb: the B operand, for the wide tile's map (a K-major B box spans the tile's BN rows)
 template <bool A_MN, bool B_MN, int MODE>
-int launch_gemm(const CUtensorMap& map_a, const CUtensorMap& map_b, const pulse_gemm_epilogue_t& ep, int m, int n, int k, int splits,
-                int kb_per_split, cudaStream_t stream) {
+int launch_gemm(const CUtensorMap& map_a, const CUtensorMap& map_b, const void* b, long long ldb, const pulse_gemm_epilogue_t& ep, int m, int n,
+                int k, int splits, int kb_per_split, cudaStream_t stream) {
   CUtensorMap map_c, map_p;
   int tma_out = 0;
   const int rc = epilogue_maps(MODE, ep, m, n, splits, &map_c, &map_p, &tma_out);
@@ -518,18 +595,30 @@ int launch_gemm(const CUtensorMap& map_a, const CUtensorMap& map_b, const pulse_
   if constexpr (MODE == kModeFwd || MODE == kModeDgrad) {
     const int s = ring_stages(tma_out != 0, ep.preact != nullptr);
     if (s == kStages && tma_out == kTmaOutF32) tma_out = 0;
-    if (s == 6) return launch_gemm_ring<A_MN, B_MN, MODE, 6>(map_a, map_b, map_c, map_p, ep, m, n, k, splits, kb_per_split, tma_out, stream);
+    if constexpr (!A_MN) {   // A MN-major is a weight gradient: those keep the narrow tile
+      // wide: the bf16 register-resident epilogue without a pre-activation (the 16 KB areas hold no pre-activation boxes)
+      if (s != kStages && tma_out == 1 && ep.preact == nullptr && !narrow_forced() &&
+          gemm_tile_n(m, n, kb_per_split, splits, gemm_num_sms(true)) == kWideBN) {
+        CUtensorMap map_bw = map_b;
+        if (!B_MN && !make_map(&map_bw, b, n, k, ldb, kWideBN)) {
+          set_error("pulse_gemm_bf16: cuTensorMapEncodeTiled failed for the wide B operand");
+          return PULSE_ERR_CUDA;
+        }
+        return launch_gemm_ring<A_MN, B_MN, MODE, kStages, kWideBN>(map_a, map_bw, map_c, map_p, ep, m, n, k, splits, kb_per_split, tma_out, stream);
+      }
+    }
+    if (s == 6) return launch_gemm_ring<A_MN, B_MN, MODE, 6, kNarrowBN>(map_a, map_b, map_c, map_p, ep, m, n, k, splits, kb_per_split, tma_out, stream);
     if constexpr (MODE == kModeFwd) {   // only the forward epilogue writes a pre-activation
-      if (s == 5) return launch_gemm_ring<A_MN, B_MN, MODE, 5>(map_a, map_b, map_c, map_p, ep, m, n, k, splits, kb_per_split, tma_out, stream);
+      if (s == 5) return launch_gemm_ring<A_MN, B_MN, MODE, 5, kNarrowBN>(map_a, map_b, map_c, map_p, ep, m, n, k, splits, kb_per_split, tma_out, stream);
     }
   }
-  return launch_gemm_ring<A_MN, B_MN, MODE, kStages>(map_a, map_b, map_c, map_p, ep, m, n, k, splits, kb_per_split, tma_out, stream);
+  return launch_gemm_ring<A_MN, B_MN, MODE, kStages, kNarrowBN>(map_a, map_b, map_c, map_p, ep, m, n, k, splits, kb_per_split, tma_out, stream);
 }
 
 template <bool A_MN, bool B_MN, int MODE, int S>
 int launch_gemm_grouped(const GemmGroup& grp, cudaStream_t stream) {
   static bool attr_set = false;
-  const int rc = set_smem_once(gemm_bf16_grouped_kernel<A_MN, B_MN, MODE, S>, smem_bytes<S>(), &attr_set);
+  const int rc = set_smem_once(gemm_bf16_grouped_kernel<A_MN, B_MN, MODE, S, kNarrowBN>, smem_bytes<S, kNarrowBN>(), &attr_set);
   if (rc != PULSE_OK) return rc;
   const int num_sms = gemm_num_sms(false);
   PULSE_REQUIRE(num_sms > 0, "pulse_gemm_bf16_grouped: cannot query the device's SM count");
@@ -537,15 +626,16 @@ int launch_gemm_grouped(const GemmGroup& grp, cudaStream_t stream) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid, 1, 1);
   cfg.blockDim = dim3(kThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem_bytes<S>();
+  cfg.dynamicSmemBytes = smem_bytes<S, kNarrowBN>();
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  PULSE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_grouped_kernel<A_MN, B_MN, MODE, S>, grp));
+  PULSE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_grouped_kernel<A_MN, B_MN, MODE, S, kNarrowBN>, grp));
   PULSE_LAUNCH_OK("gemm_bf16_grouped_kernel");
+  g_last_tile_n = kNarrowBN;
   return PULSE_OK;
 }
 
@@ -575,6 +665,17 @@ extern "C" int pulse_gemm_num_splits(int64_t k, int32_t split_k) {
   return (num_kb + kb_per_split - 1) / kb_per_split;  // every slab gets at least one k-block
 }
 
+// the shape rule alone (gemm_tile_n): the width it picks for an m x n x k GEMM with split_k on `sms` SMs.  A launch takes it only where a
+// wide instantiation applies (see launch_gemm); pulse_gemm_last_tile_n reports what a launch took.
+extern "C" int pulse_gemm_tile_n(int64_t m, int64_t n, int64_t k, int32_t split_k, int32_t sms) {
+  const int num_kb = static_cast<int>((k + 63) / 64);
+  const int splits = pulse_gemm_num_splits(k, split_k);
+  return pulse::gemm_tile_n(m, n, (num_kb + splits - 1) / splits, splits, sms);
+}
+
+// output tile width (128 or 256) of the last GEMM launch issued from the host; 0 before the first
+extern "C" int pulse_gemm_last_tile_n(void) { return pulse::g_last_tile_n; }
+
 // flags: bit 0 = A is MN-major ([K, M] row-major in memory), bit 1 = B is MN-major ([K, N] row-major in memory)
 extern "C" int pulse_gemm_bf16(const void* a, int64_t lda, const void* b, int64_t ldb, int64_t m, int64_t n, int64_t k,
                                const pulse_gemm_epilogue_t* ep, int32_t split_k, uint32_t flags, void* stream) {
@@ -598,7 +699,7 @@ extern "C" int pulse_gemm_bf16(const void* a, int64_t lda, const void* b, int64_
   PULSE_REQUIRE(!(ep->gate_mask && ep->gate), "pulse_gemm_bf16: give the ReLU gate either as bf16 activations or as bit words, not both");
   CUtensorMap map_a, map_b;
   const bool ok_a = a_mn ? make_map(&map_a, a, k, m, lda, 64) : make_map(&map_a, a, m, k, lda, BM);
-  const bool ok_b = b_mn ? make_map(&map_b, b, k, n, ldb, 64) : make_map(&map_b, b, n, k, ldb, BN);
+  const bool ok_b = b_mn ? make_map(&map_b, b, k, n, ldb, 64) : make_map(&map_b, b, n, k, ldb, kNarrowBN);
   if (!ok_a || !ok_b) {
     set_error("pulse_gemm_bf16: cuTensorMapEncodeTiled failed (driver entry point missing or bad strides)");
     return PULSE_ERR_CUDA;
@@ -610,13 +711,13 @@ extern "C" int pulse_gemm_bf16(const void* a, int64_t lda, const void* b, int64_
   // smallest epilogue specialisation that covers the request (see the MODE comment on the kernel)
   const int mode = epilogue_mode(ep);
   const int mi = (int)m, ni = (int)n, ki = (int)k;
-#define PULSE_GEMM_DISPATCH(AM, BM_)                                                                                        \
-  switch (mode) {                                                                                                           \
-    case kModeFwd: return launch_gemm<AM, BM_, kModeFwd>(map_a, map_b, *ep, mi, ni, ki, splits, kb_per_split, st);             \
-    case kModeDgrad: return launch_gemm<AM, BM_, kModeDgrad>(map_a, map_b, *ep, mi, ni, ki, splits, kb_per_split, st);         \
-    case kModeWgrad: return launch_gemm<AM, BM_, kModeWgrad>(map_a, map_b, *ep, mi, ni, ki, splits, kb_per_split, st);         \
-    case kModeDgradVec: return launch_gemm<AM, BM_, kModeDgradVec>(map_a, map_b, *ep, mi, ni, ki, splits, kb_per_split, st);   \
-    default: return launch_gemm<AM, BM_, kModeGeneric>(map_a, map_b, *ep, mi, ni, ki, splits, kb_per_split, st);               \
+#define PULSE_GEMM_DISPATCH(AM, BM_)                                                                                                 \
+  switch (mode) {                                                                                                                    \
+    case kModeFwd: return launch_gemm<AM, BM_, kModeFwd>(map_a, map_b, b, ldb, *ep, mi, ni, ki, splits, kb_per_split, st);           \
+    case kModeDgrad: return launch_gemm<AM, BM_, kModeDgrad>(map_a, map_b, b, ldb, *ep, mi, ni, ki, splits, kb_per_split, st);       \
+    case kModeWgrad: return launch_gemm<AM, BM_, kModeWgrad>(map_a, map_b, b, ldb, *ep, mi, ni, ki, splits, kb_per_split, st);       \
+    case kModeDgradVec: return launch_gemm<AM, BM_, kModeDgradVec>(map_a, map_b, b, ldb, *ep, mi, ni, ki, splits, kb_per_split, st); \
+    default: return launch_gemm<AM, BM_, kModeGeneric>(map_a, map_b, b, ldb, *ep, mi, ni, ki, splits, kb_per_split, st);             \
   }
   if (a_mn && b_mn) { PULSE_GEMM_DISPATCH(true, true) }
   if (a_mn) { PULSE_GEMM_DISPATCH(true, false) }
@@ -667,7 +768,7 @@ extern "C" int pulse_gemm_bf16_grouped(const pulse_gemm_problem_t* problems, int
     const pulse_gemm_problem_t& q = problems[i];
     GemmProblem& g = grp.p[i];
     const bool ok_a = a_mn ? make_map(&g.map_a, q.a, q.k, q.m, q.lda, 64) : make_map(&g.map_a, q.a, q.m, q.k, q.lda, BM);
-    const bool ok_b = b_mn ? make_map(&g.map_b, q.b, q.k, q.n, q.ldb, 64) : make_map(&g.map_b, q.b, q.n, q.k, q.ldb, BN);
+    const bool ok_b = b_mn ? make_map(&g.map_b, q.b, q.k, q.n, q.ldb, 64) : make_map(&g.map_b, q.b, q.n, q.k, q.ldb, kNarrowBN);
     if (!ok_a || !ok_b) {
       set_error("pulse_gemm_bf16_grouped: cuTensorMapEncodeTiled failed for problem %d", i);
       return PULSE_ERR_CUDA;
@@ -681,7 +782,7 @@ extern "C" int pulse_gemm_bf16_grouped(const pulse_gemm_problem_t* problems, int
     const int num_kb = static_cast<int>((q.k + BK - 1) / BK);
     const int splits = pulse_gemm_num_splits(q.k, q.split_k);
     g.kb_per_split = (num_kb + splits - 1) / splits;
-    items += static_cast<long long>((q.n + BN - 1) / BN) * ((q.m + BM - 1) / BM) * splits;
+    items += static_cast<long long>((q.n + kNarrowBN - 1) / kNarrowBN) * ((q.m + BM - 1) / BM) * splits;
     PULSE_REQUIRE(items < (1ll << 30), "pulse_gemm_bf16_grouped: too many work items");
     g.item_end = static_cast<int>(items);
   }

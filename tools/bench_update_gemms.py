@@ -1,4 +1,5 @@
-"""Every GEMM of one PPO + discriminator minibatch update, timed alone (CUDA events, warm L2), with its tensor / HBM floor.
+"""Every GEMM of one PPO + discriminator minibatch update, timed alone (CUDA events, warm L2), with its tensor / HBM floor, at the tile
+width the shape rule picks and with the 128 x 128 tile forced (PULSE_GEMM_BN=128).
 The epilogue arguments are the ones the update passes: the nets are bias-augmented (no bias vector, no column sums), the forward
 layers write ReLU mask words and the input-gradient GEMMs are gated by them.
 
@@ -101,10 +102,13 @@ def main():
             kw.update(colsum=torch.zeros(Np, device=dev))
         if alpha != 1.0:
             kw.update(alpha=alpha)
+        os.environ["PULSE_GEMM_BN"] = "128"   # the 128 x 128 tile, then the width the shape rule picks
+        us128 = timed(lambda: gemm(av, bv, **kw))
+        del os.environ["PULSE_GEMM_BN"]
         us = timed(lambda: gemm(av, bv, **kw))
         fl = 2.0 * M * N * K
         floor = max(fl / peaks["bf16"] / 1e6, byt / peaks["hbm"] / 1e3)
-        rows.append({"name": name, "M": M, "N": N, "K": K, "kind": kind, "us": round(us, 2), "tflops": round(fl / us / 1e6, 1),
+        rows.append({"name": name, "M": M, "N": N, "K": K, "kind": kind, "us": round(us, 2), "us_bn128": round(us128, 2), "tflops": round(fl / us / 1e6, 1),
                      "gbs": round(byt / us / 1e3, 1), "floor_us": round(floor, 2), "eff": round(floor / us, 3)})
 
     B, Bd, Bg = 16384, 12288, 4096
@@ -144,9 +148,9 @@ def main():
     nonvae("gp.dw3", Bg, 512, 1024, "nt", gate="mask", f32=True, bf16_out=False)
     tot, fl = sum(r["us"] for r in rows), sum(r["floor_us"] for r in rows)
     for r in rows:
-        print(f"{r['name']:18s} {r['kind']:5s} M={r['M']:6d} N={r['N']:5d} K={r['K']:6d}  {r['us']:8.2f} us  {r['tflops']:7.1f} TF  "
+        print(f"{r['name']:18s} {r['kind']:5s} M={r['M']:6d} N={r['N']:5d} K={r['K']:6d}  {r['us']:8.2f} us (128 x 128: {r['us_bn128']:8.2f})  {r['tflops']:7.1f} TF  "
               f"{r['gbs']:7.1f} GB/s  floor {r['floor_us']:7.2f} us  eff {r['eff']:.2f}")
-    print(f"sum {tot:.1f} us, floor {fl:.1f} us, eff {fl / tot:.3f}")
+    print(f"sum {tot:.1f} us (128 x 128 tiles: {sum(r['us_bn128'] for r in rows):.1f} us), floor {fl:.1f} us, eff {fl / tot:.3f}")
     if a.json:
         json.dump({"peaks": peaks, "cases": rows, "sum_us": tot, "floor_us": fl}, open(a.json, "w"), indent=1)
 
