@@ -287,6 +287,68 @@ typedef struct {
 int pulse_reset_ref_state(const pulse_motionlib_t* lib, const pulse_reset_args_t* args, int64_t num_envs, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Getup reset of HumanoidImGetup on the device, free of host synchronisation.  For the reset set of `base` (mask or id list), in
+ * the order of HumanoidImGetup._reset_actors (phc/env/tasks/humanoid_im_getup.py:135-182):
+ *   1. every reset env releases its current assignment: available_fall_states[fall_id_assignments[env]] = 0, stale or not;
+ *   2. recovery envs (draw < recovery_prob and terminate_buf == 1, read before anything clears it): recovery_counter <- recovery_steps,
+ *      actor state, motion id and start time kept (_reset_recovery_episode :164-166);
+ *   3. fall envs (the others whose draw < fall_prob): k distinct free states, the one with the i-th smallest key to the i-th fall env in
+ *      ascending env order (the distribution of randperm(available)[:k]); root / dof position / dof velocity copied from the fall pool,
+ *      recovery_counter <- recovery_steps, the state marked held and assigned (_reset_fall_episode :168-182).  Where the reference
+ *      asserts (fewer free states than fall envs) the surplus fall envs, the last in env order, take a reference-state episode
+ *      instead and *error grows by their number;
+ *   4. reference-state envs: pulse_reset_ref_state's start-time draw, MotionLib gather, scatter and AMP back-fill; recovery_counter <- 0;
+ *   5. every reset env: progress / reset / terminate and its contact-force rows <- 0; the int32 actor-id list (_reset_env_tensors,
+ *      humanoid.py:589-609), recovery envs included.
+ * Draws: injected per env (recovery_u, fall_u: u < p succeeds) and per fall state (fall_keys, >= 0), or Philox4x32-10 on
+ * (seed, index, offset + *offset_dev) of `base`: words 1 / 2 of env e's block are its recovery / fall draws, word 3 of state s's block
+ * its key, so none of them meets the start-time draw (word 0 of env e's block).
+ * The AMP history of fall and recovery envs depends on the state after the simulator's refresh: pulse_getup_amp_init, run after it.
+ * ---------------------------------------------------------------------------------------------- */
+#define PULSE_GETUP_REF 1
+#define PULSE_GETUP_FALL 2
+#define PULSE_GETUP_RECOVERY 3
+
+typedef struct {
+  pulse_reset_args_t base;       /* reset set, reference-state buffers, and the UNION of the reset envs in env_list / actor_list / count */
+  const float* recovery_u;       /* [N] uniform draw per env, or NULL: Philox */
+  const float* fall_u;           /* [N] uniform draw per env, or NULL: Philox */
+  const float* fall_keys;        /* [P] non-negative key per fall state, or NULL: Philox */
+  float recovery_prob;           /* _recovery_episode_prob */
+  float fall_prob;               /* _fall_init_prob */
+  int32_t recovery_steps;        /* _recovery_steps */
+  int32_t reserved;
+  int32_t* recovery_counter;     /* [N] _recovery_counter */
+  int64_t* available_fall_states;/* [P] availalbe_fall_states: 0 free, 1 held */
+  int64_t* fall_id_assignments;  /* [N] */
+  const float* fall_root_states; int64_t fall_root_stride;       /* [P, >= 13] _fall_root_states */
+  const float* fall_dof_pos; const float* fall_dof_vel;          /* [P, 69] _fall_dof_pos / _fall_dof_vel (shared strides) */
+  int64_t fall_dof_env_stride; int64_t fall_dof_elem_stride;
+  int64_t num_fall_states;       /* P */
+  int64_t* ref_list;             /* [N] out: reference-state envs, ascending */
+  int64_t* fall_list;            /* [N] out: fall envs, ascending */
+  int64_t* recovery_list;        /* [N] out: recovery envs, ascending */
+  int32_t* class_counts;         /* [3] out, device side: number of reference-state, fall and recovery envs */
+  uint8_t* env_class;            /* [N] out, optional: PULSE_GETUP_* of every reset env (other envs untouched) */
+  int32_t* error;                /* [1] in/out: += fall envs that found no free state (never cleared by the library) */
+  int64_t* fall_pick;            /* [N] scratch: fall state of the i-th fall env */
+  uint64_t* fall_key_scratch;    /* [P] scratch: (key, state) sort keys */
+} pulse_getup_reset_args_t;
+int pulse_reset_getup(const pulse_motionlib_t* lib, const pulse_getup_reset_args_t* args, int64_t num_envs, void* stream);
+
+/* The AMP history of the fall and recovery envs of the last pulse_reset_getup, from the simulator state after the refresh
+ * (humanoid_amp.py:519-533, humanoid_im_getup.py:190-196): fall envs get the current AMP observation in every row
+ * (_init_amp_obs_default), recovery envs in row 0 only.  Lists and counts are pulse_reset_getup's outputs; num_envs bounds them. */
+typedef struct {
+  const float* body_state; int64_t body_env_stride;
+  const float* dof_pos; const float* dof_vel; int64_t dof_env_stride; int64_t dof_elem_stride;
+  float* amp_obs_buf;            /* [N, num_steps, 196] */
+  int32_t num_steps; int32_t reserved;
+  const int64_t* fall_list; const int64_t* recovery_list; const int32_t* class_counts;
+} pulse_getup_amp_args_t;
+int pulse_getup_amp_init(const pulse_getup_amp_args_t* args, int64_t num_envs, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * GAE / returns.  CommonAgent.discount_values  phc/learning/common_agent.py:493-505, mb_returns =
  * mb_advs + mb_values (amp_agent.py:427), and the first half of _calc_advs (:589-599): sums for the
  * advantage mean / unbiased std.  Inputs are [T,N] time-major as in the rl_games ExperienceBuffer;

@@ -72,6 +72,26 @@ class ResetArgs(C.Structure):
     ]
 
 
+class GetupResetArgs(C.Structure):
+    _fields_ = [
+        ("base", ResetArgs), ("recovery_u", C.c_void_p), ("fall_u", C.c_void_p), ("fall_keys", C.c_void_p),
+        ("recovery_prob", C.c_float), ("fall_prob", C.c_float), ("recovery_steps", C.c_int32), ("reserved", C.c_int32),
+        ("recovery_counter", C.c_void_p), ("available_fall_states", C.c_void_p), ("fall_id_assignments", C.c_void_p),
+        ("fall_root_states", C.c_void_p), ("fall_root_stride", C.c_int64), ("fall_dof_pos", C.c_void_p), ("fall_dof_vel", C.c_void_p),
+        ("fall_dof_env_stride", C.c_int64), ("fall_dof_elem_stride", C.c_int64), ("num_fall_states", C.c_int64),
+        ("ref_list", C.c_void_p), ("fall_list", C.c_void_p), ("recovery_list", C.c_void_p), ("class_counts", C.c_void_p),
+        ("env_class", C.c_void_p), ("error", C.c_void_p), ("fall_pick", C.c_void_p), ("fall_key_scratch", C.c_void_p),
+    ]
+
+
+class GetupAmpArgs(C.Structure):
+    _fields_ = [
+        ("body_state", C.c_void_p), ("body_env_stride", C.c_int64), ("dof_pos", C.c_void_p), ("dof_vel", C.c_void_p),
+        ("dof_env_stride", C.c_int64), ("dof_elem_stride", C.c_int64), ("amp_obs_buf", C.c_void_p), ("num_steps", C.c_int32),
+        ("reserved", C.c_int32), ("fall_list", C.c_void_p), ("recovery_list", C.c_void_p), ("class_counts", C.c_void_p),
+    ]
+
+
 class WeightBlock(C.Structure):
     _fields_ = [("w", C.c_void_p), ("g", C.c_void_p), ("rows", C.c_int64), ("cols", C.c_int64), ("ld", C.c_int64), ("coef", C.c_float),
                 ("reserved", C.c_int32), ("sumsq", C.c_void_p), ("sumsq2", C.c_void_p)]
@@ -271,6 +291,7 @@ HEAD1_MAX_CTAS = 264        # PULSE_HEAD1_MAX_CTAS: rows of the pulse_head1_back
 ACT_NONE, ACT_RELU, ACT_SILU = 0, 1, 2
 Z_SAMPLE, Z_MEAN, Z_RESIDUAL = 0, 1, 2
 STEP_REWARD, STEP_RESET, STEP_OBS, STEP_ALL, STEP_ADVANCE = 1, 2, 4, 7, 8
+GETUP_REF, GETUP_FALL, GETUP_RECOVERY = 1, 2, 3
 
 # name -> (restype, argtypes); mirrors include/pulse_b200.h one to one
 SIGNATURES = {
@@ -282,6 +303,8 @@ SIGNATURES = {
     "pulse_motion_state": (C.c_int, [C.c_void_p, C.POINTER(MotionQuery), C.c_int64, C.c_void_p]),
     "pulse_im_step": (C.c_int, [C.c_void_p, C.POINTER(ImStepArgs), C.c_int64, C.c_void_p]),
     "pulse_reset_ref_state": (C.c_int, [C.c_void_p, C.POINTER(ResetArgs), C.c_int64, C.c_void_p]),
+    "pulse_reset_getup": (C.c_int, [C.c_void_p, C.POINTER(GetupResetArgs), C.c_int64, C.c_void_p]),
+    "pulse_getup_amp_init": (C.c_int, [C.POINTER(GetupAmpArgs), C.c_int64, C.c_void_p]),
     "pulse_policy_post": (C.c_int, [C.POINTER(PolicyPostArgs), C.c_int64, C.c_void_p]),
     "pulse_value_post": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
     "pulse_amp_obs_row": (C.c_int, [C.POINTER(AmpRowArgs), C.c_int64, C.c_void_p]),

@@ -6,7 +6,8 @@ Two layers:
   * `HumanoidImCompute` -- explicit-tensor API (what bench.py, the tests and the mixin call);
   * `HumanoidImB200Mixin` -- drop-in overrides with the reference's method names, to be mixed in
     front of `phc.env.tasks.humanoid_im.HumanoidIm` (see INTEGRATION.md); Isaac Gym keeps doing the
-    physics and owns the state tensors, which are read in place through their strides.
+    physics and owns the state tensors, which are read in place through their strides;
+  * `HumanoidImGetupB200Mixin` -- the same for `HumanoidImGetup`, whose getup reset it serves too.
 
 Everything runs on torch's current CUDA stream; no host synchronisation is added (the reference's
 MotionLib-cache compare, humanoid_im.py:952-953, costs one D2H sync per call and is gone).
@@ -218,29 +219,11 @@ class HumanoidImCompute:
         self.amp_obs(body_state=body, dof_pos=ms["dof_pos"], dof_vel=ms["dof_vel"], amp_obs_buf=out, shift_history=False)
         return out.view(n, steps * AMP_OBS)
 
-    def reset_envs(self, *, motion_ids: torch.Tensor, motion_start_times: torch.Tensor, motion_start_offset: torch.Tensor,
-                   global_offset: torch.Tensor, progress_buf: torch.Tensor, root_states: torch.Tensor, dof_pos: torch.Tensor,
-                   dof_vel: torch.Tensor, rigid_body_state: torch.Tensor, reset_buf: Optional[torch.Tensor] = None,
-                   env_ids: Optional[torch.Tensor] = None, terminate_buf: Optional[torch.Tensor] = None,
-                   cycle_counter: Optional[torch.Tensor] = None, contact_forces: Optional[torch.Tensor] = None,
-                   amp_obs_buf: Optional[torch.Tensor] = None, actor_ids: Optional[torch.Tensor] = None,
-                   phase: Optional[torch.Tensor] = None, seed: int = 0, offset: int = 0, obs_buf: Optional[torch.Tensor] = None,
-                   self_obs_buf: Optional[torch.Tensor] = None, amp_fresh: Optional[torch.Tensor] = None,
-                   offset_dev: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
-        """The per-step env reset of the rollout loop (`self.obs = self.env_reset(done_indices)`, amp_agent.py:352 ->
-        Humanoid.reset -> _reset_envs, humanoid.py:526-587, humanoid_amp.py:347-356, :468-488, :519-597, humanoid_im.py:921-989)
-        WITHOUT a host round trip: `pulse_reset_ref_state` (device-side compaction of `reset_buf` -- or the explicit `env_ids` --
-        start-time draw, MotionLib query, scatter into the simulator's root / dof / rigid-body views, counters cleared, AMP
-        history back-filled) followed by the fused step kernel in observation mode on the compacted list.
-        `phase`: per-ENV uniform draws (tests); None -> Philox4x32-10(seed, env, offset) inside the kernel.
-        Returns {'env_list', 'actor_list', 'count'}: device tensors for gym.set_*_tensor_indexed (count stays on the device)."""
+    def _reset_args(self, ws, *, motion_ids, motion_start_times, motion_start_offset, global_offset, progress_buf, root_states, dof_pos,
+                    dof_vel, rigid_body_state, reset_buf, env_ids, terminate_buf, cycle_counter, contact_forces, amp_obs_buf, actor_ids,
+                    phase, seed, offset, amp_fresh, offset_dev) -> "_lib.ResetArgs":
+        """Checks the reset set, the views and their strides, and fills pulse_reset_args_t (outputs: ws env_list / actor_list / count)."""
         N = int(progress_buf.shape[0])
-        dev = self.device
-        ws = getattr(self, "_reset_ws", None)
-        if ws is None or ws["env_list"].shape[0] < N:
-            ws = {"env_list": torch.zeros(N, dtype=torch.int64, device=dev), "actor_list": torch.zeros(N, dtype=torch.int32, device=dev),
-                  "count": torch.zeros(1, dtype=torch.int32, device=dev)}
-            self._reset_ws = ws
         if (reset_buf is None) == (env_ids is None):
             raise _lib.PulseError("reset_envs takes either the reset_buf mask or an explicit env_ids list")
         if rigid_body_state.dim() != 3 or rigid_body_state.shape[-1] != 13 or rigid_body_state.stride(1) != 13 or rigid_body_state.stride(2) != 1:
@@ -292,6 +275,37 @@ class HumanoidImCompute:
             a.amp_fresh = amp_fresh.data_ptr()
         if offset_dev is not None:                    # int64 / uint64 device counter added to `offset`
             a.offset_dev = offset_dev.data_ptr()
+        return a
+
+    def reset_envs(self, *, motion_ids: torch.Tensor, motion_start_times: torch.Tensor, motion_start_offset: torch.Tensor,
+                   global_offset: torch.Tensor, progress_buf: torch.Tensor, root_states: torch.Tensor, dof_pos: torch.Tensor,
+                   dof_vel: torch.Tensor, rigid_body_state: torch.Tensor, reset_buf: Optional[torch.Tensor] = None,
+                   env_ids: Optional[torch.Tensor] = None, terminate_buf: Optional[torch.Tensor] = None,
+                   cycle_counter: Optional[torch.Tensor] = None, contact_forces: Optional[torch.Tensor] = None,
+                   amp_obs_buf: Optional[torch.Tensor] = None, actor_ids: Optional[torch.Tensor] = None,
+                   phase: Optional[torch.Tensor] = None, seed: int = 0, offset: int = 0, obs_buf: Optional[torch.Tensor] = None,
+                   self_obs_buf: Optional[torch.Tensor] = None, amp_fresh: Optional[torch.Tensor] = None,
+                   offset_dev: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
+        """The per-step env reset of the rollout loop (`self.obs = self.env_reset(done_indices)`, amp_agent.py:352 ->
+        Humanoid.reset -> _reset_envs, humanoid.py:526-587, humanoid_amp.py:347-356, :468-488, :519-597, humanoid_im.py:921-989)
+        WITHOUT a host round trip: `pulse_reset_ref_state` (device-side compaction of `reset_buf` -- or the explicit `env_ids` --
+        start-time draw, MotionLib query, scatter into the simulator's root / dof / rigid-body views, counters cleared, AMP
+        history back-filled) followed by the fused step kernel in observation mode on the compacted list.
+        `phase`: per-ENV uniform draws (tests); None -> Philox4x32-10(seed, env, offset) inside the kernel.
+        Returns {'env_list', 'actor_list', 'count'}: device tensors for gym.set_*_tensor_indexed (count stays on the device)."""
+        N = int(progress_buf.shape[0])
+        dev = self.device
+        ws = getattr(self, "_reset_ws", None)
+        if ws is None or ws["env_list"].shape[0] < N:
+            ws = {"env_list": torch.zeros(N, dtype=torch.int64, device=dev), "actor_list": torch.zeros(N, dtype=torch.int32, device=dev),
+                  "count": torch.zeros(1, dtype=torch.int32, device=dev)}
+            self._reset_ws = ws
+        a = self._reset_args(ws, motion_ids=motion_ids, motion_start_times=motion_start_times, motion_start_offset=motion_start_offset,
+                             global_offset=global_offset, progress_buf=progress_buf, root_states=root_states, dof_pos=dof_pos,
+                             dof_vel=dof_vel, rigid_body_state=rigid_body_state, reset_buf=reset_buf, env_ids=env_ids,
+                             terminate_buf=terminate_buf, cycle_counter=cycle_counter, contact_forces=contact_forces,
+                             amp_obs_buf=amp_obs_buf, actor_ids=actor_ids, phase=phase, seed=seed, offset=offset, amp_fresh=amp_fresh,
+                             offset_dev=offset_dev)
         with torch.cuda.device(dev):
             _lib.check(self.lib.pulse_reset_ref_state(self.motion_lib.handle, C.byref(a), N, _lib.current_stream(dev)), "pulse_reset_ref_state")
         if obs_buf is not None:   # _compute_observations(env_ids) on the compacted list; its length stays on the device
@@ -300,6 +314,106 @@ class HumanoidImCompute:
                       motion_start_offset=motion_start_offset, global_offset=global_offset, obs_buf=obs_buf, self_obs_buf=self_obs_buf,
                       env_ids=ws["env_list"][:n_list], env_count=ws["count"], flags=_lib.STEP_OBS)
         return ws
+
+    def reset_getup(self, *, motion_ids: torch.Tensor, motion_start_times: torch.Tensor, motion_start_offset: torch.Tensor,
+                    global_offset: torch.Tensor, progress_buf: torch.Tensor, root_states: torch.Tensor, dof_pos: torch.Tensor,
+                    dof_vel: torch.Tensor, rigid_body_state: torch.Tensor, terminate_buf: torch.Tensor, recovery_counter: torch.Tensor,
+                    available_fall_states: torch.Tensor, fall_id_assignments: torch.Tensor, fall_root_states: torch.Tensor,
+                    fall_dof_pos: torch.Tensor, fall_dof_vel: torch.Tensor, recovery_prob: float, fall_prob: float, recovery_steps: int,
+                    reset_buf: Optional[torch.Tensor] = None, env_ids: Optional[torch.Tensor] = None,
+                    cycle_counter: Optional[torch.Tensor] = None, contact_forces: Optional[torch.Tensor] = None,
+                    amp_obs_buf: Optional[torch.Tensor] = None, actor_ids: Optional[torch.Tensor] = None,
+                    phase: Optional[torch.Tensor] = None, recovery_u: Optional[torch.Tensor] = None, fall_u: Optional[torch.Tensor] = None,
+                    fall_keys: Optional[torch.Tensor] = None, seed: int = 0, offset: int = 0, amp_fresh: Optional[torch.Tensor] = None,
+                    offset_dev: Optional[torch.Tensor] = None, check: bool = False) -> Dict[str, torch.Tensor]:
+        """HumanoidImGetup's reset (`_reset_actors`, humanoid_im_getup.py:135-182, + `_reset_env_tensors`) for the envs of `reset_buf`
+        or `env_ids`, in one `pulse_reset_getup` call and without a host round trip: recovery episodes (counter set, state kept), fall
+        episodes (distinct free states of the fall pool copied in), reference-state episodes (exactly `reset_envs`'s device work).
+        The getup tensors are the task's own, updated in place: `recovery_counter` (int32), `available_fall_states` /
+        `fall_id_assignments` (int64; every assignment must index the pool), `fall_root_states` [P, 13], `fall_dof_pos` /
+        `fall_dof_vel` [P, 69].
+        Draws: `phase` / `recovery_u` / `fall_u` per ENV and `fall_keys` per fall state (uniforms, tests and the mixin inject them),
+        or None -> Philox4x32-10(seed, index, offset [+ *offset_dev]) inside the kernels.
+        The simulator refresh, the observation of the reset envs and `getup_amp_init` follow.  Returns device tensors: the union
+        'env_list' / 'actor_list' / 'count' (as `reset_envs`), 'ref_list' / 'fall_list' / 'recovery_list' with 'class_counts' [3],
+        'env_class' [N] (GETUP_REF / _FALL / _RECOVERY for the reset envs) and 'error', the number of fall envs that found no free
+        state since the workspace was made (they take a reference-state episode; the reference asserts instead).  `check=True` reads
+        that word -- one host synchronisation -- and raises PulseError when it is non-zero."""
+        N = int(progress_buf.shape[0])
+        P = int(fall_root_states.shape[0])
+        dev = self.device
+        ws = getattr(self, "_getup_ws", None)
+        if ws is None or ws["env_list"].shape[0] != N or ws["fall_key_scratch"].shape[0] != P:
+            i64 = lambda: torch.zeros(N, dtype=torch.int64, device=dev)
+            ws = {"env_list": i64(), "actor_list": torch.zeros(N, dtype=torch.int32, device=dev), "count": torch.zeros(1, dtype=torch.int32, device=dev),
+                  "ref_list": i64(), "fall_list": i64(), "recovery_list": i64(), "class_counts": torch.zeros(3, dtype=torch.int32, device=dev),
+                  "env_class": torch.zeros(N, dtype=torch.uint8, device=dev), "error": torch.zeros(1, dtype=torch.int32, device=dev),
+                  "fall_pick": i64(), "fall_key_scratch": torch.zeros(P, dtype=torch.int64, device=dev)}
+            self._getup_ws = ws
+        if terminate_buf is None:
+            raise _lib.PulseError("reset_getup needs terminate_buf (it selects the recovery envs)")
+        g = _lib.GetupResetArgs()
+        g.base = self._reset_args(ws, motion_ids=motion_ids, motion_start_times=motion_start_times, motion_start_offset=motion_start_offset,
+                                  global_offset=global_offset, progress_buf=progress_buf, root_states=root_states, dof_pos=dof_pos,
+                                  dof_vel=dof_vel, rigid_body_state=rigid_body_state, reset_buf=reset_buf, env_ids=env_ids,
+                                  terminate_buf=terminate_buf, cycle_counter=cycle_counter, contact_forces=contact_forces,
+                                  amp_obs_buf=amp_obs_buf, actor_ids=actor_ids, phase=phase, seed=seed, offset=offset, amp_fresh=amp_fresh,
+                                  offset_dev=offset_dev)
+        if env_ids is not None and env_ids.numel() == 0:   # an empty tensor may have no storage: any device address serves num_ids = 0
+            g.base.env_ids_in = ws["env_list"].data_ptr()
+        for name, t, n in (("recovery_u", recovery_u, N), ("fall_u", fall_u, N), ("fall_keys", fall_keys, P)):
+            if t is not None:
+                if t.dtype != torch.float32 or not t.is_contiguous() or t.shape[0] != n:
+                    raise _lib.PulseError(f"{name} must be contiguous float32 [{n}]")
+                setattr(g, name, t.data_ptr())
+        for name, t, dt_, n in (("recovery_counter", recovery_counter, torch.int32, N), ("available_fall_states", available_fall_states, torch.int64, P),
+                                ("fall_id_assignments", fall_id_assignments, torch.int64, N)):
+            if t.dtype != dt_ or not t.is_contiguous() or t.shape[0] != n:
+                raise _lib.PulseError(f"{name}: expected contiguous {dt_} with {n} rows")
+            setattr(g, name, t.data_ptr())
+        if fall_root_states.dtype != torch.float32 or fall_root_states.stride(-1) != 1:
+            raise _lib.PulseError("fall_root_states must be float32 [P, 13] with contiguous rows")
+        if fall_dof_pos.stride() != fall_dof_vel.stride() or fall_dof_pos.dtype != torch.float32 or fall_dof_vel.dtype != torch.float32 \
+                or fall_dof_pos.shape[0] != P or fall_dof_vel.shape[0] != P:
+            raise _lib.PulseError("fall_dof_pos / fall_dof_vel must be float32 [P, 69] with shared strides")
+        g.fall_root_states, g.fall_root_stride = fall_root_states.data_ptr(), fall_root_states.stride(0)
+        g.fall_dof_pos, g.fall_dof_vel = fall_dof_pos.data_ptr(), fall_dof_vel.data_ptr()
+        g.fall_dof_env_stride, g.fall_dof_elem_stride = fall_dof_pos.stride(0), fall_dof_pos.stride(1)
+        g.num_fall_states = P
+        g.recovery_prob, g.fall_prob, g.recovery_steps = float(recovery_prob), float(fall_prob), int(recovery_steps)
+        for name in ("ref_list", "fall_list", "recovery_list", "class_counts", "env_class", "error", "fall_pick", "fall_key_scratch"):
+            setattr(g, name, ws[name].data_ptr())
+        with torch.cuda.device(dev):
+            _lib.check(self.lib.pulse_reset_getup(self.motion_lib.handle, C.byref(g), N, _lib.current_stream(dev)), "pulse_reset_getup")
+        if check:
+            self.check_getup_error()
+        return ws
+
+    def check_getup_error(self) -> None:
+        """Raises PulseError if some fall env of a `reset_getup` call found no free fall state (reads one device word: a host sync)."""
+        ws = getattr(self, "_getup_ws", None)
+        if ws is not None and int(ws["error"].item()) != 0:
+            raise _lib.PulseError(f"reset_getup: {int(ws['error'].item())} fall envs found no free fall state (the reference asserts, "
+                                  "humanoid_im_getup.py:172); they took a reference-state episode")
+
+    def getup_amp_init(self, *, body_state: torch.Tensor, dof_pos: torch.Tensor, dof_vel: torch.Tensor, amp_obs_buf: torch.Tensor) -> None:
+        """`_init_amp_obs` of the fall and recovery envs of the last `reset_getup` (humanoid_amp.py:519-533, humanoid_im_getup.py:190-196),
+        run after the simulator's refresh: the current AMP observation into every history row of a fall env, into row 0 of a recovery
+        env.  The reference-state envs were back-filled by `reset_getup` itself."""
+        ws = getattr(self, "_getup_ws", None)
+        if ws is None:
+            raise _lib.PulseError("getup_amp_init follows reset_getup")
+        a = _lib.GetupAmpArgs()
+        a.body_state, a.body_env_stride = _strided(body_state, 13)
+        if dof_pos.stride() != dof_vel.stride():
+            raise _lib.PulseError("dof_pos and dof_vel must share strides (views of one dof-state tensor)")
+        a.dof_pos, a.dof_vel, a.dof_env_stride, a.dof_elem_stride = dof_pos.data_ptr(), dof_vel.data_ptr(), dof_pos.stride(0), dof_pos.stride(1)
+        if not amp_obs_buf.is_contiguous() or amp_obs_buf.shape[-1] != AMP_OBS or amp_obs_buf.shape[0] != ws["env_list"].shape[0]:
+            raise _lib.PulseError("amp_obs_buf must be contiguous [N, steps, 196]")
+        a.amp_obs_buf, a.num_steps = amp_obs_buf.data_ptr(), int(amp_obs_buf.shape[1])
+        a.fall_list, a.recovery_list, a.class_counts = ws["fall_list"].data_ptr(), ws["recovery_list"].data_ptr(), ws["class_counts"].data_ptr()
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.pulse_getup_amp_init(C.byref(a), int(amp_obs_buf.shape[0]), _lib.current_stream(self.device)), "pulse_getup_amp_init")
 
     def task_obs(self, *, version: int, body_state: torch.Tensor, progress_buf: torch.Tensor, motion_ids: torch.Tensor,
                  motion_start_times: torch.Tensor, motion_start_offset: torch.Tensor, global_offset: torch.Tensor,
@@ -516,21 +630,15 @@ class HumanoidImB200Mixin:
         Default / Hybrid state initialisation is handed back to the reference."""
         name = getattr(getattr(self, "_state_init", None), "name", None)
         # HumanoidImGetup splits the reset envs into recovery / fall-state / reference-state episodes inside its own `_reset_actors`
-        # (humanoid_im_getup.py:135-182: Bernoulli draws, a pool of simulated fall states): that control flow stays the reference's.
+        # (humanoid_im_getup.py:135-182): HumanoidImGetupB200Mixin below serves it; behind this mixin alone it stays the reference's.
         if len(env_ids) == 0 or name not in ("Random", "Start") or hasattr(self, "_recovery_counter"):
             return super()._reset_envs(env_ids)
         if not self._pulse_ready:
             self._pulse_setup()
-        from .flags_compat import flags_test
         env_ids = env_ids.to(torch.int64).contiguous()
         self._reset_default_env_ids = []
         self._state_reset_happened = True
-        if getattr(self, "_pulse_phase", None) is None or self._pulse_phase.shape[0] != self.num_envs:
-            self._pulse_phase = torch.zeros(self.num_envs, device=self.device)
-        if name == "Start" or flags_test():                    # motion_times = 0 (humanoid_im.py:971-977)
-            self._pulse_phase.zero_()
-        else:
-            self._pulse_phase[env_ids] = torch.rand(env_ids.shape, device=self.device)
+        self._pulse_draw_phase(env_ids, name)
         self._pulse.reset_envs(env_ids=env_ids, phase=self._pulse_phase, motion_ids=self._sampled_motion_ids,
                                motion_start_times=self._motion_start_times, motion_start_offset=self._motion_start_times_offset,
                                global_offset=self._global_offset, progress_buf=self.progress_buf, cycle_counter=self._cycle_counter,
@@ -547,6 +655,15 @@ class HumanoidImB200Mixin:
         self._refresh_sim_tensors()
         self._compute_observations(env_ids)
         # _init_amp_obs: rows 0 .. steps-1 of `_amp_obs_buf[env_ids]` were written by the launch above (row 0 from the state just set)
+
+    def _pulse_draw_phase(self, env_ids, name):
+        from .flags_compat import flags_test
+        if getattr(self, "_pulse_phase", None) is None or self._pulse_phase.shape[0] != self.num_envs:
+            self._pulse_phase = torch.zeros(self.num_envs, device=self.device)
+        if name == "Start" or flags_test():                    # motion_times = 0 (humanoid_im.py:971-977)
+            self._pulse_phase.zero_()
+        else:
+            self._pulse_phase[env_ids] = torch.rand(env_ids.shape, device=self.device)
 
     def _pulse_amp_fused(self, env_ids) -> bool:
         """The fused AMP launch (history shift + current observation) covers the whole-batch call of the default configuration; one
@@ -565,3 +682,53 @@ class HumanoidImB200Mixin:
             self._pulse_setup()
         self._pulse.amp_obs(body_state=self._rigid_body_state_reshaped, dof_pos=self._dof_pos, dof_vel=self._dof_vel,
                             amp_obs_buf=self._amp_obs_buf, shift_history=True)
+
+class HumanoidImGetupB200Mixin(HumanoidImB200Mixin):
+    """`HumanoidImB200Mixin` for `phc.env.tasks.humanoid_im_getup.HumanoidImGetup` (PULSE's distillation task, env_im_vae.yaml),
+    whose reset it also serves (see INTEGRATION.md):
+
+        class HumanoidImGetupB200(HumanoidImGetupB200Mixin, HumanoidImGetup): pass
+
+    The step path is the base mixin's (recovering envs are masked inside the fused kernel through `_recovery_counter`)."""
+
+    def _reset_envs(self, env_ids):
+        """HumanoidImGetup._reset_envs (humanoid_im_getup.py:135-196 over humanoid.py:574-609, humanoid_amp.py:347-356, :519-620) with
+        `pulse_reset_getup` in place of `_reset_actors`.  After the start-time draws, the recovery / fall draws of env_ids come from
+        `torch.rand((2, n))` and one key per fall state from `torch.rand(P)`, so `torch.manual_seed` fixes them.  The reference's
+        `_reset_env_tensors` and `_refresh_sim_tensors` follow; what would sync on a data-dependent list is replaced: the `_reset_rb_*`
+        restore covers all of env_ids and keeps the saved rows where the env took a reference-state episode (a device mask), and
+        `_init_amp_obs` of the fall / recovery envs is `getup_amp_init`.  `_generate_fall_states`, `update_getup_schedule` and
+        `_update_recovery_count` stay the reference's."""
+        name = getattr(getattr(self, "_state_init", None), "name", None)
+        if len(env_ids) == 0 or name not in ("Random", "Start"):
+            return super()._reset_envs(env_ids)
+        if not self._pulse_ready:
+            self._pulse_setup()
+        env_ids = env_ids.to(torch.int64).contiguous()
+        self._reset_default_env_ids = []
+        self._pulse_draw_phase(env_ids, name)
+        n, dev = env_ids.shape[0], self.device
+        if getattr(self, "_pulse_getup_u", None) is None or self._pulse_getup_u.shape[1] != self.num_envs:
+            self._pulse_getup_u = torch.ones(2, self.num_envs, device=dev)
+        self._pulse_getup_u[:, env_ids] = torch.rand((2, n), device=dev)
+        keys = torch.rand(self._fall_root_states.shape[0], device=dev)
+        ws = self._pulse.reset_getup(
+            env_ids=env_ids, phase=self._pulse_phase, recovery_u=self._pulse_getup_u[0], fall_u=self._pulse_getup_u[1], fall_keys=keys,
+            motion_ids=self._sampled_motion_ids, motion_start_times=self._motion_start_times, motion_start_offset=self._motion_start_times_offset,
+            global_offset=self._global_offset, progress_buf=self.progress_buf, cycle_counter=self._cycle_counter, terminate_buf=self._terminate_buf,
+            root_states=self._humanoid_root_states, dof_pos=self._dof_pos, dof_vel=self._dof_vel, rigid_body_state=self._rigid_body_state_reshaped,
+            contact_forces=self._contact_forces, amp_obs_buf=self._amp_obs_buf, recovery_counter=self._recovery_counter,
+            available_fall_states=self.availalbe_fall_states, fall_id_assignments=self.fall_id_assignments,
+            fall_root_states=self._fall_root_states, fall_dof_pos=self._fall_dof_pos, fall_dof_vel=self._fall_dof_vel,
+            recovery_prob=float(self._recovery_episode_prob), fall_prob=float(self._fall_init_prob), recovery_steps=int(self._recovery_steps))
+        self._reset_fall_env_ids = []                          # _init_amp_obs_default runs below, not through the reference
+        saved = [v[env_ids].clone() for v in (self._rigid_body_pos, self._rigid_body_rot, self._rigid_body_vel, self._rigid_body_ang_vel)]
+        self._state_reset_happened = False                     # the reference's list-indexed restore is the masked one below
+        self._reset_env_tensors(env_ids)
+        self._refresh_sim_tensors()
+        is_ref = (ws["env_class"][env_ids] == _lib.GETUP_REF).view(-1, 1, 1)
+        for v, s in zip((self._rigid_body_pos, self._rigid_body_rot, self._rigid_body_vel, self._rigid_body_ang_vel), saved):
+            v[env_ids] = torch.where(is_ref, s, v[env_ids])
+        self._compute_observations(env_ids)
+        self._pulse.getup_amp_init(body_state=self._rigid_body_state_reshaped, dof_pos=self._dof_pos, dof_vel=self._dof_vel,
+                                   amp_obs_buf=self._amp_obs_buf)
