@@ -627,6 +627,13 @@ int pulse_copy_cols_bf16(const pulse_bf16_t* src, int64_t ld_src, int64_t rows, 
 int pulse_vae_reparam(const float* head, int64_t ld_head, const float* noise, int64_t ld_noise, int64_t rows, int32_t latent,
                       int32_t mode, int32_t clamp, float clamp_lo, float clamp_hi, pulse_bf16_t* z_bf16, int64_t ld_z, float* z_f32,
                       int64_t ld_zf, void* stream);
+/* PULSE_Z_SAMPLE with the noise drawn in the kernel (the distillation rollout, amp_network_z_builder.py:82-95 in eval mode):
+ * z = mu + exp(0.5*clamp(logvar, clamp_lo, clamp_hi))*eps written as bf16 into z_bf16[rows, 0:latent], latent <= 32.
+ * eps ~ N(0,1) from Philox4x32-10 keyed (seed, row*64 + j/2) with offset (*offset_dev if not NULL) + step; the two words of one call
+ * give the Box-Muller pair (j, j+1).  noise_out fp32 [rows, latent] (or NULL) receives eps. */
+int pulse_vae_reparam_philox(const float* head, int64_t ld_head, int64_t rows, int32_t latent, int32_t clamp, float clamp_lo,
+                             float clamp_hi, uint64_t seed, const uint64_t* offset_dev, uint64_t step, pulse_bf16_t* z_bf16,
+                             int64_t ld_z, float* noise_out, int64_t ld_noise, void* stream);
 
 /* kin_action_loss = mean_rows ||pred - gt||_2 (amp_agent.py:782): stats[0] += sum of row norms (fp64; caller zeroes);
  * dpred bf16 [rows, ld_d] = (pred - gt) / (||pred - gt|| * rows) (0 where the norm is 0, as torch.norm's backward), columns
@@ -668,6 +675,16 @@ int pulse_pnn_compose(const float* acts, int64_t prim_stride, int64_t ld_a, cons
  * out = freeze[d] ? 0 : offset[d] + scale[d]*action[r, d].  freeze: uint8 [dofs] or NULL. */
 int pulse_pd_targets(const float* action, int64_t ld_a, const float* offset, const float* scale, const uint8_t* freeze, int64_t rows,
                      int32_t dofs, float* out, int64_t ld_out, void* stream);
+
+/* Pre-physics step of the distillation rollout (HumanoidImDistillGetup: pre_physics_step, then _update_recovery_count,
+ * humanoid_im_getup.py:76-80) in one launch over `rows` envs:
+ *   pd_out[r, d]       = freeze[d] ? 0 : offset[d] + scale[d]*mus[r, d]     (pulse_pd_targets' arithmetic)
+ *   kin_progress[r]    = progress_buf[r]                                   (the progress record, humanoid_im_distill.py:205)
+ *   recovery_counter[r] = max(recovery_counter[r] - 1, 0)
+ * mus, pd_out and kin_progress are addressed through their row strides (experience-buffer slices). */
+int pulse_distill_pre_physics(const float* mus, int64_t ld_mus, const float* pd_offset, const float* pd_scale, const uint8_t* freeze,
+                              int64_t rows, int32_t dofs, float* pd_out, int64_t ld_pd, const int64_t* progress_buf,
+                              int64_t* kin_progress, int64_t ld_progress, int32_t* recovery_counter, void* stream);
 
 /* HumanoidReach._update_task / _reset_task (humanoid_reach.py:126-147) with the uniform draws supplied by the caller:
  * where progress >= tar_change_steps: tar_pos = (dist_max*(2u-1), dist_max*(2v-1), h_min + (h_max-h_min)*w),

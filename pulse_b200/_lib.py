@@ -356,6 +356,10 @@ SIGNATURES = {
     "pulse_copy_cols_bf16": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_vae_reparam": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_float,
                                     C.c_float, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
+    "pulse_vae_reparam_philox": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_uint64,
+                                           C.c_void_p, C.c_uint64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
+    "pulse_distill_pre_physics": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p,
+                                            C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "pulse_vae_action_loss": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_int64,
                                         C.c_void_p, C.c_void_p]),
     "pulse_vae_latent_loss": (C.c_int, [C.POINTER(VaeLatentArgs), C.c_int64, C.c_void_p]),

@@ -3,6 +3,7 @@
 // grid-stride loops, or one warp per row (lane = action / latent dimension) with fp64 atomics for the scalar statistics.
 #include <cuda_bf16.h>
 
+#include "philox.cuh"
 #include "pulse_common.cuh"
 
 namespace pulse {
@@ -59,6 +60,60 @@ __global__ void __launch_bounds__(256) vae_reparam_kernel(const float* __restric
     }
     if (zb != nullptr) zb[r * ld_z + j] = __float2bfloat16(z);
     if (zf != nullptr) zf[r * ld_zf + j] = z;
+  }
+}
+
+// z = mu + exp(0.5 clamp(logvar)) eps with eps drawn here (the reparameterisation of the distillation rollout): one thread per latent PAIR,
+// one Philox4x32-10 call keyed (seed, row * 64 + pair, offset) whose first two words give the pair's two Box-Muller normals -- the
+// indexing of policy_post_kernel.  The arithmetic after the draw is vae_reparam_kernel's PULSE_Z_SAMPLE path.
+__global__ void __launch_bounds__(256) vae_reparam_philox_kernel(const float* __restrict__ head, long long ld_head, long long rows, int latent,
+                                                                 int clamp, float lo, float hi, unsigned long long seed,
+                                                                 const unsigned long long* __restrict__ offset_dev, unsigned long long step,
+                                                                 __nv_bfloat16* __restrict__ zb, long long ld_z, float* __restrict__ noise_out,
+                                                                 long long ld_noise) {
+  const int pairs = (latent + 1) / 2;
+  const long long total = rows * pairs;
+  const unsigned long long off = offset_dev != nullptr ? *offset_dev + step : step;
+  for (long long i = blockIdx.x * 256ll + threadIdx.x; i < total; i += 256ll * gridDim.x) {
+    const long long r = i / pairs;
+    const int p = static_cast<int>(i - r * pairs);
+    const Philox4 w = philox4x32_10(seed, static_cast<unsigned long long>(r) * 64ull + static_cast<unsigned long long>(p), off);
+    float e[2];
+    box_muller(w.x, w.y, e[0], e[1]);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int j = 2 * p + h;
+      if (j >= latent) break;
+      const float mu = head[r * ld_head + j];
+      float lv = head[r * ld_head + latent + j];
+      if (clamp) lv = fminf(fmaxf(lv, lo), hi);
+      const float z = mu + expf(0.5f * lv) * e[h];
+      zb[r * ld_z + j] = __float2bfloat16(z);
+      if (noise_out != nullptr) noise_out[r * ld_noise + j] = e[h];
+    }
+  }
+}
+
+// ---- pre-physics step of the distillation rollout ---------------------------------------------------------------------------
+// pd_out = freeze ? 0 : offset + scale * mus (pd_targets_kernel's two roundings), the progress record kin_progress[r] = progress[r] and
+// HumanoidImGetup._update_recovery_count's recovery_counter = max(recovery_counter - 1, 0), in one launch: the row-wise outputs are
+// written by the thread of column 0.
+__global__ void __launch_bounds__(256) distill_pre_physics_kernel(const float* __restrict__ mus, long long ld_mus, const float* __restrict__ offset,
+                                                                  const float* __restrict__ scale, const uint8_t* __restrict__ freeze,
+                                                                  long long rows, int dofs, float* __restrict__ pd_out, long long ld_pd,
+                                                                  const long long* __restrict__ progress, long long* __restrict__ kin_progress,
+                                                                  long long ld_kp, int* __restrict__ recovery_counter) {
+  const long long total = rows * dofs;
+  for (long long i = blockIdx.x * 256ll + threadIdx.x; i < total; i += 256ll * gridDim.x) {
+    const long long r = i / dofs;
+    const int d = static_cast<int>(i - r * dofs);
+    const float v = __fadd_rn(offset[d], __fmul_rn(scale[d], mus[r * ld_mus + d]));
+    pd_out[r * ld_pd + d] = (freeze != nullptr && freeze[d]) ? 0.0f : v;
+    if (d == 0) {
+      kin_progress[r * ld_kp] = progress[r];
+      const int rc = recovery_counter[r];
+      recovery_counter[r] = rc > 1 ? rc - 1 : 0;
+    }
   }
 }
 
@@ -268,6 +323,38 @@ extern "C" int pulse_vae_reparam(const float* head, int64_t ld_head, const float
   vae_reparam_kernel<<<grid_for(rows * latent, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       head, ld_head, noise, ld_noise, rows, latent, mode, clamp, clamp_lo, clamp_hi, reinterpret_cast<__nv_bfloat16*>(z_bf16), ld_z, z_f32, ld_zf);
   PULSE_LAUNCH_OK("vae_reparam_kernel");
+  return PULSE_OK;
+}
+
+extern "C" int pulse_vae_reparam_philox(const float* head, int64_t ld_head, int64_t rows, int32_t latent, int32_t clamp, float clamp_lo,
+                                        float clamp_hi, uint64_t seed, const uint64_t* offset_dev, uint64_t step, pulse_bf16_t* z_bf16,
+                                        int64_t ld_z, float* noise_out, int64_t ld_noise, void* stream) {
+  PULSE_REQUIRE(head && z_bf16, "pulse_vae_reparam_philox: null head / z_bf16");
+  PULSE_REQUIRE(rows >= 0, "pulse_vae_reparam_philox: negative rows");
+  PULSE_REQUIRE(latent >= 1 && latent <= 32, "pulse_vae_reparam_philox: latent %d outside [1, 32]", latent);
+  PULSE_REQUIRE(ld_head >= 2 * latent && ld_z >= latent, "pulse_vae_reparam_philox: head or z row stride too small");
+  PULSE_REQUIRE(noise_out == nullptr || ld_noise >= latent, "pulse_vae_reparam_philox: noise_out row stride too small");
+  if (rows == 0) return PULSE_OK;
+  vae_reparam_philox_kernel<<<grid_for(rows * ((latent + 1) / 2), 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      head, ld_head, rows, latent, clamp, clamp_lo, clamp_hi, seed, reinterpret_cast<const unsigned long long*>(offset_dev), step,
+      reinterpret_cast<__nv_bfloat16*>(z_bf16), ld_z, noise_out, ld_noise);
+  PULSE_LAUNCH_OK("vae_reparam_philox_kernel");
+  return PULSE_OK;
+}
+
+extern "C" int pulse_distill_pre_physics(const float* mus, int64_t ld_mus, const float* pd_offset, const float* pd_scale, const uint8_t* freeze,
+                                         int64_t rows, int32_t dofs, float* pd_out, int64_t ld_pd, const int64_t* progress_buf,
+                                         int64_t* kin_progress, int64_t ld_progress, int32_t* recovery_counter, void* stream) {
+  PULSE_REQUIRE(mus && pd_offset && pd_scale && pd_out, "pulse_distill_pre_physics: null mus / pd_offset / pd_scale / pd_out");
+  PULSE_REQUIRE(progress_buf && kin_progress && recovery_counter, "pulse_distill_pre_physics: null progress_buf / kin_progress / recovery_counter");
+  PULSE_REQUIRE(rows >= 0, "pulse_distill_pre_physics: negative rows");
+  PULSE_REQUIRE(dofs >= 1, "pulse_distill_pre_physics: dofs %d < 1", dofs);
+  PULSE_REQUIRE(ld_mus >= dofs && ld_pd >= dofs && ld_progress >= 1, "pulse_distill_pre_physics: row strides too small");
+  if (rows == 0) return PULSE_OK;
+  distill_pre_physics_kernel<<<grid_for(rows * dofs, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      mus, ld_mus, pd_offset, pd_scale, freeze, rows, dofs, pd_out, ld_pd, reinterpret_cast<const long long*>(progress_buf),
+      reinterpret_cast<long long*>(kin_progress), ld_progress, recovery_counter);
+  PULSE_LAUNCH_OK("distill_pre_physics_kernel");
   return PULSE_OK;
 }
 

@@ -37,7 +37,33 @@ def discount_values(mb_fdones: torch.Tensor, mb_values: torch.Tensor, mb_rewards
     return adv, ret
 
 
-class PlayStepsB200:
+class GraphRunner:
+    """CUDA-graph runner of the rollout drivers: `_run(key, fn, *args)` executes `fn` eagerly on its first use, captures it on its second
+    use and replays it from then on; every graph shares one memory pool.  The subclass sets `dev`, `use_graphs`, `_graphs = {}` and
+    `_pool = None`."""
+
+    def _run(self, key, fn, *args):
+        if not self.use_graphs:
+            return fn(*args)
+        g = self._graphs.get(key)
+        if g is None:
+            # first use: plain eager execution (lazy workspaces, one-time attribute calls).  The segments are NOT idempotent (progress
+            # counters advance, reset / fresh flags are consumed), so nothing may run twice: the capture happens on the second use,
+            # where it only records, and the replay that follows is that use's single execution.
+            self._graphs[key] = False
+            return fn(*args)
+        if g is False:
+            torch.cuda.synchronize(self.dev)
+            if self._pool is None:
+                self._pool = torch.cuda.graph_pool_handle()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, pool=self._pool):
+                fn(*args)
+            self._graphs[key] = g
+        g.replay()
+
+
+class PlayStepsB200(GraphRunner):
     """`AMPAgent.play_steps` (phc/learning/amp_agent.py:341-439) on the device: for every step of the horizon
          env_reset(done envs) -> get_action_values -> env step (post-physics compute) -> AMP observation -> next values,
     then the discriminator rewards / reward mix / GAE / value normalisation of `play_steps` + `prepare_dataset`
@@ -155,26 +181,6 @@ class PlayStepsB200:
             self._reset_and_act(t)
 
     # ------------------------------------------------------------------ graphs
-    def _run(self, key, fn, *args):
-        if not self.use_graphs:
-            return fn(*args)
-        g = self._graphs.get(key)
-        if g is None:
-            # first use: plain eager execution (lazy workspaces, one-time attribute calls).  The segments are NOT idempotent (progress
-            # counters advance, reset / fresh flags are consumed), so nothing may run twice: the capture happens on the second use,
-            # where it only records, and the replay that follows is that use's single execution.
-            self._graphs[key] = False
-            return fn(*args)
-        if g is False:
-            torch.cuda.synchronize(self.dev)
-            if self._pool is None:
-                self._pool = torch.cuda.graph_pool_handle()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, pool=self._pool):
-                fn(*args)
-            self._graphs[key] = g
-        g.replay()
-
     def _whole_overlapped(self) -> None:
         """The horizon with the independent pieces of consecutive steps overlapped on three streams (single-graph mode, no host I/O):
              main    reset(t) -> obs of the reset envs -> normalise -> actor -> policy_post -> fused step kernel(t)

@@ -79,6 +79,8 @@ class PulseVAE:
         self.lib = _lib.load()
         self._bufs: Dict[tuple, dict] = {}
         self._side = None
+        self.rng_seed = (int(seed) * 0x9E3779B97F4A7C15 + 0x452821E638D01377) & (2 ** 64 - 1)
+        self.rng_offset = torch.zeros(1, dtype=torch.int64, device=self.device)    # uint64 counter read by pulse_vae_reparam_philox
 
     # ------------------------------------------------------------------ buffers
     def _buf(self, M: int) -> dict:
@@ -165,6 +167,31 @@ class PulseVAE:
         if self.critic is not None:
             out["values"] = self.value_rms.unnormalize(self.eval_critic(M=obs.shape[0]))
         return out
+
+    def act_into(self, obs: torch.Tensor, *, mus: torch.Tensor, rng_step: int = 0, noise_out: Optional[torch.Tensor] = None) -> None:
+        """The student's action in the distillation rollout (get_action_values in eval mode, the env stepped with `mus`,
+        amp_agent.py:359-369, amp_network_z_builder.py:82-95): normalise without a statistics update, encoder, reparameterisation
+        with the noise drawn in `pulse_vae_reparam_philox` (seed, row, latent index; offset = rng_offset + rng_step), decoder writing
+        `mus` (an [M, A] experience-buffer slice, any row stride).  `noise_out` fp32 [M, E] receives the draws (tests).  No critic:
+        its values never reach the only_kin_loss update."""
+        M = obs.shape[0]
+        b = self._buf(M)
+        self._normalize_obs(obs, b)
+        head = self.enc.forward(b["x"])
+        if noise_out is not None and (noise_out.dtype != torch.float32 or noise_out.shape != (M, self.E) or noise_out.stride(1) != 1):
+            raise _lib.PulseError(f"act_into: noise_out must be float32 [{M}, {self.E}] with contiguous rows")
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.pulse_vae_reparam_philox(head.data_ptr(), head.stride(0), M, self.E, int(self.clamp), self.clamp_lo, self.clamp_hi,
+                                                         self.rng_seed, self.rng_offset.data_ptr(), int(rng_step), b["dec_in"].data_ptr(),
+                                                         b["dec_in"].stride(0), _lib.ptr(noise_out),
+                                                         noise_out.stride(0) if noise_out is not None else 0, self._st()),
+                       "pulse_vae_reparam_philox")
+        self.dec.forward(b["dec_in"], out=mus)
+
+    def advance_rng(self, steps: int) -> None:
+        """Moves the device-side Philox offset past the `steps` draws of a rollout (CUDA-graph replays draw fresh noise)."""
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.pulse_bump_counter(self.rng_offset.data_ptr(), int(steps), self._st()), "pulse_bump_counter")
 
     # ------------------------------------------------------------------ update
     def anneal(self, epoch_num: int) -> float:
@@ -344,8 +371,8 @@ class TeacherPNN:
         self.rms.running_var.copy_(running_var.to(self.device).double())
         self.rms._refresh()
 
-    def gt_action(self, obs_buf: torch.Tensor) -> torch.Tensor:
-        """obs_buf fp32 [M, obs] raw -> fp32 [M, A] (a reused buffer)."""
+    def gt_action(self, obs_buf: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """obs_buf fp32 [M, obs] raw -> fp32 [M, A]: a reused buffer, or `out` (any row stride, e.g. an experience-buffer slice)."""
         M = obs_buf.shape[0]
         if M not in self._bufs:
             self._bufs[M] = {"x": torch.zeros(M, self.Kp, device=self.device, dtype=torch.bfloat16),
@@ -355,12 +382,16 @@ class TeacherPNN:
         for k, col in enumerate(self.cols):
             col.forward(b["x"], out=b["acts"][k])
         w = self.composer.forward(b["x"])
+        if out is None:
+            out = b["out"]
+        elif out.dtype != torch.float32 or out.shape != (M, self.A) or out.stride(1) != 1:
+            raise _lib.PulseError(f"gt_action: out must be float32 [{M}, {self.A}] with contiguous rows")
         with torch.cuda.device(self.device):
             _lib.check(self.lib.pulse_pnn_compose(b["acts"].data_ptr(), b["acts"].stride(0), b["acts"].stride(1), w.data_ptr(), w.stride(0),
                                                   {"silu": _lib.ACT_SILU, "relu": _lib.ACT_RELU, None: _lib.ACT_NONE}[self.composer_act], M, self.A,
-                                                  self.num_prim, b["out"].data_ptr(), b["out"].stride(0), _lib.current_stream(self.device)),
+                                                  self.num_prim, out.data_ptr(), out.stride(0), _lib.current_stream(self.device)),
                        "pulse_pnn_compose")
-        return b["out"]
+        return out
 
 
 def pd_targets(actions: torch.Tensor, offset: torch.Tensor, scale: torch.Tensor, out: Optional[torch.Tensor] = None,
