@@ -1,0 +1,343 @@
+"""Teacher-forced float64 references of the update's links, each with its own rounding bound.
+
+A link is one GEMM or one element-wise kernel of the update.  Its reference is recomputed in float64 from the operands the kernels
+themselves produced and stored (the bf16 activations, mask words and gradients in the workspaces, the bf16 weight mirror as it was
+before the call), so an error in one link does not propagate into the next and every link can be held to a tight bound:
+
+* GEMM, fp32 output:  |y - y64| <= c * u32 * sqrt(K) * (|A| . |B|)     u32 = 2^-24, c = 4, K = the full reduction length (however the
+  kernel split it).  This is the probabilistic bound of Higham and Mary with enough margin for partial sums that are truncated rather
+  than rounded to nearest at every step (wgmma's fp32 accumulation).  A link over it but under the deterministic K * u32 bound is
+  reported with that ratio as well; the bound is not loosened.
+* bf16 output: one more rounding, 2^-8 * |y64|.
+* ReLU mask words written by a kernel: every bit must be y64 > 0 wherever |y64| exceeds the bound; inside it the bit may go either way,
+  and that ambiguous fraction must stay below 1e-3 so that the check cannot become vacuous.
+* element-wise kernels: the bound follows the fp32 operations the kernel performs (a few u32 per operation), plus the bf16 rounding.
+
+Every comparator raises BoundError (an AssertionError) naming the link, and records the largest err / tol in a Report.
+Everything here is plain torch and runs on the CPU as well as on the device.
+"""
+import math
+from typing import List, Optional
+
+import torch
+
+U32 = 2.0 ** -24     # fp32 unit round-off
+UBF = 2.0 ** -8      # bf16 unit round-off
+C_GEMM = 4.0
+AMBIGUOUS_MAX = 1e-3
+
+
+class BoundError(AssertionError):
+    pass
+
+
+def f64(t: torch.Tensor) -> torch.Tensor:
+    return t.detach().to(torch.float64)
+
+
+def f32r(x: float) -> float:
+    """x rounded to fp32: the value a kernel receives for a float argument."""
+    return float(torch.tensor(x, dtype=torch.float32))
+
+
+class Report:
+    """Per-link margins: the largest err / tol, the ambiguous-mask fraction, the excluded rows."""
+
+    def __init__(self, title: str):
+        self.title = title
+        self.rows: List[tuple] = []
+
+    def add(self, link: str, ratio: float, ambiguous: Optional[float] = None, excluded: Optional[str] = None) -> None:
+        self.rows.append((link, ratio, ambiguous, excluded))
+
+    def text(self) -> str:
+        out = [f"== {self.title}"]
+        for link, r, amb, exc in self.rows:
+            s = f"  {link:<44s} err/tol {r:8.4f}"
+            if amb is not None:
+                s += f"  ambiguous {amb:.2e}"
+            if exc is not None:
+                s += f"  excluded {exc}"
+            out.append(s)
+        return "\n".join(out)
+
+
+def _ratio(got: torch.Tensor, ref: torch.Tensor, tol: torch.Tensor):
+    err = (f64(got) - ref).abs()
+    r = torch.where(tol > 0, err / torch.where(tol > 0, tol, torch.ones_like(tol)), torch.where(err > 0, torch.full_like(err, math.inf), torch.zeros_like(err)))
+    if r.numel() == 0:
+        return 0.0, None
+    k = int(torch.argmax(r))
+    return float(r.reshape(-1)[k]), k
+
+
+def check(rep: Optional[Report], link: str, got: torch.Tensor, ref: torch.Tensor, tol: torch.Tensor, det_tol: Optional[torch.Tensor] = None) -> float:
+    """|got - ref| <= tol element-wise (ref, tol float64 of got's shape).  det_tol: the deterministic bound, reported on failure."""
+    if got.shape != ref.shape:
+        raise BoundError(f"{link}: shape {tuple(got.shape)} vs reference {tuple(ref.shape)}")
+    r, k = _ratio(got, ref, tol)
+    if rep is not None:
+        rep.add(link, r)
+    if not r < 1.0:
+        idx = tuple(int(i) for i in torch.unravel_index(torch.tensor(k), got.shape)) if k is not None else ()
+        msg = (f"{link}: err/tol {r:.3f} at {idx}: got {float(got.reshape(-1)[k])!r}, reference {float(ref.reshape(-1)[k])!r}, "
+               f"tol {float(tol.reshape(-1)[k]):.3e}")
+        if det_tol is not None:
+            rd, _ = _ratio(got, ref, det_tol)
+            msg += f"; against the deterministic K*u32 bound: {rd:.3f}"
+        raise BoundError(msg)
+    return r
+
+
+def check_exact(rep: Optional[Report], link: str, got: torch.Tensor, ref: torch.Tensor) -> None:
+    bad = (f64(got) != f64(ref))
+    if rep is not None:
+        rep.add(link + " (exact)", float(bad.any()))
+    if bad.any():
+        k = int(torch.nonzero(bad.reshape(-1))[0])
+        raise BoundError(f"{link}: {int(bad.sum())} elements differ; first at flat index {k}: {float(got.reshape(-1)[k])!r} "
+                         f"vs {float(ref.reshape(-1)[k])!r}")
+
+
+# ---------------------------------------------------------------------------------------------------------------------- GEMM links
+class Gemm:
+    """y64 = alpha * (A . B) [* gate] in float64 with its accumulation bound `acc` (before any output rounding)."""
+
+    def __init__(self, a: torch.Tensor, b: torch.Tensor, alpha: float = 1.0, gate: Optional[torch.Tensor] = None,
+                 bias: Optional[torch.Tensor] = None, c: float = C_GEMM):
+        a, b = f64(a), f64(b)
+        self.K = a.shape[1]
+        y, ap = a @ b, a.abs() @ b.abs()
+        if bias is not None:                      # fp32 epilogue add: one more term, one more rounding
+            y, ap = y + f64(bias), ap + f64(bias).abs()
+            self.K += 1
+        self.acc = c * U32 * math.sqrt(self.K) * ap
+        self.det = self.K * U32 * ap
+        if bias is not None:
+            self.acc = self.acc + U32 * y.abs()
+            self.det = self.det + U32 * y.abs()
+        if alpha != 1.0:                          # fp32 multiply of the accumulator
+            y, self.acc, self.det = alpha * y, abs(alpha) * self.acc + U32 * abs(alpha) * y.abs(), abs(alpha) * self.det + U32 * abs(alpha) * y.abs()
+        if gate is not None:                      # the kernel's own mask: gated elements are exactly zero
+            g = gate.to(torch.float64)
+            y, self.acc, self.det = y * g, self.acc * g, self.det * g
+        self.y = y
+
+    def tol(self, bf16: bool) -> torch.Tensor:
+        return self.acc * (1 + UBF) + UBF * self.y.abs() if bf16 else self.acc
+
+    def det_tol(self, bf16: bool) -> torch.Tensor:
+        return self.det * (1 + UBF) + UBF * self.y.abs() if bf16 else self.det
+
+    def check(self, rep: Optional[Report], link: str, got: torch.Tensor) -> float:
+        bf16 = got.dtype == torch.bfloat16
+        return check(rep, link, got, self.y, self.tol(bf16), self.det_tol(bf16))
+
+
+def unpack_mask(words: torch.Tensor, n: int, m: int) -> torch.Tensor:
+    """ReLU mask words int32 [ceil(n/32), >= m] (bit i of word (c, r) = column 32 c + i of row r) -> bool [m, n]."""
+    w = words[:, :m].to(torch.int64) & 0xFFFFFFFF
+    bits = (w[:, :, None] >> torch.arange(32, device=words.device)) & 1          # [W, m, 32]
+    return bits.permute(1, 0, 2).reshape(m, -1)[:, :n].bool()
+
+
+def pack_mask(bits: torch.Tensor) -> torch.Tensor:
+    """Inverse of unpack_mask: bool [m, n] -> int32 [ceil(n/32), m]."""
+    m, n = bits.shape
+    wn = (n + 31) // 32
+    full = torch.zeros(m, wn * 32, dtype=torch.int64, device=bits.device)
+    full[:, :n] = bits.to(torch.int64)
+    w = (full.view(m, wn, 32) << torch.arange(32, device=bits.device)).sum(-1)
+    w = torch.where(w >= 2 ** 31, w - 2 ** 32, w)
+    return w.T.contiguous().to(torch.int32)
+
+
+def check_mask(rep: Optional[Report], link: str, words: torch.Tensor, g: Gemm, n: int, m: int) -> float:
+    """Mask words a forward epilogue wrote for y = g.y: bit = y64 > 0 wherever |y64| exceeds the bound; bits past column n are 0."""
+    bits = unpack_mask(words, ((n + 31) // 32) * 32, m)
+    if bits[:, n:].any():
+        raise BoundError(f"{link}: mask bits set past column {n}")
+    bits = bits[:, :n]
+    tol = g.tol(False)
+    sure = g.y.abs() > tol
+    wrong = sure & (bits != (g.y > 0))
+    amb = float((~sure).double().mean())
+    if rep is not None:
+        rep.add(link, float(wrong.any()), ambiguous=amb)
+    if wrong.any():
+        r, c = (int(i) for i in torch.nonzero(wrong)[0])
+        raise BoundError(f"{link}: {int(wrong.sum())} mask bits contradict the sign of y64, first at row {r} column {c} "
+                         f"(y64 {float(g.y[r, c]):.3e}, bound {float(tol[r, c]):.3e})")
+    if not amb < AMBIGUOUS_MAX:
+        raise BoundError(f"{link}: {amb:.2e} of the mask bits lie within the bound (limit {AMBIGUOUS_MAX})")
+    return amb
+
+
+def sum_tol(terms_abs_sum: torch.Tensor, n: int, c: float = C_GEMM) -> torch.Tensor:
+    """Bound of an fp32 sum of n terms whose magnitudes add up to terms_abs_sum (same model as the GEMM bound)."""
+    return c * U32 * math.sqrt(max(n, 1)) * terms_abs_sum
+
+
+# ---------------------------------------------------------------------------------------------------------------- element-wise links
+def normalize_ref(x: torch.Tensor, mean: torch.Tensor, rstd: torch.Tensor):
+    """clamp((x - mean) * rstd, +-5) -> bf16: two fp32 roundings then one bf16 rounding."""
+    x, m, r = f64(x), f64(mean), f64(rstd)
+    y = torch.clamp((x - m) * r, -5.0, 5.0)
+    tol = UBF * y.abs() + 3 * U32 * (x.abs() + m.abs()) * r.abs() * (1 + UBF)
+    return y, tol
+
+
+def silu_tol(pre: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """Fast-math SiLU epilogue (ex2.approx / rcp.approx) on the bf16 pre-activation -- or, in a column group that reaches past N, on the
+    fp32 accumulator, at most one bf16 rounding (2^-8 |pre|) away, |silu'| <= 1.1 -- and one bf16 rounding of the result."""
+    shift = 1.1 * UBF * pre.abs() * (1 + UBF)
+    return UBF * (s.abs() + shift) + shift + (8 + 2 * pre.abs()) * U32 * (s.abs() + pre.abs())
+
+
+def silu64(z: torch.Tensor) -> torch.Tensor:
+    return z * torch.sigmoid(z)
+
+
+def silu_grad64(z: torch.Tensor) -> torch.Tensor:
+    s = torch.sigmoid(z)
+    return s * (1 + z * (1 - s))
+
+
+def silu_grad_err(z: torch.Tensor) -> torch.Tensor:
+    """Bound of |act_grad_fast(z) - silu'(z)| for the dgrad gate (fast-math exp / divide, four fp32 operations)."""
+    return (16 + 4 * z.abs()) * U32 * (1 + z.abs())
+
+
+def ppo_loss_ref(mu, value, actions, old_nlp, adv, ret, logstd, old_mu=None, e_clip=0.2, critic_coef=5.0, bounds_coef=10.0):
+    """pulse_ppo_loss on the kernel's own mu / value: float64 autograd of the oracle's ppo_total_loss (dmu, dv), the per-row statistics
+    and the bounds of the fp32 kernel.  Rows whose branch decision lies within rounding of its threshold are flagged `ambiguous`."""
+    from oracle import pulse_oracle as po
+    M, A = mu.shape
+    mu64 = f64(mu).requires_grad_(True)
+    v64 = f64(value).reshape(M).requires_grad_(True)
+    act, onl, adv64, ret64, ls = f64(actions), f64(old_nlp), f64(adv), f64(ret), f64(logstd)
+    r = po.ppo_total_loss(mu64, v64, onl, adv64, ret64, act, ls, e_clip=e_clip, critic_coef=critic_coef, bounds_coef=bounds_coef)
+    dmu, dv = torch.autograd.grad(r["loss"], (mu64, v64))
+    with torch.no_grad():
+        sg = torch.exp(ls)
+        z = (act - mu64) / sg
+        nlp = r["neglogp"]
+        d = onl - nlp
+        ratio = torch.exp(d)
+        nlp_mag = 0.5 * (z * z).sum(-1) + 0.5 * math.log(2 * math.pi) * A + ls.abs().sum()
+        ratio_rel = 16 * U32 * nlp_mag + U32 * d.abs() + 4 * U32            # error of nlp, of the difference, of expf
+        lo, hi = 1.0 - f32r(e_clip), 1.0 + f32r(e_clip)
+        win = 2 * ratio * ratio_rel
+        ambiguous = ((ratio - lo).abs() <= win) | ((ratio - hi).abs() <= win)
+        mu_d = mu64.detach()
+        bnd_edge = ((mu_d.abs() - 1.0).abs() <= 4 * U32 * mu_d.abs()).any(-1)     # |mu| ~ 1: the bound loss's kink
+        ambiguous = ambiguous | bnd_edge
+        rc = torch.clamp(ratio, lo, hi)
+        active = (-adv64 * ratio) >= (-adv64 * rc)
+        dnlp_dmu = -(act - mu_d) / (sg * sg)
+        ta = torch.where(active, adv64 * ratio, torch.zeros_like(ratio))[:, None] * dnlp_dmu / M
+        hi_t, lo_t = torch.clamp_min(mu_d - 1.0, 0.0), torch.clamp_max(mu_d + 1.0, 0.0)
+        tb = bounds_coef * 2.0 * (hi_t + lo_t) / M
+        tol_mu = UBF * dmu.abs() + (1 + UBF) * ((ratio_rel[:, None] + 8 * U32) * ta.abs() + 8 * U32 * tb.abs())
+        tol_v = UBF * dv.abs() + 6 * U32 * (critic_coef * 2.0 * (ret64.abs() + v64.detach().abs()) / M)
+        a_loss = torch.maximum(-adv64 * ratio, -adv64 * rc)
+        c_loss = (ret64 - v64.detach()) ** 2
+        b_loss = (hi_t ** 2 + lo_t ** 2).sum(-1)
+        stats = [a_loss.sum(), c_loss.sum(), b_loss.sum(), None, ((ratio - 1.0).abs() > f32r(e_clip)).double().sum(), nlp.sum()]
+        stats_tol = [(adv64.abs() * ratio * (ratio_rel + 4 * U32)).sum(), (8 * U32 * ((ret64.abs() + v64.detach().abs()) ** 2)).sum(),
+                     (8 * U32 * (hi_t.abs() + lo_t.abs() + 1) ** 2).sum(), None, float(ambiguous.sum()), (16 * U32 * nlp_mag).sum()]
+        if old_mu is not None:
+            sg2 = sg * sg
+            dd = f64(old_mu) - mu_d
+            frac = (sg2 + dd * dd) / (2.0 * (sg2 + f32r(1e-5)))
+            stats[3] = (math.log(1.0 + f32r(1e-5)) + frac - 0.5).sum()
+            # per term: expf(logstd), the squares, the difference old_mu - mu and the quotient, a few u32 of (1 + frac) each
+            stats_tol[3] = (16 * U32 * (1.5 + frac + dd.abs() * (f64(old_mu).abs() + mu_d.abs()) / sg2)).sum()
+    return {"dmu": dmu, "dv": dv, "tol_mu": tol_mu, "tol_v": tol_v, "ambiguous": ambiguous, "stats": stats, "stats_tol": stats_tol,
+            "ratio": ratio, "active": active}
+
+
+def disc_loss_ref(logits: torch.Tensor, n_agent: int, scale: float):
+    """pulse_disc_loss: dlogit = 0.5 * scale * d(mean BCE)/dl per batch (agent rows target 0, demo rows target 1), the statistics."""
+    l = f64(logits).reshape(-1)
+    n = l.shape[0]
+    n_demo = n - n_agent
+    sg = torch.sigmoid(l)
+    agent = torch.arange(n, device=l.device) < n_agent
+    g = torch.where(agent, 0.5 * scale * sg / n_agent, 0.5 * scale * (sg - 1.0) / n_demo)
+    cnt = torch.where(agent, torch.full_like(l, float(n_agent)), torch.full_like(l, float(n_demo)))
+    tol = UBF * g.abs() + 8 * U32 * 0.5 * scale * (sg + 1.0) / cnt
+    sp = torch.nn.functional.softplus(l)
+    spm = torch.nn.functional.softplus(-l)
+    stats = [sp[agent].sum(), spm[~agent].sum(), (l[agent] < 0).double().sum(), (l[~agent] > 0).double().sum()]
+    stats_tol = [(8 * U32 * (sp[agent] + l[agent].abs() + 1)).sum(), (8 * U32 * (spm[~agent] + l[~agent].abs() + 1)).sum(), 0.0, 0.0]
+    return g, tol, stats, stats_tol
+
+
+def adam_ref(p, g, m, v, step: int, *, lr: float, max_norm: float, b1: float = 0.9, b2: float = 0.999, eps: float = 1e-8,
+             sumsq_rel: float = 16 * U32):
+    """clip_grad_norm_(max_norm) + torch.optim.Adam step number step + 1 in float64 on fp32 state, with the bounds of the fp32 kernel.
+    The constants are the fp32 values the kernel receives.  Returns (p, m, v, tol_p, tol_m, tol_v, clipped, norm_margin)."""
+    lr, b1, b2, eps = f32r(lr), f32r(b1), f32r(b2), f32r(eps)
+    p, g, m, v = f64(p), f64(g), f64(m), f64(v)
+    t = step + 1
+    norm = float(torch.sqrt((g * g).sum()))
+    scale, clipped, margin = 1.0, False, math.inf
+    if max_norm and max_norm > 0:
+        mn = f32r(max_norm)
+        scale = min(1.0, mn / (norm + f32r(1e-6)))
+        clipped = scale < 1.0
+        margin = abs(norm / mn - 1.0)
+    gs = g * scale
+    rel_g = (sumsq_rel + 4 * U32 if clipped else 0.0) + U32
+    dg = gs.abs() * rel_g
+    m1 = b1 * m + (1 - b1) * gs
+    v1 = b2 * v + (1 - b2) * gs * gs
+    dm = 2 * U32 * (b1 * m.abs() + (1 - b1) * gs.abs()) + (1 - b1) * dg + U32 * m1.abs()
+    dv = 3 * U32 * (b2 * v + (1 - b2) * gs * gs) + (1 - b2) * 2 * gs.abs() * dg
+    bc1, bc2 = 1 - b1 ** t, 1 - b2 ** t
+    rel_bc1 = 8 * U32 * b1 ** t / bc1 + U32          # powf: a few ulp of b^t, then the subtraction
+    rel_bc2 = 8 * U32 * b2 ** t / bc2 + U32
+    s = torch.sqrt(v1) / math.sqrt(bc2)
+    den = s + eps
+    st = (lr / bc1) * m1 / den
+    p1 = p - st
+    rel_v = torch.where(v1 > 0, dv / torch.where(v1 > 0, v1, torch.ones_like(v1)), torch.zeros_like(v1))
+    dden = s * (0.5 * rel_v + 0.5 * rel_bc2 + 4 * U32) + U32 * den
+    dst = st.abs() * (rel_bc1 + 4 * U32) + (lr / bc1) * (dm / den + m1.abs() * dden / (den * den))
+    dp = U32 * (p1.abs() + p.abs()) + dst
+    return p1, m1, v1, dp, dm, dv, clipped, margin
+
+
+def latent_loss_tol(enc, pri, noise, dz, progress, E: int, T: int, kld_coef: float, ar1_coef: float, clamp=(-5.0, 2.0), phi: float = 0.99):
+    """Bounds of pulse_vae_latent_loss's head gradients (d_enc, d_prior) from the fp32 operations it performs, float64 [M, 2E] each."""
+    enc, pri, noise, dz = f64(enc), f64(pri), f64(noise), f64(dz)
+    M = enc.shape[0]
+    qm, pm = enc[:, :E], pri[:, :E]
+    qv, pv = torch.clamp(enc[:, E:], *clamp), torch.clamp(pri[:, E:], *clamp)
+    kc = kld_coef / M
+    ipv, ratio, dm = torch.exp(-pv), torch.exp(qv - pv), qm - pm
+    ddm = U32 * (qm.abs() + pm.abs())
+    dratio = ratio * (U32 * (qv - pv).abs() + 3 * U32)
+    t_qm = kc * ipv * (ddm + 4 * U32 * dm.abs()) + U32 * dz.abs()
+    t_qv = kc * 0.5 * (dratio + U32 * (ratio + 1)) + 6 * U32 * (dz * 0.5 * torch.exp(0.5 * qv) * noise).abs()
+    t_pv = kc * 0.5 * (dratio + 2 * dm.abs() * ddm * ipv + 6 * U32 * dm * dm * ipv + U32 * (1 + ratio + dm * dm * ipv))
+    t_pm = t_qm - U32 * dz.abs()
+    if ar1_coef:
+        pairs = (M // T) * (T - 1)
+        c = ar1_coef / pairs
+        prog = progress.to(torch.int64)
+        t = torch.arange(M, device=enc.device) % T
+        keep = torch.zeros(M, dtype=torch.bool, device=enc.device)        # pair (r - 1, r)
+        keep[1:] = ((prog[1:] - prog[:-1]) == 1) & ~((prog[1:] <= 2) | (prog[:-1] <= 2)) & (t[1:] > 0)
+        e = torch.zeros_like(qm)
+        e[1:] = qm[1:] - f32r(phi) * qm[:-1]
+        de = torch.zeros_like(qm)
+        de[1:] = U32 * (qm[1:].abs() + 2 * qm[:-1].abs())
+        nrm = e.norm(dim=-1, keepdim=True)
+        dn = (e.abs() * de).sum(-1, keepdim=True) / nrm.clamp_min(1e-300) + (E + 4) * U32 * nrm
+        term = c * (de / nrm.clamp_min(1e-300) + e.abs() * dn / nrm.clamp_min(1e-300) ** 2 + 4 * U32 * e.abs() / nrm.clamp_min(1e-300))
+        term = torch.where(keep[:, None] & (nrm > 0), term, torch.zeros_like(term))
+        t_qm = t_qm + term
+        t_qm[:-1] = t_qm[:-1] + f32r(phi) * term[1:]
+    return torch.cat([t_qm, t_qv], 1), torch.cat([t_pm, t_pv], 1)
