@@ -329,14 +329,17 @@ class PPOPolicy:
         single = reducer is not None and os.environ.get("PULSE_GRAD_REDUCE", "single") != "chain"
         if single:
             reducer = None
+        # with a prefetch, this minibatch's AMP batches are normalised here, before the fork: the next minibatch's, on the prefetch stream,
+        # merge into the same discriminator input statistics and must come after them
+        amp_here = not prepared and prefetch is not None
         if not prepared:
-            self.prepare_inputs(obs, None, update_obs_rms, slot)
+            self.prepare_inputs(obs, amp if amp_here else None, update_obs_rms, slot)
         if pref_at == "start":
             fork_prefetch()
         if amp is not None:                                  # (agent, replay, demo) AMP observation batches: disc_coef * disc_loss
             s_disc.wait_stream(main)
             with torch.cuda.stream(s_disc):
-                self.disc.loss_backward(*amp, slot=slot, prepared=prepared)
+                self.disc.loss_backward(*amp, slot=slot, prepared=prepared or amp_here)
                 if reducer is not None:
                     d0, d1 = self.disc.mlp.param_span()
                     reducer.reduce(self.flat.grads[d0:d1], 2)

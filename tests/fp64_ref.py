@@ -208,6 +208,57 @@ def silu_grad_err(z: torch.Tensor) -> torch.Tensor:
     return (16 + 4 * z.abs()) * U32 * (1 + z.abs())
 
 
+def silu_gated(g: "Gemm", pre: torch.Tensor):
+    """A dgrad GEMM gated in its epilogue by silu'(pre) of the kernel's own bf16 pre-activation: (y64, accumulation bound before the
+    bf16 output rounding).  Check with check(..., y, acc * (1 + UBF) + UBF * |y|)."""
+    z = f64(pre)
+    sg = silu_grad64(z)
+    y = g.y * sg
+    return y, g.acc * sg.abs() + g.y.abs() * silu_grad_err(z) + U32 * y.abs()
+
+
+SILU_GRAD_ARGMAX = 2.3993572805154675      # z tanh(z / 2) = 2: where |silu'| peaks (1.09984 at +z*, 0.09984 at -z*)
+
+
+def silu_grad_absmax(lo: torch.Tensor, hi: torch.Tensor) -> torch.Tensor:
+    """max |silu'(z)| over [lo, hi]: the end points, and the two extrema of silu' where they lie inside."""
+    m = torch.maximum(silu_grad64(lo).abs(), silu_grad64(hi).abs())
+    for z in (SILU_GRAD_ARGMAX, -SILU_GRAD_ARGMAX):
+        inside = (lo <= z) & (z <= hi)
+        m = torch.where(inside, torch.maximum(m, silu_grad64(torch.tensor(z, dtype=torch.float64)).abs()), m)
+    return m
+
+
+def silu_gemm_tol(g: "Gemm") -> torch.Tensor:
+    """SiLU in the forward epilogue, rounded to bf16 -- the eval path, where no pre-activation is stored.  The register epilogue applies
+    it to the accumulator rounded to bf16 (fp32 only in a column group that reaches past N), so its argument lies within
+    w = acc + one bf16 rounding of y: max |silu'| over [y - w, y + w] times w, the fast-math SiLU evaluation (as in silu_tol), one bf16
+    rounding of the result."""
+    w = g.acc * (1 + UBF) + UBF * g.y.abs()
+    z = g.y.abs() + w
+    s = silu64(g.y)
+    shift = silu_grad_absmax(g.y - w, g.y + w) * w + (8 + 2 * z) * U32 * (s.abs() + z)
+    return shift + UBF * (s.abs() + shift)
+
+
+def gaussian_sample_ref(mu: torch.Tensor, eps: torch.Tensor, logstd: torch.Tensor):
+    """pulse_gaussian_sample on the kernel's own mu: actions = mu + exp(logstd) eps and neglogp = 0.5 sum z^2 + 0.5 log(2 pi) A +
+    sum logstd with z = (a - mu) / sigma, float64, with the bounds of the fp32 kernel (expf, the product and the sum for a; for z the
+    cancellation a - mu, the quotient; then the per-lane and warp sums of A terms and the fp32 constant 0.5f * log(2 pi)f * A)."""
+    mu, eps, ls = f64(mu), f64(eps), f64(logstd)
+    A = mu.shape[1]
+    sg = torch.exp(ls)
+    a = mu + sg * eps
+    tol_a = U32 * a.abs() + 3 * U32 * (sg * eps).abs()
+    dz = (tol_a + U32 * (a - mu).abs()) / sg + 3 * U32 * eps.abs()
+    z2 = eps * eps
+    nlp = 0.5 * z2.sum(-1) + 0.5 * math.log(2 * math.pi) * A + ls.sum()
+    c32 = 0.5 * f32r(1.8378770664093453) * A
+    tol_n = (0.5 * (2 * eps.abs() * dz + dz * dz + U32 * z2).sum(-1) + 0.5 * A * U32 * z2.sum(-1) + A * U32 * ls.abs().sum()
+             + abs(c32 - 0.5 * math.log(2 * math.pi) * A) + 2 * U32 * c32 + 2 * U32 * (nlp.abs() + c32 + ls.abs().sum()))
+    return a, tol_a, nlp, tol_n
+
+
 def ppo_loss_ref(mu, value, actions, old_nlp, adv, ret, logstd, old_mu=None, e_clip=0.2, critic_coef=5.0, bounds_coef=10.0):
     """pulse_ppo_loss on the kernel's own mu / value: float64 autograd of the oracle's ppo_total_loss (dmu, dv), the per-row statistics
     and the bounds of the fp32 kernel.  Rows whose branch decision lies within rounding of its threshold are flagged `ambiguous`."""
