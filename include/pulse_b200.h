@@ -411,14 +411,13 @@ typedef struct {
 #define PULSE_GEMM_A_MN 1u   /* A is given as [K, M] row-major (the reduction dimension is the ROW index) */
 #define PULSE_GEMM_B_MN 2u   /* B is given as [K, N] row-major */
 
-/* lda / ldb in elements, multiples of 8, >= K; A and B 16-byte aligned.  split_k > 1: fp32 slabs only
- * (slab z at out_f32 + z*split_stride); pulse_gemm_num_splits gives the number of slabs actually written. */
-int pulse_gemm_bf16_nt(const void* a, int64_t lda, const void* b, int64_t ldb, int64_t m, int64_t n, int64_t k,
-                       const pulse_gemm_epilogue_t* ep, int32_t split_k, void* stream);
-/* General form: D[M,N] = epilogue(sum_k A(m,k) B(n,k)).  flags select, per operand, K-major storage (A[M,K] / B[N,K],
- * the NT case above) or MN-major storage (A[K,M] / B[K,N] row-major), so activations, output gradients and weights
- * are consumed exactly as they sit in memory:  dgrad dX = dY . W  -> A = dY (K-major), B = W [N_out,K_in] as MN-major;
- * wgrad dW = dY^T X -> A = dY [batch,N] MN-major, B = X [batch,K] MN-major.  No transposed copies anywhere. */
+/* D[M,N] = epilogue(sum_k A(m,k) B(n,k)).  flags select, per operand, K-major storage (A[M,K] / B[N,K]) or MN-major
+ * storage (A[K,M] / B[K,N] row-major), so activations, output gradients and weights are consumed exactly as they sit in
+ * memory:  forward Y = X . W^T -> A = X, B = W, both K-major;  dgrad dX = dY . W  -> A = dY (K-major), B = W [N_out,K_in]
+ * as MN-major;  wgrad dW = dY^T X -> A = dY [batch,N] MN-major, B = X [batch,K] MN-major.  No transposed copies anywhere.
+ * lda / ldb in elements, multiples of 8, >= the contiguous extent (K for K-major storage); A and B 16-byte aligned.
+ * split_k > 1: fp32 slabs only (slab z at out_f32 + z*split_stride); pulse_gemm_num_splits gives the number of slabs
+ * actually written. */
 int pulse_gemm_bf16(const void* a, int64_t lda, const void* b, int64_t ldb, int64_t m, int64_t n, int64_t k,
                     const pulse_gemm_epilogue_t* ep, int32_t split_k, uint32_t flags, void* stream);
 int pulse_gemm_num_splits(int64_t k, int32_t split_k);
@@ -427,18 +426,6 @@ int pulse_gemm_num_splits(int64_t k, int32_t split_k);
  * under PULSE_GEMM_BN=128 or PULSE_GEMM_STAGES=4.  pulse_gemm_last_tile_n: the width the last GEMM launch took (0 before the first). */
 int pulse_gemm_tile_n(int64_t m, int64_t n, int64_t k, int32_t split_k, int32_t sms);
 int pulse_gemm_last_tile_n(void);
-
-/* Several GEMMs of the same kind in ONE persistent launch (work items of all problems concatenated): forward groups
- * (flags 0), ReLU-dgrad groups (PULSE_GEMM_B_MN) or weight-gradient groups (PULSE_GEMM_A_MN | PULSE_GEMM_B_MN, fp32 atomic
- * accumulation), at most 4 problems.  Validated against single launches by tests/test_gpu_grouped.py; off by default. */
-typedef struct {
-  const void* a; int64_t lda;
-  const void* b; int64_t ldb;
-  int64_t m, n, k;
-  pulse_gemm_epilogue_t ep;
-  int32_t split_k, reserved;
-} pulse_gemm_problem_t;
-int pulse_gemm_bf16_grouped(const pulse_gemm_problem_t* problems, int32_t count, uint32_t flags, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Element-wise / reduction kernels around the GEMMs.

@@ -150,11 +150,6 @@ class GemmEpilogue(C.Structure):
 GEMM_A_MN, GEMM_B_MN = 1, 2
 
 
-class GemmProblem(C.Structure):
-    _fields_ = [("a", C.c_void_p), ("lda", C.c_int64), ("b", C.c_void_p), ("ldb", C.c_int64), ("m", C.c_int64), ("n", C.c_int64),
-                ("k", C.c_int64), ("ep", GemmEpilogue), ("split_k", C.c_int32), ("reserved", C.c_int32)]
-
-
 class PpoLossArgs(C.Structure):
     _fields_ = [
         ("mu", C.c_void_p), ("ld_mu", C.c_int64), ("value", C.c_void_p), ("ld_value", C.c_int64), ("actions", C.c_void_p),
@@ -316,14 +311,11 @@ SIGNATURES = {
     "pulse_amp_obs": (C.c_int, [C.POINTER(AmpObsArgs), C.c_int64, C.c_void_p]),
     "pulse_gae": (C.c_int, [C.POINTER(GaeArgs), C.c_int32, C.c_int64, C.c_void_p]),
     "pulse_normalize_advantages": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
-    "pulse_gemm_bf16_nt": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
-                                     C.POINTER(GemmEpilogue), C.c_int32, C.c_void_p]),
     "pulse_gemm_bf16": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                                   C.POINTER(GemmEpilogue), C.c_int32, C.c_uint32, C.c_void_p]),
     "pulse_gemm_num_splits": (C.c_int, [C.c_int64, C.c_int32]),
     "pulse_gemm_tile_n": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32]),
     "pulse_gemm_last_tile_n": (C.c_int, []),
-    "pulse_gemm_bf16_grouped": (C.c_int, [C.POINTER(GemmProblem), C.c_int32, C.c_uint32, C.c_void_p]),
     "pulse_normalize_to_bf16": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                           C.c_void_p, C.c_int64, C.c_float, C.c_void_p]),
     "pulse_normalize_moments": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,

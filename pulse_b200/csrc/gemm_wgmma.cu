@@ -366,27 +366,7 @@ __device__ __forceinline__ void stage_tile_bf16(const float* d, unsigned stage, 
 // smallest one that covers the request.
 enum : int { kModeGeneric = 0, kModeFwd = 1, kModeDgrad = 2, kModeWgrad = 3, kModeDgradVec = 4 };
 
-// ---- grouped launch: several problems of the same operand majors / epilogue mode in ONE persistent launch ------------------
-constexpr int kMaxGroup = 4;
-struct GemmProblem {
-  CUtensorMap map_a, map_b, map_c, map_p;
-  pulse_gemm_epilogue_t ep;
-  int M, N, K, kb_per_split;
-  int item_end;   // cumulative work items (tiles x split-K slices) up to and including this problem
-  int tma_out;
-  int pad[2];
-};
-struct GemmGroup {
-  GemmProblem p[kMaxGroup];
-  int count, total_items;
-};
-
-#define PULSE_GEMM_GROUPED 0
 #include "gemm_kernel.inc"
-#undef PULSE_GEMM_GROUPED
-#define PULSE_GEMM_GROUPED 1
-#include "gemm_kernel.inc"
-#undef PULSE_GEMM_GROUPED
 
 // ---- host side: tensor maps through the driver entry point (no link-time libcuda dependency) ------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -490,17 +470,17 @@ int epilogue_maps(int mode, const pulse_gemm_epilogue_t& ep, long long m, long l
   return PULSE_OK;
 }
 
-int gemm_num_sms(bool honour_limit) {
-  static int num_sms = 0, limited = 0;
-  if (num_sms == 0) {
-    int dev = 0;
+int gemm_num_sms() {
+  static int limited = 0;
+  if (limited == 0) {
+    int dev = 0, num_sms = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 0;
     // PULSE_GEMM_SMS=n: leave SMs free for a concurrent collective (the persistent grid otherwise owns the whole GPU)
     limited = num_sms;
     const char* e = getenv("PULSE_GEMM_SMS");
     if (e != nullptr && atoi(e) >= 1 && atoi(e) < num_sms) limited = atoi(e);
   }
-  return honour_limit ? limited : num_sms;
+  return limited;
 }
 
 // Ring depth of a launch whose epilogue is register-resident (reg_epi) or not: see GemmSmem.  PULSE_GEMM_STAGES=4 keeps every launch
@@ -554,7 +534,7 @@ int launch_gemm_ring(const CUtensorMap& map_a, const CUtensorMap& map_b, const C
   static bool attr_set = false;
   const int rc = set_smem_once(gemm_bf16_kernel<A_MN, B_MN, MODE, S, BN>, smem_bytes<S, BN>(), &attr_set);
   if (rc != PULSE_OK) return rc;
-  const int num_sms = gemm_num_sms(true);
+  const int num_sms = gemm_num_sms();
   PULSE_REQUIRE(num_sms > 0, "pulse_gemm_bf16: cannot query the device's SM count");
   // persistent: one CTA per SM loops over the work items
   const long long total = static_cast<long long>((n + BN - 1) / BN) * ((m + BM - 1) / BM) * splits;
@@ -598,7 +578,7 @@ int launch_gemm(const CUtensorMap& map_a, const CUtensorMap& map_b, const void* 
     if constexpr (!A_MN) {   // A MN-major is a weight gradient: those keep the narrow tile
       // wide: the bf16 register-resident epilogue without a pre-activation (the 16 KB areas hold no pre-activation boxes)
       if (s != kStages && tma_out == 1 && ep.preact == nullptr && !narrow_forced() &&
-          gemm_tile_n(m, n, kb_per_split, splits, gemm_num_sms(true)) == kWideBN) {
+          gemm_tile_n(m, n, kb_per_split, splits, gemm_num_sms()) == kWideBN) {
         CUtensorMap map_bw = map_b;
         if (!B_MN && !make_map(&map_bw, b, n, k, ldb, kWideBN)) {
           set_error("pulse_gemm_bf16: cuTensorMapEncodeTiled failed for the wide B operand");
@@ -613,30 +593,6 @@ int launch_gemm(const CUtensorMap& map_a, const CUtensorMap& map_b, const void* 
     }
   }
   return launch_gemm_ring<A_MN, B_MN, MODE, kStages, kNarrowBN>(map_a, map_b, map_c, map_p, ep, m, n, k, splits, kb_per_split, tma_out, stream);
-}
-
-template <bool A_MN, bool B_MN, int MODE, int S>
-int launch_gemm_grouped(const GemmGroup& grp, cudaStream_t stream) {
-  static bool attr_set = false;
-  const int rc = set_smem_once(gemm_bf16_grouped_kernel<A_MN, B_MN, MODE, S, kNarrowBN>, smem_bytes<S, kNarrowBN>(), &attr_set);
-  if (rc != PULSE_OK) return rc;
-  const int num_sms = gemm_num_sms(false);
-  PULSE_REQUIRE(num_sms > 0, "pulse_gemm_bf16_grouped: cannot query the device's SM count");
-  const unsigned grid = static_cast<unsigned>(grp.total_items < num_sms ? grp.total_items : num_sms);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid, 1, 1);
-  cfg.blockDim = dim3(kThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem_bytes<S, kNarrowBN>();
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  PULSE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_grouped_kernel<A_MN, B_MN, MODE, S, kNarrowBN>, grp));
-  PULSE_LAUNCH_OK("gemm_bf16_grouped_kernel");
-  g_last_tile_n = kNarrowBN;
-  return PULSE_OK;
 }
 
 int epilogue_mode(const pulse_gemm_epilogue_t* ep) {
@@ -724,87 +680,4 @@ extern "C" int pulse_gemm_bf16(const void* a, int64_t lda, const void* b, int64_
   if (b_mn) { PULSE_GEMM_DISPATCH(false, true) }
   PULSE_GEMM_DISPATCH(false, false)
 #undef PULSE_GEMM_DISPATCH
-}
-
-extern "C" int pulse_gemm_bf16_nt(const void* a, int64_t lda, const void* b, int64_t ldb, int64_t m, int64_t n, int64_t k,
-                                  const pulse_gemm_epilogue_t* ep, int32_t split_k, void* stream) {
-  return pulse_gemm_bf16(a, lda, b, ldb, m, n, k, ep, split_k, 0u, stream);
-}
-
-// Several GEMMs of the same kind (operand majors `flags`, same epilogue specialisation) in ONE persistent launch: the work items
-// of all problems are concatenated, so the tail of one problem fills with tiles of the next and the per-launch prologue / drain
-// is paid once (actor + critic layers of a PPO minibatch, or the weight gradients of several layers).
-// Nothing calls it unless PULSE_GROUPED=1 (pulse_b200/dense.py).
-extern "C" int pulse_gemm_bf16_grouped(const pulse_gemm_problem_t* problems, int32_t count, uint32_t flags, void* stream) {
-  using namespace pulse;
-  PULSE_REQUIRE(problems != nullptr && count >= 1 && count <= kMaxGroup, "pulse_gemm_bf16_grouped: 1..%d problems", kMaxGroup);
-  PULSE_REQUIRE((flags & ~3u) == 0, "pulse_gemm_bf16_grouped: bad flags");
-  const bool a_mn = flags & PULSE_GEMM_A_MN, b_mn = flags & PULSE_GEMM_B_MN;
-  int mode = -1;
-  for (int i = 0; i < count; ++i) {
-    const pulse_gemm_problem_t& q = problems[i];
-    PULSE_REQUIRE(q.a && q.b, "pulse_gemm_bf16_grouped: null operand in problem %d", i);
-    PULSE_REQUIRE(q.m > 0 && q.n > 0 && q.k > 0 && q.m < (1ll << 31) && q.n < (1ll << 31) && q.k < (1ll << 31), "pulse_gemm_bf16_grouped: bad shape in problem %d", i);
-    PULSE_REQUIRE(q.lda >= (a_mn ? q.m : q.k) && q.ldb >= (b_mn ? q.n : q.k) && (q.lda % 8) == 0 && (q.ldb % 8) == 0,
-                  "pulse_gemm_bf16_grouped: leading dimensions of problem %d must cover the contiguous extent and be multiples of 8", i);
-    PULSE_REQUIRE(aligned16(q.a) && aligned16(q.b), "pulse_gemm_bf16_grouped: operands of problem %d must be 16-byte aligned", i);
-    PULSE_REQUIRE(q.ep.out || q.ep.out_t || q.ep.out_f32, "pulse_gemm_bf16_grouped: problem %d has no output", i);
-    PULSE_REQUIRE(q.split_k >= 1, "pulse_gemm_bf16_grouped: split_k must be >= 1");
-    PULSE_REQUIRE(q.split_k == 1 || (q.ep.out_f32 && q.ep.accumulate && !q.ep.out && !q.ep.out_t && !q.ep.bias && q.ep.act == PULSE_ACT_NONE && !q.ep.gate &&
-                                     !q.ep.preact && !q.ep.colsum),
-                  "pulse_gemm_bf16_grouped: split-K only with fp32 atomic accumulation");
-    const int mq = epilogue_mode(&q.ep);
-    PULSE_REQUIRE(mode < 0 || mq == mode, "pulse_gemm_bf16_grouped: problem %d needs a different epilogue specialisation than problem 0", i);
-    mode = mq;
-  }
-  PULSE_REQUIRE(mode == kModeFwd || mode == kModeDgrad || mode == kModeWgrad, "pulse_gemm_bf16_grouped: forward, ReLU-dgrad and wgrad groups only");
-  PULSE_REQUIRE((mode == kModeFwd && !a_mn && !b_mn) || (mode == kModeDgrad && !a_mn && b_mn) || (mode == kModeWgrad && a_mn && b_mn),
-                "pulse_gemm_bf16_grouped: operand majors do not match the group kind (fwd K/K, dgrad K/MN, wgrad MN/MN)");
-  GemmGroup grp;
-  memset(&grp, 0, sizeof(grp));
-  grp.count = count;
-  long long items = 0;
-  for (int i = 0; i < count; ++i) {
-    const pulse_gemm_problem_t& q = problems[i];
-    GemmProblem& g = grp.p[i];
-    const bool ok_a = a_mn ? make_map(&g.map_a, q.a, q.k, q.m, q.lda, 64) : make_map(&g.map_a, q.a, q.m, q.k, q.lda, BM);
-    const bool ok_b = b_mn ? make_map(&g.map_b, q.b, q.k, q.n, q.ldb, 64) : make_map(&g.map_b, q.b, q.n, q.k, q.ldb, kNarrowBN);
-    if (!ok_a || !ok_b) {
-      set_error("pulse_gemm_bf16_grouped: cuTensorMapEncodeTiled failed for problem %d", i);
-      return PULSE_ERR_CUDA;
-    }
-    g.ep = q.ep;
-    const int rc = epilogue_maps(mode, q.ep, q.m, q.n, 1, &g.map_c, &g.map_p, &g.tma_out);
-    if (rc != PULSE_OK) return rc;
-    g.M = static_cast<int>(q.m);
-    g.N = static_cast<int>(q.n);
-    g.K = static_cast<int>(q.k);
-    const int num_kb = static_cast<int>((q.k + BK - 1) / BK);
-    const int splits = pulse_gemm_num_splits(q.k, q.split_k);
-    g.kb_per_split = (num_kb + splits - 1) / splits;
-    items += static_cast<long long>((q.n + kNarrowBN - 1) / kNarrowBN) * ((q.m + BM - 1) / BM) * splits;
-    PULSE_REQUIRE(items < (1ll << 30), "pulse_gemm_bf16_grouped: too many work items");
-    g.item_end = static_cast<int>(items);
-  }
-  grp.total_items = static_cast<int>(items);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // the deep ring only when every problem takes the register-resident epilogue
-  bool reg_epi = true, preact = false;
-  for (int i = 0; i < count; ++i) {
-    reg_epi = reg_epi && grp.p[i].tma_out;
-    preact = preact || problems[i].ep.preact != nullptr;
-  }
-  const int s = ring_stages(mode != kModeWgrad && reg_epi, preact);
-  for (int i = 0; i < count; ++i)
-    if (s == kStages && grp.p[i].tma_out == kTmaOutF32) grp.p[i].tma_out = 0;
-  if (mode == kModeFwd) {
-    if (s == 6) return launch_gemm_grouped<false, false, kModeFwd, 6>(grp, st);
-    if (s == 5) return launch_gemm_grouped<false, false, kModeFwd, 5>(grp, st);
-    return launch_gemm_grouped<false, false, kModeFwd, kStages>(grp, st);
-  }
-  if (mode == kModeDgrad) {
-    if (s == 6) return launch_gemm_grouped<false, true, kModeDgrad, 6>(grp, st);
-    return launch_gemm_grouped<false, true, kModeDgrad, kStages>(grp, st);
-  }
-  return launch_gemm_grouped<true, true, kModeWgrad, kStages>(grp, st);
 }

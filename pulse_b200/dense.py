@@ -1,4 +1,4 @@
-"""Dense layers on the H100 tensor cores: thin host wrapper over `pulse_gemm_bf16_nt` (wgmma / TMA).
+"""Dense layers on the H100 tensor cores: thin host wrapper over `pulse_gemm_bf16` (wgmma / TMA).
 
 `gemm_nt(a, b)` computes a @ b.T for bf16 row-major a [M,K], b [N,K] with fp32 accumulation and a fused
 epilogue (bias, ReLU / SiLU, activation-derivative gating, transposed copy, fp32 output, split-K slabs).
@@ -134,100 +134,3 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
         _lib.check(lib.pulse_gemm_bf16(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), M, N, K, C.byref(ep), split_k, flags,
                                        _lib.current_stream(a.device)), "pulse_gemm_bf16")
 
-
-def _prepare(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False, bias: Optional[torch.Tensor] = None, act=None,
-         gate: Optional[torch.Tensor] = None, gate_mode=None, alpha: float = 1.0, out: Optional[torch.Tensor] = None,
-         out_t: Optional[torch.Tensor] = None, out_f32: Optional[torch.Tensor] = None, preact: Optional[torch.Tensor] = None,
-         colsum: Optional[torch.Tensor] = None, accumulate: bool = False, split_k: int = 1, sumsq: Optional[torch.Tensor] = None,
-         relu_mask: Optional[torch.Tensor] = None, gate_mask: Optional[torch.Tensor] = None) -> tuple:
-    """Argument checks + epilogue descriptor of one problem of a grouped launch (same rules as gemm(), which stays the
-    validated single-problem path and is deliberately left untouched)."""
-    _check_bf16(a, "a")
-    _check_bf16(b, "b")
-    (K, M) = a.shape if a_mn else (a.shape[1], a.shape[0])
-    (Kb, N) = b.shape if b_mn else (b.shape[1], b.shape[0])
-    if K != Kb:
-        raise _lib.PulseError(f"K mismatch: a {tuple(a.shape)} (mn={a_mn}) vs b {tuple(b.shape)} (mn={b_mn})")
-    ep = _lib.GemmEpilogue()
-    ep.alpha = alpha
-    ep.act = ACT[act] if not isinstance(act, int) else act
-    if bias is not None:
-        if bias.dtype != torch.float32 or bias.numel() != N or not bias.is_contiguous():
-            raise _lib.PulseError("bias must be contiguous fp32 [N]")
-        ep.bias = bias.data_ptr()
-    if gate is not None:
-        _check_bf16(gate, "gate")
-        ep.gate, ep.ldg = gate.data_ptr(), gate.stride(0)
-        ep.gate_mode = ACT[gate_mode] if not isinstance(gate_mode, int) else gate_mode
-    if out is not None:
-        _check_bf16(out, "out")
-        if out.shape[0] < M or out.shape[1] < N:
-            raise _lib.PulseError("out too small")
-        ep.out, ep.ldo = out.data_ptr(), out.stride(0)
-    if out_t is not None:
-        _check_bf16(out_t, "out_t")
-        if out_t.shape[0] < N or out_t.shape[1] < M:
-            raise _lib.PulseError("out_t too small")
-        ep.out_t, ep.ldot = out_t.data_ptr(), out_t.stride(0)
-    if preact is not None:
-        _check_bf16(preact, "preact")
-        ep.preact, ep.ldp = preact.data_ptr(), preact.stride(0)
-    if out_f32 is not None:
-        if out_f32.dtype != torch.float32 or out_f32.stride(-1) != 1:
-            raise _lib.PulseError("out_f32 must be fp32 with contiguous rows")
-        if out_f32.dim() == 3:  # [splits, M, N] slabs
-            if out_f32.shape[0] < num_splits(K, split_k):
-                raise _lib.PulseError("out_f32 has fewer slabs than split-K needs")
-            ep.split_stride, ep.ldf = out_f32.stride(0), out_f32.stride(1)
-        else:
-            if split_k != 1 and not accumulate:
-                raise _lib.PulseError("split_k > 1 needs a [splits, M, N] out_f32 or accumulate=True")
-            ep.ldf = out_f32.stride(0)
-        ep.out_f32 = out_f32.data_ptr()
-        ep.accumulate = int(accumulate)
-    if colsum is not None:
-        if colsum.dtype != torch.float32 or colsum.numel() < N:
-            raise _lib.PulseError("colsum must be fp32 [N]")
-        ep.colsum = colsum.data_ptr()
-    if sumsq is not None:
-        if sumsq.dtype != torch.float64 or sumsq.numel() < 1:
-            raise _lib.PulseError("sumsq must be an fp64 accumulator")
-        ep.sumsq = sumsq.data_ptr()
-    for name, t in (("relu_mask", relu_mask), ("gate_mask", gate_mask)):      # ReLU masks as bit words, [ceil(N/32), >= M] int32, chunk-major
-        if t is not None:
-            if t.dtype != torch.int32 or t.dim() != 2 or t.stride(1) != 1 or t.shape[0] * 32 < N or t.shape[1] < M:
-                raise _lib.PulseError(f"{name} must be int32 [ceil(N/32), >= M] with contiguous rows, got {t.dtype} {tuple(t.shape)}")
-            if name == "relu_mask":
-                ep.relu_mask, ep.ld_rmask = t.data_ptr(), t.stride(0)
-            else:
-                ep.gate_mask, ep.ld_gmask = t.data_ptr(), t.stride(0)
-    flags = (_lib.GEMM_A_MN if a_mn else 0) | (_lib.GEMM_B_MN if b_mn else 0)
-    return ep, M, N, K, flags, split_k
-
-
-def grouped_enabled() -> bool:
-    """PULSE_GROUPED=1 routes the actor + critic layers of a PPO minibatch through grouped launches (default off: validated by
-    tests/test_gpu_grouped.py, not faster than the three-stream path)."""
-    import os
-    return os.environ.get("PULSE_GROUPED", "0") == "1"
-
-
-def gemm_grouped(problems) -> None:
-    """problems: list of (a, b, kwargs) with the keyword arguments of gemm(); all of the same kind (forward / ReLU dgrad /
-    weight gradient: same a_mn, b_mn and epilogue specialisation), at most 4.  One persistent launch."""
-    lib = _lib.load()
-    if not 1 <= len(problems) <= 4:
-        raise _lib.PulseError("gemm_grouped takes 1..4 problems")
-    arr = (_lib.GemmProblem * len(problems))()
-    flags0 = None
-    for i, (a, b, kw) in enumerate(problems):
-        ep, M, N, K, flags, split_k = _prepare(a, b, **kw)
-        if flags0 is None:
-            flags0 = flags
-        elif flags != flags0:
-            raise _lib.PulseError("gemm_grouped: all problems must share the operand majors")
-        arr[i].a, arr[i].lda, arr[i].b, arr[i].ldb = a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0)
-        arr[i].m, arr[i].n, arr[i].k, arr[i].ep, arr[i].split_k = M, N, K, ep, split_k
-    dev = problems[0][0].device
-    with torch.cuda.device(dev):
-        _lib.check(lib.pulse_gemm_bf16_grouped(arr, len(problems), flags0, _lib.current_stream(dev)), "pulse_gemm_bf16_grouped")

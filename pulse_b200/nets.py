@@ -415,7 +415,7 @@ class MLP:
         l = self.layers[i]
         return not self.headless and i == len(self.layers) - 1 and i > 0 and l.N == 1 and self.layers[i - 1].act == "relu" and l.Kp <= 2048
 
-    # ---- per-layer GEMM arguments, shared by the single-problem path below and the grouped (lock-step) path ----------------------
+    # ---- per-layer GEMM arguments ------------------------------------------------------------------------------------------------
     def _fwd_problem(self, i: int, h: torch.Tensor, ws: dict, train: bool):
         l = self.layers[i]
         kw = dict(bias=None if self.aug else l.bias, act=l.act, out=ws["act"][i], preact=ws["pre"][i] if train else None)
@@ -570,67 +570,3 @@ def normalize_to_bf16(x: torch.Tensor, mean: Optional[torch.Tensor], rstd: Optio
                                                _lib.current_stream(x.device)),
                    "pulse_normalize_to_bf16")
 
-
-# ---------------------------------------------------------------------------------------------------------------------------
-# Lock-step execution of several MLPs of the same depth through GROUPED launches (pulse_gemm_bf16_grouped): the hidden layers of
-# all nets in one persistent launch per layer, likewise their weight-gradient and their dgrad GEMMs.  Validated against the
-# three-stream path by tests/test_gpu_grouped.py; used only when PULSE_GROUPED=1 (dense.grouped_enabled()).  MLP.forward / MLP.backward
-# above remain the validated path and are not touched by this code.
-# ---------------------------------------------------------------------------------------------------------------------------
-def forward_lockstep(mlps: Sequence["MLP"], xs: Sequence[torch.Tensor], train: bool = False) -> List[torch.Tensor]:
-    from .dense import gemm_grouped
-    depth = len(mlps[0].layers)
-    if any(len(m.layers) != depth for m in mlps) or any(x.shape[0] != xs[0].shape[0] for x in xs):
-        raise _lib.PulseError("forward_lockstep needs nets of the same depth on batches of the same size")
-    M = xs[0].shape[0]
-    wss = [m._workspace(M, train) for m in mlps]
-    hs = list(xs)
-    for i in range(depth - 1):
-        gemm_grouped([m._fwd_problem(i, h, ws, train) for m, ws, h in zip(mlps, wss, hs)])
-        hs = [ws["act"][i] for ws in wss]
-    outs = []
-    for m, ws, h, x in zip(mlps, wss, hs, xs):       # heads: the single-net code of MLP.forward (GEMV kernel or fp32-output GEMM)
-        i = depth - 1
-        l = m.layers[i]
-        if m._head1(i):
-            bias = m._zero_bias() if m.aug else l.bias
-            with torch.cuda.device(m.flat.device):
-                _lib.check(_lib.load().pulse_head1_forward(h.data_ptr(), h.stride(0), M, l.Kp, l.w_bf16.data_ptr(), bias.data_ptr(),
-                                                           ws["out"].data_ptr(), ws["out"].stride(0), _lib.current_stream(m.flat.device)),
-                           "pulse_head1_forward")
-        else:
-            gemm_nt(h[:, :l.Kp], l.w_bf16, bias=None if m.aug else l.bias, act=None, out_f32=ws["out"])
-        if train:
-            m._ws[(M, True)]["x"] = x
-        outs.append(ws["out"])
-    return outs
-
-
-def backward_lockstep(mlps: Sequence["MLP"], douts: Sequence[torch.Tensor], M: int) -> None:
-    """ADDS the weight / bias gradients of every net into its flat gradient buffer (see MLP.backward)."""
-    from .dense import gemm_grouped
-    depth = len(mlps[0].layers)
-    wss = [m._ws[(M, True)] for m in mlps]
-    dys, tops = [], []
-    for m, ws, dy in zip(mlps, wss, douts):           # heads first, per net (MLP.backward's head handling)
-        dy, top = m._backward_head(ws, dy, M)
-        dys.append(dy)
-        tops.append(top)
-    for i in reversed(range(depth)):
-        live = [j for j in range(len(mlps)) if tops[j] >= i]     # a fused single-output head has consumed the top layer of its net
-        if not live:
-            continue
-        wg, dg = [], []
-        for j in live:
-            m, ws, dy = mlps[j], wss[j], dys[j]
-            x_in = ws["x"] if i == 0 else ws["act"][i - 1]
-            wg.append(m._wgrad_problem(i, dy, x_in, ws))
-            if i > 0:
-                if m.layers[i - 1].act != "relu":
-                    raise _lib.PulseError("backward_lockstep groups ReLU nets only (the grouped dgrad kernel is the ReLU-gate specialisation)")
-                dg.append(m._dgrad_problem(i, dy, ws))
-        gemm_grouped(wg)
-        if dg:
-            gemm_grouped(dg)
-            for j in live:
-                dys[j] = wss[j]["dact"][i - 1]

@@ -97,8 +97,6 @@ class RunningMeanStdB200:
 
 
 class PPOPolicy:
-    grouped_ok = True    # PULSE_GROUPED may run actor + critic in lock step (subclasses whose nets do not fit it set False)
-
     def __init__(self, obs_size: int = 934, num_actions: int = 69, units: Sequence[int] = (1024, 512), act: str = "relu",
                  logstd: float = -2.9, device="cuda:0", seed: int = 0, lr: float = 2e-5, e_clip: float = 0.2, critic_coef: float = 5.0,
                  bounds_coef: float = 10.0, grad_norm: float = 50.0, normalize_value: bool = True, with_disc: bool = False,
@@ -166,13 +164,8 @@ class PPOPolicy:
         M = obs.shape[0]
         b = self._buf(M, False)
         self._normalize_eval(obs, b)
-        from .dense import grouped_enabled
-        if self.grouped_ok and grouped_enabled():   # experimental (default off): actor + critic hidden layers in one grouped launch per layer
-            from .nets import forward_lockstep
-            mu, value = forward_lockstep((self.actor, self.critic), (b["x"], b["x"]))
-        else:
-            mu = self.actor.forward(b["x"])
-            value = self.critic.forward(b["x"])
+        mu = self.actor.forward(b["x"])
+        value = self.critic.forward(b["x"])
         if eps is None:
             eps = torch.randn(M, self.A, device=self.device)
         with torch.cuda.device(self.device):
@@ -343,9 +336,7 @@ class PPOPolicy:
                 if reducer is not None:
                     d0, d1 = self.disc.mlp.param_span()
                     reducer.reduce(self.flat.grads[d0:d1], 2)
-        from .dense import grouped_enabled
-        grouped = self.grouped_ok and grouped_enabled()    # PULSE_GROUPED=1: actor + critic in lock step through grouped launches (experimental, default off)
-        mu, value = self._forward_train(b, slot, grouped)
+        mu, value = self._forward_train(b, slot)
         a = _lib.PpoLossArgs(
             mu=mu.data_ptr(), ld_mu=mu.stride(0), value=value.data_ptr(), ld_value=value.stride(0), actions=actions.data_ptr(),
             old_neglogp=old_neglogp.data_ptr(), advantages=advantages.data_ptr(), returns=returns.data_ptr(),
@@ -357,7 +348,7 @@ class PPOPolicy:
             _lib.check(self.lib.pulse_ppo_loss(C.byref(a), M, _lib.current_stream(self.device)), "pulse_ppo_loss")
         if pref_at == "loss":
             fork_prefetch()
-        self._backward_train(b, M, grouped, reducer)
+        self._backward_train(b, M, reducer)
         if amp is not None:
             main.wait_stream(s_disc)
         if pref_at == "reduce":
@@ -375,12 +366,9 @@ class PPOPolicy:
             main.wait_stream(s_pref)
         return self.stats
 
-    def _forward_train(self, b: dict, slot: int, grouped: bool):
+    def _forward_train(self, b: dict, slot: int):
         """Training forward pass of the policy nets on operand slot `slot` of the minibatch buffers: (mu, value), fp32."""
         x = b["x2"][slot]
-        if grouped:
-            from .nets import forward_lockstep
-            return forward_lockstep((self.actor, self.critic), (x, x), train=True)
         main, s_critic = torch.cuda.current_stream(self.device), self._side[0]
         s_critic.wait_stream(main)
         with torch.cuda.stream(s_critic):
@@ -389,17 +377,9 @@ class PPOPolicy:
         main.wait_stream(s_critic)
         return mu, value
 
-    def _backward_train(self, b: dict, M: int, grouped: bool, reducer) -> None:
+    def _backward_train(self, b: dict, M: int, reducer) -> None:
         """Backward pass of the policy nets from the loss kernel's output gradients b['dmu'] / b['dv']; `reducer` (multi-GPU, per-chain
         gradient exchange) averages each net's gradient slice once it is complete."""
-        if grouped:
-            from .nets import backward_lockstep
-            backward_lockstep((self.actor, self.critic), (b["dmu"], b["dv"]), M)
-            if reducer is not None:                      # lock-step path: actor + critic slices are adjacent, one reduction
-                a0, _ = self.actor.param_span()
-                _, c1 = self.critic.param_span()
-                reducer.reduce(self.flat.grads[a0:c1], 0)
-            return
         main, s_critic = torch.cuda.current_stream(self.device), self._side[0]
         s_critic.wait_stream(main)
         with torch.cuda.stream(s_critic):

@@ -32,8 +32,6 @@ from .ppo import PPOPolicy
 
 
 class SeptPolicy(PPOPolicy):
-    grouped_ok = False
-
     def __init__(self, self_obs_size: int = 358, task_obs_size_detail: Optional[Dict[str, int]] = None, task_units: Sequence[int] = (512, 256),
                  units: Sequence[int] = (2048, 1024, 512), act: str = "silu", num_actions: int = 32, with_disc: bool = True,
                  task_act: Optional[str] = None, logstd: float = -1.0, **kw):
@@ -110,12 +108,12 @@ class SeptPolicy(PPOPolicy):
         if amp is not None:
             self.disc.prepare_inputs(*amp, slot=slot)
 
-    def _forward_train(self, b: dict, slot: int, grouped: bool):
+    def _forward_train(self, b: dict, slot: int):
         self.task.forward(b["t2"][slot], train=True, out=b["x2"][slot][:, :self.E])
-        return super()._forward_train(b, slot, False)
+        return super()._forward_train(b, slot)
 
-    def _backward_train(self, b: dict, M: int, grouped: bool, reducer) -> None:
-        super()._backward_train(b, M, False, None)          # reducer is None: chain exchange refused in _reducer
+    def _backward_train(self, b: dict, M: int, reducer) -> None:
+        super()._backward_train(b, M, None)                 # reducer is None: chain exchange refused in _reducer
         gemm(b["dpre0"], self._w0_cat[:, :self.E], b_mn=True, gate=self.task.top_preact(M), gate_mode="silu", out=b["demb"])
         self.task.backward(b["demb"], M)
 

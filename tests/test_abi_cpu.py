@@ -38,14 +38,14 @@ def test_struct_sizes_match_header(lib):
     import subprocess
     import tempfile
     from pulse_b200 import _lib
-    src = '#include <stdio.h>\n#include "pulse_b200.h"\nint main(){printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(pulse_motionlib_desc_t), sizeof(pulse_motion_query_t), sizeof(pulse_im_step_args_t), sizeof(pulse_amp_obs_args_t), sizeof(pulse_gae_args_t), sizeof(pulse_gemm_epilogue_t), sizeof(pulse_ppo_loss_args_t), sizeof(pulse_vae_latent_args_t), sizeof(pulse_reach_step_args_t), sizeof(pulse_loader_args_t), sizeof(pulse_gemm_problem_t), sizeof(pulse_reset_args_t), sizeof(pulse_policy_post_args_t), sizeof(pulse_amp_row_args_t), sizeof(pulse_peer_adam_args_t), sizeof(pulse_eval_args_t), sizeof(pulse_task_obs_args_t), sizeof(pulse_ztask_step_args_t));return 0;}\n'
+    src = '#include <stdio.h>\n#include "pulse_b200.h"\nint main(){printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(pulse_motionlib_desc_t), sizeof(pulse_motion_query_t), sizeof(pulse_im_step_args_t), sizeof(pulse_amp_obs_args_t), sizeof(pulse_gae_args_t), sizeof(pulse_gemm_epilogue_t), sizeof(pulse_ppo_loss_args_t), sizeof(pulse_vae_latent_args_t), sizeof(pulse_reach_step_args_t), sizeof(pulse_loader_args_t), sizeof(pulse_reset_args_t), sizeof(pulse_policy_post_args_t), sizeof(pulse_amp_row_args_t), sizeof(pulse_peer_adam_args_t), sizeof(pulse_eval_args_t), sizeof(pulse_task_obs_args_t), sizeof(pulse_ztask_step_args_t));return 0;}\n'
     with tempfile.TemporaryDirectory() as d:
         open(os.path.join(d, "s.c"), "w").write(src)
         subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), os.path.join(d, "s.c"), "-o", os.path.join(d, "s")])
         sizes = [int(x) for x in subprocess.check_output([os.path.join(d, "s")]).split()]
     assert sizes == [C.sizeof(_lib.MotionLibDesc), C.sizeof(_lib.MotionQuery), C.sizeof(_lib.ImStepArgs), C.sizeof(_lib.AmpObsArgs),
                      C.sizeof(_lib.GaeArgs), C.sizeof(_lib.GemmEpilogue), C.sizeof(_lib.PpoLossArgs), C.sizeof(_lib.VaeLatentArgs),
-                     C.sizeof(_lib.ReachStepArgs), C.sizeof(_lib.LoaderArgs), C.sizeof(_lib.GemmProblem), C.sizeof(_lib.ResetArgs), C.sizeof(_lib.PolicyPostArgs),
+                     C.sizeof(_lib.ReachStepArgs), C.sizeof(_lib.LoaderArgs), C.sizeof(_lib.ResetArgs), C.sizeof(_lib.PolicyPostArgs),
                      C.sizeof(_lib.AmpRowArgs), C.sizeof(_lib.PeerAdamArgs), C.sizeof(_lib.EvalArgs), C.sizeof(_lib.TaskObsArgs), C.sizeof(_lib.ZTaskStepArgs)]
 
 

@@ -1,7 +1,7 @@
 """The update's links, element by element, against float64 references fed the kernels' own operands (tests/fp64_ref.py).
 
 PPO with the AMP discriminator (one train_minibatch at the production minibatch, M = 16384 with B = 4096 AMP rows, and at a ragged
-one, M = 5000 with B = 1000) in every GEMM mode -- default, PULSE_GEMM_BN=128, PULSE_GEMM_STAGES=4, PULSE_GROUPED=1 -- and the PULSE
+one, M = 5000 with B = 1000) in every GEMM mode -- default, PULSE_GEMM_BN=128, PULSE_GEMM_STAGES=4 -- and the PULSE
 VAE at the im_z_fit.yaml widths (optimize_kin(step=False) at M = 16384 and M = 4064).  Every link has its own tight bound, so a
 missing k-block, a split-K slice added twice, a mask read from the wrong rows, a dropped bias column or a wrong coefficient fails
 here even where the cosine checks of test_gpu_ppo.py / test_gpu_vae.py (against fp32 autograd) cannot see it.
@@ -66,7 +66,7 @@ def _disc_stats(pol):
     return f64(r.running_mean).clone(), f64(r.running_var).clone(), float(r.count)
 
 
-MODES = {"default": {}, "bn128": {"PULSE_GEMM_BN": "128"}, "stages4": {"PULSE_GEMM_STAGES": "4"}, "grouped": {"PULSE_GROUPED": "1"}}
+MODES = {"default": {}, "bn128": {"PULSE_GEMM_BN": "128"}, "stages4": {"PULSE_GEMM_STAGES": "4"}}
 
 
 @pytest.mark.parametrize("M,B", [(16384, 4096), (5000, 1000)])
