@@ -733,6 +733,111 @@ typedef struct {
 } pulse_ztask_step_args_t;
 int pulse_ztask_step(const pulse_ztask_step_args_t* args, int64_t num_envs, void* stream);
 
+/* The observation-only part of pulse_reach_step / pulse_ztask_step over env_list[0 .. *count) (device-side count, num_envs bounds it):
+ * _compute_observations(env_ids) of the reset envs.  The same per-env code as the step kernels writes the same rows bit for bit; no
+ * reward, reset or terminate word and no other row is written.  The argument structs are the step's; only the observation inputs
+ * (body_state, tar_pos / tar_speed / target_states, obs_buf) are read. */
+int pulse_reach_obs_list(const pulse_reach_step_args_t* args, const int64_t* env_list, const int32_t* count, int64_t num_envs, void* stream);
+int pulse_ztask_obs_list(const pulse_ztask_step_args_t* args, const int64_t* env_list, const int32_t* count, int64_t num_envs, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Reference-state reset of the latent-space tasks HumanoidReach(Z) / HumanoidSpeed(Z) / HumanoidStrike(Z), free of host
+ * synchronisation: HumanoidAMPTask._reset_envs for StateInit.Random / Start and humanoid_type "smpl", without its observation and
+ * _reset_task (those follow: the task's observation over env_list, then pulse_ztask_reset_task).  For the reset set (reset_buf mask
+ * or env id list), two launches:
+ *   1. ordered compaction into env_list / actor_list / tar_actor_list and a device-side count;
+ *   2. one warp per (reset env, AMP history step k):
+ *      - clip: sample_motions (motion_lib_base.py:395-398), a new clip per reset env: injected, or an inverse-CDF search of a
+ *        Philox uniform over sampling_cdf (zero-weight clips are never drawn);
+ *      - start time: sample_time_interval (:411-420) for PULSE_ZINIT_RANDOM, 0 for PULSE_ZINIT_START;
+ *      - get_motion_state without offset, then the SMPL ground fix of _get_fixed_smpl_state_from_motionlib (humanoid_amp.py:382-430):
+ *        d = (floor[f0] + root_z) - 0.02 with f0 the unblended frame, root_z -= d and every body z -= d;
+ *      - pose_mode: AS_IS; ROOT_XY_ZERO (humanoid_reach.py:46-48, humanoid_strike.py:147-150: root xy <- 0, bodies keep theirs);
+ *        FACE_X (humanoid_speed.py:251-270: the heading inverse of root_rot, or of remove_base_rot(root_rot) when !upright, rotates
+ *        root_rot, the bodies about the root, body rotations, root velocity, root angular velocity and body velocities; body angular
+ *        velocities and dofs stay);
+ *      - _set_env_state (humanoid_amp.py:565-597) into the root, dof and rigid-body views, _sampled_motion_ids / _motion_start_times
+ *        (:484-485), and _reset_env_tensors (humanoid.py:589-609): progress / reset / terminate and contact forces <- 0;
+ *      - strike (target_states != NULL): _reset_target (humanoid_strike.py:124-145) around the new root xy;
+ *      - AMP history (humanoid_amp.py:519-563): row 0 from the rigid bodies and dofs just written (what _compute_amp_observations
+ *        reads after the _reset_rb_* restore), rows k >= 1 from the UNADJUSTED motion at t0 - k*dt.  amp_width 196 is the layout of
+ *        pulse_reset_ref_state, 195 the same without the root height (ampRootHeightObs False, :305-306).
+ * Draws: injected per ENV, or Philox4x32-10 on (seed, index, offset + *offset_dev), one word per draw:
+ *   index e            x: start-time phase (the word pulse_reset_ref_state uses)   y: clip   z: strike near   w: strike distance
+ *   index e + 2^32     x: strike bearing   y: strike yaw
+ *   index e + 2^33     pulse_ztask_reset_task: x, y, z task uniforms, w change steps
+ * ---------------------------------------------------------------------------------------------- */
+#define PULSE_ZTASK_REACH 3
+#define PULSE_ZPOSE_AS_IS 0
+#define PULSE_ZPOSE_ROOT_XY_ZERO 1
+#define PULSE_ZPOSE_FACE_X 2
+#define PULSE_ZINIT_RANDOM 0
+#define PULSE_ZINIT_START 1
+#define PULSE_AMP_OBS_NO_HEIGHT 195
+
+typedef struct {
+  int64_t* reset_buf;            /* [N] mask mode: envs with reset_buf != 0 are reset; cleared for them */
+  const int64_t* env_ids_in;     /* list mode: ascending env ids [num_ids] (an id outside [0, N) or not above its predecessor is
+                                    skipped); NULL = mask mode */
+  int64_t num_ids;
+  const int64_t* motion_ids_in;  /* [N] injected clip per env, or NULL: Philox + inverse CDF */
+  const float* motion_u;         /* [N] injected clip uniform per env (inverse CDF), or NULL; ignored with motion_ids_in */
+  const float* phase;            /* [N] injected start-time uniform per env, or NULL: Philox */
+  const float* strike_u;         /* [N, 4] injected strike uniforms (near, distance, bearing, yaw) per env, or NULL: Philox */
+  const float* sampling_cdf;     /* [num_motions] inclusive fp32 prefix sum of _sampling_batch_prob; required without motion_ids_in */
+  uint64_t seed, offset;
+  const uint64_t* offset_dev;    /* optional device-side counter added to `offset` */
+  const float* floor;            /* [floor_len >= total_frames] per-frame min vertex z - root joint z at zero translation */
+  int64_t floor_len;
+  int32_t pose_mode;             /* PULSE_ZPOSE_* */
+  int32_t upright;               /* _has_upright_start (FACE_X heading and the AMP rotation features) */
+  int32_t state_init;            /* PULSE_ZINIT_* */
+  int32_t amp_width;             /* 196 or 195 */
+  int32_t num_amp_steps;         /* numAMPObsSteps; 0 with amp_obs_buf NULL */
+  float dt;                      /* control dt */
+  float* amp_obs_buf;            /* [N, num_amp_steps, amp_width] or NULL */
+  int64_t* sampled_motion_ids;   /* [N] <- clip */
+  float* motion_start_times;     /* [N] <- start time */
+  int64_t* progress_buf;         /* [N] <- 0 */
+  int64_t* terminate_buf;        /* [N] <- 0 (may be NULL) */
+  float* root_states; int64_t root_env_stride;
+  float* dof_pos; float* dof_vel; int64_t dof_env_stride; int64_t dof_elem_stride;
+  float* rigid_body_state; int64_t body_env_stride;      /* [N, bodies_per_env, 13], required */
+  float* contact_forces; int64_t contact_env_stride; int32_t contact_bodies;   /* <- 0; may be NULL */
+  int32_t reserved;
+  float* target_states; int64_t target_env_stride;       /* strike: [N, 13] view of the target actor's root state; NULL otherwise */
+  float near_prob, near_dist, tar_dist_min, tar_dist_max;
+  const int32_t* actor_ids;      /* [N] _humanoid_actor_ids or NULL (env id) */
+  const int32_t* tar_actor_ids;  /* [N] _tar_actor_ids or NULL (env id) */
+  int64_t* env_list;             /* [N] out: the reset env ids, ascending */
+  int32_t* actor_list;           /* [N] out, optional */
+  int32_t* tar_actor_list;       /* [N] out, optional */
+  int32_t* count;                /* [1] out, device side */
+} pulse_ztask_reset_args_t;
+int pulse_reset_ztask(const pulse_motionlib_t* lib, const pulse_ztask_reset_args_t* args, int64_t num_envs, void* stream);
+
+/* _reset_task of the reach and speed tasks over the env list of pulse_reset_ztask (run after the observation, as the reference does),
+ * draws injected per env or Philox words of index e + 2^33:
+ *   PULSE_ZTASK_REACH  humanoid_reach.py:134-146  tar_pos = (dist_max (2u - 1), dist_max (2v - 1), height_scale w + height_min)
+ *   PULSE_ZTASK_SPEED  humanoid_speed.py:166-175  tar_speed = speed_scale u + speed_min
+ * and change_steps = progress + randint(steps_min, steps_max); from a Philox word w, steps_min + (w (steps_max - steps_min)) >> 32. */
+typedef struct {
+  int32_t kind; int32_t reserved;
+  const int64_t* env_list; const int32_t* count;
+  const float* rand;             /* injected: reach [N, 3], speed [N]; or NULL: Philox */
+  const int64_t* steps_in;       /* injected randint results [N], or NULL: Philox */
+  uint64_t seed, offset;
+  const uint64_t* offset_dev;
+  const int64_t* progress_buf;
+  int64_t* change_steps;         /* _tar_change_steps / _speed_change_steps */
+  float* tar_pos;                /* reach [N, 3] */
+  float* tar_speed;              /* speed [N] */
+  float dist_max, height_scale, height_min, speed_scale, speed_min;
+  int32_t reserved2;
+  int64_t steps_min, steps_max;
+} pulse_ztask_task_args_t;
+int pulse_ztask_reset_task(const pulse_ztask_task_args_t* args, int64_t num_envs, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Pedestrian terrain task HumanoidPedestrianTerrain(Z) (phc/env/tasks/humanoid_pedestrian_terrain.py): post_physics_step in one launch,
  * one warp per env, selected by PULSE_STEP_REWARD / RESET / OBS:

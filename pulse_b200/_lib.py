@@ -204,7 +204,35 @@ class ZTaskStepArgs(C.Structure):
     ]
 
 
-ZTASK_SPEED, ZTASK_STRIKE = 1, 2
+ZTASK_SPEED, ZTASK_STRIKE, ZTASK_REACH = 1, 2, 3
+ZPOSE_AS_IS, ZPOSE_ROOT_XY_ZERO, ZPOSE_FACE_X = 0, 1, 2
+ZINIT_RANDOM, ZINIT_START = 0, 1
+
+
+class ZTaskResetArgs(C.Structure):
+    _fields_ = [
+        ("reset_buf", C.c_void_p), ("env_ids_in", C.c_void_p), ("num_ids", C.c_int64), ("motion_ids_in", C.c_void_p), ("motion_u", C.c_void_p), ("phase", C.c_void_p),
+        ("strike_u", C.c_void_p), ("sampling_cdf", C.c_void_p), ("seed", C.c_uint64), ("offset", C.c_uint64), ("offset_dev", C.c_void_p),
+        ("floor", C.c_void_p), ("floor_len", C.c_int64), ("pose_mode", C.c_int32), ("upright", C.c_int32), ("state_init", C.c_int32),
+        ("amp_width", C.c_int32), ("num_amp_steps", C.c_int32), ("dt", C.c_float), ("amp_obs_buf", C.c_void_p),
+        ("sampled_motion_ids", C.c_void_p), ("motion_start_times", C.c_void_p), ("progress_buf", C.c_void_p), ("terminate_buf", C.c_void_p),
+        ("root_states", C.c_void_p), ("root_env_stride", C.c_int64), ("dof_pos", C.c_void_p), ("dof_vel", C.c_void_p),
+        ("dof_env_stride", C.c_int64), ("dof_elem_stride", C.c_int64), ("rigid_body_state", C.c_void_p), ("body_env_stride", C.c_int64),
+        ("contact_forces", C.c_void_p), ("contact_env_stride", C.c_int64), ("contact_bodies", C.c_int32), ("reserved", C.c_int32),
+        ("target_states", C.c_void_p), ("target_env_stride", C.c_int64), ("near_prob", C.c_float), ("near_dist", C.c_float),
+        ("tar_dist_min", C.c_float), ("tar_dist_max", C.c_float), ("actor_ids", C.c_void_p), ("tar_actor_ids", C.c_void_p),
+        ("env_list", C.c_void_p), ("actor_list", C.c_void_p), ("tar_actor_list", C.c_void_p), ("count", C.c_void_p),
+    ]
+
+
+class ZTaskTaskArgs(C.Structure):
+    _fields_ = [
+        ("kind", C.c_int32), ("reserved", C.c_int32), ("env_list", C.c_void_p), ("count", C.c_void_p), ("rand", C.c_void_p),
+        ("steps_in", C.c_void_p), ("seed", C.c_uint64), ("offset", C.c_uint64), ("offset_dev", C.c_void_p), ("progress_buf", C.c_void_p),
+        ("change_steps", C.c_void_p), ("tar_pos", C.c_void_p), ("tar_speed", C.c_void_p), ("dist_max", C.c_float), ("height_scale", C.c_float),
+        ("height_min", C.c_float), ("speed_scale", C.c_float), ("speed_min", C.c_float), ("reserved2", C.c_int32),
+        ("steps_min", C.c_int64), ("steps_max", C.c_int64),
+    ]
 
 
 class TerrainStepArgs(C.Structure):
@@ -363,6 +391,10 @@ SIGNATURES = {
                                           C.c_int64, C.c_void_p]),
     "pulse_reach_step": (C.c_int, [C.POINTER(ReachStepArgs), C.c_int64, C.c_void_p]),
     "pulse_ztask_step": (C.c_int, [C.POINTER(ZTaskStepArgs), C.c_int64, C.c_void_p]),
+    "pulse_reach_obs_list": (C.c_int, [C.POINTER(ReachStepArgs), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "pulse_ztask_obs_list": (C.c_int, [C.POINTER(ZTaskStepArgs), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "pulse_reset_ztask": (C.c_int, [C.c_void_p, C.POINTER(ZTaskResetArgs), C.c_int64, C.c_void_p]),
+    "pulse_ztask_reset_task": (C.c_int, [C.POINTER(ZTaskTaskArgs), C.c_int64, C.c_void_p]),
     "pulse_terrain_step": (C.c_int, [C.POINTER(TerrainStepArgs), C.c_int64, C.c_void_p]),
     "pulse_traj_reset": (C.c_int, [C.POINTER(TrajResetArgs), C.c_void_p]),
     "pulse_terrain_heights": (C.c_int, [C.POINTER(TerrainHeightsArgs), C.c_void_p]),

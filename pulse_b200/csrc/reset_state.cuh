@@ -8,40 +8,18 @@
 //                           humanoid.py:589-609); every k writes its AMP observation row (_init_amp_obs, humanoid_amp.py:519-563).
 // HBM-bound gather / scatter: ~44 KB of packed frame records per reset env (20 rows x 2 208 B), ~11 KB written.
 #pragma once
+#include "compact.cuh"
 #include "philox.cuh"
 #include "humanoid_obs.cuh"
 
 namespace pulse {
 namespace {
 
-constexpr int kCompactThreads = 1024;
-
 // Env behind candidate i of a reset set: entry i of the explicit id list, or i itself when reset_buf[i] != 0 (mask mode); -1 if none.
 __device__ __forceinline__ long long reset_candidate(const pulse_reset_args_t& a, long long i, long long n) {
   if (i >= n) return -1;
   if (a.env_ids_in != nullptr) return a.env_ids_in[i];
   return a.reset_buf[i] != 0 ? i : -1;
-}
-
-// One round of an ordered compaction over a CTA of kCompactThreads threads, called by all of them together: a thread with `take`
-// gets slot *base + (takers before it in thread order), -1 otherwise; *base (shared) then advances by the round's takers.
-__device__ __forceinline__ int compact_slot(bool take, int* warp_cnt, int* base) {
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const unsigned m = __ballot_sync(kFull, take);
-  if (lane == 0) warp_cnt[wid] = __popc(m);
-  __syncthreads();
-  int before = 0, total = 0;
-#pragma unroll 1
-  for (int w = 0; w < kCompactThreads / 32; ++w) {
-    const int c = warp_cnt[w];
-    if (w < wid) before += c;
-    total += c;
-  }
-  const int pos = take ? *base + before + __popc(m & ((1u << lane) - 1u)) : -1;
-  __syncthreads();
-  if (tid == 0) *base += total;
-  __syncthreads();
-  return pos;
 }
 
 __global__ void __launch_bounds__(256) reset_ref_state_kernel(const pulse_motionlib_desc_t lib, const pulse_reset_args_t a) {

@@ -151,6 +151,15 @@ class MotionLibB200:
     def sample_motions(self, n):
         return torch.multinomial(self._sampling_batch_prob, num_samples=n, replacement=True).to(self._device)
 
+    def sampling_cdf(self) -> torch.Tensor:
+        """Inclusive fp32 prefix sum of `_sampling_batch_prob` on the device: the kernels draw clips by an inverse-CDF search of it.
+        Rebuilt whenever `_sampling_batch_prob` is replaced or changed in place (the tensor's version counter), without reading it."""
+        p = self._sampling_batch_prob
+        if getattr(self, "_cdf_src", None) is not p or self._cdf_version != p._version:
+            self._cdf = torch.cumsum(p.to(self._device, torch.float32), 0).contiguous()
+            self._cdf_src, self._cdf_version = p, p._version
+        return self._cdf
+
     def sample_time(self, motion_ids, truncate_time=None):
         phase = torch.rand(motion_ids.shape, device=self._device)
         motion_len = self._motion_lengths[motion_ids]

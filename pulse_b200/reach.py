@@ -63,7 +63,21 @@ class ReachTaskB200:
     def post_physics_step(self, rigid_body_state: torch.Tensor, progress_buf: torch.Tensor, contact_forces: Optional[torch.Tensor] = None) -> None:
         """_compute_reward + _compute_reset + _compute_observations (humanoid.py:1315-1330 order) in one launch.
         rigid_body_state fp32 [N, B_env >= 24, 13] (Isaac Gym view, read in place); contact_forces fp32 [N, B_env, 3]."""
-        a = _lib.ReachStepArgs(
+        a = self._step_args(rigid_body_state, progress_buf, contact_forces)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.pulse_reach_step(C.byref(a), self.num_envs, _lib.current_stream(self.device)), "pulse_reach_step")
+
+    def observe_list(self, rigid_body_state: torch.Tensor, env_list: torch.Tensor, count: torch.Tensor, progress_buf: torch.Tensor,
+                     contact_forces: Optional[torch.Tensor] = None) -> None:
+        """_compute_observations(env_ids) for the envs env_list[0 .. *count) (int64 list, int32 device-side count): the rows
+        post_physics_step writes for them, bit for bit, and nothing else."""
+        a = self._step_args(rigid_body_state, progress_buf, contact_forces)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.pulse_reach_obs_list(C.byref(a), env_list.data_ptr(), count.data_ptr(), self.num_envs,
+                                                     _lib.current_stream(self.device)), "pulse_reach_obs_list")
+
+    def _step_args(self, rigid_body_state, progress_buf, contact_forces):
+        return _lib.ReachStepArgs(
             body_state=rigid_body_state.data_ptr(), body_env_stride=rigid_body_state.stride(0),
             contact_forces=contact_forces.data_ptr() if contact_forces is not None else None,
             contact_env_stride=contact_forces.stride(0) if contact_forces is not None else 0,
@@ -71,5 +85,3 @@ class ReachTaskB200:
             contact_body_mask=self.contact_body_mask, reach_body_id=self.reach_body_id, enable_early_termination=int(self.enable_early_termination),
             max_episode_length=self.max_episode_length, obs_buf=self.obs_buf.data_ptr(), obs_stride=self.obs_buf.stride(0),
             rew_buf=self.rew_buf.data_ptr(), reset_buf=self.reset_buf.data_ptr(), terminate_buf=self._terminate_buf.data_ptr())
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.pulse_reach_step(C.byref(a), self.num_envs, _lib.current_stream(self.device)), "pulse_reach_step")

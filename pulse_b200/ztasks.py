@@ -60,6 +60,11 @@ class _ZTaskBase:
         with torch.cuda.device(self.device):
             _lib.check(self.lib.pulse_ztask_step(C.byref(a), self.num_envs, _lib.current_stream(self.device)), "pulse_ztask_step")
 
+    def _launch_list(self, a, env_list: torch.Tensor, count: torch.Tensor) -> None:
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.pulse_ztask_obs_list(C.byref(a), env_list.data_ptr(), count.data_ptr(), self.num_envs,
+                                                     _lib.current_stream(self.device)), "pulse_ztask_obs_list")
+
 
 class SpeedTaskB200(_ZTaskBase):
     """HumanoidSpeed (humanoid_speed.py:17-240): run along +x at a commanded speed."""
@@ -103,6 +108,13 @@ class SpeedTaskB200(_ZTaskBase):
             a.dof_vel, a.dof_env_stride, a.dof_elem_stride = dof_vel.data_ptr(), dof_vel.stride(0), dof_vel.stride(1)
         self._launch(a)
 
+    def observe_list(self, rigid_body_state: torch.Tensor, env_list: torch.Tensor, count: torch.Tensor, progress_buf: torch.Tensor,
+                     contact_forces: Optional[torch.Tensor] = None) -> None:
+        """_compute_observations(env_ids) for the envs env_list[0 .. *count): post_physics_step's rows for them, nothing else."""
+        a = self._args(rigid_body_state, progress_buf, contact_forces)
+        a.tar_speed = self._tar_speed.data_ptr()
+        self._launch_list(a, env_list, count)
+
 
 class StrikeTaskB200(_ZTaskBase):
     """HumanoidStrike (humanoid_strike.py:17-240): walk to a standing target and knock it over."""
@@ -145,3 +157,10 @@ class StrikeTaskB200(_ZTaskBase):
         a.target_states, a.target_env_stride = target_states.data_ptr(), target_states.stride(0)
         a.tar_contact_forces, a.tar_contact_env_stride = tar_contact_forces.data_ptr(), tar_contact_forces.stride(0)
         self._launch(a)
+
+    def observe_list(self, rigid_body_state: torch.Tensor, env_list: torch.Tensor, count: torch.Tensor, progress_buf: torch.Tensor,
+                     target_states: torch.Tensor, contact_forces: Optional[torch.Tensor] = None) -> None:
+        """_compute_observations(env_ids) for the envs env_list[0 .. *count): post_physics_step's rows for them, nothing else."""
+        a = self._args(rigid_body_state, progress_buf, contact_forces)
+        a.target_states, a.target_env_stride = target_states.data_ptr(), target_states.stride(0)
+        self._launch_list(a, env_list, count)
