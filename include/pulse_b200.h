@@ -766,6 +766,7 @@ int pulse_ztask_obs_list(const pulse_ztask_step_args_t* args, const int64_t* env
  *   index e            x: start-time phase (the word pulse_reset_ref_state uses)   y: clip   z: strike near   w: strike distance
  *   index e + 2^32     x: strike bearing   y: strike yaw
  *   index e + 2^33     pulse_ztask_reset_task: x, y, z task uniforms, w change steps
+ *   index e + 3 * 2^32 pulse_ztask_pre_physics (_update_task of the rollout): x, y, z task uniforms, w change steps
  * ---------------------------------------------------------------------------------------------- */
 #define PULSE_ZTASK_REACH 3
 #define PULSE_ZPOSE_AS_IS 0
@@ -837,6 +838,72 @@ typedef struct {
   int64_t steps_min, steps_max;
 } pulse_ztask_task_args_t;
 int pulse_ztask_reset_task(const pulse_ztask_task_args_t* args, int64_t num_envs, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Rollout glue of the latent-space tasks (AMPAgent.play_steps, phc/learning/amp_agent.py:341-439, over HumanoidReachZ / HumanoidSpeedZ /
+ * HumanoidStrikeZ; HumanoidZ.step -> step_z, phc/env/tasks/humanoid_z.py:157-173), written into experience-buffer slices.
+ *
+ * pulse_latent_post: what pulse_policy_post followed by pulse_vae_reparam(PULSE_Z_RESIDUAL) do, in one launch, one warp per row:
+ *   a_z = mu + exp(logstd) * eps (eps injected, or Philox4x32-10 keyed (seed, row, *rng_offset + rng_step) exactly as
+ *   pulse_policy_post draws it), neglogp, the de-normalised value (running_mean_std.py:84-87), and z = prior_mu + a_z
+ *   (HumanoidZ.compute_z_actions, humanoid_z.py:104-107) as bf16 into the decoder operand's latent columns.  Every output is bit-equal
+ *   to the two-launch composition.  pulse_z_task.yaml has clip_actions False and project_to_norm(.., "none") is the identity, so a_z is
+ *   neither clamped nor projected.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  const float* mu; int64_t ld_mu;            /* [rows, latent] latent policy head output */
+  const float* logstd;                       /* [latent] */
+  const float* eps; int64_t ld_eps;          /* [rows, latent] injected standard-normal draws, or NULL -> Philox */
+  uint64_t seed; const uint64_t* rng_offset; uint64_t rng_step;
+  int32_t latent; int32_t reserved;          /* 1 .. 128 */
+  float* actions; int64_t ld_actions;        /* out: a_z */
+  float* neglogp; int64_t ld_neglogp;        /* out, element stride */
+  const float* value; int64_t ld_value;      /* [rows] normalised critic output */
+  const double* value_mean; const double* value_var; float value_eps; int32_t reserved2;   /* RunningMeanStd of the value (NULL = identity) */
+  float* values_out; int64_t ld_values;      /* out */
+  const float* prior_mu; int64_t ld_prior;   /* [rows, >= latent] frozen prior head; columns [0, latent) = prior mean */
+  pulse_bf16_t* z_bf16; int64_t ld_z;        /* out: z into columns [0, latent) of the decoder operand rows */
+} pulse_latent_post_args_t;
+int pulse_latent_post(const pulse_latent_post_args_t* args, int64_t rows, void* stream);
+
+/* pulse_ztask_pre_physics: the pre-physics work of one latent-task step over num_envs envs in one launch:
+ *   pd_out[e, d]   = freeze[d] ? 0 : pd_offset[d] + pd_scale[d] * action[e, d]      (pulse_pd_targets' arithmetic; humanoid.py:1222-1247)
+ *   prev_root_pos[e] = root_states[e, 0:3]                                          (speed, strike; humanoid_speed.py:73-76)
+ *   _update_task where progress_buf[e] >= change_steps[e]   (reach humanoid_reach.py:127-146, speed humanoid_speed.py:157-175):
+ *     PULSE_ZTASK_REACH  tar_pos = (dist_max (2u - 1), dist_max (2v - 1), (height_max - height_min) w + height_min), the arithmetic of
+ *                        pulse_reach_update_task
+ *     PULSE_ZTASK_SPEED  tar_speed = speed_scale u + speed_min (two roundings, as the tensor expression of the reference)
+ *     change_steps = progress + randint(steps_min, steps_max);  PULSE_ZTASK_STRIKE has no _update_task
+ *   Only due envs are written.  Draws: injected per ENV (rand: reach [N, 3], speed [N]; steps_in int64 [N]) or the Philox4x32-10 words of
+ *     index e + 3 * 2^32   x, y, z task uniforms, w change steps (steps_min + (w (steps_max - steps_min)) >> 32)
+ *   on (seed, index, offset + *offset_dev): a fourth index plane beside the three of pulse_reset_ztask / pulse_ztask_reset_task
+ *   (e, e + 2^32, e + 2^33), so a step that resets an env and later updates its task draws from different words. */
+typedef struct {
+  int32_t kind; int32_t dofs;
+  const float* action; int64_t ld_action;    /* [N, dofs] decoder output */
+  const float* pd_offset; const float* pd_scale; const uint8_t* freeze;   /* [dofs]; freeze may be NULL */
+  float* pd_out; int64_t ld_pd;
+  const float* root_states; int64_t root_env_stride; float* prev_root_pos;   /* speed, strike: [N, >= 3] view, [N, 3]; NULL for reach */
+  const int64_t* progress_buf;
+  int64_t* change_steps;                     /* reach, speed: _tar_change_steps / _speed_change_steps */
+  float* tar_pos;                            /* reach [N, 3] */
+  float* tar_speed;                          /* speed [N] */
+  const float* rand;                         /* injected uniforms, or NULL: Philox */
+  const int64_t* steps_in;                   /* injected randint results, or NULL: Philox */
+  uint64_t seed, offset;
+  const uint64_t* offset_dev;
+  float dist_max, height_min, height_max, speed_scale, speed_min;
+  int32_t reserved;
+  int64_t steps_min, steps_max;
+} pulse_ztask_pre_physics_args_t;
+int pulse_ztask_pre_physics(const pulse_ztask_pre_physics_args_t* args, int64_t num_envs, void* stream);
+
+/* Post-physics step of the rollout (humanoid.py:1315-1346): `progress_buf += 1` inside the kernel (the argument structs' progress_buf is
+ * written here), then the per-env code of pulse_reach_step / pulse_ztask_step, then dones[e] = float(reset_buf[e]) (amp_agent.py:380).
+ * obs_buf / obs_stride address the next step's experience slice, rew_buf the step's reward row.  Outputs are bit-equal to advancing
+ * the counter and calling the plain step. */
+int pulse_reach_rollout_step(const pulse_reach_step_args_t* args, float* dones, int64_t num_envs, void* stream);
+int pulse_ztask_rollout_step(const pulse_ztask_step_args_t* args, float* dones, int64_t num_envs, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Pedestrian terrain task HumanoidPedestrianTerrain(Z) (phc/env/tasks/humanoid_pedestrian_terrain.py): post_physics_step in one launch,

@@ -235,6 +235,32 @@ class ZTaskTaskArgs(C.Structure):
     ]
 
 
+class LatentPostArgs(C.Structure):
+    _fields_ = [
+        ("mu", C.c_void_p), ("ld_mu", C.c_int64), ("logstd", C.c_void_p), ("eps", C.c_void_p), ("ld_eps", C.c_int64),
+        ("seed", C.c_uint64), ("rng_offset", C.c_void_p), ("rng_step", C.c_uint64), ("latent", C.c_int32), ("reserved", C.c_int32),
+        ("actions", C.c_void_p), ("ld_actions", C.c_int64), ("neglogp", C.c_void_p), ("ld_neglogp", C.c_int64),
+        ("value", C.c_void_p), ("ld_value", C.c_int64), ("value_mean", C.c_void_p), ("value_var", C.c_void_p), ("value_eps", C.c_float),
+        ("reserved2", C.c_int32), ("values_out", C.c_void_p), ("ld_values", C.c_int64), ("prior_mu", C.c_void_p), ("ld_prior", C.c_int64),
+        ("z_bf16", C.c_void_p), ("ld_z", C.c_int64),
+    ]
+
+
+class ZTaskPrePhysicsArgs(C.Structure):
+    _fields_ = [
+        ("kind", C.c_int32), ("dofs", C.c_int32), ("action", C.c_void_p), ("ld_action", C.c_int64), ("pd_offset", C.c_void_p),
+        ("pd_scale", C.c_void_p), ("freeze", C.c_void_p), ("pd_out", C.c_void_p), ("ld_pd", C.c_int64), ("root_states", C.c_void_p),
+        ("root_env_stride", C.c_int64), ("prev_root_pos", C.c_void_p), ("progress_buf", C.c_void_p), ("change_steps", C.c_void_p),
+        ("tar_pos", C.c_void_p), ("tar_speed", C.c_void_p), ("rand", C.c_void_p), ("steps_in", C.c_void_p), ("seed", C.c_uint64),
+        ("offset", C.c_uint64), ("offset_dev", C.c_void_p), ("dist_max", C.c_float), ("height_min", C.c_float), ("height_max", C.c_float),
+        ("speed_scale", C.c_float), ("speed_min", C.c_float), ("reserved", C.c_int32), ("steps_min", C.c_int64), ("steps_max", C.c_int64),
+    ]
+
+
+# Philox index planes of the latent tasks' draws (include/pulse_b200.h): index = env + plane
+ZTASK_PLANE_RESET, ZTASK_PLANE_STRIKE, ZTASK_PLANE_RESET_TASK, ZTASK_PLANE_UPDATE_TASK = 0, 1 << 32, 2 << 32, 3 << 32
+
+
 class TerrainStepArgs(C.Structure):
     _fields_ = [
         ("flags", C.c_uint32), ("upright", C.c_int32), ("body_state", C.c_void_p), ("body_env_stride", C.c_int64),
@@ -395,6 +421,10 @@ SIGNATURES = {
     "pulse_ztask_obs_list": (C.c_int, [C.POINTER(ZTaskStepArgs), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_reset_ztask": (C.c_int, [C.c_void_p, C.POINTER(ZTaskResetArgs), C.c_int64, C.c_void_p]),
     "pulse_ztask_reset_task": (C.c_int, [C.POINTER(ZTaskTaskArgs), C.c_int64, C.c_void_p]),
+    "pulse_latent_post": (C.c_int, [C.POINTER(LatentPostArgs), C.c_int64, C.c_void_p]),
+    "pulse_ztask_pre_physics": (C.c_int, [C.POINTER(ZTaskPrePhysicsArgs), C.c_int64, C.c_void_p]),
+    "pulse_reach_rollout_step": (C.c_int, [C.POINTER(ReachStepArgs), C.c_void_p, C.c_int64, C.c_void_p]),
+    "pulse_ztask_rollout_step": (C.c_int, [C.POINTER(ZTaskStepArgs), C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_terrain_step": (C.c_int, [C.POINTER(TerrainStepArgs), C.c_int64, C.c_void_p]),
     "pulse_traj_reset": (C.c_int, [C.POINTER(TrajResetArgs), C.c_void_p]),
     "pulse_terrain_heights": (C.c_int, [C.POINTER(TerrainHeightsArgs), C.c_void_p]),

@@ -11,16 +11,10 @@
 //                       their previous row from the rows `pulse_reset_ref_state` back-filled (`fresh` flags, cleared here).
 #include "philox.cuh"
 #include "humanoid_obs.cuh"
+#include "value_unnorm.cuh"
 
 namespace pulse {
 namespace {
-
-// RunningMeanStd.forward(unnorm=True): clamp(y, -5, 5) * sqrt(var.float() + eps) + mean.float()
-__device__ __forceinline__ float value_unnorm(float y, const double* mean, const double* var, float eps) {
-  if (mean == nullptr) return y;
-  const float sd = sqrtf(__fadd_rn(static_cast<float>(var[0]), eps));
-  return __fadd_rn(__fmul_rn(fminf(fmaxf(y, -5.0f), 5.0f), sd), static_cast<float>(mean[0]));
-}
 
 __global__ void __launch_bounds__(128) policy_post_kernel(const pulse_policy_post_args_t a, long long rows) {
   const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;

@@ -6,12 +6,11 @@
 //           reset = compute_humanoid_reset
 //   strike  compute_strike_observations / compute_strike_reward  phc/env/tasks/humanoid_strike.py:270-328,
 //           reset = the strike variant of compute_humanoid_reset  :330-375
-#include "humanoid_obs.cuh"
+// The per-env device code is ztask_env.cuh's, shared with the rollout step kernels of ztask_rollout.cu.
+#include "ztask_env.cuh"
 
 namespace pulse {
 namespace {
-
-constexpr int kZB = PULSE_NUM_BODIES;
 
 __global__ void __launch_bounds__(256) reach_update_task_kernel(const long long* __restrict__ progress, long long* __restrict__ change,
                                                                 float* __restrict__ tar, const float* __restrict__ u,
@@ -27,54 +26,6 @@ __global__ void __launch_bounds__(256) reach_update_task_kernel(const long long*
   }
 }
 
-// One env of the reach step, lane = body.  kObsOnly: the observation alone (the reset envs' _compute_observations(env_ids)).
-template <bool kObsOnly>
-__device__ __forceinline__ void reach_env(const pulse_reach_step_args_t& a, long long e, int lane) {
-  const int j = lane;
-  const bool body = j < kZB;
-  const float* bs = a.body_state + e * a.body_env_stride + (body ? j : 0) * 13;
-  Vec3 p = {bs[0], bs[1], bs[2]}, v = {bs[7], bs[8], bs[9]}, w = {bs[10], bs[11], bs[12]};
-  Quat q = {bs[3], bs[4], bs[5], bs[6]};
-  const Vec3 p_root = {__shfl_sync(kFull, p.x, 0), __shfl_sync(kFull, p.y, 0), __shfl_sync(kFull, p.z, 0)};
-  const Quat q_root = {__shfl_sync(kFull, q.x, 0), __shfl_sync(kFull, q.y, 0), __shfl_sync(kFull, q.z, 0), __shfl_sync(kFull, q.w, 0)};
-  float hs, hc;
-  heading_half(q_root, hs, hc);
-  const Yaw yr = make_yaw(Quat{0.0f, 0.0f, -hs, hc});
-  float* o = a.obs_buf + e * a.obs_stride;
-  if (body) {  // store_self_obs's layout written out, for the reason given in im_step.cu
-    if (j == 0) o[0] = p_root.z;
-    else {
-      const Vec3 lp = yaw_rot(yr, p - p_root);
-      o[1 + 3 * (j - 1)] = lp.x; o[2 + 3 * (j - 1)] = lp.y; o[3 + 3 * (j - 1)] = lp.z;
-    }
-    float six[6];
-    qsix(yaw_mul_left(-hs, hc, q), six);
-#pragma unroll
-    for (int i = 0; i < 6; ++i) o[70 + 6 * j + i] = six[i];
-    const Vec3 lv = yaw_rot(yr, v), lw = yaw_rot(yr, w);
-    o[214 + 3 * j] = lv.x; o[215 + 3 * j] = lv.y; o[216 + 3 * j] = lv.z;
-    o[286 + 3 * j] = lw.x; o[287 + 3 * j] = lw.y; o[288 + 3 * j] = lw.z;
-  }
-  const Vec3 tar = {a.tar_pos[3 * e], a.tar_pos[3 * e + 1], a.tar_pos[3 * e + 2]};
-  const FallFlags fall = fall_flags(a, e, j, body, p.z);
-  const bool any_contact = __any_sync(kFull, fall.contact), any_height = __any_sync(kFull, fall.height);
-  // the reach body's position, broadcast
-  const int rb = a.reach_body_id;
-  const Vec3 pr = {__shfl_sync(kFull, p.x, rb), __shfl_sync(kFull, p.y, rb), __shfl_sync(kFull, p.z, rb)};
-  if (lane == 0) {
-    const Vec3 lt = yaw_rot(yr, tar - p_root);  // compute_location_observations (humanoid_reach.py:224-236)
-    o[PULSE_SELF_OBS + 0] = lt.x; o[PULSE_SELF_OBS + 1] = lt.y; o[PULSE_SELF_OBS + 2] = lt.z;
-    if constexpr (!kObsOnly) {
-      const Vec3 d = tar - pr;                  // compute_reach_reward (:238-250)
-      a.rew_buf[e] = expf(-4.0f * (d.x * d.x + d.y * d.y + d.z * d.z));
-      const long long prog = a.progress_buf[e];
-      const long long term = (any_contact && any_height && prog > 1) ? 1 : 0;
-      a.terminate_buf[e] = term;
-      a.reset_buf[e] = prog >= a.max_episode_length - 1 ? 1 : term;
-    }
-  }
-}
-
 __global__ void __launch_bounds__(256) reach_step_kernel(const pulse_reach_step_args_t a, long long n) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (long long e = blockIdx.x * 8ll + warp; e < n; e += 8ll * gridDim.x) reach_env<false>(a, e, lane);
@@ -85,89 +36,6 @@ __global__ void __launch_bounds__(256) reach_obs_list_kernel(const pulse_reach_s
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const long long n = *count;
   for (long long i = blockIdx.x * 8ll + warp; i < n; i += 8ll * gridDim.x) reach_env<true>(a, env_list[i], lane);
-}
-
-// One env of the speed / strike step, lane = body.  kObsOnly: the observation alone.
-template <bool kObsOnly>
-__device__ __forceinline__ void ztask_env(const pulse_ztask_step_args_t& a, long long e, int lane) {
-  const int j = lane;
-  const bool body = j < kZB;
-  const float* bs = a.body_state + e * a.body_env_stride + (body ? j : 0) * 13;
-  const Vec3 p = {bs[0], bs[1], bs[2]}, v = {bs[7], bs[8], bs[9]}, w = {bs[10], bs[11], bs[12]};
-  const Quat q = {bs[3], bs[4], bs[5], bs[6]};
-  const Vec3 p_root = {__shfl_sync(kFull, p.x, 0), __shfl_sync(kFull, p.y, 0), __shfl_sync(kFull, p.z, 0)};
-  const Quat q_root = {__shfl_sync(kFull, q.x, 0), __shfl_sync(kFull, q.y, 0), __shfl_sync(kFull, q.z, 0), __shfl_sync(kFull, q.w, 0)};
-  float hs, hc;
-  heading_half(q_root, hs, hc);
-  const Yaw yr = make_yaw(Quat{0.0f, 0.0f, -hs, hc});
-  float* o = a.obs_buf + e * a.obs_stride;
-  if (body) store_self_obs(o, j, p, p_root, q, v, w, hs, hc, yr);
-  const FallFlags fall = fall_flags(a, e, j, body, p.z);
-  // strike: a body that is neither a ground-contact body nor a strike body pressing harder than 50 N (humanoid_strike.py:356-364)
-  bool hard_contact = false;
-  if (a.enable_early_termination && body && a.contact_forces != nullptr && !(((a.contact_body_mask | a.strike_body_mask) >> j) & 1u)) {
-    const float* cf = a.contact_forces + e * a.contact_env_stride + j * 3;
-    hard_contact = fabsf(cf[0]) > 50.0f || fabsf(cf[1]) > 50.0f || fabsf(cf[2]) > 50.0f;
-  }
-  const bool any_contact = __any_sync(kFull, fall.contact), any_height = __any_sync(kFull, fall.height);
-  const bool any_hard = __any_sync(kFull, hard_contact);
-  // power term of the speed task: -c * sum |tau * qdot|, zero for progress <= 3 (humanoid_speed.py:215-222)
-  const float power = a.kind == PULSE_ZTASK_SPEED && a.dof_force != nullptr ? dof_power(a, e, lane) : 0.0f;
-  if (lane == 0) {
-    const long long prog = a.progress_buf[e];
-    const float* pr = a.prev_root_pos + 3 * e;
-    const float vx = (p_root.x - pr[0]) / a.dt, vy = (p_root.y - pr[1]) / a.dt;   // root_vel = delta_root_pos / dt
-    float* t = o + PULSE_SELF_OBS;
-    bool failed = any_contact && any_height;
-    if (a.kind == PULSE_ZTASK_SPEED) {
-      // observation: heading-frame x axis (first two components) and the target speed (:310-325)
-      const Vec3 d = yaw_rot(yr, Vec3{1.0f, 0.0f, 0.0f});
-      const float ts = a.tar_speed[e];
-      t[0] = d.x; t[1] = d.y; t[2] = ts;
-      if constexpr (kObsOnly) return;
-      const float err = ts - vx;
-      float rew = expf(-0.25f * (err * err + 0.1f * vy * vy));                    // :327-343
-      if (a.reward_raw != nullptr) a.reward_raw[e * a.raw_stride] = rew;
-      if (a.dof_force != nullptr) {
-        const float pw = prog <= 3 ? 0.0f : -a.power_coefficient * power;
-        rew += pw;
-        if (a.reward_raw != nullptr) a.reward_raw[e * a.raw_stride + 1] = pw;
-      }
-      a.rew_buf[e] = rew;
-    } else {
-      const float* ts = a.target_states + e * a.target_env_stride;
-      const Vec3 tp = {ts[0], ts[1], ts[2]};
-      const Quat tq = {ts[3], ts[4], ts[5], ts[6]};
-      // observation (:270-293): target position relative to the root with the ABSOLUTE height, 6D rotation, velocities, heading frame
-      const Vec3 lp = yaw_rot(yr, Vec3{tp.x - p_root.x, tp.y - p_root.y, tp.z});
-      t[0] = lp.x; t[1] = lp.y; t[2] = lp.z;
-      qsix(yaw_mul_left(-hs, hc, tq), t + 3);
-      const Vec3 lv = yaw_rot(yr, Vec3{ts[7], ts[8], ts[9]}), lw = yaw_rot(yr, Vec3{ts[10], ts[11], ts[12]});
-      t[9] = lv.x; t[10] = lv.y; t[11] = lv.z;
-      t[12] = lw.x; t[13] = lw.y; t[14] = lw.z;
-      if constexpr (kObsOnly) return;
-      // reward (:295-328)
-      const float rot_err = 2.0f * tq.w * tq.w - 1.0f + 2.0f * tq.z * tq.z;      // z component of quat_rotate(tar_rot, [0, 0, 1])
-      const float rot_r = fmaxf(1.0f - rot_err, 0.0f);
-      float dx = tp.x - p_root.x, dy = tp.y - p_root.y;
-      const float dn = fmaxf(sqrtf(dx * dx + dy * dy), 1e-12f);                    // torch.nn.functional.normalize (eps 1e-12)
-      dx /= dn; dy /= dn;
-      const float dir_speed = dx * vx + dy * vy;
-      const float verr = fmaxf(1.0f - dir_speed, 0.0f);
-      float vel_r = expf(-4.0f * verr * verr);
-      if (dir_speed <= 0.0f) vel_r = 0.0f;
-      float rew = 0.6f * rot_r + 0.4f * vel_r;
-      if (rot_err < 0.2f) rew = 1.0f;
-      a.rew_buf[e] = rew;
-      // reset (:330-375): also fails when the target is pushed (> 50 N horizontally) while a non-strike body presses hard
-      const float* tc = a.tar_contact_forces + e * a.tar_contact_env_stride;
-      const bool tar_contact = fabsf(tc[0]) > 50.0f || fabsf(tc[1]) > 50.0f;
-      failed = failed || (a.enable_early_termination && tar_contact && any_hard);
-    }
-    const long long term = (a.enable_early_termination && failed && prog > 1) ? 1 : 0;
-    a.terminate_buf[e] = term;
-    a.reset_buf[e] = prog >= a.max_episode_length - 1 ? 1 : term;
-  }
 }
 
 __global__ void __launch_bounds__(256) ztask_step_kernel(const pulse_ztask_step_args_t a, long long n) {

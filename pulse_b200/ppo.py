@@ -185,18 +185,7 @@ class PPOPolicy:
         pd = (offset [A], scale [A], out [M, A]).  `side`: a second CUDA stream -- the critic's forward pass then runs beside the
         actor's (at the per-rank env counts of a multi-GPU run neither fills the GPU)."""
         M = obs.shape[0]
-        b = self._buf(M, False)
-        self.obs_rms.normalize_into(obs, b["x"])
-        if side is not None and values is not None:      # actor | critic on two streams (fork / join: still one CUDA-graph segment)
-            main = torch.cuda.current_stream(self.device)
-            side.wait_stream(main)
-            with torch.cuda.stream(side):
-                value = self.critic.forward(b["x"])
-            self.actor.forward(b["x"], out=mus)
-            main.wait_stream(side)
-        else:
-            self.actor.forward(b["x"], out=mus)
-            value = self.critic.forward(b["x"]) if values is not None else None
+        value = self.heads_into(obs, mus=mus, with_value=values is not None, side=side)
         a = _lib.PolicyPostArgs(mu=mus.data_ptr(), ld_mu=mus.stride(0), logstd=self.logstd.data_ptr(), seed=self.rng_seed,
                                 rng_offset=self.rng_offset.data_ptr(), rng_step=int(rng_step), num_actions=self.A,
                                 actions=actions.data_ptr(), ld_actions=actions.stride(0), neglogp=neglogp.data_ptr(), ld_neglogp=neglogp.stride(0))
@@ -210,6 +199,23 @@ class PPOPolicy:
             a.pd_offset, a.pd_scale, a.pd_targets, a.ld_pd = pd[0].data_ptr(), pd[1].data_ptr(), pd[2].data_ptr(), pd[2].stride(0)
         with torch.cuda.device(self.device):
             _lib.check(self.lib.pulse_policy_post(C.byref(a), M, _lib.current_stream(self.device)), "pulse_policy_post")
+
+    def heads_into(self, obs: torch.Tensor, *, mus: torch.Tensor, with_value: bool = True, side=None) -> Optional[torch.Tensor]:
+        """The network half of get_action_values: normalise `obs`, the actor head into `mus` ([M, A] slice, any row stride) and, with
+        `with_value`, the critic; returns its NORMALISED value [M, 1] (a reused workspace) or None.  `side`: the critic runs on that
+        stream beside the actor and is joined before returning."""
+        b = self._buf(obs.shape[0], False)
+        self.obs_rms.normalize_into(obs, b["x"])
+        if side is not None and with_value:              # actor | critic on two streams (fork / join: still one CUDA-graph segment)
+            main = torch.cuda.current_stream(self.device)
+            side.wait_stream(main)
+            with torch.cuda.stream(side):
+                value = self.critic.forward(b["x"])
+            self.actor.forward(b["x"], out=mus)
+            main.wait_stream(side)
+            return value
+        self.actor.forward(b["x"], out=mus)
+        return self.critic.forward(b["x"]) if with_value else None
 
     def critic_values_into(self, obs: torch.Tensor, out: torch.Tensor, terminate: Optional[torch.Tensor] = None, slot: int = 0,
                            after_normalize=None) -> None:

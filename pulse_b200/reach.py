@@ -20,6 +20,8 @@ SMPL_BODY_NAMES = ['Pelvis', 'L_Hip', 'L_Knee', 'L_Ankle', 'L_Toe', 'R_Hip', 'R_
 
 
 class ReachTaskB200:
+    kind, obs_size = _lib.ZTASK_REACH, REACH_OBS
+
     def __init__(self, num_envs: int, device="cuda:0", reach_body_name: str = "R_Hand", contact_bodies: Sequence[str] = ("R_Ankle", "L_Ankle", "R_Toe", "L_Toe"),
                  tar_change_steps_min: int = 100, tar_change_steps_max: int = 200, tar_dist_max: float = 1.0, tar_height_min: float = 0.5,
                  tar_height_max: float = 1.5, max_episode_length: int = 300, enable_early_termination: bool = True, termination_height: float = 0.15):

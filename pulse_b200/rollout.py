@@ -37,6 +37,22 @@ def discount_values(mb_fdones: torch.Tensor, mb_values: torch.Tensor, mb_rewards
     return adv, ret
 
 
+def finish_returns(pol, dones: torch.Tensor, values: torch.Tensor, mb_rewards: torch.Tensor, next_values: torch.Tensor, adv_out: torch.Tensor,
+                   ret_out: torch.Tensor, gamma: float, tau: float) -> None:
+    """The end of `play_steps` + `prepare_dataset` shared by the rollout drivers: GAE + returns (common_agent.py:493-505) and advantage
+    normalisation (:589-599) into `adv_out`, value / return normalisation in training mode into `ret_out` (prepare_dataset :372-374: each
+    tensor is normalised with the statistics BEFORE its own merge, running_mean_std.py:69-109).  Inputs time-major [T, n(, 1)], outputs
+    env-major flat [n*T]."""
+    adv, ret = discount_values(dones, values, mb_rewards, next_values, gamma=gamma, tau=tau, normalize_advantage=True)
+    adv_out.copy_(adv)
+    if pol.value_rms is not None:
+        pol.value_rms.update(values.view(-1, 1))                                 # values: normalised copy unused (clip_value False), stats merged
+        ret_out.copy_(pol.value_rms.normalize_values(ret.view(-1, 1)).view(-1))  # returns see the statistics that include the values batch ...
+        pol.value_rms.update(ret.view(-1, 1))                                    # ... and are merged afterwards
+    else:
+        ret_out.copy_(ret)
+
+
 class GraphRunner:
     """CUDA-graph runner of the rollout drivers: `_run(key, fn, *args)` executes `fn` eagerly on its first use, captures it on its second
     use and replays it from then on; every graph shares one memory pool.  The subclass sets `dev`, `use_graphs`, `_graphs = {}` and
@@ -285,12 +301,5 @@ class PlayStepsB200(GraphRunner):
             mb_rewards = self.task_w * self.rewards.unsqueeze(-1) + self.disc_w * disc_r.view(n, T).t().unsqueeze(-1)
         else:
             mb_rewards = self.rewards.unsqueeze(-1)
-        adv, ret = discount_values(self.dones, self.values, mb_rewards, self.next_values, gamma=self.gamma, tau=self.tau, normalize_advantage=True)
-        self.adv.copy_(adv)
-        if pol.value_rms is not None:
-            pol.value_rms.update(self.values.view(T * n, 1))                         # values: normalised copy unused (clip_value False), stats merged
-            self.ret.copy_(pol.value_rms.normalize_values(ret.view(-1, 1)).view(-1))  # returns see the statistics that include the values batch ...
-            pol.value_rms.update(ret.view(-1, 1))                                    # ... and are merged afterwards
-        else:
-            self.ret.copy_(ret)
+        finish_returns(pol, self.dones, self.values, mb_rewards, self.next_values, self.adv, self.ret, self.gamma, self.tau)
         pol.advance_rng(T)

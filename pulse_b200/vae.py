@@ -270,6 +270,14 @@ class PulseVAE:
         """HumanoidZ.compute_z_actions, z_type 'vae' + use_vae_prior: z = prior_mu(self_obs) + action_z;
         actions = decoder([clamp(self_obs, +-5), z]).  The prior sees the UNCLAMPED normalised self observation (:87 vs :147).
         obs_buf fp32 [M, >= S] raw; frozen `obs_rms` = the checkpoint's running_mean_std."""
+        prior_head, dec_in = self.z_prior(obs_buf)
+        self._reparam(prior_head, action_z, _lib.Z_RESIDUAL, dec_in, obs_buf.shape[0])
+        return self.dec.forward(dec_in)
+
+    def z_prior(self, obs_buf: torch.Tensor):
+        """The part of compute_z_actions that does not depend on the action: the unclamped normalised self observation into the prior
+        operand, the clamped one into the decoder operand's self-observation columns, the prior MLP.  Returns (prior head fp32 [M, 2E],
+        decoder operand bf16 [M, Kp] whose columns [0, E) await z); `self.dec.forward(operand)` decodes."""
         M = obs_buf.shape[0]
         b = self._buf(M)
         E, S = self.E, self.S
@@ -281,9 +289,7 @@ class PulseVAE:
             _lib.check(self.lib.pulse_normalize_cols(obs_buf.data_ptr(), obs_buf.stride(0), M, S, rms.mean_f32.data_ptr(), rms.rstd_f32.data_ptr(),
                                                      5.0, b["dec_in"][:, E:].data_ptr(), b["dec_in"].stride(0), S, self._st()),
                        "pulse_normalize_cols")
-        prior_head = self.prior.forward(b["prior_in"])
-        self._reparam(prior_head, action_z, _lib.Z_RESIDUAL, b["dec_in"], M)
-        return self.dec.forward(b["dec_in"])
+        return self.prior.forward(b["prior_in"]), b["dec_in"]
 
     # ------------------------------------------------------------------ checkpoint keys (rl_games layout)
     def state_dict(self) -> Dict[str, torch.Tensor]:
