@@ -7,8 +7,10 @@
   compute_error_vel / _accel  (requirement.txt:20, unpinned) that is NOT under /root/reference.  Restated from its published
   p_mpjpe                     source: per-frame global / root-relative MPJPE in mm, finite-difference velocity / acceleration
                               errors, Procrustes-aligned MPJPE (the VideoPose3D `p_mpjpe`).]  PARITY UNPINNED for these four:
-                              no copy of smpl_sim exists in this container to generate fixtures from; the kernel is compared with
-                              this restatement only.
+                              no copy of smpl_sim exists to generate fixtures from.  tests/eval_fp64.py evaluates the same
+                              definitions in float64 with a bound on the kernel's fp32 deviation; tests/test_gpu_eval_fp64.py holds
+                              the kernel to it frame by frame (frame classes listed there and in DESIGN.md §7), and
+                              tests/test_eval_fp64_cpu.py checks that reference, and this fp32 restatement against it.
 The bookkeeping half (post_step) follows code that IS under /root/reference and is cited line by line.
 """
 from collections import defaultdict
