@@ -767,6 +767,9 @@ int pulse_ztask_obs_list(const pulse_ztask_step_args_t* args, const int64_t* env
  *   index e + 2^32     x: strike bearing   y: strike yaw
  *   index e + 2^33     pulse_ztask_reset_task: x, y, z task uniforms, w change steps
  *   index e + 3 * 2^32 pulse_ztask_pre_physics (_update_task of the rollout): x, y, z task uniforms, w change steps
+ *   index e + 4 * 2^32 pulse_traj_reset_list: counter PULSE_TRAJ_VERTS * (offset + *offset_dev) + k, k <= PULSE_TRAJ_VERTS - 1
+ *                      (the pedestrian terrain task's waypoints; block k < S: segment k, block S: heading and speed)
+ * pulse_reset_terrain reads index e as above, with word z as the spawn location (w unused).
  * ---------------------------------------------------------------------------------------------- */
 #define PULSE_ZTASK_REACH 3
 #define PULSE_ZPOSE_AS_IS 0
@@ -978,6 +981,50 @@ typedef struct {
   float* heights; int64_t heights_stride;
 } pulse_terrain_heights_args_t;
 int pulse_terrain_heights(const pulse_terrain_heights_args_t* args, void* stream);
+
+/* pulse_traj_reset_list: TrajGenerator.reset (phc/utils/traj_generator.py:57-112) over the env list and device-side count of a reset
+ * (pulse_reset_terrain's env_list / count), one thread per listed env, starting at root_states[e, 0:2] (_reset_task,
+ * humanoid_pedestrian_terrain.py:480-485, reads _humanoid_root_states after the reset).  rand [N, PULSE_TRAJ_DRAWS] injects the draws
+ * per ENV (layout of pulse_traj_reset); NULL takes them from Philox4x32-10 on (seed, e + 4 * 2^32, PULSE_TRAJ_VERTS * (offset +
+ * *offset_dev) + k): two resets of one env at different offsets never share a block.  Parameters as pulse_traj_reset. */
+typedef struct {
+  const int64_t* env_list; const int32_t* count;
+  const float* root_states; int64_t root_env_stride;         /* [N, >= 2] view: the start xy */
+  const float* rand;                                         /* [N, PULSE_TRAJ_DRAWS] or NULL */
+  uint64_t seed, offset; const uint64_t* offset_dev;
+  float dtheta_scale, dspeed_scale, seg_dt, speed_min, speed_max, sharp_turn_prob;
+  float* verts;                                              /* [N, PULSE_TRAJ_VERTS, 3] */
+} pulse_traj_list_args_t;
+int pulse_traj_reset_list(const pulse_traj_list_args_t* args, int64_t num_envs, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Reference-state reset of the pedestrian terrain task, free of host synchronisation: HumanoidPedestrianTerrain._reset_ref_state_init
+ * (humanoid_pedestrian_terrain.py:527-589) with _sample_ref_state (:488-525), _set_env_state, _reset_env_tensors and _init_amp_obs,
+ * for humanoid_type "smpl".  The launches and the per-warp work of pulse_reset_ztask (args as there, pose_mode AS_IS, state_init
+ * RANDOM: the terrain task's _sample_ref_state always calls _sample_time, for StateInit Start too; no strike target), with the
+ * spawn in place of the pose adjustment:
+ *   - location: Terrain.sample_valid_locations (:1175-1189), new_xy = (coord_x[l], coord_y[l]) with l injected per env
+ *     (loc_ids_in, the np.random.randint draw) or (word z * num_locations) >> 32; l is written to loc_ids_out when given;
+ *   - diff = new_xy - root_xy; root_xy = new_xy; root_z += mean of get_center_heights at the new root (:690-716: the center points
+ *     rotated by the yaw of the root, or of remove_base_rot(root) when !upright);
+ *   - rigid-body xy += diff.  The rigid bodies' z is NOT lifted (the reference adds the lift to key_pos only, twice, and never
+ *     reads key_pos again), so AMP row 0, built from the rigid bodies, carries the unlifted root height.
+ * The walkable table is Terrain.__init__'s (:1160-1171): the cells with walkable_field == 0 inside the border, scaled by
+ * horizontal_scale.  A plane (heightfield NULL) has no table: the reference cannot spawn on it and neither can this entry point.
+ * The observation of the reset envs follows (pulse_terrain_step, PULSE_STEP_OBS over env_list / count), then
+ * pulse_traj_reset_list, as in the reference (humanoid.py:574-587, humanoid_amp_task.py:73-76).
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  const int16_t* heightfield; int64_t hf_rows, hf_cols;      /* required (no plane) */
+  float horizontal_scale, vertical_scale;
+  const float* center_points; int64_t num_center_points;     /* [num_center_points, 3], 1 ..= 32 */
+  const float* coord_x; const float* coord_y;                /* [num_locations] walkable table (coord_{x,y}_scale) */
+  int64_t num_locations;                                     /* 1 .. 2^32 - 1 */
+  const int64_t* loc_ids_in;                                 /* [N] injected location index per env (clamped to the table), or NULL */
+  int64_t* loc_ids_out;                                      /* [N] out: the location index of each reset env; may be NULL */
+} pulse_terrain_spawn_args_t;
+int pulse_reset_terrain(const pulse_motionlib_t* lib, const pulse_ztask_reset_args_t* args, const pulse_terrain_spawn_args_t* spawn,
+                        int64_t num_envs, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Task observation for every observation version / tracked-body subset / number of future samples (SURVEY 8f-4): replaces the

@@ -299,6 +299,32 @@ TRAJ_DRAWS = 4 * (TRAJ_VERTS - 1) + 2
 HEIGHTS_CENTER, HEIGHTS_GRID = 1, 2
 
 
+class TrajListArgs(C.Structure):
+    _fields_ = [
+        ("env_list", C.c_void_p), ("count", C.c_void_p), ("root_states", C.c_void_p), ("root_env_stride", C.c_int64), ("rand", C.c_void_p),
+        ("seed", C.c_uint64), ("offset", C.c_uint64), ("offset_dev", C.c_void_p), ("dtheta_scale", C.c_float), ("dspeed_scale", C.c_float),
+        ("seg_dt", C.c_float), ("speed_min", C.c_float), ("speed_max", C.c_float), ("sharp_turn_prob", C.c_float), ("verts", C.c_void_p),
+    ]
+
+
+class TerrainSpawnArgs(C.Structure):
+    _fields_ = [
+        ("heightfield", C.c_void_p), ("hf_rows", C.c_int64), ("hf_cols", C.c_int64), ("horizontal_scale", C.c_float), ("vertical_scale", C.c_float),
+        ("center_points", C.c_void_p), ("num_center_points", C.c_int64), ("coord_x", C.c_void_p), ("coord_y", C.c_void_p),
+        ("num_locations", C.c_int64), ("loc_ids_in", C.c_void_p), ("loc_ids_out", C.c_void_p),
+    ]
+
+
+TRAJ_LIST_PLANE = 4 << 32      # Philox index plane of pulse_traj_reset_list: index = env + TRAJ_LIST_PLANE
+
+
+def traj_list_philox_blocks(env: int, offset: int, offset_dev: int = 0):
+    """The Philox4x32-10 blocks (index, counters) one `pulse_traj_reset_list` reset of `env` reads, as the kernel keys them:
+    index env + 4 * 2^32, counters TRAJ_VERTS * (offset + offset_dev) + k for k in [0, TRAJ_VERTS)."""
+    base = (TRAJ_VERTS * ((offset + offset_dev) % 2 ** 64)) % 2 ** 64
+    return env + TRAJ_LIST_PLANE, [(base + k) % 2 ** 64 for k in range(TRAJ_VERTS)]
+
+
 class TaskObsArgs(C.Structure):
     _fields_ = [
         ("body_state", C.c_void_p), ("body_env_stride", C.c_int64), ("track_ids", C.c_void_p),
@@ -428,6 +454,8 @@ SIGNATURES = {
     "pulse_terrain_step": (C.c_int, [C.POINTER(TerrainStepArgs), C.c_int64, C.c_void_p]),
     "pulse_traj_reset": (C.c_int, [C.POINTER(TrajResetArgs), C.c_void_p]),
     "pulse_terrain_heights": (C.c_int, [C.POINTER(TerrainHeightsArgs), C.c_void_p]),
+    "pulse_traj_reset_list": (C.c_int, [C.POINTER(TrajListArgs), C.c_int64, C.c_void_p]),
+    "pulse_reset_terrain": (C.c_int, [C.c_void_p, C.POINTER(ZTaskResetArgs), C.POINTER(TerrainSpawnArgs), C.c_int64, C.c_void_p]),
     "pulse_task_obs_size": (C.c_int, [C.c_int32, C.c_int32, C.c_int32]),
     "pulse_im_task_obs": (C.c_int, [C.POINTER(TaskObsArgs), C.c_void_p]),
     "pulse_eval_step": (C.c_int, [C.POINTER(EvalArgs), C.c_void_p]),

@@ -1,0 +1,181 @@
+// The per-warp reference-state reset shared by pulse_reset_ztask (ztask_reset.cu) and pulse_reset_terrain (terrain_reset.cu):
+//   reset_compact_kernel  one CTA: the ordered compaction of compact.cuh turns the reset mask or id list into the ascending env list,
+//                         the humanoid and target actor lists and a device-side count;
+//   reset_warps           one warp per (reset env, AMP history step k): clip and start-time draws, MotionLib gather, SMPL ground fix
+//                         from the per-frame floor table, the caller's adjustment of the root and bodies, the scatter into the
+//                         simulator's views, counters and the AMP rows (195- or 196-float layout).
+// The entry points, argument structs and Philox word layout are documented in include/pulse_b200.h.
+#pragma once
+#include "compact.cuh"
+#include "humanoid_obs.cuh"
+#include "philox.cuh"
+
+namespace pulse {
+namespace {
+
+constexpr int kResetWarps = 8;
+
+__global__ void __launch_bounds__(kCompactThreads) reset_compact_kernel(const pulse_ztask_reset_args_t a, long long num_envs) {
+  __shared__ int warp_cnt[kCompactThreads / 32];
+  __shared__ int base;
+  if (threadIdx.x == 0) base = 0;
+  __syncthreads();
+  const long long n = a.env_ids_in != nullptr ? a.num_ids : num_envs;
+  for (long long c0 = 0; c0 < n; c0 += kCompactThreads) {
+    const long long i = c0 + threadIdx.x;
+    long long env = -1;
+    if (i < n && a.env_ids_in == nullptr) env = a.reset_buf[i] != 0 ? i : -1;
+    if (i < n && a.env_ids_in != nullptr) {   // an id outside [0, N) or not above its predecessor is skipped: each env is written once
+      env = a.env_ids_in[i];
+      if (env < 0 || env >= num_envs || (i > 0 && a.env_ids_in[i - 1] >= env)) env = -1;
+    }
+    const int pos = compact_slot(env >= 0, warp_cnt, &base);
+    if (pos < 0) continue;
+    a.env_list[pos] = env;
+    if (a.actor_list != nullptr) a.actor_list[pos] = a.actor_ids != nullptr ? a.actor_ids[env] : static_cast<int>(env);
+    if (a.tar_actor_list != nullptr) a.tar_actor_list[pos] = a.tar_actor_ids != nullptr ? a.tar_actor_ids[env] : static_cast<int>(env);
+  }
+  if (threadIdx.x == 0) *a.count = base;
+}
+
+// sample_motions: the first clip whose inclusive CDF exceeds u * total (a zero-weight clip never does before its predecessor).
+__device__ __forceinline__ long long pick_motion(const float* cdf, long long m, float u) {
+  const float total = cdf[m - 1];
+  float v = __fmul_rn(u, total);
+  if (v >= total) v = nextafterf(total, 0.0f);
+  long long lo = 0, hi = m - 1;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (cdf[mid] > v) hi = mid;
+    else lo = mid + 1;
+  }
+  return lo;
+}
+
+// build_amp_observations_smpl into the warp's staging row, then `width` floats of it to `out`: 196 is the whole row, 195 drops the
+// root height.  A non-upright start takes the heading and root rotation feature of remove_base_rot(q0).
+template <class JointFn, class KeyPosFn>
+__device__ __forceinline__ void store_amp_row(float* out, int width, float* stage, int lane, Vec3 p0, Quat q0, Vec3 v0, Vec3 w0, bool upright,
+                                              JointFn joint, KeyPosFn key_pos) {
+  store_amp_obs(stage, lane, p0, base_rot_removed(q0, upright), v0, w0, joint, key_pos);
+  __syncwarp();
+  const int skip = PULSE_AMP_OBS - width;
+  for (int c = lane; c < width; c += 32) out[c] = stage[skip + c];
+  __syncwarp();
+}
+
+// The work of one warp.  `adjust(e, lane, r0, off, p, rq, v, rp, rr, rv, rw)` runs on every lane after the ground fix: lane j holds
+// body j's position, rotation and velocity (p, rq, v), every lane the root's (rp, rr, rv, rw); r0 is Philox block (seed, e, off)
+// when a draw is not injected or `more_draws` is set, zero otherwise.  What it leaves is what _set_env_state writes.
+template <class Adjust>
+__device__ __forceinline__ void reset_warps(const pulse_motionlib_desc_t& lib, const pulse_ztask_reset_args_t& a, bool more_draws, float* stage,
+                                            const Adjust& adjust) {
+  const int lane = threadIdx.x & 31;
+  const long long warp0 = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const long long nwarps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
+  const int steps = a.amp_obs_buf != nullptr ? a.num_amp_steps : 1;
+  const long long items = static_cast<long long>(*a.count) * steps;
+  const unsigned long long off = a.offset + (a.offset_dev != nullptr ? *a.offset_dev : 0ull);
+  const bool upright = a.upright != 0;
+  const float step30 = static_cast<float>(1.0 / 30.0);
+  for (long long it = warp0; it < items; it += nwarps) {
+    const long long i = it / steps;
+    const int k = static_cast<int>(it - i * steps);
+    const long long e = a.env_list[i];
+    Philox4 r0{0u, 0u, 0u, 0u};
+    if ((a.motion_ids_in == nullptr && a.motion_u == nullptr) || a.phase == nullptr || more_draws)
+      r0 = philox4x32_10(a.seed, static_cast<unsigned long long>(e), off);
+    const long long mid = a.motion_ids_in != nullptr ? a.motion_ids_in[e]
+                          : pick_motion(a.sampling_cdf, lib.num_motions, a.motion_u != nullptr ? a.motion_u[e] : u01(r0.y));
+    const float mlen = lib.lengths[mid];
+    float t0 = 0.0f;
+    if (a.state_init == PULSE_ZINIT_RANDOM) {   // sample_time_interval: ((phase * motion_len) / curr_fps).long() * curr_fps
+      const float ph = a.phase != nullptr ? a.phase[e] : u01(r0.x);
+      t0 = __fmul_rn(__ll2float_rn(static_cast<long long>(__fdiv_rn(__fmul_rn(ph, mlen), step30))), step30);
+    }
+    const float t = k == 0 ? t0 : __fadd_rn(t0, __fmul_rn(-a.dt, static_cast<float>(k)));
+    long long i0, i1;
+    float b;
+    frame_blend_rn(t, mlen, lib.num_frames[mid], lib.dt[mid], i0, i1, b);
+    const long long f0 = i0 + lib.length_starts[mid], f1 = i1 + lib.length_starts[mid];
+    const float* r0p = lib.frame_rec + f0 * PULSE_FRAME_REC;
+    const float* r1p = lib.frame_rec + f1 * PULSE_FRAME_REC;
+    const float* x0 = lib.aux_rec + f0 * PULSE_AUX_REC;
+    const float* x1 = lib.aux_rec + f1 * PULSE_AUX_REC;
+
+    if (k > 0) {   // _init_amp_obs_ref: the motion at t0 - k dt as it is, without the ground fix or the pose adjustment
+      const Vec3 p0 = {lerp_rn(r0p[0], r1p[0], b), lerp_rn(r0p[1], r1p[1], b), lerp_rn(r0p[2], r1p[2], b)};
+      const Vec3 v0 = {lerp_rn(r0p[168], r1p[168], b), lerp_rn(r0p[169], r1p[169], b), lerp_rn(r0p[170], r1p[170], b)};
+      const Vec3 w0 = {lerp_rn(r0p[240], r1p[240], b), lerp_rn(r0p[241], r1p[241], b), lerp_rn(r0p[242], r1p[242], b)};
+      const Quat q0 = slerp(ldq4(r0p + 72), ldq4(r1p + 72), b);
+      const auto joint = [&](int jt) {
+        return AmpJoint{quat_exp_map(slerp(ldq4(x0 + 4 * (jt + 1)), ldq4(x1 + 4 * (jt + 1)), b)),
+                        {lerp_rn(x0[96 + 3 * jt], x1[96 + 3 * jt], b), lerp_rn(x0[97 + 3 * jt], x1[97 + 3 * jt], b),
+                         lerp_rn(x0[98 + 3 * jt], x1[98 + 3 * jt], b)}};
+      };
+      const auto key_pos = [&](int kb) {
+        return Vec3{lerp_rn(r0p[3 * kb], r1p[3 * kb], b), lerp_rn(r0p[3 * kb + 1], r1p[3 * kb + 1], b), lerp_rn(r0p[3 * kb + 2], r1p[3 * kb + 2], b)};
+      };
+      store_amp_row(a.amp_obs_buf + (e * a.num_amp_steps + k) * a.amp_width, a.amp_width, stage, lane, p0, q0, v0, w0, upright, joint, key_pos);
+      continue;
+    }
+
+    // ---- the reset state: lane j holds body j -----------------------------------------------------------------------------------
+    const int j = lane < PULSE_NUM_BODIES ? lane : 0;
+    Vec3 p = {lerp_rn(r0p[3 * j], r1p[3 * j], b), lerp_rn(r0p[3 * j + 1], r1p[3 * j + 1], b), lerp_rn(r0p[3 * j + 2], r1p[3 * j + 2], b)};
+    Vec3 v = {lerp_rn(r0p[168 + 3 * j], r1p[168 + 3 * j], b), lerp_rn(r0p[169 + 3 * j], r1p[169 + 3 * j], b),
+              lerp_rn(r0p[170 + 3 * j], r1p[170 + 3 * j], b)};
+    const Vec3 w = {lerp_rn(r0p[240 + 3 * j], r1p[240 + 3 * j], b), lerp_rn(r0p[241 + 3 * j], r1p[241 + 3 * j], b),
+                    lerp_rn(r0p[242 + 3 * j], r1p[242 + 3 * j], b)};
+    Quat rq = slerp(ldq4(r0p + 72 + 4 * j), ldq4(r1p + 72 + 4 * j), b);
+    // ground fix (humanoid_amp.py:382-430): d = min_v (V - (J0 - root)).z - 0.02 = (floor(f0) + root z) - 0.02
+    const float root_z = __shfl_sync(kFull, p.z, 0);
+    const float d = __fsub_rn(__fadd_rn(a.floor[f0], root_z), 0.02f);
+    p.z = __fsub_rn(p.z, d);
+    Vec3 rp = {__shfl_sync(kFull, p.x, 0), __shfl_sync(kFull, p.y, 0), __shfl_sync(kFull, p.z, 0)};
+    Quat rr = {__shfl_sync(kFull, rq.x, 0), __shfl_sync(kFull, rq.y, 0), __shfl_sync(kFull, rq.z, 0), __shfl_sync(kFull, rq.w, 0)};
+    Vec3 rv = {__shfl_sync(kFull, v.x, 0), __shfl_sync(kFull, v.y, 0), __shfl_sync(kFull, v.z, 0)};
+    Vec3 rw = {__shfl_sync(kFull, w.x, 0), __shfl_sync(kFull, w.y, 0), __shfl_sync(kFull, w.z, 0)};
+    adjust(e, lane, r0, off, p, rq, v, rp, rr, rv, rw);
+    if (lane < PULSE_NUM_BODIES) {   // _set_env_state (humanoid_amp.py:565-597)
+      float* bs = a.rigid_body_state + e * a.body_env_stride + j * PULSE_BODY_STATE_W;
+      bs[0] = p.x; bs[1] = p.y; bs[2] = p.z; bs[3] = rq.x; bs[4] = rq.y; bs[5] = rq.z; bs[6] = rq.w;
+      bs[7] = v.x; bs[8] = v.y; bs[9] = v.z; bs[10] = w.x; bs[11] = w.y; bs[12] = w.z;
+      if (j >= 1) {   // dof_pos = exp_map(slerp(local rotations)) of joints 1..23
+        const Vec3 em = quat_exp_map(slerp(ldq4(x0 + 4 * j), ldq4(x1 + 4 * j), b));
+        float* dp = a.dof_pos + e * a.dof_env_stride + 3 * (j - 1) * a.dof_elem_stride;
+        dp[0] = em.x; dp[a.dof_elem_stride] = em.y; dp[2 * a.dof_elem_stride] = em.z;
+      }
+    }
+    for (int c = lane; c < PULSE_NUM_DOF; c += 32) a.dof_vel[e * a.dof_env_stride + c * a.dof_elem_stride] = lerp_rn(x0[96 + c], x1[96 + c], b);
+    if (a.contact_forces != nullptr)
+      for (int c = lane; c < a.contact_bodies * 3; c += 32) a.contact_forces[e * a.contact_env_stride + c] = 0.0f;
+    if (lane == 0) {
+      float* rs = a.root_states + e * a.root_env_stride;
+      rs[0] = rp.x; rs[1] = rp.y; rs[2] = rp.z; rs[3] = rr.x; rs[4] = rr.y; rs[5] = rr.z; rs[6] = rr.w;
+      rs[7] = rv.x; rs[8] = rv.y; rs[9] = rv.z; rs[10] = rw.x; rs[11] = rw.y; rs[12] = rw.z;
+      a.sampled_motion_ids[e] = mid;   // humanoid_amp.py:484-485
+      a.motion_start_times[e] = t0;
+      a.progress_buf[e] = 0;           // _reset_env_tensors (humanoid.py:603-606)
+      if (a.reset_buf != nullptr) a.reset_buf[e] = 0;
+      if (a.terminate_buf != nullptr) a.terminate_buf[e] = 0;
+    }
+    if (a.amp_obs_buf == nullptr) continue;
+    // row 0: _compute_amp_observations(env_ids) of the rigid bodies and dofs just written
+    __syncwarp();
+    const float* bs = a.rigid_body_state + e * a.body_env_stride;
+    const float* dp = a.dof_pos + e * a.dof_env_stride;
+    const float* dv = a.dof_vel + e * a.dof_env_stride;
+    const long long ds = a.dof_elem_stride;
+    const auto joint = [&](int jt) {
+      return AmpJoint{{dp[(3 * jt + 0) * ds], dp[(3 * jt + 1) * ds], dp[(3 * jt + 2) * ds]},
+                      {dv[(3 * jt + 0) * ds], dv[(3 * jt + 1) * ds], dv[(3 * jt + 2) * ds]}};
+    };
+    const auto key_pos = [&](int kb) { return ldv(bs + kb * PULSE_BODY_STATE_W); };
+    store_amp_row(a.amp_obs_buf + e * a.num_amp_steps * a.amp_width, a.amp_width, stage, lane, ldv(bs), ldq(bs + 3), ldv(bs + 7), ldv(bs + 10),
+                  upright, joint, key_pos);
+  }
+}
+
+}  // namespace
+}  // namespace pulse

@@ -3,36 +3,24 @@
 //                         _compute_reward :871-896, _compute_reset :849-869 -> compute_humanoid_reset :1477-1531,
 //                         _compute_humanoid_obs :195-223, _compute_task_obs :385-440 (compute_location_observations :1588-1616,
 //                         get_heights :718-772 at the head pose :296-311, get_center_heights :690-716).
-//   traj_reset_kernel     TrajGenerator.reset (phc/utils/traj_generator.py:57-112), one thread per reset env.
+//   traj_reset_kernel     TrajGenerator.reset (phc/utils/traj_generator.py:57-112), one thread per reset env;
+//   traj_list_kernel      the same over the device-side env list of a reset (pulse_traj_reset_list).
 //   terrain_heights_kernel get_center_heights / get_heights alone (the spawn lift of _reset_ref_state_init :527-584).
-// Height sampling is Terrain.world_points_to_map / sample_height_points (:1191-1198, :1261-1267); trajectory lookups are
+// Height sampling (terrain_height.cuh) is Terrain.world_points_to_map / sample_height_points (:1191-1198, :1261-1267); trajectory lookups are
 // TrajGenerator.calc_pos (traj_generator.py:148-165).
 //
 // Cell indices, the reset mask and the trajectory segment indices are integers decided by fp32 arithmetic, so the operations that
 // feed them keep the reference's order with round-to-nearest intrinsics (no FMA contraction), as in im_step.cu.  Everything else
 // is under the 1e-4 float tolerance of the observations and rewards.
-#include "humanoid_obs.cuh"
 #include "philox.cuh"
+#include "terrain_height.cuh"
 
 namespace pulse {
 namespace {
 
 constexpr int kTB = PULSE_NUM_BODIES;
 constexpr int kVerts = PULSE_TRAJ_VERTS;
-
-// isaacgym.torch_utils.quat_apply [3P-memory]: t = 2 (xyz x b); b + w t + xyz x t, in this order.
-__device__ __forceinline__ Vec3 cross_rn(Vec3 a, Vec3 b) {
-  return {__fsub_rn(__fmul_rn(a.y, b.z), __fmul_rn(a.z, b.y)), __fsub_rn(__fmul_rn(a.z, b.x), __fmul_rn(a.x, b.z)),
-          __fsub_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x))};
-}
-__device__ __forceinline__ Vec3 quat_apply_rn(Quat q, Vec3 b) {
-  const Vec3 u = {q.x, q.y, q.z};
-  Vec3 t = cross_rn(u, b);
-  t = {__fmul_rn(t.x, 2.0f), __fmul_rn(t.y, 2.0f), __fmul_rn(t.z, 2.0f)};
-  const Vec3 c = cross_rn(u, t);
-  return {__fadd_rn(__fadd_rn(b.x, __fmul_rn(q.w, t.x)), c.x), __fadd_rn(__fadd_rn(b.y, __fmul_rn(q.w, t.y)), c.y),
-          __fadd_rn(__fadd_rn(b.z, __fmul_rn(q.w, t.z)), c.z)};
-}
+constexpr unsigned long long kTrajListStream = 4ull << 32;   // Philox index e + 4 * 2^32: pulse_traj_reset_list
 
 // calc_heading_quat / calc_heading_quat_inv (phc/utils/torch_utils.py:200-240) in the angle form the reference computes: heading =
 // atan2 of the rotated x axis, quat_from_angle_axis(+-heading, z) incl. its final quat_unit.  The height-map points rotate by it, so
@@ -47,45 +35,6 @@ __device__ __forceinline__ Quat heading_quat_ref(Quat q, bool inverse) {
   sincosf(__fmul_rn(h, 0.5f), &sn, &cs);
   const float n = fmaxf(__fsqrt_rn(__fadd_rn(__fmul_rn(sn, sn), __fmul_rn(cs, cs))), 1e-9f);
   return {0.0f, 0.0f, __fdiv_rn(sn, n), __fdiv_rn(cs, n)};
-}
-
-// quat_apply_yaw (:1571-1576): x = y = 0, normalize, quat_apply
-__device__ __forceinline__ Quat yaw_only(Quat q) {
-  const float n = fmaxf(__fsqrt_rn(__fadd_rn(__fmul_rn(q.z, q.z), __fmul_rn(q.w, q.w))), 1e-9f);
-  return {0.0f, 0.0f, __fdiv_rn(q.z, n), __fdiv_rn(q.w, n)};
-}
-
-struct HeightField {
-  const int16_t* hf;
-  long long rows, cols;
-  float hscale, vscale;
-};
-
-// Terrain.world_points_to_map + sample_height_points (:1191-1198, :1261-1267): long(x / horizontal_scale) truncates toward zero,
-// the indices clip to [0, dim - 2], height = min(hf[px, py], hf[px + 1, py + 1]) * vertical_scale.  A plane (hf == NULL) is flat 0.
-__device__ __forceinline__ float sample_height(const HeightField& t, float x, float y) {
-  if (t.hf == nullptr) return 0.0f;
-  long long px = static_cast<long long>(__fdiv_rn(x, t.hscale));
-  long long py = static_cast<long long>(__fdiv_rn(y, t.hscale));
-  px = min(max(px, 0ll), t.rows - 2);
-  py = min(max(py, 0ll), t.cols - 2);
-  const int h1 = __ldg(t.hf + px * t.cols + py), h2 = __ldg(t.hf + (px + 1) * t.cols + py + 1);
-  return __fmul_rn(static_cast<float>(min(h1, h2)), t.vscale);
-}
-
-// world point = quat_apply(q, offset) + origin (get_heights :734-742, get_center_heights :703-711)
-__device__ __forceinline__ float height_at(const HeightField& t, Quat q, const float* off, Vec3 origin) {
-  const Vec3 r = quat_apply_rn(q, Vec3{off[0], off[1], off[2]});
-  return sample_height(t, __fadd_rn(r.x, origin.x), __fadd_rn(r.y, origin.y));
-}
-
-// mean of get_center_heights over the points (lanes < count hold one point each); the result is in every lane
-__device__ __forceinline__ float center_height(const HeightField& t, const float* pts, int count, Quat q_root, Vec3 p_root, bool upright,
-                                               int lane) {
-  const Quat qy = yaw_only(base_rot_removed(q_root, upright));
-  float h = 0.0f;
-  for (int i = lane; i < count; i += 32) h += height_at(t, qy, pts + 3 * i, p_root);
-  return warp_sum(h) / static_cast<float>(count);
 }
 
 // TrajGenerator.calc_pos (traj_generator.py:148-165): phase = clip(t / (num_verts * dt), 0, 1) -- num_verts, not num_segs, as in the
@@ -212,28 +161,24 @@ __global__ void __launch_bounds__(256) terrain_step_kernel(const pulse_terrain_s
 // TrajGenerator.reset (traj_generator.py:57-112) for one env.  Injected draws per env (PULSE_TRAJ_DRAWS = 4 * S + 2, S = num_verts - 1):
 // [0, S) turn angles, [S, 2S) sharp-turn angles, [2S, 3S) sharp-turn coins (sharp where u < sharp_turn_prob, the bernoulli draw),
 // [3S, 4S) speed changes, 4S initial heading, 4S + 1 initial speed.  Column 0 of the first four rows is overwritten, as in the
-// reference.  Without injected draws, Philox block (seed, env, offset + k) supplies the four draws of segment k and block
-// (seed, env, offset + S) the initial heading and speed: a different stream from torch's generator, the same distribution.
-// torch.cumsum on the CPU accumulates fp32 in double; so do the two running sums here.
-__global__ void __launch_bounds__(128) traj_reset_kernel(const pulse_traj_reset_args_t a) {
+// reference.  Without injected draws, Philox block (seed, index, ctr0 + k) supplies the four draws of segment k and block
+// (seed, index, ctr0 + S) the initial heading and speed: a different stream from torch's generator, the same distribution.
+// torch.cumsum on the CPU accumulates fp32 in double; so do the two running sums here.  Args is pulse_traj_reset_args_t or
+// pulse_traj_list_args_t (the same trajectory parameters).
+template <class Args>
+__device__ __forceinline__ void traj_generate(const Args& a, float* vt, float x0, float y0, const float* rin, unsigned long long index,
+                                              unsigned long long ctr0) {
   constexpr int S = kVerts - 1;
-  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
-  if (i >= a.num_ids) return;
-  const long long e = a.env_ids[i];
-  const float* rin = a.rand != nullptr ? a.rand + i * PULSE_TRAJ_DRAWS : nullptr;
-  const unsigned long long off = a.offset + (a.offset_dev != nullptr ? *a.offset_dev : 0ull);
   float u_head, u_v0;
   if (rin != nullptr) {
     u_head = rin[4 * S];
     u_v0 = rin[4 * S + 1];
   } else {
-    const Philox4 b = philox4x32_10(a.seed, static_cast<unsigned long long>(e), off + S);
+    const Philox4 b = philox4x32_10(a.seed, index, ctr0 + S);
     u_head = u01(b.x);
     u_v0 = u01(b.y);
   }
   const float pi = 3.14159265358979f;
-  const float x0 = a.init_pos[i * a.init_stride], y0 = a.init_pos[i * a.init_stride + 1];
-  float* vt = a.verts + e * (kVerts * 3);
   vt[0] = x0;
   vt[1] = y0;
   double ang = 0.0, px = 0.0, py = 0.0;
@@ -246,7 +191,7 @@ __global__ void __launch_bounds__(128) traj_reset_kernel(const pulse_traj_reset_
       coin = rin[2 * S + k];
       u_speed = rin[3 * S + k];
     } else {
-      const Philox4 b = philox4x32_10(a.seed, static_cast<unsigned long long>(e), off + k);
+      const Philox4 b = philox4x32_10(a.seed, index, ctr0 + k);
       u_turn = u01(b.x);
       u_sharp = u01(b.y);
       coin = u01(b.z);
@@ -273,6 +218,29 @@ __global__ void __launch_bounds__(128) traj_reset_kernel(const pulse_traj_reset_
     vt[3 * (k + 1)] = static_cast<float>(px);
     vt[3 * (k + 1) + 1] = static_cast<float>(py);
     vt[3 * (k + 1) + 2] = 0.0f;
+  }
+}
+
+// pulse_traj_reset: row i of the id list; Philox keyed (seed, env, offset + *offset_dev + k).
+__global__ void __launch_bounds__(128) traj_reset_kernel(const pulse_traj_reset_args_t a) {
+  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  if (i >= a.num_ids) return;
+  const long long e = a.env_ids[i];
+  const unsigned long long off = a.offset + (a.offset_dev != nullptr ? *a.offset_dev : 0ull);
+  traj_generate(a, a.verts + e * (kVerts * 3), a.init_pos[i * a.init_stride], a.init_pos[i * a.init_stride + 1],
+                a.rand != nullptr ? a.rand + i * PULSE_TRAJ_DRAWS : nullptr, static_cast<unsigned long long>(e), off);
+}
+
+// pulse_traj_reset_list: the envs of a device-side list, starting at root_states[e, 0:2]; draws per ENV, or Philox keyed
+// (seed, e + 4 * 2^32, PULSE_TRAJ_VERTS * (offset + *offset_dev) + k), so resets at different offsets never share a block.
+__global__ void __launch_bounds__(128) traj_list_kernel(const pulse_traj_list_args_t a) {
+  const long long n = *a.count;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long e = a.env_list[i];
+    const unsigned long long off = a.offset + (a.offset_dev != nullptr ? *a.offset_dev : 0ull);
+    const float* rs = a.root_states + e * a.root_env_stride;
+    traj_generate(a, a.verts + e * (kVerts * 3), rs[0], rs[1], a.rand != nullptr ? a.rand + e * PULSE_TRAJ_DRAWS : nullptr,
+                  static_cast<unsigned long long>(e) + kTrajListStream, static_cast<unsigned long long>(kVerts) * off);
   }
 }
 
@@ -361,5 +329,19 @@ extern "C" int pulse_terrain_heights(const pulse_terrain_heights_args_t* args, v
   if (st != PULSE_OK) return st;
   terrain_heights_kernel<<<grid_for(a.num_rows, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
   PULSE_LAUNCH_OK("terrain_heights_kernel");
+  return PULSE_OK;
+}
+
+extern "C" int pulse_traj_reset_list(const pulse_traj_list_args_t* args, int64_t num_envs, void* stream) {
+  using namespace pulse;
+  PULSE_REQUIRE(args != nullptr, "pulse_traj_reset_list: null args");
+  const pulse_traj_list_args_t& a = *args;
+  PULSE_REQUIRE(num_envs >= 0 && num_envs < (1ll << 31), "pulse_traj_reset_list: num_envs %lld outside [0, 2^31)", (long long)num_envs);
+  PULSE_REQUIRE(a.env_list && a.count && a.root_states && a.verts, "pulse_traj_reset_list: null list / count / root_states / verts");
+  PULSE_REQUIRE(a.root_env_stride >= 2, "pulse_traj_reset_list: root_env_stride < 2");
+  PULSE_REQUIRE(a.seg_dt > 0.0f && a.speed_max >= a.speed_min, "pulse_traj_reset_list: bad trajectory parameters");
+  if (num_envs == 0) return PULSE_OK;
+  traj_list_kernel<<<grid_for(num_envs, 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(a);
+  PULSE_LAUNCH_OK("traj_list_kernel");
   return PULSE_OK;
 }

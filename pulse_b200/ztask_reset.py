@@ -62,6 +62,7 @@ class ZTaskResetB200:
         if state_init not in _INIT:
             raise _lib.PulseError(f"state_init {state_init!r}: the device reset serves Random and Start")
         self.kind, self.motion_lib, self.device = kind, motion_lib, motion_lib._device
+        self.pose_mode, self.init_code = _POSE[kind], _INIT[state_init]
         if floor.dtype != torch.float32 or floor.dim() != 1 or floor.device != self.device:
             raise _lib.PulseError("floor must be a float32 [F] table on the MotionLib's device")
         if floor.shape[0] < motion_lib.gts.shape[0]:
@@ -98,6 +99,20 @@ class ZTaskResetB200:
         [N, steps, 195 | 196].  `env_ids` must be ascending (what `nonzero` returns): an id out of range or not above its predecessor
         is skipped.  Injected draws are per ENV: `motion_ids` int64 [N] (the clips themselves) or `motion_u` [N] (uniforms turned into
         clips through the sampling CDF), `phase` [N], `strike_u` [N, 4]; None -> Philox on (seed, env, offset [+ *offset_dev]).  Returns the workspace {'env_list', 'actor_list', 'tar_actor_list', 'count'} (device)."""
+        a, ws = self._args(root_states=root_states, dof_pos=dof_pos, dof_vel=dof_vel, rigid_body_state=rigid_body_state, progress_buf=progress_buf,
+                           sampled_motion_ids=sampled_motion_ids, motion_start_times=motion_start_times, reset_buf=reset_buf, env_ids=env_ids,
+                           terminate_buf=terminate_buf, contact_forces=contact_forces, amp_obs_buf=amp_obs_buf, actor_ids=actor_ids,
+                           target_states=target_states, tar_actor_ids=tar_actor_ids, motion_ids=motion_ids, motion_u=motion_u, phase=phase,
+                           strike_u=strike_u, seed=seed, offset=offset, offset_dev=offset_dev)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.pulse_reset_ztask(self.motion_lib.handle, C.byref(a), int(progress_buf.shape[0]), _lib.current_stream(self.device)),
+                       "pulse_reset_ztask")
+        return ws
+
+    def _args(self, *, root_states, dof_pos, dof_vel, rigid_body_state, progress_buf, sampled_motion_ids, motion_start_times, reset_buf, env_ids,
+              terminate_buf, contact_forces, amp_obs_buf, actor_ids, target_states, tar_actor_ids, motion_ids, motion_u, phase, strike_u, seed,
+              offset, offset_dev):
+        """The checked `pulse_ztask_reset_args_t` of a `reset_envs` call, and the workspace it writes."""
         N = int(progress_buf.shape[0])
         dev = self.device
         if (reset_buf is None) == (env_ids is None):
@@ -149,7 +164,7 @@ class ZTaskResetB200:
         if offset_dev is not None:
             a.offset_dev = offset_dev.data_ptr()
         a.floor, a.floor_len = self.floor.data_ptr(), int(self.floor.shape[0])
-        a.pose_mode, a.upright, a.state_init, a.dt = _POSE[self.kind], int(self.upright), _INIT[self.state_init], self.dt
+        a.pose_mode, a.upright, a.state_init, a.dt = self.pose_mode, int(self.upright), self.init_code, self.dt
         if amp_obs_buf is not None:
             if not amp_obs_buf.is_contiguous() or amp_obs_buf.dim() != 3 or amp_obs_buf.shape[0] != N or amp_obs_buf.shape[-1] != self.amp_width:
                 raise _lib.PulseError(f"amp_obs_buf must be contiguous [N, steps, {self.amp_width}]")
@@ -181,9 +196,7 @@ class ZTaskResetB200:
         a.env_list, a.actor_list, a.count = ws["env_list"].data_ptr(), ws["actor_list"].data_ptr(), ws["count"].data_ptr()
         if self.kind == "strike":
             a.tar_actor_list = ws["tar_actor_list"].data_ptr()
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.pulse_reset_ztask(self.motion_lib.handle, C.byref(a), N, _lib.current_stream(self.device)), "pulse_reset_ztask")
-        return ws
+        return a, ws
 
     def observe(self, task, rigid_body_state: torch.Tensor, progress_buf: torch.Tensor, **kw) -> None:
         """_compute_observations(env_ids) of the envs of the last `reset_envs`, run after the simulator's refresh: `task` is the
@@ -244,6 +257,27 @@ _KEY_BODY_IDS = (7, 3, 22, 17)                                                  
 _DOF_SUBSET = tuple(k for k in range(69) if (k // 3) not in (3, 7, 17, 22))        # humanoid.py:397,417-421
 
 
+def smpl_reset_tables(task, ml, who: str):
+    """The checks shared by the device resets' mixins and what they build once per MotionLib load: the task's MotionLib as a
+    `MotionLibB200` and the floor table of its one body shape.  Refuses, naming the option, what the device reset does not serve."""
+    if getattr(task, "humanoid_type", None) != "smpl":
+        raise _lib.PulseError(f"{who}: humanoid_type {getattr(task, 'humanoid_type', None)!r}, the device reset serves 'smpl'")
+    if int(getattr(task, "amp_obs_v", 1)) != 1:
+        raise _lib.PulseError(f"{who}: amp_obs_v {task.amp_obs_v}, the device AMP rows are amp_obs_v 1")
+    if tuple(int(i) for i in task._key_body_ids.tolist()) != _KEY_BODY_IDS:
+        raise _lib.PulseError(f"{who}: keyBodies (_key_body_ids) other than R_Ankle, L_Ankle, R_Wrist, L_Wrist")
+    if not getattr(task, "_has_dof_subset", False) or tuple(int(i) for i in task.dof_subset.tolist()) != _DOF_SUBSET:
+        raise _lib.PulseError(f"{who}: a dof_subset (_has_dof_subset) other than the one without toes and hands")
+    shapes = task.humanoid_shapes
+    if bool((shapes != shapes[0:1]).any()):              # once per MotionLib load: one host read
+        raise _lib.PulseError(f"{who}: shape variation (humanoid_shapes rows differ); the floor table is per shape")
+    gender = int(shapes[0, 0])
+    parser = {0: "smpl_parser_n", 1: "smpl_parser_m", 2: "smpl_parser_f"}[gender]
+    pml = ml if isinstance(ml, MotionLibB200) else MotionLibB200.from_reference(ml, device=task.device)
+    pml._sampling_batch_prob = ml._sampling_batch_prob
+    return pml, smpl_ground_table(pml._motion_aa, getattr(task, parser), shapes[0, 1:].float())
+
+
 class HumanoidZTaskResetB200Mixin:
     """`_reset_envs` of HumanoidReach(Z) / HumanoidSpeed(Z) / HumanoidStrike(Z) on the device.  Usage:
 
@@ -270,22 +304,7 @@ class HumanoidZTaskResetB200Mixin:
         if getattr(self, "_pulse_zr", None) is not None and self._pulse_zr_src is ml.gts:
             self._pulse_zr.motion_lib._sampling_batch_prob = ml._sampling_batch_prob     # follows the reference's sampling weights
             return self._pulse_zr
-        if getattr(self, "humanoid_type", None) != "smpl":
-            raise _lib.PulseError(f"HumanoidZTaskResetB200Mixin: humanoid_type {getattr(self, 'humanoid_type', None)!r}, the device reset serves 'smpl'")
-        if int(getattr(self, "amp_obs_v", 1)) != 1:
-            raise _lib.PulseError(f"HumanoidZTaskResetB200Mixin: amp_obs_v {self.amp_obs_v}, the device AMP rows are amp_obs_v 1")
-        if tuple(int(i) for i in self._key_body_ids.tolist()) != _KEY_BODY_IDS:
-            raise _lib.PulseError("HumanoidZTaskResetB200Mixin: keyBodies (_key_body_ids) other than R_Ankle, L_Ankle, R_Wrist, L_Wrist")
-        if not getattr(self, "_has_dof_subset", False) or tuple(int(i) for i in self.dof_subset.tolist()) != _DOF_SUBSET:
-            raise _lib.PulseError("HumanoidZTaskResetB200Mixin: a dof_subset (_has_dof_subset) other than the one without toes and hands")
-        shapes = self.humanoid_shapes
-        if bool((shapes != shapes[0:1]).any()):              # once per MotionLib load: one host read
-            raise _lib.PulseError("HumanoidZTaskResetB200Mixin: shape variation (humanoid_shapes rows differ); the floor table is per shape")
-        gender = int(shapes[0, 0])
-        parser = {0: "smpl_parser_n", 1: "smpl_parser_m", 2: "smpl_parser_f"}[gender]
-        pml = ml if isinstance(ml, MotionLibB200) else MotionLibB200.from_reference(ml, device=self.device)
-        pml._sampling_batch_prob = ml._sampling_batch_prob
-        floor = smpl_ground_table(pml._motion_aa, getattr(self, parser), shapes[0, 1:].float())
+        pml, floor = smpl_reset_tables(self, ml, "HumanoidZTaskResetB200Mixin")
         kind = self._pulse_ztask_kind()
         kw = {}
         if kind == "strike":
