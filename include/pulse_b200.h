@@ -953,6 +953,14 @@ typedef struct {
 } pulse_terrain_step_args_t;
 int pulse_terrain_step(const pulse_terrain_step_args_t* args, int64_t num_envs, void* stream);
 
+/* Post-physics step of the terrain task's rollout (humanoid.py:1315-1346): `progress_buf += 1` inside the kernel (the struct's
+ * progress_buf is written here; the new value is broadcast to the env's warp, which never reads the counter from memory), then the
+ * per-env code of pulse_terrain_step with flags PULSE_STEP_ALL (the only flags accepted; no env_ids), then dones[e] =
+ * float(reset_buf[e]) (amp_agent.py:380).  obs_buf / obs_stride address the next step's experience slice, rew_buf the step's reward
+ * row.  Argument checks as pulse_terrain_step, plus dones != NULL.  Outputs are bit-equal to advancing the counter and calling
+ * pulse_terrain_step(PULSE_STEP_ALL). */
+int pulse_terrain_rollout_step(const pulse_terrain_step_args_t* args, float* dones, int64_t num_envs, void* stream);
+
 /* TrajGenerator.reset (phc/utils/traj_generator.py:57-112) for num_ids envs, one thread each: random turns (sharp turns with
  * probability sharp_turn_prob), the clipped speed recurrence, waypoints from init_pos's xy (row i belongs to env_ids[i]).  rand
  * [num_ids, PULSE_TRAJ_DRAWS] injects the uniform draws (layout in terrain.cu); NULL draws them with Philox4x32-10 keyed by

@@ -7,13 +7,16 @@ There is no CPU fallback: importing the compute modules without the built librar
 from . import _lib  # noqa: F401
 from ._lib import PulseError  # noqa: F401
 
-__all__ = ["PulseError", "TerrainResetB200", "ZTaskStepsB200"]
+__all__ = ["PulseError", "TerrainResetB200", "TerrainStepsB200", "ZTaskStepsB200"]
 
 
 def __getattr__(name):
     if name == "ZTaskStepsB200":           # resolved on first use: importing the package alone does not import torch
         from .ztask_rollout import ZTaskStepsB200
         return ZTaskStepsB200
+    if name == "TerrainStepsB200":
+        from .terrain_rollout import TerrainStepsB200
+        return TerrainStepsB200
     if name == "TerrainResetB200":
         from .terrain_reset import TerrainResetB200
         return TerrainResetB200

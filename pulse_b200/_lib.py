@@ -452,6 +452,7 @@ SIGNATURES = {
     "pulse_reach_rollout_step": (C.c_int, [C.POINTER(ReachStepArgs), C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_ztask_rollout_step": (C.c_int, [C.POINTER(ZTaskStepArgs), C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_terrain_step": (C.c_int, [C.POINTER(TerrainStepArgs), C.c_int64, C.c_void_p]),
+    "pulse_terrain_rollout_step": (C.c_int, [C.POINTER(TerrainStepArgs), C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_traj_reset": (C.c_int, [C.POINTER(TrajResetArgs), C.c_void_p]),
     "pulse_terrain_heights": (C.c_int, [C.POINTER(TerrainHeightsArgs), C.c_void_p]),
     "pulse_traj_reset_list": (C.c_int, [C.POINTER(TrajListArgs), C.c_int64, C.c_void_p]),

@@ -1,0 +1,229 @@
+"""The task-independent part of the latent-space rollout drivers (`ZTaskStepsB200`, `TerrainStepsB200`): the experience buffers, the
+action half of a step (the policy's heads beside the frozen prior, `pulse_latent_post`, the decoder), the next values, the launch
+schedules, `play_steps`, `finish` and the PPO update (`AMPAgent.play_steps` + `train_epoch`, phc/learning/amp_agent.py:341-439,
+:462-548; `HumanoidZ.step -> step_z`, humanoid_z.py:157-173)."""
+import ctypes as C
+from typing import Callable, Optional
+
+import torch
+
+from . import _lib
+from .rollout import GraphRunner, finish_returns
+
+
+class LatentStepsB200(GraphRunner):
+    """One horizon of a latent-space task per `play_steps()`.  A subclass supplies the task's pieces of a step:
+         `_reset(t)`           the reset of the done envs (Philox draws keyed (reset_seed, env, t + the policy's device offset)), which
+                               leaves the reset's workspace {'env_list', 'count', ...} in `reset_ws`;
+         `_reset_obs(t)`       the observation of the reset envs into obses[:, t], then the task's `_reset_task`;
+         `_pre_physics(dec, t)` what the step does with the decoder output `dec` [n, 69] before the physics (PD targets into pd_tar, ...);
+         `_env_step(t)`        the rollout step kernel (progress += 1, reward, reset, next observation) into obses[:, t+1] / obs_carry,
+                               rewards[t], dones[t], reset_buf, terminate_buf;
+         `first_observation()` the observation of the initial state into obs_carry.
+    For every step t, in the reference's order: `_reset(t)`, the `refresh(t, ws)` hook if set, `_reset_obs(t)`; `get_action_values`
+    (the policy's `heads_into`, actor beside critic, and beside both the frozen prior MLP on obses[:, t, :358] with the clamped self
+    observation columns of the decoder operand: neither depends on the action); `pulse_latent_post` (a_z = mu + exp(logstd) eps into
+    actions[:, t], neglogp[:, t], the de-normalised value into values[t] and z = prior_mu + a_z into the decoder operand; the latent
+    tasks' configs have clip_actions False and `project_to_norm(.., "none")` is the identity, so a_z is neither clamped nor projected);
+    the decoder MLP on [clamp(norm(s), +-5) | z] (HumanoidZ.compute_z_actions); `_pre_physics`; the caller's `physics(t)` hook;
+    `_env_step(t)`; next_values[t] = critic(obses[:, t+1]) (1 - terminate) on the critic's second operand slot.
+    `finish()` then computes GAE, normalised advantages and value-normalised returns from the task reward alone (task_reward_w 1,
+    disc_reward_w 0) and `train_epoch()` runs the PPO update.
+
+    The experience buffers are env-major (`obses[n, T, W]`, `actions[n, T, E]`, `mus[n, T, E]`, `neglogp[n, T]`; `adv[n*T]`, `ret[n*T]`), so
+    a minibatch is a contiguous row range; `values`, `next_values` [T, n, 1], `rewards`, `dones` [T, n] are time-major as GAE reads them.
+
+    Launch structure.  With no hooks the horizon is ONE CUDA graph over four streams:
+         main    reset(t) -> obs of the reset envs -> reset_task -> normalise -> actor -> latent_post -> decoder -> pre_physics -> step kernel(t)
+         side A  critic(obs t) beside the actor
+         side P  prior operands + prior MLP(obs t) beside actor and critic
+         side B  next values of step t (normalise -> critic -> value_post) beside reset(t+1) / actor(t+1)
+       Hazards, all stream dependencies inside the captured graph: P starts after the observation of the reset envs (it reads obses[:, t]
+       and rewrites the decoder operand's self columns, which decoder(t-1) on main has read by then); latent_post waits for A (value) and
+       P (prior mean, decoder operand); the observation of the reset envs overwrites rows of obses[:, t+1] that B's normalise reads (main
+       waits for the event B records after it); the step kernel(t+1) rewrites `terminate_buf` that B's value_post reads (main waits for B);
+       B starts after the step kernel(t).  A and B use separate critic operands and workspaces (slot 0 / slot 1).  The reset does not
+       clear `terminate_buf`: the step kernel rewrites it for every env each step and nothing reads it in between.
+       With `physics` / `refresh` hooks the steps run as graph segments between the hook calls (reset | act | post), each with the same
+       forks joined inside the segment.  `use_graphs=False` runs the same entry points on one stream in the order above.
+       No ATen elementwise op, boolean-mask index or host synchronisation is inside the loop."""
+
+    def _setup(self, task, reset, policy, vae, sim: dict, horizon: int, obs_width: int, pd_offset: Optional[torch.Tensor],
+               pd_scale: Optional[torch.Tensor], pd_freeze: Optional[torch.Tensor], use_graphs: bool, gamma: float, tau: float,
+               reset_seed: int) -> None:
+        """The buffers and state every driver shares; the subclass calls it after its checks."""
+        self.task, self.reset, self.policy, self.vae, self.sim, self.T = task, reset, policy, vae, sim, int(horizon)
+        self.dev = policy.device
+        self.lib = _lib.load()
+        n = self.n
+        T, W, E, A, dev = self.T, int(obs_width), vae.E, vae.A, self.dev
+        z = lambda *s, **k: torch.zeros(*s, device=dev, **k)
+        self.obses, self.obs_carry = z(n, T, W), z(n, W)
+        self.actions, self.mus, self.neglogp = z(n, T, E), z(n, T, E), z(n, T)
+        self.values, self.next_values = z(T, n, 1), z(T, n, 1)
+        self.rewards, self.dones = z(T, n), z(T, n)
+        self.reset_buf, self.terminate_buf = z(n, dtype=torch.long), z(n, dtype=torch.long)
+        self.adv, self.ret = z(n * T), z(n * T)
+        self.pd_tar = z(n, A)
+        self.pd = (pd_offset if pd_offset is not None else z(A), pd_scale if pd_scale is not None else torch.ones(A, device=dev))
+        if pd_freeze is not None and (pd_freeze.dtype != torch.uint8 or pd_freeze.numel() != A):
+            raise _lib.PulseError(f"pd_freeze must be uint8 [{A}]")
+        self.pd_freeze = pd_freeze
+        self.gamma, self.tau = gamma, tau
+        self.reset_seed = (int(reset_seed) * 0x9E3779B97F4A7C15 + 0x13198A2E03707344) & (2 ** 64 - 1)
+        self.use_graphs = use_graphs
+        self._graphs, self._pool = {}, None
+        self.physics: Optional[Callable[[int], None]] = None           # physics(t): between the pre-physics work and the step kernel
+        self.refresh: Optional[Callable[[int, dict], None]] = None     # refresh(t, ws): after the reset, before the reset envs' observation
+        self.reset_ws = None
+        self.z_actions = None          # the decoder's output of the last step, fp32 [n, 69] (a reused workspace)
+        self._streams = None
+
+    # ------------------------------------------------------------------ the task's pieces (subclass)
+    def _reset(self, t: int) -> None:
+        raise NotImplementedError
+
+    def _reset_obs(self, t: int) -> None:
+        raise NotImplementedError
+
+    def _pre_physics(self, dec: torch.Tensor, t: int) -> None:
+        raise NotImplementedError
+
+    def _env_step(self, t: int) -> None:
+        raise NotImplementedError
+
+    def first_observation(self) -> None:
+        raise NotImplementedError
+
+    # ------------------------------------------------------------------ the shared pieces of one step
+    def _launch(self, name: str, *args) -> None:
+        with torch.cuda.device(self.dev):
+            _lib.check(getattr(self.lib, name)(*args, _lib.current_stream(self.dev)), name)
+
+    def _act(self, t: int, side_a=None, side_p=None) -> None:
+        """get_action_values (amp_agent.py:359-378), HumanoidZ.compute_z_actions (humanoid_z.py:75-155) and the task's pre-physics work."""
+        pol, vae, n = self.policy, self.vae, self.n
+        obs, mus = self.obses[:, t], self.mus[:, t]
+        main = torch.cuda.current_stream(self.dev)
+        if side_p is not None:
+            side_p.wait_stream(main)
+            with torch.cuda.stream(side_p):
+                prior_head, dec_in = vae.z_prior(obs)
+        else:
+            prior_head, dec_in = vae.z_prior(obs)
+        value = pol.heads_into(obs, mus=mus, side=side_a)
+        if side_p is not None:
+            main.wait_stream(side_p)
+        actions, neglogp, values = self.actions[:, t], self.neglogp[:, t], self.values[t]
+        rms = pol.value_rms
+        a = _lib.LatentPostArgs(mu=mus.data_ptr(), ld_mu=mus.stride(0), logstd=pol.logstd.data_ptr(), seed=pol.rng_seed,
+                                rng_offset=pol.rng_offset.data_ptr(), rng_step=t, latent=vae.E, actions=actions.data_ptr(),
+                                ld_actions=actions.stride(0), neglogp=neglogp.data_ptr(), ld_neglogp=neglogp.stride(0),
+                                value=value.data_ptr(), ld_value=value.stride(0), values_out=values.data_ptr(), ld_values=values.stride(0),
+                                prior_mu=prior_head.data_ptr(), ld_prior=prior_head.stride(0), z_bf16=dec_in.data_ptr(), ld_z=dec_in.stride(0))
+        if rms is not None:
+            a.value_mean, a.value_var, a.value_eps = rms.running_mean.data_ptr(), rms.running_var.data_ptr(), rms.eps
+        self._launch("pulse_latent_post", C.byref(a), n)
+        self.z_actions = dec = vae.dec.forward(dec_in)
+        self._pre_physics(dec, t)
+
+    def _next_obs(self, t: int) -> torch.Tensor:
+        return self.obses[:, t + 1] if t + 1 < self.T else self.obs_carry
+
+    def _next_values(self, t: int, after_normalize=None) -> None:
+        """`next_vals = _eval_critic(obs); next_vals *= 1 - terminated` (amp_agent.py:396-398), on the critic's second operand slot."""
+        self.policy.critic_values_into(self._next_obs(t), self.next_values[t].view(-1), terminate=self.terminate_buf, slot=1,
+                                       after_normalize=after_normalize)
+
+    def _sides(self):
+        if self._streams is None:
+            self._streams = tuple(torch.cuda.Stream(self.dev) for _ in range(3))
+        return self._streams
+
+    # ------------------------------------------------------------------ schedules
+    def _sequential(self) -> None:
+        """The horizon on one stream, hooks included, in the order of the class docstring."""
+        for t in range(self.T):
+            self._reset(t)
+            if self.refresh is not None:
+                self.refresh(t, self.reset_ws)
+            self._reset_obs(t)
+            self._act(t)
+            if self.physics is not None:
+                self.physics(t)
+            self._env_step(t)
+            self._next_values(t)
+
+    def _whole_overlapped(self) -> None:
+        """The horizon without hooks over main + sides A, P, B (hazards: class docstring)."""
+        main = torch.cuda.current_stream(self.dev)
+        A, P, B = self._sides()
+        norm_done = None
+        for t in range(self.T):
+            self._reset(t)
+            if norm_done is not None:
+                main.wait_event(norm_done)                           # B has read obses[:, t]
+            self._reset_obs(t)
+            self._act(t, A, P)
+            if t > 0:
+                main.wait_stream(B)                                  # value_post(t-1) has read terminate_buf
+            self._env_step(t)
+            B.wait_stream(main)
+            with torch.cuda.stream(B):
+                norm_done = torch.cuda.Event()
+                self._next_values(t, after_normalize=lambda ev=norm_done: ev.record(B))
+        main.wait_stream(B)
+
+    def _act_segment(self, t: int) -> None:
+        self._reset_obs(t)
+        self._act(t, *self._sides()[:2])
+
+    def _post_segment(self, t: int) -> None:
+        self._env_step(t)
+        self._next_values(t)
+
+    def play_steps(self) -> None:
+        """One horizon.  The first observation is the last next-observation of the previous horizon.  Afterwards the policy's Philox
+        offset (shared with the reset and task draws) moves past the horizon."""
+        self.obses[:, 0].copy_(self.obs_carry)
+        if not self.use_graphs:
+            self._sequential()
+        elif self.physics is None and self.refresh is None:
+            self._run(("horizon",), self._whole_overlapped)
+        else:
+            for t in range(self.T):
+                self._run(("reset", t), self._reset, t)
+                if self.refresh is not None:
+                    self.refresh(t, self.reset_ws)
+                self._run(("act", t), self._act_segment, t)
+                if self.physics is not None:
+                    self.physics(t)
+                self._run(("post", t), self._post_segment, t)
+        self.policy.advance_rng(self.T)
+
+    # ------------------------------------------------------------------ after the horizon
+    def finish(self) -> None:
+        """GAE + returns, advantage normalisation and value / return normalisation (`rollout.finish_returns`) from the task reward alone:
+        task_reward_w 1, disc_reward_w 0 (`_combine_rewards`, amp_agent.py:1011-1025)."""
+        finish_returns(self.policy, self.dones, self.values, self.rewards.unsqueeze(-1), self.next_values, self.adv, self.ret, self.gamma, self.tau)
+
+    def _update_mb(self, i: int, mb: int) -> None:
+        r0, r1 = i * mb, (i + 1) * mb
+        rows = self.n * self.T
+        self.policy.train_minibatch(self.obses.view(rows, -1)[r0:r1], self.actions.view(rows, -1)[r0:r1], self.neglogp.view(rows)[r0:r1],
+                                    self.adv[r0:r1], self.ret[r0:r1], old_mu=self.mus.view(rows, -1)[r0:r1])
+
+    def train_epoch(self, mini_epochs: int = 6, minibatch: int = 16384) -> torch.Tensor:
+        """The PPO update of one epoch (`train_epoch` -> `calc_gradients`, amp_agent.py:462-548, :605-760, without the discriminator
+        term): `mini_epochs` passes over the horizon's experience in contiguous minibatches of min(minibatch, n*T) rows, one
+        `train_minibatch` each with old_mu = mus; every minibatch index is one CUDA graph.  Returns the policy's stats tensor,
+        accumulated over the epoch (cleared at its start)."""
+        rows = self.n * self.T
+        mb = min(int(minibatch), rows)
+        if mb <= 0 or rows % mb:
+            raise _lib.PulseError(f"minibatch {minibatch} must divide the {rows} rows of a horizon")
+        self.policy.reset_stats()
+        for _ in range(mini_epochs):
+            for i in range(rows // mb):
+                self._run(("update", i, mb), self._update_mb, i, mb)
+        return self.policy.stats

@@ -205,7 +205,7 @@ class PPOPolicy:
         `with_value`, the critic; returns its NORMALISED value [M, 1] (a reused workspace) or None.  `side`: the critic runs on that
         stream beside the actor and is joined before returning."""
         b = self._buf(obs.shape[0], False)
-        self.obs_rms.normalize_into(obs, b["x"])
+        self._normalize_eval(obs, b)
         if side is not None and with_value:              # actor | critic on two streams (fork / join: still one CUDA-graph segment)
             main = torch.cuda.current_stream(self.device)
             side.wait_stream(main)
@@ -232,12 +232,15 @@ class PPOPolicy:
         self.obs_rms.normalize_into(obs, x)
         if after_normalize is not None:
             after_normalize()
-        value = self.critic.forward(x, slot=slot)
+        self._value_post(self.critic.forward(x, slot=slot), terminate, out)
+
+    def _value_post(self, value: torch.Tensor, terminate: Optional[torch.Tensor], out: torch.Tensor) -> None:
+        """`pulse_value_post`: out = de-normalised `value` (* (1 - terminate) when given)."""
         rms = self.value_rms
         with torch.cuda.device(self.device):
             _lib.check(self.lib.pulse_value_post(value.data_ptr(), value.stride(0), rms.running_mean.data_ptr() if rms is not None else None,
                                                  rms.running_var.data_ptr() if rms is not None else None, rms.eps if rms is not None else 0.0,
-                                                 _lib.ptr(terminate), out.data_ptr(), out.stride(0), M, _lib.current_stream(self.device)),
+                                                 _lib.ptr(terminate), out.data_ptr(), out.stride(0), value.shape[0], _lib.current_stream(self.device)),
                        "pulse_value_post")
 
     def advance_rng(self, steps: int) -> None:

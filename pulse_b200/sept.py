@@ -86,14 +86,28 @@ class SeptPolicy(PPOPolicy):
 
     # ------------------------------------------------------------------ rollout side
     def _normalize_eval(self, obs: torch.Tensor, b: dict) -> None:
+        """b['x'] <- [embedding | normalised self | 1 | 0...]: normalise_split, then the task encoder into its first E columns.  Run
+        once before the actor | critic fork of `heads_into`; both heads read the same operand."""
         self.obs_rms.normalize_split(obs, self.S, b["x"], self.E, b["t"], update=False)
         self.task.forward(b["t"], out=b["x"][:, :self.E])
 
-    def act_into(self, *args, **kw):
-        raise _lib.PulseError("SeptPolicy.act_into: the device-side rollout loop drives the imitation task only; use act()")
-
-    def critic_values_into(self, *args, **kw):
-        raise _lib.PulseError("SeptPolicy.critic_values_into: the device-side rollout loop drives the imitation task only; use critic_values()")
+    def critic_values_into(self, obs: torch.Tensor, out: torch.Tensor, terminate: Optional[torch.Tensor] = None, slot: int = 0,
+                           after_normalize=None) -> None:
+        """PPOPolicy.critic_values_into through the shared task encoder.  `slot` 1 uses operands of its own (x_next, t_next) and the
+        slot-1 workspaces of the encoder and the critic, none of which `heads_into` touches on slot 0, so that it may run on another
+        stream beside it; `after_normalize()` is called once `obs` has been read."""
+        M = obs.shape[0]
+        b = self._buf(M, False)
+        x, t = b["x"], b["t"]
+        if slot:
+            if "x_next" not in b:
+                b["x_next"], b["t_next"] = torch.zeros_like(b["x"]), torch.zeros_like(b["t"])
+            x, t = b["x_next"], b["t_next"]
+        self.obs_rms.normalize_split(obs, self.S, x, self.E, t, update=False)
+        if after_normalize is not None:
+            after_normalize()
+        self.task.forward(t, out=x[:, :self.E], slot=slot)
+        self._value_post(self.critic.forward(x, slot=slot), terminate, out)
 
     # ------------------------------------------------------------------ update side
     def _reducer(self, world_size: int):
