@@ -177,6 +177,21 @@ typedef struct {
 /* num_envs = number of envs processed (= len(env_ids) when env_ids is given). */
 int pulse_im_step(const pulse_motionlib_t* lib, const pulse_im_step_args_t* args, int64_t num_envs, void* stream);
 
+/* Tracked-body observation of the fused step (HumanoidImZ, env_pulse_im.yaml: trackBodies [Head, L_Hand, R_Hand], obs_v 6).
+ * pulse_im_track_step is pulse_im_step (same arguments, flags, env list, side buffers, full-body reward and reset) whose observation
+ * row is [358 self | task observation of the K tracked bodies], block-major as compute_imitation_observations_v6 / _v7
+ * (humanoid_im.py:1328-1413) over the bodies in `_track_bodies_id` order:
+ *   version 6: dp | rot6(dq) | dv | dw | R(p_ref - p_root) | rot6(q_ref)   358 + 24 K floats
+ *   version 7: dp | dv | R(p_ref - p_root)                                  358 + 9 K floats
+ * obs_stride must be at least that width; the row's columns beyond it are not written. */
+typedef struct {
+  int8_t rank[24];     /* rank[j]: position of body j in _track_bodies_id, -1 = untracked; the ranks are a permutation of 0..K-1 */
+  int32_t num_track;   /* K in [1, 24] */
+  int32_t version;     /* 6 or 7 */
+} pulse_im_track_t;
+int pulse_im_track_step(const pulse_motionlib_t* lib, const pulse_im_step_args_t* args, const pulse_im_track_t* track, int64_t num_envs,
+                        void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * AMP observation + history shift.
  *   HumanoidAMP._update_hist_amp_obs      phc/env/tasks/humanoid_amp.py:622-630

@@ -7,7 +7,7 @@ There is no CPU fallback: importing the compute modules without the built librar
 from . import _lib  # noqa: F401
 from ._lib import PulseError  # noqa: F401
 
-__all__ = ["PulseError", "TerrainResetB200", "TerrainStepsB200", "ZTaskStepsB200"]
+__all__ = ["ImZStepsB200", "PulseError", "TerrainResetB200", "TerrainStepsB200", "ZTaskStepsB200"]
 
 
 def __getattr__(name):
@@ -17,6 +17,9 @@ def __getattr__(name):
     if name == "TerrainStepsB200":
         from .terrain_rollout import TerrainStepsB200
         return TerrainStepsB200
+    if name == "ImZStepsB200":
+        from .imz_rollout import ImZStepsB200
+        return ImZStepsB200
     if name == "TerrainResetB200":
         from .terrain_reset import TerrainResetB200
         return TerrainResetB200

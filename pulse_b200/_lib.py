@@ -57,6 +57,10 @@ class ImStepArgs(C.Structure):
     ]
 
 
+class ImTrack(C.Structure):
+    _fields_ = [("rank", C.c_int8 * 24), ("num_track", C.c_int32), ("version", C.c_int32)]
+
+
 class ResetArgs(C.Structure):
     _fields_ = [
         ("reset_buf", C.c_void_p), ("env_ids_in", C.c_void_p), ("num_ids", C.c_int64), ("phase", C.c_void_p),
@@ -377,6 +381,7 @@ SIGNATURES = {
     "pulse_motionlib_destroy": (C.c_int, [C.c_void_p]),
     "pulse_motion_state": (C.c_int, [C.c_void_p, C.POINTER(MotionQuery), C.c_int64, C.c_void_p]),
     "pulse_im_step": (C.c_int, [C.c_void_p, C.POINTER(ImStepArgs), C.c_int64, C.c_void_p]),
+    "pulse_im_track_step": (C.c_int, [C.c_void_p, C.POINTER(ImStepArgs), C.POINTER(ImTrack), C.c_int64, C.c_void_p]),
     "pulse_reset_ref_state": (C.c_int, [C.c_void_p, C.POINTER(ResetArgs), C.c_int64, C.c_void_p]),
     "pulse_reset_getup": (C.c_int, [C.c_void_p, C.POINTER(GetupResetArgs), C.c_int64, C.c_void_p]),
     "pulse_getup_amp_init": (C.c_int, [C.POINTER(GetupAmpArgs), C.c_int64, C.c_void_p]),

@@ -162,6 +162,13 @@ __device__ __forceinline__ RefPose blend_pose(const float* f0, const float* f1, 
   return r;
 }
 
+// yaw_rot of a difference of the blended reference position, with the y and z products fused the way the full row's code compiles
+// them (fma(s, v.y, wz2 * v.x), fma(s, v.z, zz2 * v.z)).  Which product of a * b + c * d the compiler fuses follows the code around
+// it; the tracked row pins it with intrinsics so its columns stay the full row's bit for bit.
+__device__ __forceinline__ Vec3 yaw_rot_pinned(Yaw y, Vec3 v) {
+  return {v.x * y.s - y.wz2 * v.y, __fmaf_rn(y.s, v.y, __fmul_rn(y.wz2, v.x)), __fmaf_rn(y.s, v.z, __fmul_rn(y.zz2, v.z))};
+}
+
 // ---- planner: one pass plans kBatch groups (lane = group-in-batch * 8 + env slot) ----------------------
 __device__ __forceinline__ void plan_batch(const pulse_motionlib_desc_t& lib, const pulse_im_step_args_t& a, long long num_envs,
                                            long long ngroups, long long first_group, long long group_stride,
@@ -306,8 +313,10 @@ __device__ __forceinline__ PowerOps power_load(const pulse_im_step_args_t& a, lo
   return o;
 }
 
+// kTrack: the observation row is [self | task observation of the tracked bodies] (pulse_im_track_t) instead of the 934-float row
+template <bool kTrack>
 __global__ void __launch_bounds__(kThreads, 1) im_step_kernel(const pulse_motionlib_desc_t lib, const pulse_im_step_args_t a,
-                                                              long long num_envs) {
+                                                              long long num_envs, const pulse_im_track_t tr) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   CtaSmem& sm = *reinterpret_cast<CtaSmem*>(smem_raw);
   const int tid = threadIdx.x;
@@ -377,6 +386,7 @@ __global__ void __launch_bounds__(kThreads, 1) im_step_kernel(const pulse_motion
   const float term_j = do_reset ? a.termination_distances[j] : 0.0f;
   float(*red)[kRed][kNB + 1] = sm.red[team];
   unsigned* fallen = sm.fallen[team];
+  const int rank = kTrack ? tr.rank[j] : -1;   // body j's place in the tracked row, -1 = untracked
   PowerOps pw_ops = {};
   if (do_power && team < my_groups) pw_ops = power_load(a, num_envs, blockIdx.x + team * (long long)gridDim.x, k, j);
   for (long long n = team; n < my_groups; n += kTeams) {
@@ -447,7 +457,8 @@ __global__ void __launch_bounds__(kThreads, 1) im_step_kernel(const pulse_motion
       orow = a.obs_buf + P.env * a.obs_stride;
       ophase = static_cast<int>((reinterpret_cast<uintptr_t>(orow) >> 2) & 3);
       // global 16-byte boundaries coincide with shared ones; a row starting 3 floats past a boundary would need 937 staging floats:
-      // it is written straight to global memory instead (never the case for [N, 934]-strided buffers: 934 k = 0 or 2 mod 4)
+      // it is written straight to global memory instead (never the case for [N, 934]-strided buffers: 934 k = 0 or 2 mod 4; every
+      // fourth row of a tracked v7 row with odd K, 358 + 9 K floats wide)
       float* o = ophase == 3 ? orow : blk + ophase;
       // self observation, store_self_obs's layout written out: through the helper ptxas fuses the other product of yaw_rot's
       // a * b - c * d, which moves the result by an ulp
@@ -458,12 +469,37 @@ __global__ void __launch_bounds__(kThreads, 1) im_step_kernel(const pulse_motion
       stv(o + 286 + 3 * j, yaw_rot(yr, w));
       // task observation v6 (humanoid_im.py:1328-1378), block-major
       float* t = o + PULSE_SELF_OBS;
-      stv(t + 3 * j, yaw_rot(yr, r2.p - p));
-      qsix(yaw_mul_right(yaw_mul_left(-hs, hc, qmul(r2.q, qconj(q))), hs, hc), t + 72 + 6 * j);
-      stv(t + 216 + 3 * j, yaw_rot(yr, r2.v - v));
-      stv(t + 288 + 3 * j, yaw_rot(yr, r2.w - w));
-      stv(t + 360 + 3 * j, yaw_rot(yr, r2.p - p_root));
-      qsix(yaw_mul_left(-hs, hc, r2.q), t + 432 + 6 * j);
+      if constexpr (kTrack) {
+        // the tracked subset: the full row's pieces, each block K bodies wide, body j at its rank in _track_bodies_id (v7, :1381-1413,
+        // keeps dp | dv | R(p_ref - p_root)).  Every thread computes all six pieces in this block, without a branch, as the full row
+        // does, so the compiler orders and fuses their products as there; for the two pieces rotated from the blended reference
+        // position it still picks the other product of y and z to fuse, and yaw_rot_pinned fixes that.  The columns are then the full
+        // row's bit for bit (the PTX expression trees of the six pieces match; tests/test_gpu_imz_rollout.py checks the values).
+        // What is not part of the row goes to a 24-float sink at the end of the env's frame slots, past the staged row (the row
+        // reaches it only at K = 24, when every body is tracked); nothing reads the sink.
+        const int K = tr.num_track;
+        const bool v6 = tr.version == 6, on = rank >= 0;
+        float* sink = blk + (kFrameBlock - 24);
+        float* const d[6] = {on ? t + 3 * rank : sink,
+                             on && v6 ? t + 3 * K + 6 * rank : sink + 3,
+                             on ? t + (v6 ? 9 : 3) * K + 3 * rank : sink + 9,
+                             on && v6 ? t + 12 * K + 3 * rank : sink + 12,
+                             on ? t + (v6 ? 15 : 6) * K + 3 * rank : sink + 15,
+                             on && v6 ? t + 18 * K + 6 * rank : sink + 18};
+        stv(d[0], yaw_rot_pinned(yr, r2.p - p));
+        qsix(yaw_mul_right(yaw_mul_left(-hs, hc, qmul(r2.q, qconj(q))), hs, hc), d[1]);
+        stv(d[2], yaw_rot(yr, r2.v - v));
+        stv(d[3], yaw_rot(yr, r2.w - w));
+        stv(d[4], yaw_rot_pinned(yr, r2.p - p_root));
+        qsix(yaw_mul_left(-hs, hc, r2.q), d[5]);
+      } else {
+        stv(t + 3 * j, yaw_rot(yr, r2.p - p));
+        qsix(yaw_mul_right(yaw_mul_left(-hs, hc, qmul(r2.q, qconj(q))), hs, hc), t + 72 + 6 * j);
+        stv(t + 216 + 3 * j, yaw_rot(yr, r2.v - v));
+        stv(t + 288 + 3 * j, yaw_rot(yr, r2.w - w));
+        stv(t + 360 + 3 * j, yaw_rot(yr, r2.p - p_root));
+        qsix(yaw_mul_left(-hs, hc, r2.q), t + 432 + 6 * j);
+      }
       // reference-pose side buffers (humanoid_im.py:835-848)
       if (a.ref_body_pos != nullptr) stv(a.ref_body_pos + P.env * (kNB * 3) + 3 * j, r2.p);
       if (a.ref_body_vel != nullptr) stv(a.ref_body_vel + P.env * (kNB * 3) + 3 * j, r2.v);
@@ -492,8 +528,9 @@ __global__ void __launch_bounds__(kThreads, 1) im_step_kernel(const pulse_motion
 
     // ---- epilogue ---------------------------------------------------------------------------------------------
     if (valid && do_obs) {
-      const int head = (4 - ophase) & 3;         // floats before the first 16-byte boundary
-      const int nmid = ((kObs - head) / 4) * 4;  // floats in the aligned middle
+      const int width = kTrack ? PULSE_SELF_OBS + (tr.version == 6 ? 24 : 9) * tr.num_track : kObs;   // floats in the row
+      const int head = (4 - ophase) & 3;          // floats before the first 16-byte boundary
+      const int nmid = ((width - head) / 4) * 4;  // floats in the aligned middle
       const float* o = ophase == 3 ? orow : blk + ophase;
       if (ophase != 3) {
         if (j == 0) {
@@ -503,7 +540,7 @@ __global__ void __launch_bounds__(kThreads, 1) im_step_kernel(const pulse_motion
           if (j - 1 < head) orow[j - 1] = o[j - 1];
         } else if (j <= 6) {
           const int i = head + nmid + (j - 4);
-          if (i < kObs) orow[i] = o[i];
+          if (i < width) orow[i] = o[i];
         }
       }
       if (a.self_obs_buf != nullptr) {
@@ -572,48 +609,45 @@ __global__ void __launch_bounds__(kThreads, 1) im_step_kernel(const pulse_motion
   }
 }
 
-}  // namespace
-}  // namespace pulse
 
-extern "C" int pulse_im_step(const pulse_motionlib_t* lib, const pulse_im_step_args_t* args, int64_t num_envs,
-                             void* stream) {
-  using namespace pulse;
-  PULSE_REQUIRE(lib != nullptr && args != nullptr, "pulse_im_step: null lib/args");
-  PULSE_REQUIRE(num_envs >= 0, "pulse_im_step: negative num_envs");
+// Argument checks and launch shared by both entry points; `who` names the entry point in the messages, `width` is the row's float count.
+template <bool kTrack>
+int im_step_launch(const char* who, const pulse_motionlib_t* lib, const pulse_im_step_args_t& a, const pulse_im_track_t& tr, int width,
+                   int64_t num_envs, void* stream) {
+  PULSE_REQUIRE(num_envs >= 0, "%s: negative num_envs", who);
   if (num_envs == 0) return PULSE_OK;
-  const pulse_im_step_args_t& a = *args;
-  PULSE_REQUIRE(a.env_count == nullptr || a.env_ids != nullptr, "pulse_im_step: env_count limits an env_ids list");
-  PULSE_REQUIRE((a.flags & PULSE_STEP_ALL) != 0 && (a.flags & ~(PULSE_STEP_ALL | PULSE_STEP_ADVANCE)) == 0, "pulse_im_step: bad flags 0x%x", a.flags);
-  PULSE_REQUIRE(!(a.flags & PULSE_STEP_ADVANCE) || a.progress_rw != nullptr, "pulse_im_step: PULSE_STEP_ADVANCE needs the writable progress_rw");
+  PULSE_REQUIRE(a.env_count == nullptr || a.env_ids != nullptr, "%s: env_count limits an env_ids list", who);
+  PULSE_REQUIRE((a.flags & PULSE_STEP_ALL) != 0 && (a.flags & ~(PULSE_STEP_ALL | PULSE_STEP_ADVANCE)) == 0, "%s: bad flags 0x%x", who, a.flags);
+  PULSE_REQUIRE(!(a.flags & PULSE_STEP_ADVANCE) || a.progress_rw != nullptr, "%s: PULSE_STEP_ADVANCE needs the writable progress_rw", who);
   PULSE_REQUIRE(a.body_state && a.progress_buf && a.motion_ids && a.motion_start_times && a.motion_start_offset &&
-                    a.global_offset, "pulse_im_step: null state/task buffer");
-  PULSE_REQUIRE(a.body_env_stride >= PULSE_NUM_BODIES * PULSE_BODY_STATE_W, "pulse_im_step: body_env_stride %lld < 312",
+                    a.global_offset, "%s: null state/task buffer", who);
+  PULSE_REQUIRE(a.body_env_stride >= PULSE_NUM_BODIES * PULSE_BODY_STATE_W, "%s: body_env_stride %lld < 312", who,
                 (long long)a.body_env_stride);
-  PULSE_REQUIRE((reinterpret_cast<uintptr_t>(a.body_state) & 3u) == 0, "pulse_im_step: body_state not 4-byte aligned");
-  PULSE_REQUIRE(aligned16(lib->d.frame_rec), "pulse_im_step: frame records not 16-byte aligned");
+  PULSE_REQUIRE((reinterpret_cast<uintptr_t>(a.body_state) & 3u) == 0, "%s: body_state not 4-byte aligned", who);
+  PULSE_REQUIRE(aligned16(lib->d.frame_rec), "%s: frame records not 16-byte aligned", who);
   if (a.flags & PULSE_STEP_REWARD) {
-    PULSE_REQUIRE(a.rew_buf != nullptr, "pulse_im_step: rew_buf is null");
+    PULSE_REQUIRE(a.rew_buf != nullptr, "%s: rew_buf is null", who);
     if (a.dof_force) {
-      PULSE_REQUIRE(a.dof_vel != nullptr, "pulse_im_step: dof_force given without dof_vel");
-      PULSE_REQUIRE(!a.reward_raw || a.raw_stride >= 5, "pulse_im_step: raw_stride must be >= 5 with the power term");
+      PULSE_REQUIRE(a.dof_vel != nullptr, "%s: dof_force given without dof_vel", who);
+      PULSE_REQUIRE(!a.reward_raw || a.raw_stride >= 5, "%s: raw_stride must be >= 5 with the power term", who);
     } else {
-      PULSE_REQUIRE(!a.reward_raw || a.raw_stride >= 4, "pulse_im_step: raw_stride must be >= 4");
+      PULSE_REQUIRE(!a.reward_raw || a.raw_stride >= 4, "%s: raw_stride must be >= 4", who);
     }
   }
   if (a.flags & PULSE_STEP_RESET) {
-    PULSE_REQUIRE(a.reset_buf && a.terminate_buf && a.termination_distances, "pulse_im_step: null reset buffer");
-    PULSE_REQUIRE(a.recovery_counter == nullptr || a.progress_rw != nullptr, "pulse_im_step: recovery_counter needs the writable progress_rw");
-    PULSE_REQUIRE((a.reset_body_mask & 0xffffffu) != 0, "pulse_im_step: empty reset_body_mask");
+    PULSE_REQUIRE(a.reset_buf && a.terminate_buf && a.termination_distances, "%s: null reset buffer", who);
+    PULSE_REQUIRE(a.recovery_counter == nullptr || a.progress_rw != nullptr, "%s: recovery_counter needs the writable progress_rw", who);
+    PULSE_REQUIRE((a.reset_body_mask & 0xffffffu) != 0, "%s: empty reset_body_mask", who);
   }
   if (a.flags & PULSE_STEP_OBS) {
-    PULSE_REQUIRE(a.obs_buf != nullptr && a.obs_stride >= PULSE_IM_OBS, "pulse_im_step: obs_buf null or obs_stride < 934");
-    PULSE_REQUIRE((reinterpret_cast<uintptr_t>(a.obs_buf) & 3u) == 0, "pulse_im_step: obs_buf misaligned");
-    PULSE_REQUIRE(!a.ref_dof_pos || lib->d.aux_rec, "pulse_im_step: ref_dof_pos needs the aux records");
+    PULSE_REQUIRE(a.obs_buf != nullptr && a.obs_stride >= width, "%s: obs_buf null or obs_stride < %d", who, width);
+    PULSE_REQUIRE((reinterpret_cast<uintptr_t>(a.obs_buf) & 3u) == 0, "%s: obs_buf misaligned", who);
+    PULSE_REQUIRE(!a.ref_dof_pos || lib->d.aux_rec, "%s: ref_dof_pos needs the aux records", who);
   }
   static bool attr_set = false;
   const size_t smem = sizeof(CtaSmem);
   if (!attr_set) {
-    PULSE_CUDA_OK(cudaFuncSetAttribute(im_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PULSE_CUDA_OK(cudaFuncSetAttribute(im_step_kernel<kTrack>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
   static int max_ctas = 0;
@@ -621,13 +655,45 @@ extern "C" int pulse_im_step(const pulse_motionlib_t* lib, const pulse_im_step_a
     int dev = 0, sms = 0, per_sm = 0;
     PULSE_CUDA_OK(cudaGetDevice(&dev));
     PULSE_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    PULSE_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, im_step_kernel, kThreads, smem));
-    PULSE_REQUIRE(per_sm >= 1, "pulse_im_step: kernel does not fit on this device (smem %zu B)", smem);
+    PULSE_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, im_step_kernel<kTrack>, kThreads, smem));
+    PULSE_REQUIRE(per_sm >= 1, "%s: kernel does not fit on this device (smem %zu B)", who, smem);
     max_ctas = sms * per_sm;  // persistent: one resident wave
   }
   const long long ngroups = (num_envs + kEnvs - 1) / kEnvs;
   const unsigned grid = static_cast<unsigned>(ngroups < max_ctas ? ngroups : max_ctas);
-  im_step_kernel<<<grid, kThreads, smem, static_cast<cudaStream_t>(stream)>>>(lib->d, a, (long long)num_envs);
+  im_step_kernel<kTrack><<<grid, kThreads, smem, static_cast<cudaStream_t>(stream)>>>(lib->d, a, (long long)num_envs, tr);
   PULSE_LAUNCH_OK("im_step_kernel");
   return PULSE_OK;
+}
+
+}  // namespace
+}  // namespace pulse
+
+extern "C" int pulse_im_step(const pulse_motionlib_t* lib, const pulse_im_step_args_t* args, int64_t num_envs,
+                             void* stream) {
+  using namespace pulse;
+  PULSE_REQUIRE(lib != nullptr && args != nullptr, "pulse_im_step: null lib/args");
+  return im_step_launch<false>("pulse_im_step", lib, *args, pulse_im_track_t{}, kObs, num_envs, stream);
+}
+
+extern "C" int pulse_im_track_step(const pulse_motionlib_t* lib, const pulse_im_step_args_t* args, const pulse_im_track_t* track,
+                                   int64_t num_envs, void* stream) {
+  using namespace pulse;
+  const char* who = "pulse_im_track_step";
+  PULSE_REQUIRE(lib != nullptr && args != nullptr, "%s: null lib/args", who);
+  PULSE_REQUIRE(track != nullptr, "%s: null track", who);
+  const pulse_im_track_t& tr = *track;
+  PULSE_REQUIRE(tr.num_track >= 1 && tr.num_track <= kNB, "%s: num_track %d outside [1, 24]", who, tr.num_track);
+  PULSE_REQUIRE(tr.version == 6 || tr.version == 7, "%s: version %d (the tracked row is built for 6 and 7)", who, tr.version);
+  unsigned seen = 0u;
+  for (int j = 0; j < kNB; ++j) {
+    const int r = tr.rank[j];
+    if (r < 0) continue;
+    PULSE_REQUIRE(r < tr.num_track && !((seen >> r) & 1u), "%s: rank is not a permutation of 0..num_track-1 (body %d has rank %d)", who, j, r);
+    seen |= 1u << r;
+  }
+  PULSE_REQUIRE(__builtin_popcount(seen) == tr.num_track, "%s: rank is not a permutation of 0..num_track-1 (%d of %d ranks given)", who,
+                __builtin_popcount(seen), tr.num_track);
+  const int width = PULSE_SELF_OBS + (tr.version == 6 ? 24 : 9) * tr.num_track;
+  return im_step_launch<true>(who, lib, *args, tr, width, num_envs, stream);
 }

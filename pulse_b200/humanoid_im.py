@@ -44,6 +44,19 @@ class ImConfig:
     max_episode_length: int = 300
     use_mean_reset: bool = False     # flags.im_eval and not strict_eval
     num_amp_obs_steps: int = 10
+    track_body_ids: Optional[Sequence[int]] = None   # _track_bodies_id: None = all 24 bodies, the 934-float row
+    obs_version: int = 6             # obs_v of the tracked row: 6 or 7 (humanoid_im.py:1328-1413)
+
+
+TRACK_BLOCKS = {6: ((0, 3), (72, 6), (216, 3), (288, 3), (360, 3), (432, 6)), 7: ((0, 3), (216, 3), (360, 3))}   # (offset, width) in v6
+
+
+def track_columns(version: int, track_ids: Sequence[int]) -> torch.Tensor:
+    """Column of the full-body v6 task block (576 floats) behind each column of the tracked task block: v6 and v7 of a body subset are
+    column selections of the full v6 pieces, block-major over the bodies in `track_ids` order."""
+    if int(version) not in TRACK_BLOCKS:
+        raise _lib.PulseError(f"tracked observation version {version}: have 6 and 7")
+    return torch.tensor([off + w * int(j) + c for off, w in TRACK_BLOCKS[int(version)] for j in track_ids for c in range(w)], dtype=torch.int64)
 
 
 def _strided(t: torch.Tensor, inner: int):
@@ -63,6 +76,40 @@ class HumanoidImCompute:
         self.reset_body_mask = 0
         for j in self.cfg.reset_body_ids:
             self.reset_body_mask |= 1 << int(j)
+        self.track = None
+        ids = self.cfg.track_body_ids
+        if ids is not None:
+            ids = [int(j) for j in ids]
+            if not ids or len(set(ids)) != len(ids) or not all(0 <= j < NUM_BODIES for j in ids):
+                raise _lib.PulseError(f"track_body_ids must be distinct body ids in [0, {NUM_BODIES}), got {ids}")
+            if int(self.cfg.obs_version) not in TRACK_BLOCKS:
+                raise _lib.PulseError(f"tracked observation version {self.cfg.obs_version}: have 6 and 7")
+            self.track = _lib.ImTrack(num_track=len(ids), version=int(self.cfg.obs_version))
+            for j in range(NUM_BODIES):
+                self.track.rank[j] = ids.index(j) if j in ids else -1
+
+    @classmethod
+    def from_task(cls, task, **cfg) -> "HumanoidImCompute":
+        """The compute of a live HumanoidIm task: its MotionLib (packed once), step dt, reward, reset and AMP settings and termination
+        distances; `cfg` sets further ImConfig fields (the tracked observation)."""
+        ml = task._motion_lib
+        motion_lib = ml if isinstance(ml, MotionLibB200) else MotionLibB200.from_reference(ml, device=task.device)
+        c = ImConfig(
+            dt=float(torch.tensor(task.dt, dtype=torch.float32)), reward_specs={k: float(v) for k, v in task.reward_specs.items()},
+            power_reward=bool(task.power_reward), power_coefficient=float(task.power_coefficient),
+            reset_body_ids=tuple(int(i) for i in task._reset_bodies_id.tolist()),
+            enable_early_termination=bool(task._enable_early_termination), cycle_motion=bool(task.cycle_motion),
+            max_episode_length=int(task.max_episode_length), num_amp_obs_steps=int(getattr(task, "_num_amp_obs_steps", 10)), **cfg)
+        comp = cls(motion_lib, c)
+        comp.termination_distances = task._termination_distances.reshape(-1)[:NUM_BODIES].to(task.device, torch.float32).contiguous()
+        return comp
+
+    @property
+    def obs_size(self) -> int:
+        """Floats of the observation row `step` writes: 934, or 358 + 24 K (v6) / 358 + 9 K (v7) for K tracked bodies."""
+        if self.track is None:
+            return IM_OBS
+        return SELF_OBS + sum(w for _, w in TRACK_BLOCKS[self.track.version]) * self.track.num_track
 
     # ------------------------------------------------------------------------------------------
     def step(self, *, body_state: torch.Tensor, progress_buf: torch.Tensor, motion_ids: torch.Tensor,
@@ -77,7 +124,8 @@ class HumanoidImCompute:
              env_count: Optional[torch.Tensor] = None, recovery_counter: Optional[torch.Tensor] = None,
              fdones_out: Optional[torch.Tensor] = None, advance: bool = False) -> None:
         """One fused launch.  `body_state` is the [N, bodies_per_env, 13] rigid-body-state view (or its
-        [:, :24] slice); `dof_vel` may be the strided Isaac Gym view dof_state[..., 1]."""
+        [:, :24] slice); `dof_vel` may be the strided Isaac Gym view dof_state[..., 1].  With `track_body_ids` configured the
+        observation row is the tracked one (`obs_size` floats, `pulse_im_track_step`); reward and reset stay full-body."""
         c = self.cfg
         a = _lib.ImStepArgs()
         if body_state.dim() != 3 or body_state.shape[-1] != 13 or body_state.stride(-1) != 1 or body_state.stride(1) != 13:
@@ -114,8 +162,8 @@ class HumanoidImCompute:
         a.enable_early_termination = int(c.enable_early_termination)
         a.use_mean_reset = int(c.use_mean_reset)
         if flags & _lib.STEP_OBS:
-            if obs_buf is None or obs_buf.dtype != torch.float32 or obs_buf.stride(-1) != 1 or obs_buf.shape[-1] < IM_OBS:
-                raise _lib.PulseError("obs_buf must be float32 [N, >=934] with contiguous rows")
+            if obs_buf is None or obs_buf.dtype != torch.float32 or obs_buf.stride(-1) != 1 or obs_buf.shape[-1] < self.obs_size:
+                raise _lib.PulseError(f"obs_buf must be float32 [N, >={self.obs_size}] with contiguous rows")
             a.obs_buf, a.obs_stride = obs_buf.data_ptr(), obs_buf.stride(0)
             if self_obs_buf is not None:
                 a.self_obs_buf = self_obs_buf.data_ptr()
@@ -157,7 +205,11 @@ class HumanoidImCompute:
             a.flags = flags | _lib.STEP_ADVANCE
             a.progress_rw = progress_buf.data_ptr()
         with torch.cuda.device(self.device):
-            _lib.check(self.lib.pulse_im_step(self.motion_lib.handle, C.byref(a), n, _lib.current_stream(self.device)), "pulse_im_step")
+            if self.track is None:
+                _lib.check(self.lib.pulse_im_step(self.motion_lib.handle, C.byref(a), n, _lib.current_stream(self.device)), "pulse_im_step")
+            else:
+                _lib.check(self.lib.pulse_im_track_step(self.motion_lib.handle, C.byref(a), C.byref(self.track), n, _lib.current_stream(self.device)),
+                           "pulse_im_track_step")
 
     # ------------------------------------------------------------------------------------------
     def amp_obs(self, *, body_state: torch.Tensor, dof_pos: torch.Tensor, dof_vel: torch.Tensor, amp_obs_buf: torch.Tensor,
@@ -483,16 +535,8 @@ class HumanoidImB200Mixin:
     _pulse_ready = False
 
     def _pulse_setup(self):
-        ml = self._motion_lib
-        self._pulse_motion_lib = ml if isinstance(ml, MotionLibB200) else MotionLibB200.from_reference(ml, device=self.device)
-        cfg = ImConfig(
-            dt=float(torch.tensor(self.dt, dtype=torch.float32)), reward_specs={k: float(v) for k, v in self.reward_specs.items()},
-            power_reward=bool(self.power_reward), power_coefficient=float(self.power_coefficient),
-            reset_body_ids=tuple(int(i) for i in self._reset_bodies_id.tolist()),
-            enable_early_termination=bool(self._enable_early_termination), cycle_motion=bool(self.cycle_motion),
-            max_episode_length=int(self.max_episode_length), num_amp_obs_steps=int(getattr(self, "_num_amp_obs_steps", 10)))
-        self._pulse = HumanoidImCompute(self._pulse_motion_lib, cfg)
-        self._pulse.termination_distances = self._termination_distances.reshape(-1)[:NUM_BODIES].to(self.device, torch.float32).contiguous()
+        self._pulse = HumanoidImCompute.from_task(self)
+        self._pulse_motion_lib = self._pulse.motion_lib
         self._pulse_fused_pending = False
         self._pulse_pass_time = torch.zeros(self.num_envs, dtype=torch.uint8, device=self.device)
         unsupported = (getattr(self, "self_obs_v", 1) != 1 or getattr(self, "zero_out_far", False) or getattr(self, "_occl_training", False)
