@@ -93,7 +93,7 @@ class ImZStepsB200(LatentStepsB200):
     Out of scope: the discriminator (pulse_z_vr.yaml still trains it with disc_coef 5 although disc_reward_w is 0; leaving it out does
     not change the reward, but it removes the discriminator's gradients from the shared gradient-norm clip, so the reset is called
     without an AMP buffer); the fut_tracks windows, observation versions 1/2/3/8/9, non-upright starts, zero_out_far and occlusion;
-    multi-GPU; the smplx humanoid; an agent mixin (INTEGRATION.md wires the hooks); the IMAmpAgent evaluation loop."""
+    multi-GPU; the smplx humanoid; an agent mixin (INTEGRATION.md wires the hooks).  The IMAmpAgent evaluation pass is `evaluate`."""
 
     def __init__(self, comp: HumanoidImCompute, policy, vae, sim: dict, horizon: int = 32, pd_offset: Optional[torch.Tensor] = None,
                  pd_scale: Optional[torch.Tensor] = None, pd_freeze: Optional[torch.Tensor] = None, use_graphs: bool = True,
@@ -143,3 +143,12 @@ class ImZStepsB200(LatentStepsB200):
         self.comp.step(flags=_lib.STEP_OBS, obs_buf=self.obs_carry, **self._state())
         self.reset_buf.zero_()
         self.terminate_buf.zero_()
+
+    def evaluate(self, dataset, physics=None, auto_pmcp: bool = False, auto_pmcp_soft: bool = False, **kw):
+        """`IMAmpAgent.eval` (im_amp.py:136-242) of this policy over every clip of `dataset` (a MotionDatasetB200) on this driver's
+        simulator tensors, then every env reset into training and the optional PMCP update: `evaluation.EvalStepsB200` (`kw`: its
+        poll_every / use_graphs / strict_eval / eval_body_ids).  The pass is `self.eval_steps` while it runs: `physics(t)` applies
+        its `pd_tar` and may read its task-side state (`progress_buf`, `motion_start_times`, ...)."""
+        from .evaluation import EvalStepsB200
+        self.eval_steps = EvalStepsB200(self, physics=physics, **kw)
+        return self.eval_steps.run(dataset, auto_pmcp=auto_pmcp, auto_pmcp_soft=auto_pmcp_soft)

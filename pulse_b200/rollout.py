@@ -287,6 +287,15 @@ class PlayStepsB200(GraphRunner):
         """Live durations of the fused step kernel launches of the LAST horizon (graph-safe events)."""
         return [a.elapsed_ms(b) for a, b in self.step_events] if self.step_events is not None else []
 
+    def evaluate(self, dataset, physics=None, auto_pmcp: bool = False, auto_pmcp_soft: bool = False, **kw):
+        """`IMAmpAgent.eval` (im_amp.py:136-242) of this policy over every clip of `dataset` (a MotionDatasetB200) on this driver's
+        simulator tensors, then every env reset into training and the optional PMCP update: `evaluation.EvalStepsB200` (`kw`: its
+        poll_every / use_graphs / strict_eval / eval_body_ids).  The pass is `self.eval_steps` while it runs: `physics(t)` applies
+        its `pd_tar` and may read its task-side state (`progress_buf`, `motion_start_times`, ...)."""
+        from .evaluation import EvalStepsB200
+        self.eval_steps = EvalStepsB200(self, physics=physics, **kw)
+        return self.eval_steps.run(dataset, auto_pmcp=auto_pmcp, auto_pmcp_soft=auto_pmcp_soft)
+
     # ------------------------------------------------------------------ after the horizon
     def finish(self) -> None:
         """Discriminator rewards over the whole horizon (amp_agent.py:422-424, :1027-1041), `_combine_rewards` (:1011-1025), GAE +
