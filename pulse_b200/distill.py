@@ -190,6 +190,17 @@ class DistillStepsB200(GraphRunner):
         self.reset_buf.zero_()
         self.terminate_buf.zero_()
 
+    def evaluate(self, dataset, physics=None, auto_pmcp: bool = False, auto_pmcp_soft: bool = False, **kw):
+        """`IMAmpAgent.eval` (im_amp.py:136-242) of the student over every clip of `dataset` (a MotionDatasetB200) on this driver's
+        simulator tensors: z = the posterior mean, the decoder's action, no teacher.  Then every env is reset into training through
+        the getup reset (training probabilities; recovery episodes on the envs the pass's last step terminated) and the optional PMCP
+        update (env_im_vae.yaml: auto_pmcp_soft): `evaluation.EvalStepsB200` (`kw`: its poll_every / use_graphs / strict_eval /
+        eval_body_ids).  The pass is `self.eval_steps` while it runs: `physics(t)` applies its `pd_tar` and may read its task-side
+        state (`progress_buf`, `motion_start_times`, ...)."""
+        from .evaluation import EvalStepsB200
+        self.eval_steps = EvalStepsB200(self, physics=physics, **kw)
+        return self.eval_steps.run(dataset, auto_pmcp=auto_pmcp, auto_pmcp_soft=auto_pmcp_soft)
+
     # ------------------------------------------------------------------ update
     def _update_mb(self, i: int, minibatch: int, update_obs_rms: bool) -> None:
         r0, r1 = i * minibatch, (i + 1) * minibatch

@@ -14,9 +14,9 @@ Host-side mirror of `IMAmpAgent.eval` / `_post_step_eval` (phc/learning/im_amp.p
 
 `EvalMetricsB200` is the device state of one chunk; `EvalLoopB200` drives chunks through caller-supplied callbacks (reset, step,
 load chunk), so it runs in front of Isaac Gym, of the stand-in task of the tests, or of a synthetic simulator.  `EvalStepsB200` is the
-pass of a training driver (`PlayStepsB200`: HumanoidIm, `ImZStepsB200`: the VR task): its policy acts deterministically on the
-simulator tensors of the driver through the existing kernels, chunk after chunk of a `MotionDatasetB200`, with `EvalLoopB200` as the
-chunk loop.  `eval_config` / `eval_settings` are the settings of the pass (im_amp.py:160-182) on a step configuration / on a live task.
+pass of a training driver (`PlayStepsB200`: HumanoidIm, `ImZStepsB200`: the VR task, `DistillStepsB200`: the PULSE student of
+HumanoidImDistillGetup): its policy acts deterministically on the simulator tensors of the driver through the existing kernels,
+chunk after chunk of a `MotionDatasetB200`, with `EvalLoopB200` as the chunk loop.  `eval_config` / `eval_settings` are the settings of the pass (im_amp.py:160-182) on a step configuration / on a live task.
 """
 import contextlib
 import dataclasses
@@ -234,10 +234,27 @@ def update_training_data(motion_dataset, failed_keys, auto_pmcp: bool = False, a
         motion_dataset.update_soft_sampling_weight(list(failed_keys))
 
 
+def driver_kind(driver) -> str:
+    """The policy an `EvalStepsB200` pass runs for `driver`: "im" (PlayStepsB200, the actor's mean), "vr" (ImZStepsB200, the latent
+    policy's mean through the frozen prior and decoder) or "distill" (DistillStepsB200, the VAE student at its posterior mean)."""
+    from .distill import DistillStepsB200
+    from .imz_rollout import ImZStepsB200
+    from .rollout import PlayStepsB200
+    if isinstance(driver, ImZStepsB200):
+        return "vr"
+    if isinstance(driver, PlayStepsB200):
+        return "im"
+    if isinstance(driver, DistillStepsB200):
+        return "distill"
+    raise _lib.PulseError(f"EvalStepsB200 evaluates PlayStepsB200 and ImZStepsB200 (the imitation and VR policies) and DistillStepsB200 "
+                          f"(the distillation student), not {type(driver).__name__}")
+
+
 class EvalStepsB200(GraphRunner):
     """One `IMAmpAgent.eval` pass (im_amp.py:136-242) of a training driver's policy over all `num_unique` clips of a `MotionDatasetB200`,
-    on the driver's simulator tensors and step configuration: `PlayStepsB200` (HumanoidIm, im.yaml) or `ImZStepsB200` (HumanoidImZ,
-    pulse_z_vr.yaml).  `EvalLoopB200` is the chunk loop; this class supplies its callbacks:
+    on the driver's simulator tensors and step configuration: `PlayStepsB200` (HumanoidIm, im.yaml), `ImZStepsB200` (HumanoidImZ,
+    pulse_z_vr.yaml) or `DistillStepsB200` (HumanoidImDistillGetup, env_im_vae.yaml + im_z_fit.yaml: the VAE student).  `EvalLoopB200`
+    is the chunk loop; this class supplies its callbacks:
         load_chunk(start_idx)  `dataset.load_motions(N, random_sample=False, start_idx, eval_mode=True)`: clips (start_idx + e) % U, no
                                heading draw; a new MotionLibB200 and a new step compute over it with `eval_config`'s settings;
         reset_all()            every env at motion time 0 (`flags.test`): `pulse_reset_ref_state` with the start-time phase injected as 0,
@@ -246,6 +263,8 @@ class EvalStepsB200(GraphRunner):
                                  1. the reset of the envs done at the previous step (again at motion time 0, im_amp.py:202);
                                  2. the deterministic action: HumanoidIm: the actor's mu on the normalised observation, `pulse_pd_targets`;
                                     VR task: z = prior_mu + mu (`pulse_latent_post` with zero noise), the frozen decoder, `pulse_pd_targets`;
+                                    student: `eval_actor(use_mean=True)` -- z = vae_mu (amp_network_z_builder.py:94-95), the decoder --
+                                    and `pulse_pd_targets`; the teacher is not run (humanoid_im_distill.py:152, flags.test);
                                  3. the `physics(t)` hook (it applies `pd_tar`);
                                  4. the fused step (`pulse_im_step` / `pulse_im_track_step`, STEP_ALL | STEP_ADVANCE) with the eval settings;
                                  5. `body_pos_gt` = MotionLibB200's query at progress * dt + start + offset after the step, the time the
@@ -259,19 +278,19 @@ class EvalStepsB200(GraphRunner):
     PD targets) and shares only the simulator tensors and the policy's evaluation workspaces with the driver.  No running statistic
     moves (the observation normaliser is read in evaluation mode; no value, AMP or optimiser state is touched) and the driver's graphs,
     buffers and MotionLib stay as they are.  Afterwards every env is reset into training through the driver's reset (im_amp.py:234)
-    and the training observation is written to the driver's `obs_carry`."""
+    and the training observation is written to the driver's `obs_carry`.
+    The student's pass needs no getup state of its own: at the pass's getup probabilities 0 (im_amp.py:167-172) every reset is a
+    reference-state episode that zeroes the recovery counter, so the recovery masking never fires and the pass is the HumanoidIm
+    pass; the driver's getup tensors (recovery counter, fall pool and its assignments) are not touched.  Its reset into training
+    is the getup reset with the training probabilities, after the pass's last terminate flags are copied into the driver's
+    `terminate_buf`: the recovery episodes fall on the envs the pass terminated."""
 
     def __init__(self, driver, physics: Optional[Callable[[int], None]] = None, poll_every: int = 8, use_graphs: bool = True,
                  strict_eval: bool = False, eval_body_ids: Sequence[int] = ALL_BODIES):
-        from .imz_rollout import ImZStepsB200
-        from .rollout import PlayStepsB200
-        if isinstance(driver, ImZStepsB200):
-            self.vr = True
-        elif isinstance(driver, PlayStepsB200):
-            self.vr = False
-        else:
-            raise _lib.PulseError(f"EvalStepsB200 evaluates PlayStepsB200 and ImZStepsB200, not {type(driver).__name__}")
-        self.driver, self.policy, self.sim = driver, driver.policy, driver.sim
+        self.kind = driver_kind(driver)
+        self.vr = self.kind == "vr"
+        self.driver, self.sim = driver, driver.sim
+        self.policy = driver.vae if self.kind == "distill" else driver.policy
         self.dev, n = driver.dev, int(driver.n)
         self.n = n
         self.cfg = eval_config(driver.comp.cfg, strict_eval, eval_body_ids)
@@ -288,7 +307,8 @@ class EvalStepsB200(GraphRunner):
         self.obs, self.rew = z(n, driver.comp.obs_size), z(n)
         A = driver.pd[0].shape[0]
         self.pd_tar = z(n, A)
-        self.mus = z(n, self.policy.A)
+        if self.kind != "distill":                                               # the student's mu is a view of its decoder's workspace
+            self.mus = z(n, self.policy.A)
         if self.vr:                                                              # pulse_latent_post's operands: zero noise, unused value
             E = self.policy.A
             self.eps, self.actions, self.neglogp = z(n, E), z(n, E), z(n)
@@ -319,6 +339,9 @@ class EvalStepsB200(GraphRunner):
         """get_action(obs, is_determenistic=True) (im_amp.py:44-75) and the PD targets of pre_physics_step."""
         from .vae import pd_targets
         pol, d = self.policy, self.driver
+        if self.kind == "distill":                                              # z = vae_mu (Z_MEAN), decoder; no teacher (flags.test)
+            pd_targets(pol.eval_actor(self.obs, use_mean=True)["mus"], d.pd[0], d.pd[1], out=self.pd_tar, freeze=d.pd_freeze)
+            return
         if not self.vr:
             pol.heads_into(self.obs, mus=self.mus, with_value=False)
             pd_targets(self.mus, d.pd[0], d.pd[1], out=self.pd_tar)
@@ -393,6 +416,17 @@ class EvalStepsB200(GraphRunner):
                 d.refresh(0, d.reset_ws)
             ws = d.reset_ws
             d.comp.step(flags=_lib.STEP_OBS, obs_buf=d.obs_carry, env_ids=ws["env_list"], env_count=ws["count"], **d._state())
+        elif self.kind == "distill":
+            # the getup reset with the training probabilities: recovery episodes fall on the envs the pass's last step terminated
+            # (`_reset_actors` reads `_terminate_buf`, humanoid_im_getup.py:135-162) and keep the state the pass left them in
+            d.terminate_buf.copy_(self.terminate_buf)
+            d._reset(0)
+            if d.refresh is not None:
+                d.refresh(0, d.reset_ws)
+            ws = d.reset_ws
+            d.comp.step(body_state=s["body_state"], progress_buf=s["progress_buf"], motion_ids=s["motion_ids"], motion_start_times=s["motion_start_times"],
+                        motion_start_offset=s["motion_start_offset"], global_offset=s["global_offset"], obs_buf=d.obs_carry,
+                        env_ids=ws["env_list"][:d.n], env_count=ws["count"], flags=_lib.STEP_OBS)
         else:
             d.comp.reset_envs(motion_ids=s["motion_ids"], motion_start_times=s["motion_start_times"], motion_start_offset=s["motion_start_offset"],
                               global_offset=s["global_offset"], progress_buf=s["progress_buf"], root_states=s["root_states"], dof_pos=s["dof_pos"],
@@ -400,7 +434,7 @@ class EvalStepsB200(GraphRunner):
                               cycle_counter=s.get("cycle_counter"), contact_forces=s.get("contact_forces"), amp_obs_buf=d.amp_init,
                               actor_ids=s.get("actor_ids"), seed=d.reset_seed, offset=0, offset_dev=d.policy.rng_offset, obs_buf=d.obs_carry,
                               amp_fresh=d.amp_fresh)
-        self.policy.advance_rng(1)                             # the start-time draws above used block `rng_offset + 0`
+        self.policy.advance_rng(1)                             # the reset's draws above used block `rng_offset + 0`
 
     # ------------------------------------------------------------------ the pass
     def run(self, dataset, auto_pmcp: bool = False, auto_pmcp_soft: bool = False) -> Dict:
