@@ -5,11 +5,10 @@ import math
 
 import torch
 
-from tests.fp64_ref import (U32, UBF, Gemm, adam_ref, check, check_exact, check_mask, disc_loss_ref, f64, normalize_ref, ppo_loss_ref,
+from tests.fp64_ref import (U32, U64, UBF, Gemm, adam_ref, check, check_exact, check_mask, disc_loss_ref, f64, normalize_ref, ppo_loss_ref,
                             silu64, silu_gated, silu_gemm_tol, silu_tol, sum_tol, unpack_mask)
 
 BF = torch.bfloat16
-U64 = 2.0 ** -53     # fp64 unit round-off
 
 
 def _sync(t):
@@ -130,17 +129,20 @@ def check_grads(rep, name, mlp, wgrad, bgrad, extra=None):
             check(rep, f"{name} L{i} db (column sums)", l.bias_grad, *bgrad[i])
 
 
-def check_mlp_eval(rep, name, mlp, snap, x, M, top_out=None):
-    """Forward links of one MLP from its evaluation workspace (no pre-activation stored: a SiLU is applied to the fp32 accumulator,
-    fp64_ref.silu_gemm_tol).  Headless nets: the top activation is read from `top_out` when given."""
-    ws, L = mlp._ws[(M, False)], mlp.layers
+def check_mlp_eval(rep, name, mlp, snap, x, M, top_out=None, slot=0):
+    """Forward links of one MLP from its evaluation workspace `slot` (no pre-activation stored: a SiLU is applied to the fp32 accumulator,
+    fp64_ref.silu_gemm_tol).  The top output is read from `top_out` when given: the activation window of a headless net, or the fp32
+    head a headed net wrote through forward(out=) (an experience slice, any row stride).  A head1 top layer (pulse_head1_forward, the
+    GEMV of a single-output head on a ReLU layer) is a Gemm over its bf16 input and weight row -- with a bias-augmented net the input's
+    ones column times the bias column, otherwise one fp32 bias add."""
+    ws, L = mlp._ws[(M, False) if slot == 0 else (M, False, slot)], mlp.layers
     h = x
     for i, l in enumerate(L):
         g = Gemm(h[:M, :l.Kp], _w(snap, mlp.flat, l).T, bias=None if mlp.aug else _b(snap, mlp.flat, l))
         if i == len(L) - 1 and not mlp.headless:
-            if mlp._head1(i):
-                raise NotImplementedError("the head1 GEMV's eval output is not checked here")
-            g.check(rep, f"{name} L{i} eval head (fp32)", ws["out"][:M])
+            out = ws["out"] if top_out is None else top_out
+            where = ", in the slice" if top_out is not None else ""
+            g.check(rep, f"{name} L{i} eval head (fp32{', head1 GEMV' if mlp._head1(i) else ''}{where})", out[:M, :l.N])
             break
         window = i == len(L) - 1 and top_out is not None
         act = top_out if window else ws["act"][i]
@@ -219,8 +221,8 @@ def rms_f32(mean, var, count, batches):
     return mean.float(), 1.0 / torch.sqrt(var.float() + 1e-5)
 
 
-def _check_normalized(rep, link, out, x, mean32, rstd32, cols, one_col, slack=0.0):
-    y, tol = normalize_ref(x, mean32, rstd32)
+def _check_normalized(rep, link, out, x, mean32, rstd32, cols, one_col, slack=0.0, clamp=5.0):
+    y, tol = normalize_ref(x, mean32, rstd32, clamp)
     check(rep, link, out[:, :cols], y, tol + slack * y.abs())
     _check_pads(rep, link, out, one_col + 1 if one_col is not None else cols, one_col)
 

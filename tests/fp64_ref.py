@@ -23,6 +23,7 @@ import torch
 
 U32 = 2.0 ** -24     # fp32 unit round-off
 UBF = 2.0 ** -8      # bf16 unit round-off
+U64 = 2.0 ** -53     # fp64 unit round-off
 C_GEMM = 4.0
 AMBIGUOUS_MAX = 1e-3
 
@@ -100,6 +101,28 @@ def check_exact(rep: Optional[Report], link: str, got: torch.Tensor, ref: torch.
 
 
 # ---------------------------------------------------------------------------------------------------------------------- GEMM links
+def kernel_gemm(a, b, kblock=64, skip=None, dup_slice=None, slices=1):
+    """CPU simulation of the GEMM kernels for the self-tests: fp32 accumulation of bf16 a [M, K] . b [K, N] block by block (each block
+    product in fp32).  skip = (k-block, column slice): that k-block is left out of those columns.  slices / dup_slice: the reduction split
+    into `slices` contiguous slices summed in order, slice `dup_slice` added twice."""
+    a32, b32 = a.float(), b.float()
+    K = a.shape[1]
+    per = -(-K // slices)
+    out = torch.zeros(a.shape[0], b.shape[1])
+    for s in range(slices):
+        part = torch.zeros_like(out)
+        for k0 in range(s * per, min(K, (s + 1) * per), kblock):
+            k1 = min(k0 + kblock, (s + 1) * per, K)
+            blk = a32[:, k0:k1] @ b32[k0:k1]
+            if skip is not None and skip[0] == k0 // kblock:
+                blk[:, skip[1]] = 0.0
+            part += blk
+        out += part
+        if s == dup_slice:
+            out += part
+    return out
+
+
 class Gemm:
     """y64 = alpha * (A . B) [* gate] in float64 with its accumulation bound `acc` (before any output rounding)."""
 
@@ -179,10 +202,12 @@ def sum_tol(terms_abs_sum: torch.Tensor, n: int, c: float = C_GEMM) -> torch.Ten
 
 
 # ---------------------------------------------------------------------------------------------------------------- element-wise links
-def normalize_ref(x: torch.Tensor, mean: torch.Tensor, rstd: torch.Tensor):
-    """clamp((x - mean) * rstd, +-5) -> bf16: two fp32 roundings then one bf16 rounding."""
+def normalize_ref(x: torch.Tensor, mean: torch.Tensor, rstd: torch.Tensor, clamp: Optional[float] = 5.0):
+    """clamp((x - mean) * rstd, +-clamp) -> bf16 (clamp None: unclamped): two fp32 roundings then one bf16 rounding."""
     x, m, r = f64(x), f64(mean), f64(rstd)
-    y = torch.clamp((x - m) * r, -5.0, 5.0)
+    y = (x - m) * r
+    if clamp is not None:
+        y = torch.clamp(y, -clamp, clamp)
     tol = UBF * y.abs() + 3 * U32 * (x.abs() + m.abs()) * r.abs() * (1 + UBF)
     return y, tol
 
@@ -257,6 +282,201 @@ def gaussian_sample_ref(mu: torch.Tensor, eps: torch.Tensor, logstd: torch.Tenso
     tol_n = (0.5 * (2 * eps.abs() * dz + dz * dz + U32 * z2).sum(-1) + 0.5 * A * U32 * z2.sum(-1) + A * U32 * ls.abs().sum()
              + abs(c32 - 0.5 * math.log(2 * math.pi) * A) + 2 * U32 * c32 + 2 * U32 * (nlp.abs() + c32 + ls.abs().sum()))
     return a, tol_a, nlp, tol_n
+
+
+def value_unnorm_ref(y: torch.Tensor, mean: torch.Tensor, var: torch.Tensor, eps: float, terminate: Optional[torch.Tensor] = None):
+    """value_unnorm.cuh on the kernel's own normalised value y: clamp(y, +-5) * sqrt(var.float() + eps) + mean.float() [* (1 - terminate)],
+    float64.  fp32: the add under the root, the root (half the relative error of its argument, plus its own rounding), the product and
+    the sum -- one u32 each; the terminate factor is exactly 0 or 1."""
+    c = torch.clamp(f64(y), -5.0, 5.0)
+    m = float(mean.reshape(-1)[0].float())
+    sd = math.sqrt(float(var.reshape(-1)[0].float()) + f32r(eps))
+    v = c * sd + m
+    tol = 3 * U32 * (c * sd).abs() + U32 * v.abs()
+    if terminate is not None:
+        keep = 1.0 - f64(terminate)
+        v, tol = v * keep, tol * keep
+    return v, tol
+
+
+def pd_targets_exact(actions: torch.Tensor, offset: torch.Tensor, scale: torch.Tensor, freeze: Optional[torch.Tensor] = None):
+    """Humanoid._action_to_pd_targets as the kernels round it: fp32(offset + fp32(scale * a)), two separate roundings -- exact, so the
+    kernel's targets must match bit for bit (frozen dofs: exactly 0)."""
+    t = offset.float()[None, :] + scale.float()[None, :] * actions.float()
+    if freeze is not None:
+        t = torch.where(freeze.bool()[None, :], torch.zeros_like(t), t)
+    return t
+
+
+def policy_post_ref(mu, eps, logstd, eps_tol=None, value=None, value_mean=None, value_var=None, value_eps=1e-5):
+    """policy_post_kernel on the kernel's own head output mu: actions and neglogp through gaussian_sample_ref (same fp32 operations),
+    the de-normalised value (value_unnorm_ref).  eps_tol: the draws are the fp64 regeneration of the kernel's Philox noise
+    (philox_normals_ref), off by at most eps_tol -- it widens the action bound by sigma * eps_tol and neglogp's by sum (|eps| + eps_tol/2)
+    eps_tol.  The PD targets are exact: pd_targets_exact on the kernel's actions.  Returns {name: (value, tol)} in float64."""
+    a, tol_a, nlp, tol_n = gaussian_sample_ref(mu, eps, logstd)
+    if eps_tol is not None:
+        et = f64(eps_tol)
+        tol_a = tol_a + torch.exp(f64(logstd)) * et
+        tol_n = tol_n + ((f64(eps).abs() + 0.5 * et) * et).sum(-1)
+    out = {"actions": (a, tol_a), "neglogp": (nlp, tol_n)}
+    if value is not None:
+        out["values"] = value_unnorm_ref(value, value_mean, value_var, value_eps) if value_mean is not None else (f64(value), torch.zeros_like(f64(value)))
+    return out
+
+
+def latent_post_ref(mu, eps, logstd, prior_mu, actions, eps_tol=None, value=None, value_mean=None, value_var=None, value_eps=1e-5):
+    """latent_post_kernel on the kernel's own head mu and prior mean: policy_post_ref's actions, neglogp and value (the same draws and
+    arithmetic), and the decoder's latent z = bf16(fp32(prior_mu + a)) from the kernel's own actions -- two correctly rounded
+    operations, so "z" is exact (bf16)."""
+    out = policy_post_ref(mu, eps, logstd, eps_tol=eps_tol, value=value, value_mean=value_mean, value_var=value_var, value_eps=value_eps)
+    out["z"] = (prior_mu.float() + actions.float()).to(torch.bfloat16)
+    return out
+
+
+def philox_normals_ref(seed: int, index, offset):
+    """Box-Muller (philox.cuh) in float64 on the Philox4x32-10 blocks (seed, index, offset) regenerated on the host: returns
+    (n0, n1, tol0, tol1), the normals of words x / y, float64 tensors of index's shape.
+
+    The kernel forms u1 = (x >> 8 + 1) 2^-24 and u2 = (y >> 8) 2^-24 exactly, then r = sqrtf(-2 __logf(u1)) and __sincosf(2 pi_f32 u2).
+    __logf is lg2.approx.f32 times ln 2 (one fp32 multiply).  The error figures below are the ones the CUDA C++ programming guide gives
+    for __logf and __sinf / __cosf (2^-21.41 absolute on [0.5, 2], 3 ulp elsewhere; 2^-21.41 absolute on [-pi, pi]) and the PTX ISA
+    manual for lg2.approx.f32 and sin.approx / cos.approx.f32; the looser figure is used wherever the two differ.  The logarithm:
+    E_log = max(2^-21.41, 3 ulp of |ln u1|) plus the multiply by ln 2; r then carries sqrt(r^2 + 2 E_log) - r (finite as r -> 0,
+    where u1 -> 1) plus the rounding of the root.  The sine and cosine: 2^-20.5 over [-pi, pi].  The argument 2 pi u2 covers [0, 2 pi),
+    and neither document gives a figure on (pi, 2 pi); there this bound takes 2^-20, an assumption (twice the [-pi, pi] figure, for the
+    range reduction's extra rounding at 2 pi), which no test isolates: the GPU checks confirm only that the combined bound holds.  The
+    argument itself is off by one rounding of the product (the reference uses the same fp32 constant 2 pi_f32).
+    All of it stays near 1e-6 for most draws (below 1e-4 as u1 -> 1), far below the O(1) difference of a draw from another Philox
+    block."""
+    import numpy as np
+    from tests.philox_ref import philox4x32_10
+    x, y, _, _ = philox4x32_10(seed, index, offset)
+    u1 = ((x >> np.uint64(8)).astype(np.float64) + 1.0) / 16777216.0
+    u2 = (y >> np.uint64(8)).astype(np.float64) / 16777216.0
+    ln = np.log(u1)
+    r = np.sqrt(-2.0 * ln)
+    two_pi_f32 = float(np.float32(2 * math.pi))
+    arg = two_pi_f32 * u2
+    c, s = np.cos(arg), np.sin(arg)
+    e_log = np.maximum(2.0 ** -21.41, 3 * 2 * U32 * np.abs(ln)) + U32 * np.abs(ln)        # + the fp32 multiply by ln 2
+    dr = 2 * e_log / (np.sqrt(r * r + 2 * e_log) + r) + U32 * r                                 # -2 ln exact; sqrtf rounds once
+    e_trig = np.where(arg <= math.pi, 2.0 ** -20.5, 2.0 ** -20) + U32 * arg       # the reference uses 2 pi_f32: one rounding of the product
+    n0, n1 = r * c, r * s
+    t0 = dr * np.abs(c) + r * e_trig + U32 * np.abs(n0) + dr * e_trig
+    t1 = dr * np.abs(s) + r * e_trig + U32 * np.abs(n1) + dr * e_trig
+    to = lambda v: torch.from_numpy(np.ascontiguousarray(v, dtype=np.float64))
+    return to(n0), to(n1), to(t0), to(t1)
+
+
+def philox_pair_normals(seed: int, rows: int, width: int, offset: int, stride: int = 64):
+    """The normals of a [rows, width] draw laid out as the kernels lay it: columns (2p, 2p + 1) are the Box-Muller pair of block
+    (seed, row * stride + p, offset).  Returns (n, tol) float64 [rows, width]."""
+    import numpy as np
+    pairs = (width + 1) // 2
+    idx = (np.arange(rows, dtype=np.uint64)[:, None] * np.uint64(stride) + np.arange(pairs, dtype=np.uint64)[None, :]).reshape(-1)
+    n0, n1, t0, t1 = philox_normals_ref(seed, idx, offset)
+    n = torch.stack([n0, n1], -1).reshape(rows, 2 * pairs)[:, :width]
+    t = torch.stack([t0, t1], -1).reshape(rows, 2 * pairs)[:, :width]
+    return n, t
+
+
+def pnn_compose_ref(w: torch.Tensor, acts: torch.Tensor, act: Optional[str]):
+    """pnn_compose_kernel on the kernel's own composer head w [M, K] and primitive outputs acts [K, M, A]: sum_k act(w_k) a_k, float64.
+    fp32: act(w) (SiLU as w / (1 + expf(-w)): expf, the add, the quotient -- 4 u32 of |silu| plus expf's 2 ulp carried through), then
+    K fused multiply-adds -- one rounding each, bounded by K u32 sum |act(w_k) a_k|."""
+    w64, a64 = f64(w), f64(acts)
+    if act == "silu":
+        g = silu64(w64)
+        eg = 6 * U32 * (g.abs() + (w64 * torch.sigmoid(w64) * (1 - torch.sigmoid(w64))).abs())
+    elif act == "relu":
+        g, eg = torch.relu(w64), torch.zeros_like(w64)
+    else:
+        g, eg = w64, torch.zeros_like(w64)
+    K = w.shape[1]
+    terms = g.T[:, :, None] * a64                       # [K, M, A]
+    y = terms.sum(0)
+    tol = K * U32 * terms.abs().sum(0) + (eg.T[:, :, None] * a64.abs()).sum(0) + U32 * y.abs()
+    return y, tol
+
+
+def reparam_ref(head: torch.Tensor, noise: torch.Tensor, mode: str, latent: int, clamp: bool = True, lo: float = -5.0, hi: float = 2.0,
+                noise_tol: Optional[torch.Tensor] = None):
+    """vae_reparam_kernel / vae_reparam_philox_kernel on the kernel's own head [M, >= 2 latent], rounded to bf16, float64:
+    'sample'   z = mu + exp(0.5 clamp(logvar)) eps   (0.5 lv exact; expf within 2 ulp, 4 u32; the product and the sum, one rounding each:
+               5 u32 |sigma eps| + u32 |z| covers them whether or not the compiler contracts them into one fma),
+    'mean'     z = mu                                 (exact: the bf16 rounding of mu),
+    'residual' z = mu + eps                           (one rounding).
+    noise_tol: eps is the fp64 regeneration of the kernel's draws (philox_normals_ref), off by at most noise_tol."""
+    h = f64(head)
+    mu = h[:, :latent]
+    if mode == "mean":
+        return mu, UBF * mu.abs()
+    e = f64(noise)[:, :latent]
+    if mode == "residual":
+        z = mu + e
+        tol = U32 * z.abs()
+        if noise_tol is not None:
+            tol = tol + f64(noise_tol)
+    else:
+        lv = h[:, latent:2 * latent]
+        if clamp:
+            lv = torch.clamp(lv, lo, hi)
+        sg = torch.exp(0.5 * lv)
+        z = mu + sg * e
+        tol = U32 * z.abs() + 5 * U32 * (sg * e).abs()
+        if noise_tol is not None:
+            tol = tol + sg * f64(noise_tol)
+    return z, UBF * z.abs() + (1 + UBF) * tol
+
+
+def gae_ref(rewards, values, next_values, dones, gamma: float, tau: float):
+    """gae_kernel in float64 on fp32 time-major [T, N] inputs: delta = r + g V' - V, last = delta + (g tau)(1 - d) last, ret = last + V,
+    with the kernel's fp32 constant g tau = fp32(fp32(g) fp32(tau)) (an exact product, rounded once).  The bound is carried backwards
+    step by step: delta costs three roundings (u32 |g V'|, u32 |r + g V'|, u32 |delta|); each step adds delta's error, the rounding of
+    the product (u32 |c (1-d) last|) and of the sum (u32 |last|) to the error of the step after it, shrunk by c (1 - d).  So it scales
+    with |r|, |V| and |V'| and grows along t only as far as the discounting lets it.  Returns (adv, tol_adv, ret, tol_ret) time-major."""
+    r, v, nv, d = f64(rewards), f64(values), f64(next_values), f64(dones)
+    g = f32r(gamma)
+    c = f32r(g * f32r(tau))
+    T = r.shape[0]
+    adv, ret = torch.zeros_like(r), torch.zeros_like(r)
+    ta, tr = torch.zeros_like(r), torch.zeros_like(r)
+    last, err = torch.zeros_like(r[0]), torch.zeros_like(r[0])
+    for t in range(T - 1, -1, -1):
+        gv = g * nv[t]
+        s = r[t] + gv
+        delta = s - v[t]
+        e_delta = U32 * (gv.abs() + s.abs() + delta.abs())
+        carry = c * (1.0 - d[t]) * last                 # c (1 - d) is exact in fp32: d is 0 or 1
+        e_prod = c * (1.0 - d[t]) * err + U32 * (carry.abs() + c * err)
+        last = delta + carry
+        err = e_delta + e_prod + U32 * (last.abs() + e_delta + e_prod)
+        adv[t], ta[t] = last, err
+        ret[t] = last + v[t]
+        tr[t] = err + U32 * (ret[t].abs() + err)
+    return adv, ta, ret, tr
+
+
+def adv_normalize_ref(adv: torch.Tensor):
+    """normalize_adv_kernel on the kernel's own fp32 advantages a (flat [n]): (a - fp32(mean)) / (fp32(sqrt(unbiased var)) + 1e-8f),
+    float64.  The fp64 sums are exact to n u64 of sum |a| and sum a^2 (any order); mean and variance follow within a few u64 per
+    operation, which may move fp32(mean) / fp32(sqrt var) by one rounding each: u32 |mean| / den and u32 |y| (twice: the root and the
+    +1e-8f add).  Then the fp32 difference (u32 |a - mean| / den) and the quotient (u32 |y|)."""
+    a = f64(adv).reshape(-1)
+    n = a.numel()
+    s, q = a.sum(), (a * a).sum()
+    mean = s / n
+    var = torch.clamp((q - n * mean * mean) / (n - 1), min=0.0)
+    e_mean = float(U64 * a.abs().sum() + U64 * mean.abs())
+    e_var = float((n * U64 * q + 2 * n * mean.abs() * e_mean + 4 * U64 * (q + n * mean * mean)) / (n - 1))
+    sd = math.sqrt(float(var))
+    m32 = f32r(float(mean))
+    den = f32r(f32r(sd) + f32r(1e-8))
+    y = (a - m32) / den
+    e_m = e_mean + 2 * U32 * abs(m32)                           # the kernel's fp32(mean) may round the other way
+    e_den = (e_var / (2 * sd) if sd > 0 else math.sqrt(e_var)) + 4 * U32 * den
+    tol = (U32 * (a - m32).abs() + e_m) / den + y.abs() * (e_den / den + U32)
+    return y, tol
 
 
 def ppo_loss_ref(mu, value, actions, old_nlp, adv, ret, logstd, old_mu=None, e_clip=0.2, critic_coef=5.0, bounds_coef=10.0):

@@ -9,35 +9,14 @@ import math
 import pytest
 import torch
 
-from tests.fp64_ref import BoundError, Gemm, adam_ref, check, check_mask, disc_loss_ref, pack_mask, ppo_loss_ref, unpack_mask
+from tests.fp64_ref import BoundError, Gemm, adam_ref, kernel_gemm, check, check_mask, disc_loss_ref, pack_mask, ppo_loss_ref, unpack_mask
 
 BF = torch.bfloat16
+_kernel_gemm = kernel_gemm
 
 
 def _bf(g, *shape, scale=1.0):
     return (torch.randn(*shape, generator=g) * scale).to(BF)
-
-
-def _kernel_gemm(a, b, kblock=64, skip=None, dup_slice=None, slices=1):
-    """fp32 accumulation of bf16 a [M, K] . b [K, N] block by block (each block product in fp32).  skip = (k-block, column slice): that
-    k-block is left out of those columns.  slices / dup_slice: the reduction split into `slices` contiguous slices summed in order,
-    slice `dup_slice` added twice."""
-    a32, b32 = a.float(), b.float()
-    K = a.shape[1]
-    per = -(-K // slices)
-    out = torch.zeros(a.shape[0], b.shape[1])
-    for s in range(slices):
-        part = torch.zeros_like(out)
-        for k0 in range(s * per, min(K, (s + 1) * per), kblock):
-            k1 = min(k0 + kblock, (s + 1) * per, K)
-            blk = a32[:, k0:k1] @ b32[k0:k1]
-            if skip is not None and skip[0] == k0 // kblock:
-                blk[:, skip[1]] = 0.0
-            part += blk
-        out += part
-        if s == dup_slice:
-            out += part
-    return out
 
 
 def _setup(seed=0, M=96, K=512, N=256):

@@ -10,7 +10,7 @@ import torch
 
 from tests.fp64_links import _check_pads, _snapshot, _w, check, check_mlp, check_split
 from tests.fp64_ref import UBF, BoundError, Gemm, check_exact, silu64, silu_gated, silu_gemm_tol
-from tests.test_fp64_ref_cpu import _kernel_gemm
+from tests.fp64_ref import kernel_gemm as _kernel_gemm
 
 BF = torch.bfloat16
 SMALL = dict(E=24, S=22, T=36, task_units=(40, 24), N0=96, A=11, M=160)
