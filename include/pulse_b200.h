@@ -924,6 +924,82 @@ int pulse_reach_rollout_step(const pulse_reach_step_args_t* args, float* dones, 
 int pulse_ztask_rollout_step(const pulse_ztask_step_args_t* args, float* dones, int64_t num_envs, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * The PULSE-X speed task: HumanoidSpeedZ with robot=smplx_humanoid, env_pulsex_amp.yaml, learning=pulse_z_task.yaml.  The 52-body
+ * SMPL-X humanoid (bodies in SMPLH_MUJOCO_NAMES order, humanoid.py:376-377; body 0 the root; 51 joints x 3 = 153 dofs), beside the
+ * SMPL entry points above, which it leaves unchanged.  Body sets (contact bodies, termination heights) arrive as arguments; no
+ * entry point knows a body name.  The per-env device code is the SMPL step's and reset's, instantiated for 52 bodies: one warp per
+ * env, lane l holding bodies l and l + 32.
+ * ---------------------------------------------------------------------------------------------- */
+#define PULSE_SMPLX_BODIES 52
+#define PULSE_SMPLX_DOF 153          /* 51 joints x 3                                               */
+#define PULSE_SMPLX_SELF_OBS 778     /* 1 + 51*3 + 52*6 + 52*3 + 52*3, humanoid.py:1675-1731          */
+#define PULSE_SMPLX_SPEED_OBS 781    /* + compute_speed_observations (humanoid_speed.py:310-325)      */
+#define PULSE_SMPLX_FRAME_REC 676    /* packed per-frame record: pos156 | rot208 | vel156 | angvel156 */
+#define PULSE_SMPLX_AUX_REC 364      /* packed per-frame record: lrs208 | dvs153 | pad3             */
+
+/* MotionLib tables of the SMPL-X humanoid (MotionLibSMPL loaded with smplx_humanoid.xml, motion_lib_base.py:287-316), packed into
+ * the two records above by one kernel.  The handle is its own type: SMPL-X tables never reach an SMPL entry point. */
+typedef struct pulse_smplx_motionlib pulse_smplx_motionlib_t;
+typedef struct {
+  const float* gts;   /* [F,52,3] */
+  const float* grs;   /* [F,52,4] */
+  const float* lrs;   /* [F,52,4] */
+  const float* gvs;   /* [F,52,3] */
+  const float* gavs;  /* [F,52,3] */
+  const float* dvs;   /* [F,51,3] */
+  const float* lengths; const float* dt; const int64_t* num_frames; const int64_t* length_starts;   /* [M] */
+  int64_t total_frames, num_motions;
+  float* frame_rec;   /* [F, PULSE_SMPLX_FRAME_REC], 16-byte aligned, filled by pulse_smplx_motionlib_create */
+  float* aux_rec;     /* [F, PULSE_SMPLX_AUX_REC],   16-byte aligned */
+} pulse_smplx_motionlib_desc_t;
+int pulse_smplx_motionlib_create(const pulse_smplx_motionlib_desc_t* desc, void* stream, pulse_smplx_motionlib_t** out);
+int pulse_smplx_motionlib_destroy(pulse_smplx_motionlib_t* lib);
+
+/* get_motion_state (motion_lib_base.py:434-517) over the SMPL-X tables, the arithmetic of pulse_motion_state.  Any output may be NULL. */
+typedef struct {
+  const int64_t* motion_ids;   /* [n] */
+  const float* motion_times;   /* [n] */
+  const float* offset;         /* [n,3] or NULL */
+  float* root_pos; float* root_rot; float* root_vel; float* root_ang_vel;   /* [n,3] / [n,4] */
+  float* dof_pos; float* dof_vel;                                            /* [n,153] */
+  float* rg_pos; float* rb_rot; float* body_vel; float* body_ang_vel;       /* [n,52,3] / [n,52,4] */
+} pulse_smplx_motion_query_t;
+int pulse_smplx_motion_state(const pulse_smplx_motionlib_t* lib, const pulse_smplx_motion_query_t* q, int64_t n, void* stream);
+
+/* Post-physics step of the SMPL-X speed task: the self observation of compute_humanoid_observations_smpl_max with local root obs,
+ * root height and has_upright_start False (the heading of remove_base_rot(root_rot), humanoid.py:1617-1620, :1682-1684), then
+ * compute_speed_observations, whose heading is that of the RAW root rotation, compute_speed_reward and compute_humanoid_reset.
+ * obs[env] = [self 778 | heading-frame x axis 2 | target speed 1].  env_pulsex_amp.yaml has power_reward and power_usage_reward off;
+ * this step has neither term.  reward_raw (optional) receives the speed reward. */
+typedef struct {
+  int32_t enable_early_termination, reserved;
+  const float* body_state; int64_t body_env_stride;        /* [N, >=52, 13] pos quat(xyzw) linvel angvel */
+  const float* contact_forces; int64_t contact_env_stride; /* [N, >=52, 3] or NULL */
+  const float* termination_heights;                        /* [52] */
+  uint64_t contact_body_mask;                              /* bit j: body j may touch the ground (_contact_body_ids) */
+  const int64_t* progress_buf; int64_t max_episode_length;
+  const float* prev_root_pos; float dt; float reserved2;   /* [N, 3] root position before the physics step */
+  const float* tar_speed;                                  /* [N] */
+  float* obs_buf; int64_t obs_stride;                      /* [N, >= 781] */
+  float* rew_buf; float* reward_raw; int64_t raw_stride;
+  int64_t* reset_buf; int64_t* terminate_buf;
+} pulse_smplx_speed_step_args_t;
+int pulse_smplx_speed_step(const pulse_smplx_speed_step_args_t* args, int64_t num_envs, void* stream);
+/* The observation rows of the envs env_list[0 .. *count), as pulse_ztask_obs_list. */
+int pulse_smplx_speed_obs_list(const pulse_smplx_speed_step_args_t* args, const int64_t* env_list, const int32_t* count, int64_t num_envs,
+                               void* stream);
+/* progress_buf += 1, the step, dones[e] = float(reset_buf[e]), as pulse_ztask_rollout_step. */
+int pulse_smplx_speed_rollout_step(const pulse_smplx_speed_step_args_t* args, float* dones, int64_t num_envs, void* stream);
+
+/* The reference-state reset of pulse_reset_ztask for the SMPL-X speed task, no host synchronisation: the compaction, then one warp per
+ * reset env: clip and start-time draws, the 52-body gather, the SMPL ground fix from the per-frame floor table, the FACE_X pose
+ * adjustment (HumanoidSpeed._sample_ref_state, humanoid_speed.py:251-270, heading of remove_base_rot(root_rot) when !upright) and the
+ * scatter into the root, [N, >= 52, 13] rigid-body and [N, 153] dof views, counters and contact forces.  The argument struct is
+ * pulse_reset_ztask's with pose_mode PULSE_ZPOSE_FACE_X; the AMP history back-fill (amp_obs_buf) and the strike target (target_states)
+ * are refused.  _reset_task follows through pulse_ztask_reset_task, the PD targets through pulse_ztask_pre_physics (dofs 153). */
+int pulse_reset_ztask_smplx(const pulse_smplx_motionlib_t* lib, const pulse_ztask_reset_args_t* args, int64_t num_envs, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Pedestrian terrain task HumanoidPedestrianTerrain(Z) (phc/env/tasks/humanoid_pedestrian_terrain.py): post_physics_step in one launch,
  * one warp per env, selected by PULSE_STEP_REWARD / RESET / OBS:
  *   reward  _compute_reward :871-896: exp(-2 |tar - actor root|^2_xy) at tar = calc_pos(progress * dt) (fuzzy: errors < 0.0025 -> 0,

@@ -261,6 +261,30 @@ class ZTaskPrePhysicsArgs(C.Structure):
     ]
 
 
+class SmplxMotionLibDesc(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("gts", "grs", "lrs", "gvs", "gavs", "dvs", "lengths", "dt", "num_frames", "length_starts")] + [
+        ("total_frames", C.c_int64), ("num_motions", C.c_int64), ("frame_rec", C.c_void_p), ("aux_rec", C.c_void_p)]
+
+
+class SmplxMotionQuery(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in (
+        "motion_ids", "motion_times", "offset", "root_pos", "root_rot", "root_vel", "root_ang_vel", "dof_pos", "dof_vel", "rg_pos", "rb_rot",
+        "body_vel", "body_ang_vel")]
+
+
+class SmplxSpeedStepArgs(C.Structure):
+    _fields_ = [
+        ("enable_early_termination", C.c_int32), ("reserved", C.c_int32), ("body_state", C.c_void_p), ("body_env_stride", C.c_int64),
+        ("contact_forces", C.c_void_p), ("contact_env_stride", C.c_int64), ("termination_heights", C.c_void_p), ("contact_body_mask", C.c_uint64),
+        ("progress_buf", C.c_void_p), ("max_episode_length", C.c_int64), ("prev_root_pos", C.c_void_p), ("dt", C.c_float), ("reserved2", C.c_float),
+        ("tar_speed", C.c_void_p), ("obs_buf", C.c_void_p), ("obs_stride", C.c_int64), ("rew_buf", C.c_void_p), ("reward_raw", C.c_void_p),
+        ("raw_stride", C.c_int64), ("reset_buf", C.c_void_p), ("terminate_buf", C.c_void_p),
+    ]
+
+
+SMPLX_BODIES, SMPLX_DOF, SMPLX_SELF_OBS, SMPLX_SPEED_OBS = 52, 153, 778, 781
+
+
 # Philox index planes of the latent tasks' draws (include/pulse_b200.h): index = env + plane
 ZTASK_PLANE_RESET, ZTASK_PLANE_STRIKE, ZTASK_PLANE_RESET_TASK, ZTASK_PLANE_UPDATE_TASK = 0, 1 << 32, 2 << 32, 3 << 32
 
@@ -466,6 +490,13 @@ SIGNATURES = {
     "pulse_im_task_obs": (C.c_int, [C.POINTER(TaskObsArgs), C.c_void_p]),
     "pulse_eval_step": (C.c_int, [C.POINTER(EvalArgs), C.c_void_p]),
     "pulse_motionlib_load_clips": (C.c_int, [C.POINTER(LoaderArgs), C.c_void_p]),
+    "pulse_smplx_motionlib_create": (C.c_int, [C.POINTER(SmplxMotionLibDesc), C.c_void_p, C.POINTER(C.c_void_p)]),
+    "pulse_smplx_motionlib_destroy": (C.c_int, [C.c_void_p]),
+    "pulse_smplx_motion_state": (C.c_int, [C.c_void_p, C.POINTER(SmplxMotionQuery), C.c_int64, C.c_void_p]),
+    "pulse_smplx_speed_step": (C.c_int, [C.POINTER(SmplxSpeedStepArgs), C.c_int64, C.c_void_p]),
+    "pulse_smplx_speed_obs_list": (C.c_int, [C.POINTER(SmplxSpeedStepArgs), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "pulse_smplx_speed_rollout_step": (C.c_int, [C.POINTER(SmplxSpeedStepArgs), C.c_void_p, C.c_int64, C.c_void_p]),
+    "pulse_reset_ztask_smplx": (C.c_int, [C.c_void_p, C.POINTER(ZTaskResetArgs), C.c_int64, C.c_void_p]),
 }
 
 _lib = None

@@ -5,17 +5,38 @@
 
 namespace pulse {
 
+// The body layouts the latent-task step and reset code is instantiated for.  B bodies give a MotionLib frame record
+// pos 3B | rot 4B | vel 3B | angvel 3B, an aux record lrs 4B | dvs 3(B - 1) | pad, and a self observation of 1 + 3(B - 1) + 6B + 3B + 3B
+// floats.  kUpright: the step's self observation takes the heading of the root rotation itself (has_upright_start), otherwise
+// of remove_base_rot(root).  kSmplTerms: the terms only the SMPL path serves (strike, the power term, the AMP history rows).
+struct SmplLayout {
+  static constexpr int kBodies = PULSE_NUM_BODIES, kDofs = PULSE_NUM_DOF, kSelfObs = PULSE_SELF_OBS;
+  static constexpr int kFrameRec = PULSE_FRAME_REC, kAuxRec = PULSE_AUX_REC;
+  static constexpr bool kUpright = true, kSmplTerms = true;
+  using StepArgs = pulse_ztask_step_args_t;
+};
+struct SmplxLayout {
+  static constexpr int kBodies = PULSE_SMPLX_BODIES, kDofs = PULSE_SMPLX_DOF, kSelfObs = PULSE_SMPLX_SELF_OBS;
+  static constexpr int kFrameRec = PULSE_SMPLX_FRAME_REC, kAuxRec = PULSE_SMPLX_AUX_REC;
+  static constexpr bool kUpright = false, kSmplTerms = false;
+  using StepArgs = pulse_smplx_speed_step_args_t;
+};
+static_assert(3 * PULSE_SMPLX_BODIES + 4 * PULSE_SMPLX_BODIES + 6 * PULSE_SMPLX_BODIES == PULSE_SMPLX_FRAME_REC, "SMPL-X frame record");
+static_assert(4 * PULSE_SMPLX_BODIES + PULSE_SMPLX_DOF <= PULSE_SMPLX_AUX_REC && PULSE_SMPLX_AUX_REC % 4 == 0, "SMPL-X aux record");
+static_assert(1 + 3 * (PULSE_SMPLX_BODIES - 1) + 12 * PULSE_SMPLX_BODIES == PULSE_SMPLX_SELF_OBS, "SMPL-X self observation");
+
 // compute_humanoid_observations_smpl_max (humanoid.py:1675-1731) with local root obs and the root height: body j's slice of the
-// 358-float self observation [root height | 23 x position | 24 x six-D rotation | 24 x velocity | 24 x angular velocity], all in
-// the heading frame.  The heights p.z and p_root.z are taken from the task's reference (the ground, or the terrain's center
-// height); (hs, hc) is the heading's half-angle sine / cosine and yr = make_yaw of the inverse heading.  The imitation and reach
-// step kernels write the same layout inline (see im_step.cu).
+// self observation of B bodies [root height | (B-1) x position | B x six-D rotation | B x velocity | B x angular velocity] (358 floats
+// for SMPL), all in the heading frame.  The heights p.z and p_root.z are taken from the task's reference (the ground, or the
+// terrain's center height); (hs, hc) is the heading's half-angle sine / cosine and yr = make_yaw of the inverse heading.  The
+// imitation and reach step kernels write the same layout inline (see im_step.cu).
+template <int B = PULSE_NUM_BODIES>
 __device__ __forceinline__ void store_self_obs(float* o, int j, Vec3 p, Vec3 p_root, Quat q, Vec3 v, Vec3 w, float hs, float hc, Yaw yr) {
   if (j == 0) o[0] = p_root.z;
   else stv(o + 1 + 3 * (j - 1), yaw_rot(yr, p - p_root));
-  qsix(yaw_mul_left(-hs, hc, q), o + 70 + 6 * j);
-  stv(o + 214 + 3 * j, yaw_rot(yr, v));
-  stv(o + 286 + 3 * j, yaw_rot(yr, w));
+  qsix(yaw_mul_left(-hs, hc, q), o + 3 * B - 2 + 6 * j);
+  stv(o + 9 * B - 2 + 3 * j, yaw_rot(yr, v));
+  stv(o + 12 * B - 2 + 3 * j, yaw_rot(yr, w));
 }
 
 namespace {  // __constant__ tables are per module; one copy in every translation unit that builds AMP rows
@@ -79,7 +100,7 @@ struct FallFlags {
 template <class Args>
 __device__ __forceinline__ FallFlags fall_flags(const Args& a, long long e, int j, bool body, float z) {
   FallFlags f = {false, false};
-  if (a.enable_early_termination && body && !((a.contact_body_mask >> j) & 1u)) {
+  if (a.enable_early_termination && body && !((a.contact_body_mask >> j) & 1u)) {   // a 32- or 64-bit mask
     if (a.contact_forces != nullptr) {
       const float* cf = a.contact_forces + e * a.contact_env_stride + j * 3;
       f.contact = fabsf(cf[0]) > 0.1f || fabsf(cf[1]) > 0.1f || fabsf(cf[2]) > 0.1f;

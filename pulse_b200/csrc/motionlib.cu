@@ -112,6 +112,69 @@ __global__ void __launch_bounds__(128) motion_state_kernel(const pulse_motionlib
   }
 }
 
+// The SMPL-X records: one thread per (frame, float) of the frame record and the aux record (pad floats zero).
+__global__ void smplx_pack_kernel(pulse_smplx_motionlib_desc_t d) {
+  constexpr int B = PULSE_SMPLX_BODIES, FR = PULSE_SMPLX_FRAME_REC, AR = PULSE_SMPLX_AUX_REC;
+  const long long total = d.total_frames * (FR + AR);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long f = i / (FR + AR);
+    const int c = static_cast<int>(i - f * (FR + AR));
+    if (c < FR) {
+      float v;
+      if (c < 3 * B) v = d.gts[f * 3 * B + c];
+      else if (c < 7 * B) v = d.grs[f * 4 * B + (c - 3 * B)];
+      else if (c < 10 * B) v = d.gvs[f * 3 * B + (c - 7 * B)];
+      else v = d.gavs[f * 3 * B + (c - 10 * B)];
+      d.frame_rec[f * FR + c] = v;
+    } else {
+      const int k = c - FR;
+      float v = 0.0f;
+      if (k < 4 * B) v = d.lrs[f * 4 * B + k];
+      else if (k < 4 * B + PULSE_SMPLX_DOF) v = d.dvs[f * PULSE_SMPLX_DOF + (k - 4 * B)];
+      d.aux_rec[f * AR + k] = v;
+    }
+  }
+}
+
+// get_motion_state over the SMPL-X records: motion_state_kernel's arithmetic, one warp per query, lane l = bodies l and l + 32.
+__global__ void __launch_bounds__(128) smplx_motion_state_kernel(const pulse_smplx_motionlib_desc_t lib, const pulse_smplx_motion_query_t q,
+                                                                 long long n) {
+  constexpr int B = PULSE_SMPLX_BODIES;
+  const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (i >= n) return;
+  const long long mid = q.motion_ids[i];
+  long long i0, i1;
+  float b;
+  frame_blend_rn(q.motion_times[i], lib.lengths[mid], lib.num_frames[mid], lib.dt[mid], i0, i1, b);
+  const long long f0 = i0 + lib.length_starts[mid], f1 = i1 + lib.length_starts[mid];
+  const float* r0 = lib.frame_rec + f0 * PULSE_SMPLX_FRAME_REC;
+  const float* r1 = lib.frame_rec + f1 * PULSE_SMPLX_FRAME_REC;
+  const float* x0 = lib.aux_rec + f0 * PULSE_SMPLX_AUX_REC;
+  const float* x1 = lib.aux_rec + f1 * PULSE_SMPLX_AUX_REC;
+  const auto blend3 = [&](int o) { return Vec3{lerp_rn(r0[o], r1[o], b), lerp_rn(r0[o + 1], r1[o + 1], b), lerp_rn(r0[o + 2], r1[o + 2], b)}; };
+  for (int j = lane; j < B; j += 32) {
+    Vec3 p = blend3(3 * j);
+    if (q.offset) p = {__fadd_rn(p.x, q.offset[3 * i]), __fadd_rn(p.y, q.offset[3 * i + 1]), __fadd_rn(p.z, q.offset[3 * i + 2])};
+    const Vec3 v = blend3(7 * B + 3 * j), w = blend3(10 * B + 3 * j);
+    const Quat rq = slerp(ldq4(r0 + 3 * B + 4 * j), ldq4(r1 + 3 * B + 4 * j), b);
+    if (q.rg_pos) stv(q.rg_pos + (i * B + j) * 3, p);
+    if (q.body_vel) stv(q.body_vel + (i * B + j) * 3, v);
+    if (q.body_ang_vel) stv(q.body_ang_vel + (i * B + j) * 3, w);
+    if (q.rb_rot) { float* d = q.rb_rot + (i * B + j) * 4; d[0] = rq.x; d[1] = rq.y; d[2] = rq.z; d[3] = rq.w; }
+    if (j == 0) {
+      if (q.root_pos) stv(q.root_pos + 3 * i, p);
+      if (q.root_vel) stv(q.root_vel + 3 * i, v);
+      if (q.root_ang_vel) stv(q.root_ang_vel + 3 * i, w);
+      if (q.root_rot) { float* d = q.root_rot + 4 * i; d[0] = rq.x; d[1] = rq.y; d[2] = rq.z; d[3] = rq.w; }
+    } else if (q.dof_pos) {
+      stv(q.dof_pos + i * PULSE_SMPLX_DOF + 3 * (j - 1), quat_exp_map(slerp(ldq4(x0 + 4 * j), ldq4(x1 + 4 * j), b)));
+    }
+  }
+  if (q.dof_vel)
+    for (int k = lane; k < PULSE_SMPLX_DOF; k += 32) q.dof_vel[i * PULSE_SMPLX_DOF + k] = lerp_rn(x0[4 * B + k], x1[4 * B + k], b);
+}
+
 }  // namespace
 }  // namespace pulse
 
@@ -157,5 +220,41 @@ extern "C" int pulse_motion_state(const pulse_motionlib_t* lib, const pulse_moti
   const unsigned grid = static_cast<unsigned>((threads + 127) / 128);
   motion_state_kernel<<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(lib->d, *q, (long long)n);
   PULSE_LAUNCH_OK("motion_state_kernel");
+  return PULSE_OK;
+}
+
+extern "C" int pulse_smplx_motionlib_create(const pulse_smplx_motionlib_desc_t* desc, void* stream, pulse_smplx_motionlib_t** out) {
+  using namespace pulse;
+  PULSE_REQUIRE(desc != nullptr && out != nullptr, "pulse_smplx_motionlib_create: null argument");
+  const pulse_smplx_motionlib_desc_t& d = *desc;
+  PULSE_REQUIRE(d.gts && d.grs && d.lrs && d.gvs && d.gavs && d.dvs && d.lengths && d.dt && d.num_frames && d.length_starts,
+                "pulse_smplx_motionlib_create: null table pointer");
+  PULSE_REQUIRE(d.total_frames > 0 && d.num_motions > 0, "pulse_smplx_motionlib_create: empty tables (F=%lld, M=%lld)",
+                (long long)d.total_frames, (long long)d.num_motions);
+  PULSE_REQUIRE(d.frame_rec != nullptr && aligned16(d.frame_rec) && d.aux_rec != nullptr && aligned16(d.aux_rec),
+                "pulse_smplx_motionlib_create: frame_rec / aux_rec null or not 16-byte aligned");
+  const long long total = d.total_frames * (PULSE_SMPLX_FRAME_REC + PULSE_SMPLX_AUX_REC);
+  smplx_pack_kernel<<<grid_for(total, 256, 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(d);
+  PULSE_LAUNCH_OK("smplx_pack_kernel");
+  pulse_smplx_motionlib* h = static_cast<pulse_smplx_motionlib*>(malloc(sizeof(pulse_smplx_motionlib)));
+  PULSE_REQUIRE(h != nullptr, "pulse_smplx_motionlib_create: host allocation failed");
+  h->d = d;
+  *out = h;
+  return PULSE_OK;
+}
+
+extern "C" int pulse_smplx_motionlib_destroy(pulse_smplx_motionlib_t* lib) {
+  if (lib) free(lib);
+  return PULSE_OK;
+}
+
+extern "C" int pulse_smplx_motion_state(const pulse_smplx_motionlib_t* lib, const pulse_smplx_motion_query_t* q, int64_t n, void* stream) {
+  using namespace pulse;
+  PULSE_REQUIRE(lib != nullptr && q != nullptr, "pulse_smplx_motion_state: null lib/query");
+  PULSE_REQUIRE(n >= 0, "pulse_smplx_motion_state: negative n");
+  if (n == 0) return PULSE_OK;
+  PULSE_REQUIRE(q->motion_ids && q->motion_times, "pulse_smplx_motion_state: null ids/times");
+  smplx_motion_state_kernel<<<static_cast<unsigned>((n * 32 + 127) / 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(lib->d, *q, (long long)n);
+  PULSE_LAUNCH_OK("smplx_motion_state_kernel");
   return PULSE_OK;
 }

@@ -69,3 +69,7 @@ __device__ __forceinline__ T warp_sum(T v) {
 struct pulse_motionlib {
   pulse_motionlib_desc_t d;
 };
+
+struct pulse_smplx_motionlib {
+  pulse_smplx_motionlib_desc_t d;
+};

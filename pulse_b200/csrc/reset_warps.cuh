@@ -1,9 +1,9 @@
 // The per-warp reference-state reset shared by pulse_reset_ztask (ztask_reset.cu) and pulse_reset_terrain (terrain_reset.cu):
 //   reset_compact_kernel  one CTA: the ordered compaction of compact.cuh turns the reset mask or id list into the ascending env list,
 //                         the humanoid and target actor lists and a device-side count;
-//   reset_warps           one warp per (reset env, AMP history step k): clip and start-time draws, MotionLib gather, SMPL ground fix
-//                         from the per-frame floor table, the caller's adjustment of the root and bodies, the scatter into the
-//                         simulator's views, counters and the AMP rows (195- or 196-float layout).
+//   reset_warps           one warp per (reset env, AMP history step k), for a body layout (SMPL, SMPL-X): clip and start-time
+//                         draws, MotionLib gather, SMPL ground fix from the per-frame floor table, the caller's adjustment of the root
+//                         and bodies, the scatter into the simulator's views, counters and the AMP rows (195- or 196-float layout).
 // The entry points, argument structs and Philox word layout are documented in include/pulse_b200.h.
 #pragma once
 #include "compact.cuh"
@@ -64,12 +64,16 @@ __device__ __forceinline__ void store_amp_row(float* out, int width, float* stag
   __syncwarp();
 }
 
-// The work of one warp.  `adjust(e, lane, r0, off, p, rq, v, rp, rr, rv, rw)` runs on every lane after the ground fix: lane j holds
-// body j's position, rotation and velocity (p, rq, v), every lane the root's (rp, rr, rv, rw); r0 is Philox block (seed, e, off)
-// when a draw is not injected or `more_draws` is set, zero otherwise.  What it leaves is what _set_env_state writes.
-template <class Adjust>
-__device__ __forceinline__ void reset_warps(const pulse_motionlib_desc_t& lib, const pulse_ztask_reset_args_t& a, bool more_draws, float* stage,
+// The work of one warp in body layout L (lib: the layout's MotionLib descriptor).  `adjust(e, lane, r0, off, p, rq, v, rp, rr, rv, rw)`
+// runs after the ground fix once per body a lane holds (lane l holds bodies l and l + 32 where the layout has them): (p, rq, v) are
+// that body's position, rotation and velocity, (rp, rr, rv, rw) the root's in every lane; a lane's second call gets its own copy of the
+// root, so the root is adjusted once.  r0 is Philox block (seed, e, off) when a draw is not injected or `more_draws` is set, zero
+// otherwise.  What it leaves is what _set_env_state writes.  The AMP history rows are SMPL's (L::kSmplTerms).
+template <class L, class Lib, class Adjust>
+__device__ __forceinline__ void reset_warps(const Lib& lib, const pulse_ztask_reset_args_t& a, bool more_draws, float* stage,
                                             const Adjust& adjust) {
+  constexpr int B = L::kBodies, kSlots = (B + 31) / 32;
+  constexpr int kRot = 3 * B, kVel = 7 * B, kAng = 10 * B, kDvs = 4 * B;   // record offsets
   const int lane = threadIdx.x & 31;
   const long long warp0 = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const long long nwarps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
@@ -98,56 +102,74 @@ __device__ __forceinline__ void reset_warps(const pulse_motionlib_desc_t& lib, c
     float b;
     frame_blend_rn(t, mlen, lib.num_frames[mid], lib.dt[mid], i0, i1, b);
     const long long f0 = i0 + lib.length_starts[mid], f1 = i1 + lib.length_starts[mid];
-    const float* r0p = lib.frame_rec + f0 * PULSE_FRAME_REC;
-    const float* r1p = lib.frame_rec + f1 * PULSE_FRAME_REC;
-    const float* x0 = lib.aux_rec + f0 * PULSE_AUX_REC;
-    const float* x1 = lib.aux_rec + f1 * PULSE_AUX_REC;
+    const float* r0p = lib.frame_rec + f0 * L::kFrameRec;
+    const float* r1p = lib.frame_rec + f1 * L::kFrameRec;
+    const float* x0 = lib.aux_rec + f0 * L::kAuxRec;
+    const float* x1 = lib.aux_rec + f1 * L::kAuxRec;
 
-    if (k > 0) {   // _init_amp_obs_ref: the motion at t0 - k dt as it is, without the ground fix or the pose adjustment
-      const Vec3 p0 = {lerp_rn(r0p[0], r1p[0], b), lerp_rn(r0p[1], r1p[1], b), lerp_rn(r0p[2], r1p[2], b)};
-      const Vec3 v0 = {lerp_rn(r0p[168], r1p[168], b), lerp_rn(r0p[169], r1p[169], b), lerp_rn(r0p[170], r1p[170], b)};
-      const Vec3 w0 = {lerp_rn(r0p[240], r1p[240], b), lerp_rn(r0p[241], r1p[241], b), lerp_rn(r0p[242], r1p[242], b)};
-      const Quat q0 = slerp(ldq4(r0p + 72), ldq4(r1p + 72), b);
-      const auto joint = [&](int jt) {
-        return AmpJoint{quat_exp_map(slerp(ldq4(x0 + 4 * (jt + 1)), ldq4(x1 + 4 * (jt + 1)), b)),
-                        {lerp_rn(x0[96 + 3 * jt], x1[96 + 3 * jt], b), lerp_rn(x0[97 + 3 * jt], x1[97 + 3 * jt], b),
-                         lerp_rn(x0[98 + 3 * jt], x1[98 + 3 * jt], b)}};
-      };
-      const auto key_pos = [&](int kb) {
-        return Vec3{lerp_rn(r0p[3 * kb], r1p[3 * kb], b), lerp_rn(r0p[3 * kb + 1], r1p[3 * kb + 1], b), lerp_rn(r0p[3 * kb + 2], r1p[3 * kb + 2], b)};
-      };
-      store_amp_row(a.amp_obs_buf + (e * a.num_amp_steps + k) * a.amp_width, a.amp_width, stage, lane, p0, q0, v0, w0, upright, joint, key_pos);
-      continue;
-    }
-
-    // ---- the reset state: lane j holds body j -----------------------------------------------------------------------------------
-    const int j = lane < PULSE_NUM_BODIES ? lane : 0;
-    Vec3 p = {lerp_rn(r0p[3 * j], r1p[3 * j], b), lerp_rn(r0p[3 * j + 1], r1p[3 * j + 1], b), lerp_rn(r0p[3 * j + 2], r1p[3 * j + 2], b)};
-    Vec3 v = {lerp_rn(r0p[168 + 3 * j], r1p[168 + 3 * j], b), lerp_rn(r0p[169 + 3 * j], r1p[169 + 3 * j], b),
-              lerp_rn(r0p[170 + 3 * j], r1p[170 + 3 * j], b)};
-    const Vec3 w = {lerp_rn(r0p[240 + 3 * j], r1p[240 + 3 * j], b), lerp_rn(r0p[241 + 3 * j], r1p[241 + 3 * j], b),
-                    lerp_rn(r0p[242 + 3 * j], r1p[242 + 3 * j], b)};
-    Quat rq = slerp(ldq4(r0p + 72 + 4 * j), ldq4(r1p + 72 + 4 * j), b);
-    // ground fix (humanoid_amp.py:382-430): d = min_v (V - (J0 - root)).z - 0.02 = (floor(f0) + root z) - 0.02
-    const float root_z = __shfl_sync(kFull, p.z, 0);
-    const float d = __fsub_rn(__fadd_rn(a.floor[f0], root_z), 0.02f);
-    p.z = __fsub_rn(p.z, d);
-    Vec3 rp = {__shfl_sync(kFull, p.x, 0), __shfl_sync(kFull, p.y, 0), __shfl_sync(kFull, p.z, 0)};
-    Quat rr = {__shfl_sync(kFull, rq.x, 0), __shfl_sync(kFull, rq.y, 0), __shfl_sync(kFull, rq.z, 0), __shfl_sync(kFull, rq.w, 0)};
-    Vec3 rv = {__shfl_sync(kFull, v.x, 0), __shfl_sync(kFull, v.y, 0), __shfl_sync(kFull, v.z, 0)};
-    Vec3 rw = {__shfl_sync(kFull, w.x, 0), __shfl_sync(kFull, w.y, 0), __shfl_sync(kFull, w.z, 0)};
-    adjust(e, lane, r0, off, p, rq, v, rp, rr, rv, rw);
-    if (lane < PULSE_NUM_BODIES) {   // _set_env_state (humanoid_amp.py:565-597)
-      float* bs = a.rigid_body_state + e * a.body_env_stride + j * PULSE_BODY_STATE_W;
-      bs[0] = p.x; bs[1] = p.y; bs[2] = p.z; bs[3] = rq.x; bs[4] = rq.y; bs[5] = rq.z; bs[6] = rq.w;
-      bs[7] = v.x; bs[8] = v.y; bs[9] = v.z; bs[10] = w.x; bs[11] = w.y; bs[12] = w.z;
-      if (j >= 1) {   // dof_pos = exp_map(slerp(local rotations)) of joints 1..23
-        const Vec3 em = quat_exp_map(slerp(ldq4(x0 + 4 * j), ldq4(x1 + 4 * j), b));
-        float* dp = a.dof_pos + e * a.dof_env_stride + 3 * (j - 1) * a.dof_elem_stride;
-        dp[0] = em.x; dp[a.dof_elem_stride] = em.y; dp[2 * a.dof_elem_stride] = em.z;
+    if constexpr (L::kSmplTerms) {
+      if (k > 0) {   // _init_amp_obs_ref: the motion at t0 - k dt as it is, without the ground fix or the pose adjustment
+        const Vec3 p0 = {lerp_rn(r0p[0], r1p[0], b), lerp_rn(r0p[1], r1p[1], b), lerp_rn(r0p[2], r1p[2], b)};
+        const Vec3 v0 = {lerp_rn(r0p[168], r1p[168], b), lerp_rn(r0p[169], r1p[169], b), lerp_rn(r0p[170], r1p[170], b)};
+        const Vec3 w0 = {lerp_rn(r0p[240], r1p[240], b), lerp_rn(r0p[241], r1p[241], b), lerp_rn(r0p[242], r1p[242], b)};
+        const Quat q0 = slerp(ldq4(r0p + 72), ldq4(r1p + 72), b);
+        const auto joint = [&](int jt) {
+          return AmpJoint{quat_exp_map(slerp(ldq4(x0 + 4 * (jt + 1)), ldq4(x1 + 4 * (jt + 1)), b)),
+                          {lerp_rn(x0[96 + 3 * jt], x1[96 + 3 * jt], b), lerp_rn(x0[97 + 3 * jt], x1[97 + 3 * jt], b),
+                           lerp_rn(x0[98 + 3 * jt], x1[98 + 3 * jt], b)}};
+        };
+        const auto key_pos = [&](int kb) {
+          return Vec3{lerp_rn(r0p[3 * kb], r1p[3 * kb], b), lerp_rn(r0p[3 * kb + 1], r1p[3 * kb + 1], b), lerp_rn(r0p[3 * kb + 2], r1p[3 * kb + 2], b)};
+        };
+        store_amp_row(a.amp_obs_buf + (e * a.num_amp_steps + k) * a.amp_width, a.amp_width, stage, lane, p0, q0, v0, w0, upright, joint, key_pos);
+        continue;
       }
     }
-    for (int c = lane; c < PULSE_NUM_DOF; c += 32) a.dof_vel[e * a.dof_env_stride + c * a.dof_elem_stride] = lerp_rn(x0[96 + c], x1[96 + c], b);
+
+    // ---- the reset state: lane l holds bodies l (slot 0) and l + 32 (slot 1) -------------------------------------------------------
+    Vec3 p[kSlots], v[kSlots], w[kSlots];
+    Quat rq[kSlots];
+#pragma unroll
+    for (int s = 0; s < kSlots; ++s) {
+      const int j = lane + 32 * s < B ? lane + 32 * s : 0;
+      p[s] = {lerp_rn(r0p[3 * j], r1p[3 * j], b), lerp_rn(r0p[3 * j + 1], r1p[3 * j + 1], b), lerp_rn(r0p[3 * j + 2], r1p[3 * j + 2], b)};
+      v[s] = {lerp_rn(r0p[kVel + 3 * j], r1p[kVel + 3 * j], b), lerp_rn(r0p[kVel + 1 + 3 * j], r1p[kVel + 1 + 3 * j], b),
+              lerp_rn(r0p[kVel + 2 + 3 * j], r1p[kVel + 2 + 3 * j], b)};
+      w[s] = {lerp_rn(r0p[kAng + 3 * j], r1p[kAng + 3 * j], b), lerp_rn(r0p[kAng + 1 + 3 * j], r1p[kAng + 1 + 3 * j], b),
+              lerp_rn(r0p[kAng + 2 + 3 * j], r1p[kAng + 2 + 3 * j], b)};
+      rq[s] = slerp(ldq4(r0p + kRot + 4 * j), ldq4(r1p + kRot + 4 * j), b);
+    }
+    // ground fix (humanoid_amp.py:382-430): d = min_v (V - (J0 - root)).z - 0.02 = (floor(f0) + root z) - 0.02
+    const float root_z = __shfl_sync(kFull, p[0].z, 0);
+    const float d = __fsub_rn(__fadd_rn(a.floor[f0], root_z), 0.02f);
+#pragma unroll
+    for (int s = 0; s < kSlots; ++s) p[s].z = __fsub_rn(p[s].z, d);
+    Vec3 rp = {__shfl_sync(kFull, p[0].x, 0), __shfl_sync(kFull, p[0].y, 0), __shfl_sync(kFull, p[0].z, 0)};
+    Quat rr = {__shfl_sync(kFull, rq[0].x, 0), __shfl_sync(kFull, rq[0].y, 0), __shfl_sync(kFull, rq[0].z, 0), __shfl_sync(kFull, rq[0].w, 0)};
+    Vec3 rv = {__shfl_sync(kFull, v[0].x, 0), __shfl_sync(kFull, v[0].y, 0), __shfl_sync(kFull, v[0].z, 0)};
+    Vec3 rw = {__shfl_sync(kFull, w[0].x, 0), __shfl_sync(kFull, w[0].y, 0), __shfl_sync(kFull, w[0].z, 0)};
+#pragma unroll
+    for (int s = kSlots - 1; s >= 1; --s) {   // the later slots first, on copies of the root the slot-0 call then adjusts
+      Vec3 cp = rp, cv = rv, cw = rw;
+      Quat cr = rr;
+      adjust(e, lane, r0, off, p[s], rq[s], v[s], cp, cr, cv, cw);
+    }
+    adjust(e, lane, r0, off, p[0], rq[0], v[0], rp, rr, rv, rw);
+#pragma unroll
+    for (int s = 0; s < kSlots; ++s) {
+      const int j = lane + 32 * s;
+      if (j < B) {   // _set_env_state (humanoid_amp.py:565-597)
+        float* bs = a.rigid_body_state + e * a.body_env_stride + j * PULSE_BODY_STATE_W;
+        bs[0] = p[s].x; bs[1] = p[s].y; bs[2] = p[s].z; bs[3] = rq[s].x; bs[4] = rq[s].y; bs[5] = rq[s].z; bs[6] = rq[s].w;
+        bs[7] = v[s].x; bs[8] = v[s].y; bs[9] = v[s].z; bs[10] = w[s].x; bs[11] = w[s].y; bs[12] = w[s].z;
+        if (j >= 1) {   // dof_pos = exp_map(slerp(local rotations)) of joints 1..B-1
+          const Vec3 em = quat_exp_map(slerp(ldq4(x0 + 4 * j), ldq4(x1 + 4 * j), b));
+          float* dp = a.dof_pos + e * a.dof_env_stride + 3 * (j - 1) * a.dof_elem_stride;
+          dp[0] = em.x; dp[a.dof_elem_stride] = em.y; dp[2 * a.dof_elem_stride] = em.z;
+        }
+      }
+    }
+    for (int c = lane; c < L::kDofs; c += 32) a.dof_vel[e * a.dof_env_stride + c * a.dof_elem_stride] = lerp_rn(x0[kDvs + c], x1[kDvs + c], b);
     if (a.contact_forces != nullptr)
       for (int c = lane; c < a.contact_bodies * 3; c += 32) a.contact_forces[e * a.contact_env_stride + c] = 0.0f;
     if (lane == 0) {
@@ -160,20 +182,22 @@ __device__ __forceinline__ void reset_warps(const pulse_motionlib_desc_t& lib, c
       if (a.reset_buf != nullptr) a.reset_buf[e] = 0;
       if (a.terminate_buf != nullptr) a.terminate_buf[e] = 0;
     }
-    if (a.amp_obs_buf == nullptr) continue;
-    // row 0: _compute_amp_observations(env_ids) of the rigid bodies and dofs just written
-    __syncwarp();
-    const float* bs = a.rigid_body_state + e * a.body_env_stride;
-    const float* dp = a.dof_pos + e * a.dof_env_stride;
-    const float* dv = a.dof_vel + e * a.dof_env_stride;
-    const long long ds = a.dof_elem_stride;
-    const auto joint = [&](int jt) {
-      return AmpJoint{{dp[(3 * jt + 0) * ds], dp[(3 * jt + 1) * ds], dp[(3 * jt + 2) * ds]},
-                      {dv[(3 * jt + 0) * ds], dv[(3 * jt + 1) * ds], dv[(3 * jt + 2) * ds]}};
-    };
-    const auto key_pos = [&](int kb) { return ldv(bs + kb * PULSE_BODY_STATE_W); };
-    store_amp_row(a.amp_obs_buf + e * a.num_amp_steps * a.amp_width, a.amp_width, stage, lane, ldv(bs), ldq(bs + 3), ldv(bs + 7), ldv(bs + 10),
-                  upright, joint, key_pos);
+    if constexpr (L::kSmplTerms) {
+      if (a.amp_obs_buf == nullptr) continue;
+      // row 0: _compute_amp_observations(env_ids) of the rigid bodies and dofs just written
+      __syncwarp();
+      const float* bs = a.rigid_body_state + e * a.body_env_stride;
+      const float* dp = a.dof_pos + e * a.dof_env_stride;
+      const float* dv = a.dof_vel + e * a.dof_env_stride;
+      const long long ds = a.dof_elem_stride;
+      const auto joint = [&](int jt) {
+        return AmpJoint{{dp[(3 * jt + 0) * ds], dp[(3 * jt + 1) * ds], dp[(3 * jt + 2) * ds]},
+                        {dv[(3 * jt + 0) * ds], dv[(3 * jt + 1) * ds], dv[(3 * jt + 2) * ds]}};
+      };
+      const auto key_pos = [&](int kb) { return ldv(bs + kb * PULSE_BODY_STATE_W); };
+      store_amp_row(a.amp_obs_buf + e * a.num_amp_steps * a.amp_width, a.amp_width, stage, lane, ldv(bs), ldq(bs + 3), ldv(bs + 7), ldv(bs + 10),
+                    upright, joint, key_pos);
+    }
   }
 }
 

@@ -33,7 +33,7 @@ __global__ void __launch_bounds__(kResetWarps * 32) terrain_reset_kernel(const p
     p.x = __fadd_rn(p.x, dx);
     p.y = __fadd_rn(p.y, dy);
   };
-  reset_warps(lib, a, s.loc_ids_in == nullptr, stage_all[threadIdx.x >> 5], spawn);
+  reset_warps<SmplLayout>(lib, a, s.loc_ids_in == nullptr, stage_all[threadIdx.x >> 5], spawn);
 }
 
 }  // namespace

@@ -1,5 +1,5 @@
-// One env of the latent-space tasks' post-physics step (reach; speed / strike), one warp per env, lane = body: self observation, task
-// observation, reward and reset.  Shared by the step and list-observation kernels (ztask_step.cu) and by the rollout step kernels that
+// One env of the latent-space tasks' post-physics step (reach; speed / strike; the SMPL-X speed task), one warp per env, lane = body:
+// self observation, task observation, reward and reset.  Shared by the step and list-observation kernels (ztask_step.cu) and by the rollout step kernels that
 // write into experience-buffer slices (ztask_rollout.cu), so all of them produce the same rows bit for bit.
 #pragma once
 #include "humanoid_obs.cuh"
@@ -54,39 +54,74 @@ __device__ __forceinline__ void reach_env(const pulse_reach_step_args_t& a, long
   }
 }
 
-// One env of the speed / strike step.  kObsOnly: the observation alone.
-template <bool kObsOnly>
-__device__ __forceinline__ void ztask_env(const pulse_ztask_step_args_t& a, long long e, int lane) {
-  const int j = lane;
-  const bool body = j < PULSE_NUM_BODIES;
-  const float* bs = a.body_state + e * a.body_env_stride + (body ? j : 0) * 13;
-  const Vec3 p = {bs[0], bs[1], bs[2]}, v = {bs[7], bs[8], bs[9]}, w = {bs[10], bs[11], bs[12]};
-  const Quat q = {bs[3], bs[4], bs[5], bs[6]};
-  const Vec3 p_root = {__shfl_sync(kFull, p.x, 0), __shfl_sync(kFull, p.y, 0), __shfl_sync(kFull, p.z, 0)};
-  const Quat q_root = {__shfl_sync(kFull, q.x, 0), __shfl_sync(kFull, q.y, 0), __shfl_sync(kFull, q.z, 0), __shfl_sync(kFull, q.w, 0)};
+// One env of the speed / strike step in body layout L (SmplLayout: speed and strike; SmplxLayout: speed).  kObsOnly: the observation
+// alone.  Lane l holds bodies l and l + 32 (the second only where the layout has more than 32 bodies).
+template <class L>
+__device__ __forceinline__ bool ztask_is_speed(const typename L::StepArgs& a) {
+  if constexpr (L::kSmplTerms) return a.kind == PULSE_ZTASK_SPEED;
+  else return true;
+}
+
+template <class L, bool kObsOnly>
+__device__ __forceinline__ void ztask_env(const typename L::StepArgs& a, long long e, int lane) {
+  constexpr int kSlots = (L::kBodies + 31) / 32;
+  Vec3 p[kSlots], v[kSlots], w[kSlots];
+  Quat q[kSlots];
+#pragma unroll
+  for (int s = 0; s < kSlots; ++s) {
+    const int j = lane + 32 * s;
+    const float* bs = a.body_state + e * a.body_env_stride + (j < L::kBodies ? j : 0) * 13;
+    p[s] = {bs[0], bs[1], bs[2]};
+    v[s] = {bs[7], bs[8], bs[9]};
+    w[s] = {bs[10], bs[11], bs[12]};
+    q[s] = {bs[3], bs[4], bs[5], bs[6]};
+  }
+  const Vec3 p_root = {__shfl_sync(kFull, p[0].x, 0), __shfl_sync(kFull, p[0].y, 0), __shfl_sync(kFull, p[0].z, 0)};
+  const Quat q_root = {__shfl_sync(kFull, q[0].x, 0), __shfl_sync(kFull, q[0].y, 0), __shfl_sync(kFull, q[0].z, 0), __shfl_sync(kFull, q[0].w, 0)};
   float hs, hc;
   heading_half(q_root, hs, hc);
   const Yaw yr = make_yaw(Quat{0.0f, 0.0f, -hs, hc});
-  float* o = a.obs_buf + e * a.obs_stride;
-  if (body) store_self_obs(o, j, p, p_root, q, v, w, hs, hc, yr);
-  const FallFlags fall = fall_flags(a, e, j, body, p.z);
-  // strike: a body that is neither a ground-contact body nor a strike body pressing harder than 50 N (humanoid_strike.py:356-364)
-  bool hard_contact = false;
-  if (a.enable_early_termination && body && a.contact_forces != nullptr && !(((a.contact_body_mask | a.strike_body_mask) >> j) & 1u)) {
-    const float* cf = a.contact_forces + e * a.contact_env_stride + j * 3;
-    hard_contact = fabsf(cf[0]) > 50.0f || fabsf(cf[1]) > 50.0f || fabsf(cf[2]) > 50.0f;
+  // the self observation's heading: the root's own (upright start) or that of remove_base_rot(root) (humanoid.py:1682-1684); the
+  // task observation below keeps the root's own either way (compute_speed_observations reads the raw root rotation)
+  float shs = hs, shc = hc;
+  Yaw syr = yr;
+  if constexpr (!L::kUpright) {
+    heading_half(base_rot_removed(q_root, false), shs, shc);
+    syr = make_yaw(Quat{0.0f, 0.0f, -shs, shc});
   }
-  const bool any_contact = __any_sync(kFull, fall.contact), any_height = __any_sync(kFull, fall.height);
-  const bool any_hard = __any_sync(kFull, hard_contact);
-  // power term of the speed task: -c * sum |tau * qdot|, zero for progress <= 3 (humanoid_speed.py:215-222)
-  const float power = a.kind == PULSE_ZTASK_SPEED && a.dof_force != nullptr ? dof_power(a, e, lane) : 0.0f;
+  float* o = a.obs_buf + e * a.obs_stride;
+  bool contact = false, height = false, hard_contact = false;
+#pragma unroll
+  for (int s = 0; s < kSlots; ++s) {
+    const int j = lane + 32 * s;
+    const bool body = j < L::kBodies;
+    if (body) store_self_obs<L::kBodies>(o, j, p[s], p_root, q[s], v[s], w[s], shs, shc, syr);
+    const FallFlags fall = fall_flags(a, e, j, body, p[s].z);
+    contact = contact || fall.contact;
+    height = height || fall.height;
+    if constexpr (L::kSmplTerms) {
+      // strike: a body that is neither a ground-contact body nor a strike body pressing harder than 50 N (humanoid_strike.py:356-364)
+      if (a.enable_early_termination && body && a.contact_forces != nullptr && !(((a.contact_body_mask | a.strike_body_mask) >> j) & 1u)) {
+        const float* cf = a.contact_forces + e * a.contact_env_stride + j * 3;
+        hard_contact = hard_contact || fabsf(cf[0]) > 50.0f || fabsf(cf[1]) > 50.0f || fabsf(cf[2]) > 50.0f;
+      }
+    }
+  }
+  const bool any_contact = __any_sync(kFull, contact), any_height = __any_sync(kFull, height);
+  bool any_hard = false;
+  float power = 0.0f;
+  if constexpr (L::kSmplTerms) {
+    any_hard = __any_sync(kFull, hard_contact);
+    // power term of the speed task: -c * sum |tau * qdot|, zero for progress <= 3 (humanoid_speed.py:215-222)
+    power = a.kind == PULSE_ZTASK_SPEED && a.dof_force != nullptr ? dof_power(a, e, lane) : 0.0f;
+  }
   if (lane == 0) {
     const long long prog = a.progress_buf[e];
     const float* pr = a.prev_root_pos + 3 * e;
     const float vx = (p_root.x - pr[0]) / a.dt, vy = (p_root.y - pr[1]) / a.dt;   // root_vel = delta_root_pos / dt
-    float* t = o + PULSE_SELF_OBS;
+    float* t = o + L::kSelfObs;
     bool failed = any_contact && any_height;
-    if (a.kind == PULSE_ZTASK_SPEED) {
+    if (ztask_is_speed<L>(a)) {
       // observation: heading-frame x axis (first two components) and the target speed (:310-325)
       const Vec3 d = yaw_rot(yr, Vec3{1.0f, 0.0f, 0.0f});
       const float ts = a.tar_speed[e];
@@ -95,13 +130,15 @@ __device__ __forceinline__ void ztask_env(const pulse_ztask_step_args_t& a, long
       const float err = ts - vx;
       float rew = expf(-0.25f * (err * err + 0.1f * vy * vy));                    // :327-343
       if (a.reward_raw != nullptr) a.reward_raw[e * a.raw_stride] = rew;
-      if (a.dof_force != nullptr) {
-        const float pw = prog <= 3 ? 0.0f : -a.power_coefficient * power;
-        rew += pw;
-        if (a.reward_raw != nullptr) a.reward_raw[e * a.raw_stride + 1] = pw;
+      if constexpr (L::kSmplTerms) {
+        if (a.dof_force != nullptr) {
+          const float pw = prog <= 3 ? 0.0f : -a.power_coefficient * power;
+          rew += pw;
+          if (a.reward_raw != nullptr) a.reward_raw[e * a.raw_stride + 1] = pw;
+        }
       }
       a.rew_buf[e] = rew;
-    } else {
+    } else if constexpr (L::kSmplTerms) {
       const float* ts = a.target_states + e * a.target_env_stride;
       const Vec3 tp = {ts[0], ts[1], ts[2]};
       const Quat tq = {ts[3], ts[4], ts[5], ts[6]};

@@ -5,6 +5,7 @@
 //                         gather, SMPL ground fix, _set_env_state, counters, AMP rows) with the task's pose adjustment and the strike
 //                         target;
 //   ztask_task_kernel     (pulse_ztask_reset_task) the reach / speed _reset_task over the same list, after the observation.
+// pulse_reset_ztask_smplx runs the first two for the SMPL-X speed task: ztask_reset_kernel<SmplxLayout>, without AMP rows or target.
 // The entry points, argument structs and Philox word layout are documented in include/pulse_b200.h.
 #include "reset_warps.cuh"
 
@@ -14,8 +15,9 @@ namespace {
 constexpr unsigned long long kStrikeStream = 1ull << 32;   // Philox index e + 2^32: strike bearing / yaw
 constexpr unsigned long long kTaskStream = 2ull << 32;     // Philox index e + 2^33: _reset_task draws
 
-__global__ void __launch_bounds__(kResetWarps * 32) ztask_reset_kernel(const pulse_motionlib_desc_t lib, const pulse_ztask_reset_args_t a) {
-  __shared__ float stage_all[kResetWarps][PULSE_AMP_OBS];
+template <class L, class Lib>
+__global__ void __launch_bounds__(kResetWarps * 32) ztask_reset_kernel(const Lib lib, const pulse_ztask_reset_args_t a) {
+  __shared__ float stage_all[kResetWarps][L::kSmplTerms ? PULSE_AMP_OBS : 1];
   const bool upright = a.upright != 0;
   const auto adjust = [&](long long e, int lane, const Philox4& r0, unsigned long long off, Vec3& p, Quat& rq, Vec3& v, Vec3& rp, Quat& rr,
                           Vec3& rv, Vec3& rw) {
@@ -51,7 +53,7 @@ __global__ void __launch_bounds__(kResetWarps * 32) ztask_reset_kernel(const pul
       for (int c = 7; c < 13; ++c) ts[c] = 0.0f;
     }
   };
-  reset_warps(lib, a, a.target_states != nullptr && a.strike_u == nullptr, stage_all[threadIdx.x >> 5], adjust);
+  reset_warps<L>(lib, a, a.target_states != nullptr && a.strike_u == nullptr, stage_all[threadIdx.x >> 5], adjust);
 }
 
 __global__ void __launch_bounds__(256) ztask_task_kernel(const pulse_ztask_task_args_t a) {
@@ -110,7 +112,7 @@ extern "C" int pulse_reset_ztask(const pulse_motionlib_t* lib, const pulse_ztask
   reset_compact_kernel<<<1, kCompactThreads, 0, st>>>(a, (long long)num_envs);
   PULSE_LAUNCH_OK("reset_compact_kernel");
   const long long upper = (a.env_ids_in != nullptr ? a.num_ids : num_envs) * (a.amp_obs_buf != nullptr ? a.num_amp_steps : 1);
-  ztask_reset_kernel<<<grid_for(upper, kResetWarps), kResetWarps * 32, 0, st>>>(lib->d, a);
+  ztask_reset_kernel<SmplLayout><<<grid_for(upper, kResetWarps), kResetWarps * 32, 0, st>>>(lib->d, a);
   PULSE_LAUNCH_OK("ztask_reset_kernel");
   return PULSE_OK;
 }
@@ -129,5 +131,37 @@ extern "C" int pulse_ztask_reset_task(const pulse_ztask_task_args_t* args, int64
   if (num_envs == 0) return PULSE_OK;
   ztask_task_kernel<<<grid_for(num_envs, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
   PULSE_LAUNCH_OK("ztask_task_kernel");
+  return PULSE_OK;
+}
+
+extern "C" int pulse_reset_ztask_smplx(const pulse_smplx_motionlib_t* lib, const pulse_ztask_reset_args_t* args, int64_t num_envs, void* stream) {
+  using namespace pulse;
+  PULSE_REQUIRE(lib != nullptr && args != nullptr, "pulse_reset_ztask_smplx: null lib/args");
+  const pulse_ztask_reset_args_t& a = *args;
+  PULSE_REQUIRE(num_envs >= 0 && num_envs < (1ll << 31), "pulse_reset_ztask_smplx: num_envs %lld outside [0, 2^31)", (long long)num_envs);
+  PULSE_REQUIRE(a.reset_buf != nullptr || a.env_ids_in != nullptr, "pulse_reset_ztask_smplx: neither a reset mask nor an env id list");
+  PULSE_REQUIRE(a.env_ids_in == nullptr || (a.num_ids >= 0 && a.num_ids <= num_envs), "pulse_reset_ztask_smplx: num_ids %lld outside [0, %lld]",
+                (long long)a.num_ids, (long long)num_envs);
+  PULSE_REQUIRE(a.env_list != nullptr && a.count != nullptr, "pulse_reset_ztask_smplx: env_list / count outputs are required");
+  PULSE_REQUIRE(a.sampled_motion_ids && a.motion_start_times && a.progress_buf, "pulse_reset_ztask_smplx: null task buffer");
+  PULSE_REQUIRE(a.root_states && a.dof_pos && a.dof_vel && a.rigid_body_state, "pulse_reset_ztask_smplx: null simulator tensor");
+  PULSE_REQUIRE(a.root_env_stride >= PULSE_BODY_STATE_W && a.dof_elem_stride >= 1 && a.dof_env_stride >= PULSE_SMPLX_DOF * a.dof_elem_stride &&
+                a.body_env_stride >= PULSE_SMPLX_BODIES * PULSE_BODY_STATE_W, "pulse_reset_ztask_smplx: bad root / dof / rigid-body strides");
+  PULSE_REQUIRE(a.contact_forces == nullptr || (a.contact_bodies >= 0 && a.contact_env_stride >= 3 * a.contact_bodies),
+                "pulse_reset_ztask_smplx: bad contact-force strides");
+  PULSE_REQUIRE(a.amp_obs_buf == nullptr, "pulse_reset_ztask_smplx: the AMP history back-fill is not served for SMPL-X (amp_obs_buf must be NULL)");
+  PULSE_REQUIRE(a.target_states == nullptr, "pulse_reset_ztask_smplx: the SMPL-X reset serves the speed task (target_states must be NULL)");
+  PULSE_REQUIRE(a.pose_mode == PULSE_ZPOSE_FACE_X, "pulse_reset_ztask_smplx: pose_mode %d, the speed task's is PULSE_ZPOSE_FACE_X", a.pose_mode);
+  PULSE_REQUIRE(a.floor != nullptr && a.floor_len >= lib->d.total_frames, "pulse_reset_ztask_smplx: floor table of %lld frames, the MotionLib has %lld",
+                (long long)a.floor_len, (long long)lib->d.total_frames);
+  PULSE_REQUIRE(a.motion_ids_in != nullptr || a.sampling_cdf != nullptr, "pulse_reset_ztask_smplx: null sampling_cdf (needed to draw the clips)");
+  PULSE_REQUIRE(a.state_init == PULSE_ZINIT_RANDOM || a.state_init == PULSE_ZINIT_START, "pulse_reset_ztask_smplx: unknown state_init %d", a.state_init);
+  if (num_envs == 0) return PULSE_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  reset_compact_kernel<<<1, kCompactThreads, 0, st>>>(a, (long long)num_envs);
+  PULSE_LAUNCH_OK("reset_compact_kernel");
+  const long long upper = a.env_ids_in != nullptr ? a.num_ids : num_envs;
+  ztask_reset_kernel<SmplxLayout><<<grid_for(upper, kResetWarps), kResetWarps * 32, 0, st>>>(lib->d, a);
+  PULSE_LAUNCH_OK("ztask_reset_kernel<SmplxLayout>");
   return PULSE_OK;
 }

@@ -5,7 +5,8 @@
 //   ztask_pre_physics_kernel  PD targets from the decoder output, prev_root_pos, and _update_task of the due envs with draws injected or
 //                             made here (Philox index plane e + 3 * 2^32);
 //   reach_rollout_kernel /    progress_buf += 1, then the per-env step code of ztask_env.cuh into the next step's observation slice and
-//   ztask_rollout_kernel      the step's reward row, then dones = float(reset).
+//   ztask_rollout_kernel      the step's reward row, then dones = float(reset); ztask_rollout_kernel<SmplxLayout> is the SMPL-X
+//                             speed task's (pulse_smplx_speed_rollout_step).
 // The entry points, argument structs and the Philox word layout are documented in include/pulse_b200.h.
 #include <cuda_bf16.h>
 
@@ -101,12 +102,13 @@ __global__ void __launch_bounds__(256) reach_rollout_kernel(const pulse_reach_st
   }
 }
 
-__global__ void __launch_bounds__(256) ztask_rollout_kernel(const pulse_ztask_step_args_t a, float* __restrict__ dones, long long n) {
+template <class L>
+__global__ void __launch_bounds__(256) ztask_rollout_kernel(const typename L::StepArgs a, float* __restrict__ dones, long long n) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   long long* progress = const_cast<long long*>(reinterpret_cast<const long long*>(a.progress_buf));
   for (long long e = blockIdx.x * 8ll + warp; e < n; e += 8ll * gridDim.x) {
     if (lane == 0) progress[e] += 1;
-    ztask_env<false>(a, e, lane);
+    ztask_env<L, false>(a, e, lane);
     if (lane == 0) dones[e] = static_cast<float>(a.reset_buf[e]);
   }
 }
@@ -193,7 +195,22 @@ extern "C" int pulse_ztask_rollout_step(const pulse_ztask_step_args_t* args, flo
     PULSE_REQUIRE(a.target_states && a.tar_contact_forces, "pulse_ztask_rollout_step: strike task needs target_states and tar_contact_forces");
     PULSE_REQUIRE(a.obs_stride >= PULSE_STRIKE_OBS, "pulse_ztask_rollout_step: obs_stride %lld < %d", (long long)a.obs_stride, PULSE_STRIKE_OBS);
   }
-  ztask_rollout_kernel<<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, dones, (long long)num_envs);
+  ztask_rollout_kernel<SmplLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, dones, (long long)num_envs);
   PULSE_LAUNCH_OK("ztask_rollout_kernel");
+  return PULSE_OK;
+}
+
+namespace pulse {
+int check_smplx_speed_args(const pulse_smplx_speed_step_args_t* args, bool step, const char* who);   // ztask_step.cu
+}  // namespace pulse
+
+extern "C" int pulse_smplx_speed_rollout_step(const pulse_smplx_speed_step_args_t* args, float* dones, int64_t num_envs, void* stream) {
+  using namespace pulse;
+  const int st = check_smplx_speed_args(args, true, "pulse_smplx_speed_rollout_step");
+  if (st != PULSE_OK) return st;
+  PULSE_REQUIRE(dones != nullptr, "pulse_smplx_speed_rollout_step: null dones");
+  PULSE_REQUIRE(num_envs > 0, "pulse_smplx_speed_rollout_step: num_envs must be positive");
+  ztask_rollout_kernel<SmplxLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(*args, dones, (long long)num_envs);
+  PULSE_LAUNCH_OK("ztask_rollout_kernel<SmplxLayout>");
   return PULSE_OK;
 }

@@ -6,6 +6,8 @@
 //           reset = compute_humanoid_reset
 //   strike  compute_strike_observations / compute_strike_reward  phc/env/tasks/humanoid_strike.py:270-328,
 //           reset = the strike variant of compute_humanoid_reset  :330-375
+//   smplx speed  the speed step above for the 52-body SMPL-X humanoid (env_pulsex_amp.yaml): the same per-env code instantiated for
+//           SmplxLayout, the self observation in the heading of remove_base_rot(root) (has_upright_start False)
 // The per-env device code is ztask_env.cuh's, shared with the rollout step kernels of ztask_rollout.cu.
 #include "ztask_env.cuh"
 
@@ -38,16 +40,18 @@ __global__ void __launch_bounds__(256) reach_obs_list_kernel(const pulse_reach_s
   for (long long i = blockIdx.x * 8ll + warp; i < n; i += 8ll * gridDim.x) reach_env<true>(a, env_list[i], lane);
 }
 
-__global__ void __launch_bounds__(256) ztask_step_kernel(const pulse_ztask_step_args_t a, long long n) {
+template <class L>
+__global__ void __launch_bounds__(256) ztask_step_kernel(const typename L::StepArgs a, long long n) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (long long e = blockIdx.x * 8ll + warp; e < n; e += 8ll * gridDim.x) ztask_env<false>(a, e, lane);
+  for (long long e = blockIdx.x * 8ll + warp; e < n; e += 8ll * gridDim.x) ztask_env<L, false>(a, e, lane);
 }
 
-__global__ void __launch_bounds__(256) ztask_obs_list_kernel(const pulse_ztask_step_args_t a, const long long* __restrict__ env_list,
+template <class L>
+__global__ void __launch_bounds__(256) ztask_obs_list_kernel(const typename L::StepArgs a, const long long* __restrict__ env_list,
                                                              const int* __restrict__ count) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const long long n = *count;
-  for (long long i = blockIdx.x * 8ll + warp; i < n; i += 8ll * gridDim.x) ztask_env<true>(a, env_list[i], lane);
+  for (long long i = blockIdx.x * 8ll + warp; i < n; i += 8ll * gridDim.x) ztask_env<L, true>(a, env_list[i], lane);
 }
 
 }  // namespace
@@ -74,7 +78,7 @@ extern "C" int pulse_ztask_step(const pulse_ztask_step_args_t* args, int64_t num
     PULSE_REQUIRE(a.target_states && a.tar_contact_forces, "pulse_ztask_step: strike task needs target_states and tar_contact_forces");
     PULSE_REQUIRE(a.obs_stride >= PULSE_STRIKE_OBS, "pulse_ztask_step: obs_stride %lld < %d", (long long)a.obs_stride, PULSE_STRIKE_OBS);
   }
-  ztask_step_kernel<<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, (long long)num_envs);
+  ztask_step_kernel<SmplLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, (long long)num_envs);
   PULSE_LAUNCH_OK("ztask_step_kernel");
   return PULSE_OK;
 }
@@ -131,7 +135,50 @@ extern "C" int pulse_ztask_obs_list(const pulse_ztask_step_args_t* args, const i
   PULSE_REQUIRE(a.kind != PULSE_ZTASK_STRIKE || (a.target_states && a.target_env_stride >= 13 && a.obs_stride >= PULSE_STRIKE_OBS),
                 "pulse_ztask_obs_list: strike needs target_states, obs_stride >= 373");
   if (num_envs == 0) return PULSE_OK;
-  ztask_obs_list_kernel<<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, reinterpret_cast<const long long*>(env_list), count);
+  ztask_obs_list_kernel<SmplLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, reinterpret_cast<const long long*>(env_list), count);
   PULSE_LAUNCH_OK("ztask_obs_list_kernel");
+  return PULSE_OK;
+}
+
+namespace pulse {
+// The checks of the SMPL-X speed step's arguments shared by its three entry points (`who` prefixes the messages).
+int check_smplx_speed_args(const pulse_smplx_speed_step_args_t* args, bool step, const char* who) {
+  PULSE_REQUIRE(args != nullptr, "%s: null args", who);
+  const pulse_smplx_speed_step_args_t& a = *args;
+  PULSE_REQUIRE(a.body_state && a.obs_buf && a.tar_speed, "%s: null body_state / obs_buf / tar_speed", who);
+  PULSE_REQUIRE(a.body_env_stride >= PULSE_SMPLX_BODIES * PULSE_BODY_STATE_W, "%s: body_env_stride %lld < %d", who,
+                (long long)a.body_env_stride, PULSE_SMPLX_BODIES * PULSE_BODY_STATE_W);
+  PULSE_REQUIRE(a.obs_stride >= PULSE_SMPLX_SPEED_OBS, "%s: obs_stride %lld < %d", who, (long long)a.obs_stride, PULSE_SMPLX_SPEED_OBS);
+  if (!step) return PULSE_OK;
+  PULSE_REQUIRE(a.progress_buf && a.prev_root_pos && a.rew_buf && a.reset_buf && a.terminate_buf, "%s: null buffer", who);
+  PULSE_REQUIRE(a.dt > 0.0f, "%s: dt must be positive", who);
+  PULSE_REQUIRE(!a.enable_early_termination || a.termination_heights != nullptr, "%s: termination_heights required", who);
+  PULSE_REQUIRE(a.contact_forces == nullptr || a.contact_env_stride >= PULSE_SMPLX_BODIES * 3, "%s: contact_env_stride %lld < %d", who,
+                (long long)a.contact_env_stride, PULSE_SMPLX_BODIES * 3);
+  PULSE_REQUIRE(a.reward_raw == nullptr || a.raw_stride >= 1, "%s: raw_stride too small", who);
+  return PULSE_OK;
+}
+}  // namespace pulse
+
+extern "C" int pulse_smplx_speed_step(const pulse_smplx_speed_step_args_t* args, int64_t num_envs, void* stream) {
+  using namespace pulse;
+  const int st = check_smplx_speed_args(args, true, "pulse_smplx_speed_step");
+  if (st != PULSE_OK) return st;
+  PULSE_REQUIRE(num_envs > 0, "pulse_smplx_speed_step: num_envs must be positive");
+  ztask_step_kernel<SmplxLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(*args, (long long)num_envs);
+  PULSE_LAUNCH_OK("ztask_step_kernel<SmplxLayout>");
+  return PULSE_OK;
+}
+
+extern "C" int pulse_smplx_speed_obs_list(const pulse_smplx_speed_step_args_t* args, const int64_t* env_list, const int32_t* count,
+                                          int64_t num_envs, void* stream) {
+  using namespace pulse;
+  const int st = check_smplx_speed_args(args, false, "pulse_smplx_speed_obs_list");
+  if (st != PULSE_OK) return st;
+  PULSE_REQUIRE(env_list && count && num_envs >= 0, "pulse_smplx_speed_obs_list: null env_list / count or negative num_envs");
+  if (num_envs == 0) return PULSE_OK;
+  ztask_obs_list_kernel<SmplxLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      *args, reinterpret_cast<const long long*>(env_list), count);
+  PULSE_LAUNCH_OK("ztask_obs_list_kernel<SmplxLayout>");
   return PULSE_OK;
 }

@@ -68,6 +68,8 @@ def _strided(t: torch.Tensor, inner: int):
 
 class HumanoidImCompute:
     def __init__(self, motion_lib: MotionLibB200, cfg: Optional[ImConfig] = None):
+        if getattr(motion_lib, "smplx", False):
+            raise _lib.PulseError("HumanoidImCompute serves the 24-body SMPL humanoid; the MotionLib holds 52-body SMPL-X tables")
         self.lib = _lib.load()
         self.motion_lib = motion_lib
         self.cfg = cfg or ImConfig()

@@ -16,17 +16,18 @@ class LatentStepsB200(GraphRunner):
          `_reset(t)`           the reset of the done envs (Philox draws keyed (reset_seed, env, t + the policy's device offset)), which
                                leaves the reset's workspace {'env_list', 'count', ...} in `reset_ws`;
          `_reset_obs(t)`       the observation of the reset envs into obses[:, t], then the task's `_reset_task`;
-         `_pre_physics(dec, t)` what the step does with the decoder output `dec` [n, 69] before the physics (PD targets into pd_tar, ...);
+         `_pre_physics(dec, t)` what the step does with the decoder output `dec` [n, A] before the physics (PD targets into pd_tar, ...);
          `_env_step(t)`        the rollout step kernel (progress += 1, reward, reset, next observation) into obses[:, t+1] / obs_carry,
                                rewards[t], dones[t], reset_buf, terminate_buf;
          `first_observation()` the observation of the initial state into obs_carry.
     For every step t, in the reference's order: `_reset(t)`, the `refresh(t, ws)` hook if set, `_reset_obs(t)`; `get_action_values`
-    (the policy's `heads_into`, actor beside critic, and beside both the frozen prior MLP on obses[:, t, :358] with the clamped self
+    (the policy's `heads_into`, actor beside critic, and beside both the frozen prior MLP on obses[:, t, :S] with the clamped self
     observation columns of the decoder operand: neither depends on the action); `pulse_latent_post` (a_z = mu + exp(logstd) eps into
     actions[:, t], neglogp[:, t], the de-normalised value into values[t] and z = prior_mu + a_z into the decoder operand; the latent
     tasks' configs have clip_actions False and `project_to_norm(.., "none")` is the identity, so a_z is neither clamped nor projected);
     the decoder MLP on [clamp(norm(s), +-5) | z] (HumanoidZ.compute_z_actions); `_pre_physics`; the caller's `physics(t)` hook;
     `_env_step(t)`; next_values[t] = critic(obses[:, t+1]) (1 - terminate) on the critic's second operand slot.
+    S and A are the VAE's self-observation width and dof count (358 and 69 for SMPL, 778 and 153 for SMPL-X), E its latent size.
     `finish()` then computes GAE, normalised advantages and value-normalised returns from the task reward alone (task_reward_w 1,
     disc_reward_w 0) and `train_epoch()` runs the PPO update.
 
@@ -76,7 +77,7 @@ class LatentStepsB200(GraphRunner):
         self.physics: Optional[Callable[[int], None]] = None           # physics(t): between the pre-physics work and the step kernel
         self.refresh: Optional[Callable[[int, dict], None]] = None     # refresh(t, ws): after the reset, before the reset envs' observation
         self.reset_ws = None
-        self.z_actions = None          # the decoder's output of the last step, fp32 [n, 69] (a reused workspace)
+        self.z_actions = None          # the decoder's output of the last step, fp32 [n, A] (a reused workspace)
         self._streams = None
 
     # ------------------------------------------------------------------ the task's pieces (subclass)

@@ -11,6 +11,10 @@ The clip loader (load_motions: FK, heading randomisation, velocity filters) stay
 reference for now (SURVEY.md 8f-1): build this object from the tables it produced with
 `MotionLibB200.from_reference(motion_lib)` or from raw tables with `from_tables(...)`.  `from_clips(...)` is the
 device-side loader (SURVEY 8f-1): parity green against the reference's tables (tests/test_gpu_loader.py).
+
+The tables' body count chooses the humanoid: 24 bodies is SMPL, 52 the SMPL-X humanoid of PULSE-X (smplx_humanoid.xml, 153 dofs),
+whose records (PULSE_SMPLX_FRAME_REC / PULSE_SMPLX_AUX_REC) and queries are the `pulse_smplx_*` entry points.  `from_reference` adopts a
+loaded SMPL-X MotionLib as it adopts an SMPL one; `from_clips` (the forward-kinematics loader) is SMPL only.
 """
 import ctypes as C
 from typing import Dict, Optional
@@ -21,6 +25,7 @@ from . import _lib
 
 FRAME_REC = 312
 AUX_REC = 240
+SMPLX_FRAME_REC, SMPLX_AUX_REC = 676, 364
 _TABLE_KEYS = ("gts", "grs", "lrs", "gvs", "gavs", "dvs")
 
 
@@ -37,10 +42,13 @@ class MotionLibB200:
         i64 = lambda x: x.to(dev, torch.int64).contiguous()
         self.gts, self.grs, self.lrs = f32(tables["gts"]), f32(tables["grs"]), f32(tables["lrs"])
         self.gvs, self.gavs, self.dvs = f32(tables["gvs"]), f32(tables["gavs"]), f32(tables["dvs"])
-        F = self.gts.shape[0]
-        if self.gts.shape[1:] != (24, 3) or self.grs.shape != (F, 24, 4) or self.dvs.shape != (F, 23, 3):
-            raise _lib.PulseError(f"unexpected table shapes {tuple(self.gts.shape)} {tuple(self.grs.shape)} {tuple(self.dvs.shape)}")
-        self._motion_aa = f32(tables["motion_aa"]) if tables.get("motion_aa") is not None else torch.zeros(F, 72, device=dev)
+        F, B = self.gts.shape[0], self.gts.shape[1]
+        if (B not in (24, _lib.SMPLX_BODIES) or self.gts.shape[2:] != (3,) or self.grs.shape != (F, B, 4) or self.lrs.shape != (F, B, 4)
+                or self.dvs.shape != (F, B - 1, 3)):
+            raise _lib.PulseError(f"unexpected table shapes {tuple(self.gts.shape)} {tuple(self.grs.shape)} {tuple(self.dvs.shape)}: "
+                                  "24 (SMPL) or 52 (SMPL-X) bodies")
+        self.smplx = B == _lib.SMPLX_BODIES
+        self._motion_aa = f32(tables["motion_aa"]) if tables.get("motion_aa") is not None else torch.zeros(F, 3 * B, device=dev)
         self._motion_lengths = f32(tables["lengths"])
         self._motion_num_frames = i64(tables["num_frames"])
         self._motion_dt = f32(tables["dt"])
@@ -51,11 +59,17 @@ class MotionLibB200:
         self._motion_limb_weights = (f32(tables["motion_limb_weights"]) if tables.get("motion_limb_weights") is not None
                                      else torch.zeros(M, 10, device=dev))
         self._num_motions = M
-        self.num_bodies = 24
+        self.num_bodies = B
         self.motion_ids = torch.arange(M, dtype=torch.long, device=dev)
         self._sampling_batch_prob = torch.full((M,), 1.0 / M, device=dev)
         self._time_step = torch.tensor(1 / 30, dtype=torch.float32, device=dev)  # cached: no H2D copy inside CUDA-graph capture
 
+        handle = C.c_void_p()
+        self._lib = lib
+        if self.smplx:
+            self._pack_smplx(F, M, handle)
+            self._handle = handle
+            return
         # packed records (layout: include/pulse_b200.h PULSE_FRAME_REC / PULSE_AUX_REC)
         self.frame_rec = torch.empty(F, FRAME_REC, device=dev, dtype=torch.float32)
         self.aux_rec = torch.empty(F, AUX_REC, device=dev, dtype=torch.float32)
@@ -65,11 +79,23 @@ class MotionLibB200:
             lengths=self._motion_lengths.data_ptr(), dt=self._motion_dt.data_ptr(),
             num_frames=self._motion_num_frames.data_ptr(), length_starts=self.length_starts.data_ptr(),
             total_frames=F, num_motions=M, frame_rec=self.frame_rec.data_ptr(), aux_rec=self.aux_rec.data_ptr())
-        handle = C.c_void_p()
         with torch.cuda.device(dev):
             _lib.check(lib.pulse_motionlib_create(C.byref(desc), _lib.current_stream(dev), C.byref(handle)), "pulse_motionlib_create")
         self._handle = handle
-        self._lib = lib
+
+    def _pack_smplx(self, F: int, M: int, handle) -> None:
+        """The SMPL-X records (layout: include/pulse_b200.h PULSE_SMPLX_FRAME_REC / PULSE_SMPLX_AUX_REC) and their handle."""
+        dev = self._device
+        self.frame_rec = torch.empty(F, SMPLX_FRAME_REC, device=dev, dtype=torch.float32)
+        self.aux_rec = torch.empty(F, SMPLX_AUX_REC, device=dev, dtype=torch.float32)
+        desc = _lib.SmplxMotionLibDesc(
+            gts=self.gts.data_ptr(), grs=self.grs.data_ptr(), lrs=self.lrs.data_ptr(), gvs=self.gvs.data_ptr(), gavs=self.gavs.data_ptr(),
+            dvs=self.dvs.data_ptr(), lengths=self._motion_lengths.data_ptr(), dt=self._motion_dt.data_ptr(),
+            num_frames=self._motion_num_frames.data_ptr(), length_starts=self.length_starts.data_ptr(), total_frames=F, num_motions=M,
+            frame_rec=self.frame_rec.data_ptr(), aux_rec=self.aux_rec.data_ptr())
+        with torch.cuda.device(dev):
+            _lib.check(self._lib.pulse_smplx_motionlib_create(C.byref(desc), _lib.current_stream(dev), C.byref(handle)),
+                       "pulse_smplx_motionlib_create")
 
     # ------------------------------------------------------------------ constructors
     @classmethod
@@ -78,7 +104,7 @@ class MotionLibB200:
 
     @classmethod
     def from_reference(cls, ref_lib, device=None):
-        """Adopt the tables a loaded reference MotionLibSMPL holds (after load_motions)."""
+        """Adopt the tables a loaded reference MotionLibSMPL holds (after load_motions), SMPL or SMPL-X."""
         t = {k: getattr(ref_lib, k) for k in _TABLE_KEYS}
         t.update(motion_aa=ref_lib._motion_aa, lengths=ref_lib._motion_lengths, num_frames=ref_lib._motion_num_frames,
                  dt=ref_lib._motion_dt, length_starts=ref_lib.length_starts, fps=ref_lib._motion_fps,
@@ -126,11 +152,22 @@ class MotionLibB200:
     def __del__(self):
         h = getattr(self, "_handle", None)
         if h is not None and h.value:
-            self._lib.pulse_motionlib_destroy(h)
+            (self._lib.pulse_smplx_motionlib_destroy if self.smplx else self._lib.pulse_motionlib_destroy)(h)
             self._handle = None
 
     @property
     def handle(self):
+        """The SMPL handle (`pulse_motionlib_t*`) every SMPL entry point takes; refused for SMPL-X tables, whose handle is another type."""
+        if self.smplx:
+            raise _lib.PulseError("this MotionLibB200 holds 52-body SMPL-X tables: the SMPL entry points cannot take it (smplx_handle is its "
+                                  "handle, for the PULSE-X speed task's reset)")
+        return self._handle
+
+    @property
+    def smplx_handle(self):
+        """The SMPL-X handle (`pulse_smplx_motionlib_t*`) of 52-body tables; refused for SMPL tables."""
+        if not self.smplx:
+            raise _lib.PulseError("this MotionLibB200 holds 24-body SMPL tables: it has no SMPL-X handle")
         return self._handle
 
     # ------------------------------------------------------------------ reference API
@@ -188,6 +225,8 @@ class MotionLibB200:
         times = motion_times.to(dev, torch.float32).contiguous()
         off = offset.to(dev, torch.float32).contiguous() if offset is not None else None
         mk = lambda *s: torch.empty(*s, device=dev, dtype=torch.float32)
+        if self.smplx:
+            return self._query_smplx(n, ids, times, off, want_full, diagnostics, mk), ids
         out = {"root_pos": mk(n, 3)}
         if want_full:
             out.update(root_rot=mk(n, 4), dof_pos=mk(n, 69), root_vel=mk(n, 3), root_ang_vel=mk(n, 3), dof_vel=mk(n, 69),
@@ -204,6 +243,22 @@ class MotionLibB200:
             with torch.cuda.device(dev):
                 _lib.check(self._lib.pulse_motion_state(self._handle, C.byref(q), n, _lib.current_stream(dev)), "pulse_motion_state")
         return out, ids
+
+    def _query_smplx(self, n, ids, times, off, want_full, diagnostics, mk):
+        if diagnostics:
+            raise _lib.PulseError("the SMPL-X query has no frame diagnostics")
+        B, D, dev = self.num_bodies, _lib.SMPLX_DOF, self._device
+        out = {"root_pos": mk(n, 3)}
+        if want_full:
+            out.update(root_rot=mk(n, 4), dof_pos=mk(n, D), root_vel=mk(n, 3), root_ang_vel=mk(n, 3), dof_vel=mk(n, D), rg_pos=mk(n, B, 3),
+                       rb_rot=mk(n, B, 4), body_vel=mk(n, B, 3), body_ang_vel=mk(n, B, 3))
+        q = _lib.SmplxMotionQuery(motion_ids=ids.data_ptr(), motion_times=times.data_ptr(), offset=off.data_ptr() if off is not None else None)
+        for k, v in out.items():
+            setattr(q, k, v.data_ptr())
+        if n > 0:
+            with torch.cuda.device(dev):
+                _lib.check(self._lib.pulse_smplx_motion_state(self._handle, C.byref(q), n, _lib.current_stream(dev)), "pulse_smplx_motion_state")
+        return out
 
     def get_motion_state(self, motion_ids, motion_times, offset=None, diagnostics=False):
         out, ids = self._query(motion_ids, motion_times, offset, want_full=True, diagnostics=diagnostics)

@@ -38,8 +38,10 @@ class PulseVAE:
                  kld_anneal: bool = True, ar1_coefficient: float = 0.005, use_ar1_prior: bool = True, use_vae_prior_regu: bool = False,
                  use_vae_clamped_prior: bool = True, vae_var_clamp_max: float = 2.0, horizon: int = 32, with_critic: bool = True,
                  logstd: float = -2.9):
-        if latent > 32 or latent % 8 != 0:
-            raise _lib.PulseError("latent size must be a multiple of 8 and <= 32 (env_im_vae.yaml: embedding_size 32)")
+        if latent > 128 or latent % 8 != 0:
+            # embedding_size 32 for PULSE (env_im_vae.yaml), 48 for PULSE-X (env_pulsex_amp.yaml); the encoder's training kernels
+            # (pulse_vae_reparam_philox, pulse_vae_latent_loss) serve up to 32 and refuse more, the frozen prior and decoder any size here
+            raise _lib.PulseError("latent size must be a multiple of 8 and <= 128")
         if self_obs_size % 2 != 0:
             raise _lib.PulseError("self observation size must be even (pair-wise bf16 copies)")
         self.device = torch.device(device)

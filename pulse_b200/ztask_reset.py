@@ -50,7 +50,11 @@ def _f32(t: torch.Tensor, rows: int, name: str, cols: Optional[int] = None):
 class ZTaskResetB200:
     """The reset of one latent-space task over N envs.  kind: "reach" / "speed" / "strike"; `floor` the per-frame table of
     `smpl_ground_table` (at least the MotionLib's frame count); `upright` = _has_upright_start; `amp_root_height_obs` chooses the
-    196- or 195-float AMP rows (ampRootHeightObs, False in env_pulse_amp.yaml)."""
+    196- or 195-float AMP rows (ampRootHeightObs, False in env_pulse_amp.yaml).
+
+    A 52-body MotionLib (SMPL-X, PULSE-X) serves the speed task through `pulse_reset_ztask_smplx`: views of >= 52 bodies and 153 dofs,
+    `upright` False as in env_pulsex_amp.yaml (True is refused: the SMPL-X step takes the non-upright heading), no AMP history
+    (`amp_obs_buf`) and no discriminator."""
 
     def __init__(self, kind: str, motion_lib: MotionLibB200, floor: torch.Tensor, *, upright: bool = True, state_init: str = "Random",
                  amp_root_height_obs: bool = False, dt: float = float(torch.tensor(1.0 / 60.0, dtype=torch.float32) * 2),
@@ -62,6 +66,13 @@ class ZTaskResetB200:
         if state_init not in _INIT:
             raise _lib.PulseError(f"state_init {state_init!r}: the device reset serves Random and Start")
         self.kind, self.motion_lib, self.device = kind, motion_lib, motion_lib._device
+        self.smplx = bool(getattr(motion_lib, "smplx", False))
+        if self.smplx and kind != "speed":
+            raise _lib.PulseError(f"the SMPL-X reset serves the speed task, not {kind!r}")
+        if self.smplx and upright:
+            raise _lib.PulseError("the SMPL-X reset takes upright=False (env_pulsex_amp.yaml: has_upright_start False), the heading its "
+                                  "step kernel uses")
+        self.bodies, self.dofs = (_lib.SMPLX_BODIES, _lib.SMPLX_DOF) if self.smplx else (24, 69)
         self.pose_mode, self.init_code = _POSE[kind], _INIT[state_init]
         if floor.dtype != torch.float32 or floor.dim() != 1 or floor.device != self.device:
             raise _lib.PulseError("floor must be a float32 [F] table on the MotionLib's device")
@@ -104,9 +115,9 @@ class ZTaskResetB200:
                            terminate_buf=terminate_buf, contact_forces=contact_forces, amp_obs_buf=amp_obs_buf, actor_ids=actor_ids,
                            target_states=target_states, tar_actor_ids=tar_actor_ids, motion_ids=motion_ids, motion_u=motion_u, phase=phase,
                            strike_u=strike_u, seed=seed, offset=offset, offset_dev=offset_dev)
+        fn, handle = ("pulse_reset_ztask_smplx", self.motion_lib.smplx_handle) if self.smplx else ("pulse_reset_ztask", self.motion_lib.handle)
         with torch.cuda.device(self.device):
-            _lib.check(self.lib.pulse_reset_ztask(self.motion_lib.handle, C.byref(a), int(progress_buf.shape[0]), _lib.current_stream(self.device)),
-                       "pulse_reset_ztask")
+            _lib.check(getattr(self.lib, fn)(handle, C.byref(a), int(progress_buf.shape[0]), _lib.current_stream(self.device)), fn)
         return ws
 
     def _args(self, *, root_states, dof_pos, dof_vel, rigid_body_state, progress_buf, sampled_motion_ids, motion_start_times, reset_buf, env_ids,
@@ -122,12 +133,15 @@ class ZTaskResetB200:
             if t.dtype != dtype or t.device != dev or t.shape[0] != N or not shape_ok or not layout_ok:
                 raise _lib.PulseError(f"{name} must be a {dtype} view on {dev} with {N} rows, {what}")
 
-        view(rigid_body_state, "rigid_body_state", torch.float32, rigid_body_state.dim() == 3 and rigid_body_state.shape[1] >= 24,
-             rigid_body_state.stride(1) == 13 and rigid_body_state.stride(2) == 1, "[N, B >= 24, 13] with row stride 13")
+        B, D = self.bodies, self.dofs
+        if self.smplx and amp_obs_buf is not None:
+            raise _lib.PulseError("the SMPL-X reset has no AMP history back-fill (amp_obs_buf must be None)")
+        view(rigid_body_state, "rigid_body_state", torch.float32, rigid_body_state.dim() == 3 and rigid_body_state.shape[1] >= B,
+             rigid_body_state.stride(1) == 13 and rigid_body_state.stride(2) == 1, f"[N, B >= {B}, 13] with row stride 13")
         view(root_states, "root_states", torch.float32, root_states.dim() == 2 and root_states.shape[1] >= 13, root_states.stride(1) == 1,
              "[N, >= 13] with contiguous rows")
         for name, t in (("dof_pos", dof_pos), ("dof_vel", dof_vel)):
-            view(t, name, torch.float32, t.dim() == 2 and t.shape[1] == 69, t.stride() == dof_pos.stride(), "[N, 69], dof_pos and dof_vel sharing strides")
+            view(t, name, torch.float32, t.dim() == 2 and t.shape[1] == D, t.stride() == dof_pos.stride(), f"[N, {D}], dof_pos and dof_vel sharing strides")
         if terminate_buf is not None:
             view(terminate_buf, "terminate_buf", torch.int64, terminate_buf.dim() == 1, terminate_buf.is_contiguous(), "contiguous [N]")
         if contact_forces is not None:

@@ -12,25 +12,37 @@ from .latent_rollout import LatentStepsB200
 
 _KINDS = {_lib.ZTASK_REACH: "reach", _lib.ZTASK_SPEED: "speed", _lib.ZTASK_STRIKE: "strike"}
 _WIDTHS = {"reach": 361, "speed": 361, "strike": 373}
+# per body layout: (observation width of the speed task, self observation -> dof targets of the decoder, latent size or None = any)
+_LAYOUTS = {"smpl": (None, 358, 69, None), "smplx": (_lib.SMPLX_SPEED_OBS, _lib.SMPLX_SELF_OBS, _lib.SMPLX_DOF, 48)}
+# the step's entry points per body layout: (step, list observation, rollout step) of the speed / strike tasks
+_ENTRIES = {"smpl": ("pulse_ztask_step", "pulse_ztask_obs_list", "pulse_ztask_rollout_step"),
+            "smplx": ("pulse_smplx_speed_step", "pulse_smplx_speed_obs_list", "pulse_smplx_speed_rollout_step")}
 SIM_KEYS = ("body_state", "root_states", "dof_pos", "dof_vel", "progress_buf", "sampled_motion_ids", "motion_start_times")
 STRIKE_KEYS = ("target_states", "tar_contact_forces")
 
 
 def check_pieces(task, reset, policy, vae) -> str:
     """The task kind ("reach" / "speed" / "strike") after checking that the step object, the reset, the latent policy and the frozen
-    VAE belong together; raises PulseError otherwise."""
+    VAE belong together; raises PulseError otherwise.  SMPL: observations of 361 / 361 / 373 floats, a 358 -> 69 decoder.  SMPL-X
+    (SmplxSpeedTaskB200, PULSE-X): the speed task's 781 floats, a 778 -> 153 decoder and a 48-dimensional latent (env_pulsex_amp.yaml)."""
     kind = _KINDS.get(getattr(task, "kind", None))
     if kind is None:
-        raise _lib.PulseError("ZTaskStepsB200: task must be a ReachTaskB200, SpeedTaskB200 or StrikeTaskB200")
+        raise _lib.PulseError("ZTaskStepsB200: task must be a ReachTaskB200, SpeedTaskB200, StrikeTaskB200 or SmplxSpeedTaskB200")
     if getattr(reset, "kind", None) != kind:
         raise _lib.PulseError(f"ZTaskStepsB200: the reset serves {getattr(reset, 'kind', None)!r}, the task is {kind!r}")
-    W = _WIDTHS[kind]
+    layout = getattr(task, "layout", "smpl")
+    if bool(getattr(reset, "smplx", False)) != (layout == "smplx"):
+        raise _lib.PulseError(f"ZTaskStepsB200: the task is {layout}, the reset's MotionLib has {getattr(reset, 'bodies', 24)} bodies")
+    W, S, A, E = _LAYOUTS[layout]
+    W = W or _WIDTHS[kind]
     if int(task.obs_size) != W or int(policy.obs_size) != W:
-        raise _lib.PulseError(f"ZTaskStepsB200: the {kind} observation has {W} floats, the task writes {task.obs_size} and the policy reads {policy.obs_size}")
+        raise _lib.PulseError(f"ZTaskStepsB200: the {layout} {kind} observation has {W} floats, the task writes {task.obs_size} and the policy reads {policy.obs_size}")
     if int(policy.A) != int(vae.E):
         raise _lib.PulseError(f"ZTaskStepsB200: the policy acts in {policy.A} dimensions, the VAE's latent has {vae.E}")
-    if int(vae.S) != 358 or int(vae.A) != 69:
-        raise _lib.PulseError(f"ZTaskStepsB200: the decoder must map the 358-float self observation to 69 dof targets, not {vae.S} -> {vae.A}")
+    if int(vae.S) != S or int(vae.A) != A:
+        raise _lib.PulseError(f"ZTaskStepsB200: the decoder must map the {S}-float self observation to {A} dof targets, not {vae.S} -> {vae.A}")
+    if E is not None and int(vae.E) != E:
+        raise _lib.PulseError(f"ZTaskStepsB200: the {layout} latent has {E} dimensions (embedding_size), the VAE's {vae.E}")
     if getattr(policy, "disc", None) is not None:
         raise _lib.PulseError("ZTaskStepsB200: the discriminator is not part of this driver (task reward only); build the policy without it")
     return kind
@@ -52,18 +64,25 @@ class ZTaskStepsB200(LatentStepsB200):
     sampled_motion_ids, motion_start_times; optional contact_forces, actor_ids, dof_force (the speed task's power term); strike:
     target_states, tar_contact_forces and optional tar_actor_ids.
 
+    The PULSE-X speed task (`HumanoidSpeedZ` with robot=smplx_humanoid) runs through the same driver: `task` a SmplxSpeedTaskB200,
+    `reset` a ZTaskResetB200 over a 52-body MotionLib, `policy` PPOPolicy(obs_size=781, num_actions=48), `vae` PulseVAE(self_obs_size=778,
+    num_actions=153, latent=48); the sim views hold >= 52 bodies and 153 dofs, and `dof_force` is refused (no power term).
+
     Out of scope: the discriminator (the reference still trains it here with disc_coef 5 although disc_reward_w is 0; leaving it out does
     not change the reward, but it removes the discriminator's gradients from the shared gradient-norm clip, so the reset is called
-    without an AMP buffer); multi-GPU; the smplx humanoid; Default / Hybrid state init; the power_usage_reward terms the step kernels
-    exclude."""
+    without an AMP buffer); multi-GPU; the smplx humanoid's reach and strike tasks; Default / Hybrid state init; the power_usage_reward
+    terms the step kernels exclude."""
 
     def __init__(self, task, reset, policy, vae, sim: dict, horizon: int = 32, pd_offset: Optional[torch.Tensor] = None,
                  pd_scale: Optional[torch.Tensor] = None, pd_freeze: Optional[torch.Tensor] = None, use_graphs: bool = True,
                  gamma: float = 0.99, tau: float = 0.95, reset_seed: int = 0):
         self.kind = check_pieces(task, reset, policy, vae)
+        self.layout = getattr(task, "layout", "smpl")
         missing = [k for k in SIM_KEYS + (STRIKE_KEYS if self.kind == "strike" else ()) if k not in sim]
         if missing:
             raise _lib.PulseError(f"ZTaskStepsB200: sim lacks {missing}")
+        if self.layout == "smplx" and sim.get("dof_force") is not None:
+            raise _lib.PulseError("ZTaskStepsB200: sim['dof_force'] given, but the SMPL-X speed step has no power term")
         n = self.n = int(sim["progress_buf"].shape[0])
         if n != task.num_envs:
             raise _lib.PulseError(f"ZTaskStepsB200: sim has {n} envs, the task {task.num_envs}")
@@ -77,6 +96,7 @@ class ZTaskStepsB200(LatentStepsB200):
             a = task._step_args(s["body_state"], s["progress_buf"], s.get("contact_forces"))
         else:
             a = task._args(s["body_state"], s["progress_buf"], s.get("contact_forces"))
+        if self.kind != "reach" and self.layout == "smpl":
             if self.kind == "speed":
                 a.tar_speed = task._tar_speed.data_ptr()
                 if task.power_reward:
@@ -112,14 +132,14 @@ class ZTaskStepsB200(LatentStepsB200):
         """`_compute_observations(env_ids)` of the reset envs into obses[:, t], then `_reset_task` (humanoid_amp_task.py:66-76)."""
         ws = self.reset_ws
         a = self._step_args(self.obses[:, t], self.rewards[t])
-        self._launch("pulse_reach_obs_list" if self.kind == "reach" else "pulse_ztask_obs_list", C.byref(a), ws["env_list"].data_ptr(),
+        self._launch("pulse_reach_obs_list" if self.kind == "reach" else _ENTRIES[self.layout][1], C.byref(a), ws["env_list"].data_ptr(),
                      ws["count"].data_ptr(), self.n)
         if self.kind != "strike":
             self.reset.reset_task(progress_buf=self.sim["progress_buf"], seed=self.reset_seed, offset=t, offset_dev=self.policy.rng_offset,
                                   **self._task_kw())
 
     def _pre_physics(self, dec: torch.Tensor, t: int, rand: Optional[torch.Tensor] = None, steps: Optional[torch.Tensor] = None) -> None:
-        """`pulse_ztask_pre_physics` on the decoder output `dec` [n, 69]; `rand` / `steps` inject the `_update_task` draws per env."""
+        """`pulse_ztask_pre_physics` on the decoder output `dec` [n, dofs]; `rand` / `steps` inject the `_update_task` draws per env."""
         s, task, kind = self.sim, self.task, self.kind
         p = _lib.ZTaskPrePhysicsArgs(kind=task.kind, dofs=self.vae.A, action=dec.data_ptr(), ld_action=dec.stride(0), pd_offset=self.pd[0].data_ptr(),
                                      pd_scale=self.pd[1].data_ptr(), freeze=_lib.ptr(self.pd_freeze), pd_out=self.pd_tar.data_ptr(),
@@ -140,11 +160,11 @@ class ZTaskStepsB200(LatentStepsB200):
     def _env_step(self, t: int) -> None:
         """post_physics_step (humanoid.py:1315-1346): one fused launch."""
         a = self._step_args(self._next_obs(t), self.rewards[t])
-        self._launch("pulse_reach_rollout_step" if self.kind == "reach" else "pulse_ztask_rollout_step", C.byref(a), self.dones[t].data_ptr(), self.n)
+        self._launch("pulse_reach_rollout_step" if self.kind == "reach" else _ENTRIES[self.layout][2], C.byref(a), self.dones[t].data_ptr(), self.n)
 
     def first_observation(self) -> None:
         """Observation of the initial state (Humanoid.reset -> _compute_observations at start-up): fills `obs_carry`."""
         a = self._step_args(self.obs_carry, self.rewards[0])
-        self._launch("pulse_reach_step" if self.kind == "reach" else "pulse_ztask_step", C.byref(a), self.n)
+        self._launch("pulse_reach_step" if self.kind == "reach" else _ENTRIES[self.layout][0], C.byref(a), self.n)
         self.reset_buf.zero_()
         self.terminate_buf.zero_()

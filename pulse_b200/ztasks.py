@@ -2,6 +2,7 @@
 (phc/env/tasks/humanoid_speed.py, humanoid_strike.py) for the post-physics path -- reward, reset, observation in ONE launch
 (`pulse_ztask_step`) -- and the task-state updates (`_update_task` / `_reset_task`).  Like the reach task (pulse_b200/reach.py) the policy
 acts in the frozen PULSE latent space (`PulseVAE.compute_z_actions`); Isaac Gym keeps the physics and owns the state tensors.
+`SmplxSpeedTaskB200` is the speed task of PULSE-X on the 52-body SMPL-X humanoid (`pulse_smplx_speed_step`).
 """
 import ctypes as C
 import math
@@ -164,3 +165,79 @@ class StrikeTaskB200(_ZTaskBase):
         a = self._args(rigid_body_state, progress_buf, contact_forces)
         a.target_states, a.target_env_stride = target_states.data_ptr(), target_states.stride(0)
         self._launch_list(a, env_list, count)
+
+
+class SmplxSpeedTaskB200:
+    """HumanoidSpeed(Z) for the 52-body SMPL-X humanoid of PULSE-X (`env.task=HumanoidSpeedZ env=env_pulsex_amp robot=smplx_humanoid`):
+    the post-physics step `pulse_smplx_speed_step` and `_update_task`.  The self observation takes the heading of
+    remove_base_rot(root_rot) (has_upright_start False), the task observation that of the raw root rotation, as the reference does;
+    obs = [self 778 | 3].  Bodies are given by index in the simulator's body order (SMPLH_MUJOCO_NAMES): `contact_body_ids` is the
+    task's `_contact_body_ids` (R_Ankle, L_Ankle, R_Toe, L_Toe in env_pulsex_amp.yaml).  env_pulsex_amp.yaml has power_reward and
+    power_usage_reward off; neither term is served, and a `dof_force` is refused."""
+    kind, obs_size, layout = _lib.ZTASK_SPEED, _lib.SMPLX_SPEED_OBS, "smplx"
+
+    def __init__(self, num_envs: int, device="cuda:0", *, contact_body_ids: Sequence[int], tar_speed_min: float = 0.0, tar_speed_max: float = 5.0,
+                 speed_change_steps_min: int = 100, speed_change_steps_max: int = 200, max_episode_length: int = 300,
+                 enable_early_termination: bool = True, termination_height: float = 0.15, dt: float = 1.0 / 30.0, power_reward: bool = False):
+        if power_reward:
+            raise _lib.PulseError("SmplxSpeedTaskB200: the power reward is not served for SMPL-X (env_pulsex_amp.yaml has power_reward False)")
+        B = _lib.SMPLX_BODIES
+        ids = [int(i) for i in contact_body_ids]
+        if any(i < 0 or i >= B for i in ids):
+            raise _lib.PulseError(f"SmplxSpeedTaskB200: contact_body_ids {ids} outside [0, {B})")
+        self.device, self.num_envs = torch.device(device), int(num_envs)
+        self.contact_body_mask = sum(1 << i for i in set(ids))
+        self.max_episode_length, self.enable_early_termination, self.dt = int(max_episode_length), bool(enable_early_termination), float(dt)
+        self._tar_speed_min, self._tar_speed_max = tar_speed_min, tar_speed_max
+        self._speed_change_steps_min, self._speed_change_steps_max = speed_change_steps_min, speed_change_steps_max
+        self.power_reward = False
+        dev, n = self.device, self.num_envs
+        self.termination_heights = torch.full((B,), termination_height, device=dev)
+        self._prev_root_pos = torch.zeros(n, 3, device=dev)
+        self._tar_speed = torch.ones(n, device=dev)
+        self._speed_change_steps = torch.zeros(n, dtype=torch.int64, device=dev)
+        self.obs_buf = torch.zeros(n, self.obs_size, device=dev)
+        self.rew_buf = torch.zeros(n, device=dev)
+        self.reward_raw = torch.zeros(n, 1, device=dev)
+        self.reset_buf = torch.zeros(n, dtype=torch.int64, device=dev)
+        self._terminate_buf = torch.zeros(n, dtype=torch.int64, device=dev)
+        self.lib = _lib.load()
+
+    def get_task_obs_size(self) -> int:
+        return 3
+
+    pre_physics_step = _ZTaskBase.pre_physics_step
+    update_task = SpeedTaskB200.update_task
+
+    def _args(self, rigid_body_state, progress_buf, contact_forces):
+        B = _lib.SMPLX_BODIES
+        if rigid_body_state.dim() != 3 or rigid_body_state.shape[1] < B or rigid_body_state.stride(1) != 13 or rigid_body_state.stride(2) != 1:
+            raise _lib.PulseError(f"rigid_body_state must be a [N, B>={B}, 13] view with row stride 13")
+        if contact_forces is not None and (contact_forces.dim() != 3 or contact_forces.shape[1] < B or contact_forces.stride(1) != 3
+                                           or contact_forces.stride(2) != 1):
+            raise _lib.PulseError(f"contact_forces must be a [N, B>={B}, 3] view with contiguous bodies")
+        return _lib.SmplxSpeedStepArgs(
+            enable_early_termination=int(self.enable_early_termination), body_state=rigid_body_state.data_ptr(),
+            body_env_stride=rigid_body_state.stride(0), contact_forces=contact_forces.data_ptr() if contact_forces is not None else None,
+            contact_env_stride=contact_forces.stride(0) if contact_forces is not None else 0, termination_heights=self.termination_heights.data_ptr(),
+            contact_body_mask=self.contact_body_mask, progress_buf=progress_buf.data_ptr(), max_episode_length=self.max_episode_length,
+            prev_root_pos=self._prev_root_pos.data_ptr(), dt=self.dt, tar_speed=self._tar_speed.data_ptr(), obs_buf=self.obs_buf.data_ptr(),
+            obs_stride=self.obs_buf.stride(0), rew_buf=self.rew_buf.data_ptr(), reward_raw=self.reward_raw.data_ptr(),
+            raw_stride=self.reward_raw.stride(0), reset_buf=self.reset_buf.data_ptr(), terminate_buf=self._terminate_buf.data_ptr())
+
+    def post_physics_step(self, rigid_body_state: torch.Tensor, progress_buf: torch.Tensor, contact_forces: Optional[torch.Tensor] = None,
+                          dof_force: Optional[torch.Tensor] = None) -> None:
+        """compute_speed_reward + compute_humanoid_reset + the observation in one launch."""
+        if dof_force is not None:
+            raise _lib.PulseError("SmplxSpeedTaskB200: dof_force given, but the SMPL-X speed step has no power term")
+        a = self._args(rigid_body_state, progress_buf, contact_forces)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.pulse_smplx_speed_step(C.byref(a), self.num_envs, _lib.current_stream(self.device)), "pulse_smplx_speed_step")
+
+    def observe_list(self, rigid_body_state: torch.Tensor, env_list: torch.Tensor, count: torch.Tensor, progress_buf: torch.Tensor,
+                     contact_forces: Optional[torch.Tensor] = None) -> None:
+        """_compute_observations(env_ids) for the envs env_list[0 .. *count): post_physics_step's rows for them, nothing else."""
+        a = self._args(rigid_body_state, progress_buf, contact_forces)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.pulse_smplx_speed_obs_list(C.byref(a), env_list.data_ptr(), count.data_ptr(), self.num_envs,
+                                                           _lib.current_stream(self.device)), "pulse_smplx_speed_obs_list")

@@ -1,0 +1,182 @@
+#!/usr/bin/env python
+"""The PULSE-X speed task on the device (HumanoidSpeedZ, robot=smplx_humanoid, env_pulsex_amp.yaml): full training iterations of the
+52-body SMPL-X humanoid through `ZTaskStepsB200`, measured as tools/bench_ztask_rollout.py measures the SMPL latent tasks, and the step
+kernel alone.
+
+  iteration  one horizon (device resets inside it, latent policy 2048-1024-512 SiLU over 48 latent dimensions, frozen prior + 778 -> 153
+             decoder of the PULSE-X VAE's shapes with random weights, pre-physics and step kernels; no physics), then `finish` and the
+             PPO update (6 mini-epochs of 16384-row minibatches), on synthetic 52-body MotionLib tables and simulator state.  Two arms
+             alternated iteration by iteration: graph (as shipped) and eager (use_graphs=False).  Milliseconds per horizon and update
+             from device events after --warmup, with an L2 flush before each timed region, over --iters iterations.
+  step       `pulse_smplx_speed_step` alone at --step-envs envs: device events around --step-reps back-to-back launches (one L2
+             flush before each sample), beside the bytes one env-step reads and writes as computed from the shapes (52 x 13 body
+             floats, 52 x 3 contact floats, the 781-float observation row, and the per-env scalars).  At 16384 envs a launch touches
+             ~106 MB, more than the 50 MB L2, so the back-to-back launches stream mostly from HBM.
+
+One JSON line per measurement, with the card name, power limit and maximum SM clock read in the same call.  Needs a CUDA device.
+
+  python tools/bench_smplx_speed.py [--envs 1536 8192] [--iters 5] [--warmup 2] [--step-envs 16384] [--step-reps 200]
+"""
+import argparse
+import ctypes as C
+import json
+import os
+import sys
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from tools.bench_ztask_rollout import HORIZON, MINI_EPOCHS, MINIBATCH, UNITS, gpu_info   # noqa: E402
+
+B, D, LATENT = 52, 153, 48
+CONTACT_IDS = (7, 3, 8, 4)          # R_Ankle, L_Ankle, R_Toe, L_Toe in the SMPLH_MUJOCO_NAMES order
+
+
+def tables(clips, dev, seed):
+    g = torch.Generator(device=dev).manual_seed(seed)
+    nf = torch.randint(60, 240, (clips,), device=dev, generator=g)
+    F = int(nf.sum())
+    unit = lambda q: q / q.norm(dim=-1, keepdim=True)
+    r = lambda *s: torch.randn(*s, device=dev, generator=g)
+    dt = torch.full((clips,), 1.0 / 30.0, device=dev)
+    return dict(gts=r(F, B, 3) * 0.3 + torch.tensor([0.0, 0.0, 0.9], device=dev), grs=unit(r(F, B, 4)), lrs=unit(r(F, B, 4)), gvs=r(F, B, 3),
+                gavs=r(F, B, 3), dvs=r(F, B - 1, 3), lengths=dt * (nf - 1).float(), num_frames=nf, dt=dt,
+                length_starts=torch.cumsum(nf, 0) - nf)
+
+
+def sim_state(n, dev, seed):
+    g = torch.Generator(device=dev).manual_seed(seed)
+    body = torch.zeros(n, B + 1, 13, device=dev)
+    body[..., 0:3] = torch.randn(n, B + 1, 3, device=dev, generator=g) * 0.3 + torch.tensor([0.0, 0.0, 0.9], device=dev)
+    body[..., 3:7] = torch.nn.functional.normalize(torch.randn(n, B + 1, 4, device=dev, generator=g), dim=-1)
+    body[..., 7:13] = torch.randn(n, B + 1, 6, device=dev, generator=g)
+    contact = torch.zeros(n, B + 1, 3, device=dev)
+    body[::16, 40, 2], contact[::16, 40, 2] = 0.05, 5.0                                     # fallen: reset at the second step
+    dof_state = torch.randn(n, D, 2, device=dev, generator=g)
+    return dict(body_state=body, root_states=body[:, 0].clone(), dof_pos=dof_state[:, :, 0], dof_vel=dof_state[:, :, 1], contact_forces=contact,
+                progress_buf=torch.randint(2, 300, (n,), device=dev, generator=g), sampled_motion_ids=torch.zeros(n, dtype=torch.int64, device=dev),
+                motion_start_times=torch.zeros(n, device=dev))
+
+
+def build(n, dev, use_graphs):
+    from pulse_b200.motion_lib import MotionLibB200
+    from pulse_b200.ppo import PPOPolicy
+    from pulse_b200.vae import PulseVAE
+    from pulse_b200.ztask_reset import ZTaskResetB200
+    from pulse_b200.ztask_rollout import ZTaskStepsB200
+    from pulse_b200.ztasks import SmplxSpeedTaskB200
+    ml = MotionLibB200.from_tables(tables(256, dev, 100))
+    g = torch.Generator(device=dev).manual_seed(300)
+    floor = -0.9 + 0.05 * torch.rand(ml.gts.shape[0], device=dev, generator=g)            # stand-in for the ground table
+    task = SmplxSpeedTaskB200(n, device=dev, contact_body_ids=CONTACT_IDS)
+    policy = PPOPolicy(obs_size=task.obs_size, num_actions=LATENT, units=UNITS, act="silu", device=dev, seed=0)
+    vae = PulseVAE(self_obs_size=778, num_actions=D, latent=LATENT, device=dev, with_critic=False)
+    drv = ZTaskStepsB200(task, ZTaskResetB200("speed", ml, floor, upright=False), policy, vae, sim_state(n, dev, 200), horizon=HORIZON,
+                         use_graphs=use_graphs, reset_seed=1)
+    drv.first_observation()
+    return drv
+
+
+def step_bytes():
+    """Bytes one env-step of pulse_smplx_speed_step moves, from the shapes: reads the 52 x 13 body floats, 52 x 3 contact floats, the
+    52 termination heights (cached across envs: not counted), progress, prev_root_pos and tar_speed; writes the 781-float observation
+    row, reward, reward_raw, reset and terminate."""
+    rd = {"body_state": B * 13 * 4, "contact_forces": B * 3 * 4, "progress/prev_root/tar_speed": 8 + 12 + 4}
+    wr = {"obs_row": 781 * 4, "rew/reward_raw": 8, "reset/terminate": 16}
+    return rd, wr
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--envs", type=int, nargs="+", default=[1536, 8192])
+    ap.add_argument("--iters", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--step-envs", type=int, default=16384)
+    ap.add_argument("--step-reps", type=int, default=200)
+    args = ap.parse_args()
+    if args.iters < 3:
+        raise SystemExit("at least three timed iterations")
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_smplx_speed.py needs a CUDA device")
+    from pulse_b200 import _lib
+    lib = _lib.load()
+    dev = "cuda:0"
+    info = gpu_info()
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)                  # larger than the 50 MB L2
+
+    def timed(fn):
+        flush.zero_()
+        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        s.record()
+        fn()
+        e.record()
+        return s, e
+
+    for n in args.envs:
+        arms = {"graph": build(n, dev, True), "eager": build(n, dev, False)}
+        mb = min(MINIBATCH, n * HORIZON)
+        update = lambda d: (d.finish(), d.train_epoch(mini_epochs=MINI_EPOCHS, minibatch=mb))
+        ev = {a: {"horizon": [], "update": []} for a in arms}
+        resets = {a: 0.0 for a in arms}
+        for it in range(args.warmup + args.iters):
+            for a, d in arms.items():
+                h = timed(d.play_steps)
+                done = d.dones.sum()
+                u = timed(lambda: update(d))
+                if it >= args.warmup:
+                    ev[a]["horizon"].append(h)
+                    ev[a]["update"].append(u)
+                    resets[a] += float(done)
+        torch.cuda.synchronize()
+        c0 = lib.pulse_launch_count()
+        arms["eager"].play_steps()
+        torch.cuda.synchronize()
+        launches = (lib.pulse_launch_count() - c0) / HORIZON
+        out = {"workload": "PULSE-X speed task iteration (HumanoidSpeedZ, smplx_humanoid, 52 bodies, 153 dofs): %d envs, horizon %d, latent "
+                           "policy %s SiLU over %d dims, frozen prior + 778->153 decoder, task reward only, %d mini-epochs of %d rows, no physics"
+                           % (n, HORIZON, "-".join(map(str, UNITS)), LATENT, MINI_EPOCHS, mb),
+               "gpu": info, "envs": n, "iters": args.iters, "warmup": args.warmup, "launches_per_step": round(launches, 2)}
+        for a in arms:
+            ms = {k: [s.elapsed_time(e) for s, e in v] for k, v in ev[a].items()}
+            mean = {k: sum(v) / len(v) for k, v in ms.items()}
+            out[a] = {"horizon_ms": round(mean["horizon"], 3), "horizon_ms_min_max": [round(min(ms["horizon"]), 3), round(max(ms["horizon"]), 3)],
+                      "update_ms": round(mean["update"], 3), "update_ms_min_max": [round(min(ms["update"]), 3), round(max(ms["update"]), 3)],
+                      "rollout_env_steps_per_s": round(n * HORIZON / (mean["horizon"] * 1e-3), 1),
+                      "iteration_env_steps_per_s": round(n * HORIZON / ((mean["horizon"] + mean["update"]) * 1e-3), 1),
+                      "resets_per_horizon": round(resets[a] / args.iters, 1)}
+        print(json.dumps(out), flush=True)
+        del arms
+        torch.cuda.empty_cache()
+
+    # the step kernel alone
+    from pulse_b200.ztasks import SmplxSpeedTaskB200
+    n = args.step_envs
+    task = SmplxSpeedTaskB200(n, device=dev, contact_body_ids=CONTACT_IDS)
+    s = sim_state(n, dev, 7)
+    a = task._args(s["body_state"], s["progress_buf"], s["contact_forces"])
+    st = _lib.current_stream(dev)
+    for _ in range(10):
+        _lib.check(lib.pulse_smplx_speed_step(C.byref(a), n, st), "pulse_smplx_speed_step")
+    times = []
+    for _ in range(5):
+        flush.zero_()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(args.step_reps):
+            _lib.check(lib.pulse_smplx_speed_step(C.byref(a), n, st), "pulse_smplx_speed_step")
+        e1.record()
+        torch.cuda.synchronize()
+        times.append(e0.elapsed_time(e1) * 1e3 / args.step_reps)
+    rd, wr = step_bytes()
+    per_env = sum(rd.values()) + sum(wr.values())
+    us = sorted(times)[len(times) // 2]
+    print(json.dumps({"workload": "pulse_smplx_speed_step alone: %d envs, %d back-to-back launches per sample, median of 5 samples" % (n, args.step_reps),
+                      "gpu": info, "envs": n, "kernel_us": round(us, 2), "kernel_us_samples": [round(t, 2) for t in times],
+                      "bytes_per_env_step": {"read": rd, "write": wr, "total": per_env},
+                      "achieved_GB_per_s": round(per_env * n / (us * 1e-6) / 1e9, 1)}), flush=True)
+
+
+if __name__ == "__main__":
+    main()
