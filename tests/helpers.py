@@ -19,9 +19,17 @@ def oracle_tables(device="cpu"):
     return MotionTables(**{k: v.to(device) for k, v in z.items()})
 
 
+def clip_rates(fps, num_motions):
+    """Per-clip frame rates as float64 [M]: a scalar for every clip, or a sequence repeated over the clips in order."""
+    r = torch.tensor(fps if isinstance(fps, (list, tuple)) else [fps], dtype=torch.float64)
+    return r.repeat((num_motions + r.numel() - 1) // r.numel())[:num_motions]
+
+
 def synthetic_tables(num_motions, seed=0, min_frames=5, max_frames=400, median_frames=150, fps=30.0):
     """AMASS-shaped flat MotionLib tables written directly (SURVEY 8d): unit quaternions, smooth
-    positions; bypasses the reference's 60 ms/clip loader.  Returns oracle MotionTables on CPU."""
+    positions; bypasses the reference's 60 ms/clip loader.  Returns oracle MotionTables on CPU.
+    fps: one rate, or a sequence of per-clip rates (clip_rates); length and dt follow the reference's
+    `1.0 / fps * (num_frames - 1)` and `1.0 / fps` in float64, stored as float32 (motion_lib_base.py:262-263)."""
     from oracle.pulse_oracle import MotionTables
     rng = np.random.default_rng(seed)
     nf = np.clip(np.exp(rng.normal(np.log(median_frames), 0.6, size=num_motions)).astype(np.int64), min_frames, max_frames)
@@ -43,10 +51,11 @@ def synthetic_tables(num_motions, seed=0, min_frames=5, max_frames=400, median_f
     aa = torch.randn(F, 72, generator=g)
     nf_t = torch.from_numpy(nf)
     starts = torch.cumsum(nf_t, 0) - nf_t
-    lengths = torch.tensor([(1.0 / fps) * (int(n) - 1) for n in nf], dtype=torch.float32)
-    dt = torch.full((num_motions,), 1.0 / fps, dtype=torch.float32)
+    rates = clip_rates(fps, num_motions).tolist()
+    lengths = torch.tensor([(1.0 / r) * (int(n) - 1) for r, n in zip(rates, nf)], dtype=torch.float32)
+    dt = torch.tensor([1.0 / r for r in rates], dtype=torch.float32)
     return MotionTables(gts=gts, grs=grs, lrs=lrs, gvs=gvs, gavs=gavs, dvs=dvs, motion_aa=aa, lengths=lengths,
-                        num_frames=nf_t, dt=dt, length_starts=starts, fps=torch.full((num_motions,), fps),
+                        num_frames=nf_t, dt=dt, length_starts=starts, fps=torch.tensor(rates, dtype=torch.float32),
                         motion_bodies=torch.zeros(num_motions, 17), motion_limb_weights=torch.zeros(num_motions, 10))
 
 
@@ -185,8 +194,9 @@ def _unit_quat(q):
     return q / n.unsqueeze(-1)
 
 
-def exact_tables(num_motions, seed=5, min_frames=5, max_frames=300, spread=230):
-    """oracle MotionTables with clip lengths from integer draws; unit quaternions (nearby frames), smooth-ish positions."""
+def exact_tables(num_motions, seed=5, min_frames=5, max_frames=300, spread=230, fps=30.0):
+    """oracle MotionTables with clip lengths from integer draws; unit quaternions (nearby frames), smooth-ish positions.
+    fps: one rate, or a sequence of per-clip rates (clip_rates); the rates change only lengths, dt and fps."""
     from oracle.pulse_oracle import MotionTables
     g = torch.Generator().manual_seed(seed)
     nf = torch.randint(min_frames, min_frames + spread, (num_motions,), generator=g).clamp(max=max_frames)
@@ -199,11 +209,11 @@ def exact_tables(num_motions, seed=5, min_frames=5, max_frames=300, spread=230):
     gvs, gavs, dvs = _approx_normal((F, 24, 3), g), _approx_normal((F, 24, 3), g), _approx_normal((F, 23, 3), g)
     aa = _approx_normal((F, 72), g)
     starts = torch.cumsum(nf, 0) - nf
-    fps = 30.0
-    lengths = ((nf - 1).double() * (1.0 / fps)).float()
-    dt = torch.full((num_motions,), 1.0 / fps, dtype=torch.float32)
+    rates = clip_rates(fps, num_motions)
+    lengths = ((nf - 1).double() * (1.0 / rates)).float()
+    dt = (1.0 / rates).float()
     return MotionTables(gts=gts, grs=grs, lrs=lrs, gvs=gvs, gavs=gavs, dvs=dvs, motion_aa=aa, lengths=lengths, num_frames=nf, dt=dt,
-                        length_starts=starts, fps=torch.full((num_motions,), fps), motion_bodies=torch.zeros(num_motions, 17),
+                        length_starts=starts, fps=rates.float(), motion_bodies=torch.zeros(num_motions, 17),
                         motion_limb_weights=torch.zeros(num_motions, 10))
 
 

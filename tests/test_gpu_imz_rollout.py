@@ -18,12 +18,22 @@ VR = (13, 18, 23)
 UNITS = (2048, 1536, 1024, 1024, 512, 512)     # pulse_z_vr.yaml
 
 
-@pytest.fixture(scope="module")
-def ml():
+def _motion_lib(fps):
     from pulse_b200.motion_lib import MotionLibB200
-    tb = exact_tables(CLIPS, seed=13)
+    tb = exact_tables(CLIPS, seed=13, fps=fps)
     return MotionLibB200.from_tables({k: getattr(tb, k) for k in ("gts", "grs", "lrs", "gvs", "gavs", "dvs", "motion_aa", "lengths", "num_frames",
                                                                    "dt", "length_starts")}, device=DEV), tb
+
+
+@pytest.fixture(scope="module")
+def ml():
+    return _motion_lib(30.0)
+
+
+@pytest.fixture(scope="module")
+def ml_mixed_fps():
+    """Clips at 24 to 120 fps: above 30 fps the step reads a fourth frame row straight from the records."""
+    return _motion_lib((24.0, 25.0, 29.97, 30.0, 50.0, 60.0, 120.0))
 
 
 def _sim(tb, n, seed):
@@ -80,6 +90,16 @@ def test_track_step_equals_full_row_gather(ml, ids, version, pad, advance, fast)
     """v7 over 3 bodies is 385 floats wide and (7,) 367: a dense [N, W] buffer then has every fourth row 3 floats past a 16-byte
     boundary, the rows the kernel stores directly.  `fast`: body velocities 30 times larger (differences well above 8 m/s and rad/s,
     where one rounding exceeds 1e-6).  23 bodies: the widest row beside the 24-float sink of the untracked body."""
+    _track_vs_full(ml, ids, version, pad, advance, fast)
+
+
+@pytest.mark.parametrize("ids,version,pad,advance,fast", [(VR, 6, 0, False, False), (VR, 7, 0, True, False), (tuple(range(24)), 6, 0, False, False),
+                                                          ((23, 5, 13, 0, 18), 6, 0, False, True)])
+def test_track_step_equals_full_row_gather_mixed_fps(ml_mixed_fps, ids, version, pad, advance, fast):
+    _track_vs_full(ml_mixed_fps, ids, version, pad, advance, fast)
+
+
+def _track_vs_full(ml, ids, version, pad, advance, fast):
     from pulse_b200 import _lib
     from pulse_b200.humanoid_im import SELF_OBS, HumanoidImCompute, ImConfig, track_columns
     lib, tb = ml

@@ -11,6 +11,36 @@ from tests.helpers import load_npz
 pytestmark = pytest.mark.gpu
 
 
+def _fixture_clips(z):
+    nf = z["num_frames"].tolist()
+    clips, start = [], 0
+    for i, n in enumerate(nf):
+        a, b = start, start + n
+        start = b
+        clips.append({"pose_quat_global": z["in_pose_quat_global"][a:b].numpy(), "root_trans_offset": z["in_root_trans"][a:b],
+                      "pose_aa": z["in_pose_aa"][a:b].numpy(), "fps": float(z["fps"][i])})
+    return clips
+
+
+def test_device_loader_matches_reference_tables_mixed_fps():
+    """loader_fps.npz: the reference's tables for clips at 24 to 120 fps.  Velocities scale with the rate, so their tolerances scale with
+    fps / 30 frame by frame; lengths and dt are the reference's float64 1 / fps rounded once."""
+    from pulse_b200.motion_lib import MotionLibB200
+    z = load_npz("loader_fps.npz")
+    ml = MotionLibB200.from_clips(_fixture_clips(z), z["parents"].tolist(), z["local_translation"].numpy(), "cuda:0", headings=z["headings"].numpy())
+    scale = torch.repeat_interleave(z["fps"].double() / 30.0, z["num_frames"]).reshape(-1, 1, 1)
+    for k, t, scaled in (("gts", 1e-5, False), ("grs", 1e-6, False), ("lrs", 1e-6, False), ("gvs", 2e-4, True), ("gavs", 2e-4, True),
+                         ("dvs", 1e-3, True)):
+        got, want = getattr(ml, k).cpu().double(), z[k]
+        tol = t * (scale if scaled else 1.0) + 1e-5 * want.abs()
+        bad = (got - want).abs() > tol
+        assert not bool(bad.any()), f"{k}: {int(bad.sum())} elements off, worst {float(((got - want).abs() / tol).max()):.3f} x tol"
+    fps = z["fps"].tolist()
+    nf = z["num_frames"].tolist()
+    assert torch.equal(ml._motion_lengths.cpu(), torch.tensor([1.0 / f * (n - 1) for f, n in zip(fps, nf)], dtype=torch.float32))
+    assert torch.equal(ml._motion_dt.cpu(), torch.tensor([1.0 / f for f in fps], dtype=torch.float32))
+
+
 def test_device_loader_matches_reference_tables():
     from pulse_b200.motion_lib import MotionLibB200
     z = load_npz("loader.npz")

@@ -14,11 +14,11 @@ DEV = "cuda:0"
 ATOL = 1e-4
 
 
-def _setup(n, clips=37, seed=3):
+def _setup(n, clips=37, seed=3, fps=30.0):
     from oracle import pulse_oracle as po
     from pulse_b200.humanoid_im import HumanoidImCompute
     from pulse_b200.motion_lib import MotionLibB200
-    tb = exact_tables(clips, seed=seed)
+    tb = exact_tables(clips, seed=seed, fps=fps)
     z, _ = exact_step_inputs(tb, n, seed=seed + 1)
     ml = MotionLibB200.from_tables({k: getattr(tb, k) for k in ("gts", "grs", "lrs", "gvs", "gavs", "dvs", "motion_aa", "lengths", "num_frames", "dt",
                                                                  "length_starts")}, device=DEV)
@@ -85,9 +85,12 @@ def _compare(d, exp, ids, n):
         assert torch.equal(ours.cpu()[keep], ref[keep])
 
 
-@pytest.mark.parametrize("n,frac", [(300, 0.12), (2051, 0.05), (64, 1.0)])
-def test_reset_envs_mask_mode_matches_oracle(n, frac):
-    po, tb, comp, st, g = _setup(n)
+@pytest.mark.parametrize("n,frac,fps", [pytest.param(300, 0.12, 30.0, id="300-0.12"), pytest.param(2051, 0.05, 30.0, id="2051-0.05"),
+                                        pytest.param(64, 1.0, 30.0, id="64-1.0"),
+                                        pytest.param(2051, 0.3, (24.0, 25.0, 29.97, 50.0, 60.0, 120.0), id="2051-0.3-mixed-fps")])
+def test_reset_envs_mask_mode_matches_oracle(n, frac, fps):
+    """Mixed rates run the reset kernels' own frame blend and slerp (reset_state.cuh) on clips off 30 fps, the AMP history rows included."""
+    po, tb, comp, st, g = _setup(n, fps=fps)
     mask = (torch.rand(n, generator=g) < frac)
     mask[0] = mask[n - 1] = True
     st["reset_buf"] = mask.long() * 3                      # any non-zero value marks a reset

@@ -110,16 +110,27 @@ def test_im_step_mean_reset_matches_reference_golden():
     assert torch.equal(out["terminate_buf"], z["terminate_buf_mean"])
 
 
-@pytest.mark.parametrize("n_envs,n_motions", [(1, 3), (4099, 300)])
-def test_im_step_matches_oracle_random(n_envs, n_motions):
+MIXED_RATES = (24.0, 25.0, 29.97, 30.0, 50.0, 60.0, 120.0)
+
+
+@pytest.mark.parametrize("n_envs,n_motions,fps", [pytest.param(1, 3, 30.0, id="1-3"), pytest.param(4099, 300, 30.0, id="4099-300"),
+                                                  pytest.param(4099, 300, MIXED_RATES, id="4099-300-mixed-fps")])
+def test_im_step_matches_oracle_random(n_envs, n_motions, fps):
+    """Mixed rates: above 30 fps the observation time runs more than a frame ahead of the reward time, so the reward and observation
+    queries can need four distinct frame rows; the fourth has no copy slot and is read straight from the records (im_step.cu's planner)."""
     from oracle import pulse_oracle as po
-    tb = synthetic_tables(n_motions, seed=3, max_frames=200, median_frames=60)
+    tb = synthetic_tables(n_motions, seed=3, max_frames=200, median_frames=60, fps=fps)
     z = synthetic_step_inputs(tb, n_envs, seed=5)
     ref = po.humanoid_im_step(tb, po.ImStepConfig(), z["body_state"], z["dof_vel"], z["dof_force"], z["progress_buf"], z["motion_ids"],
                               z["start_times"], z["start_offset"], z["global_offset"], z["cycle_counter"], z["reset_buf_in"])
     out = _run_step(_mlib(tb), z)
     _check_step(out, ref)
     assert 0 < int(ref["terminate_buf"].sum()) < n_envs or n_envs == 1
+    rows = torch.cat([ref["frame_idx_rew"], ref["frame_idx_obs"]], 1)
+    four = int(sum(len(set(r)) == 4 for r in rows.tolist()))
+    print(f"\n{four} of {n_envs} envs need four distinct frame rows")
+    if fps != 30.0:
+        assert four > 0
 
 
 def test_im_step_strided_unaligned_views():
