@@ -215,8 +215,9 @@ int pulse_amp_obs(const pulse_amp_obs_args_t* args, int64_t num_envs, void* stre
  *                       (Humanoid._action_to_pd_targets, humanoid.py:1392-1394).  eps: injected, or Philox4x32-10(seed,
  *                       row, *rng_offset + rng_step) drawn in the kernel (a device-side offset keeps CUDA-graph replays fresh).
  *   pulse_value_post    next_values = unnormalise(critic(next obs)) * (1 - terminated)   (amp_agent.py:396-398)
- *   pulse_amp_obs_row   AMP observation row of this step = [current 196 | first (steps-1)*196 floats of the previous row], written
- *                       into its experience slice (humanoid_amp.py:622-667 + amp_agent.py:385)
+ *   pulse_amp_obs_row   AMP observation row of this step = [current W | first (steps-1)*W floats of the previous row], written
+ *                       into its experience slice (humanoid_amp.py:622-667 + amp_agent.py:385); W = amp_width (196 by default, 195
+ *                       without the root height), the heading of remove_base_rot(q0) with remove_base_rot set
  *   pulse_bump_counter  *counter += by (one thread): advances the device-side RNG offset once per iteration
  * ---------------------------------------------------------------------------------------------- */
 typedef struct {
@@ -243,7 +244,9 @@ typedef struct {
   float* out; int64_t ld_out;                /* this step's row */
   int32_t num_steps; int32_t reserved;
   int32_t* fresh;                            /* [N] optional flags set by pulse_reset_ref_state; cleared here */
-  const float* fresh_rows;                   /* [N, num_steps, 196] the back-filled rows of reset envs */
+  const float* fresh_rows;                   /* [N, num_steps, amp_width] the back-filled rows of reset envs */
+  int32_t amp_width;                         /* 0 or 196: the whole row; 195: without the root height (ampRootHeightObs False) */
+  int32_t remove_base_rot;                   /* 0: upright start; 1: the heading and root rotation feature of remove_base_rot(q0) */
 } pulse_amp_row_args_t;
 int pulse_amp_obs_row(const pulse_amp_row_args_t* args, int64_t num_envs, void* stream);
 int pulse_bump_counter(uint64_t* counter, uint64_t by, void* stream);
@@ -784,6 +787,13 @@ int pulse_ztask_obs_list(const pulse_ztask_step_args_t* args, const int64_t* env
  *   index e + 3 * 2^32 pulse_ztask_pre_physics (_update_task of the rollout): x, y, z task uniforms, w change steps
  *   index e + 4 * 2^32 pulse_traj_reset_list: counter PULSE_TRAJ_VERTS * (offset + *offset_dev) + k, k <= PULSE_TRAJ_VERTS - 1
  *                      (the pedestrian terrain task's waypoints; block k < S: segment k, block S: heading and speed)
+ * The AMP demo and replay rings (pulse_amp_demo_fetch, pulse_amp_replay_store, pulse_amp_ring_sample) key their draws by the ring's own
+ * seed, one index plane per draw (PULSE_PLANE_* below, i.e. index i + plane * 2^32), counter = the ring's draw or permutation counter:
+ *   index i + 5 * 2^32 x: demo clip of fetched row i (inverse CDF)       counter ctr[PULSE_RING_DRAWS]
+ *   index i + 6 * 2^32 x: demo start-time phase of fetched row i         counter ctr[PULSE_RING_DRAWS]
+ *   index r + 7 * 2^32 x: replay keep mask of stored row r (u < p)       counter ctr[PULSE_RING_DRAWS]
+ *   index 8 * 2^32     x, y, z, w: Feistel round keys of the subset      counter ctr[PULSE_RING_DRAWS]
+ *   index 9 * 2^32     x, y, z, w: Feistel round keys of the sampling permutation   counter ctr[PULSE_RING_PERM_KEY]
  * pulse_reset_terrain reads index e as above, with word z as the spawn location (w unused).
  * ---------------------------------------------------------------------------------------------- */
 #define PULSE_ZTASK_REACH 3
@@ -832,6 +842,8 @@ typedef struct {
   int32_t* actor_list;           /* [N] out, optional */
   int32_t* tar_actor_list;       /* [N] out, optional */
   int32_t* count;                /* [1] out, device side */
+  int32_t* amp_fresh;            /* [N] optional: set to 1 for every reset env -- pulse_amp_obs_row then takes that env's history from
+                                    amp_obs_buf (the back-filled rows) at the next step; requires amp_obs_buf */
 } pulse_ztask_reset_args_t;
 int pulse_reset_ztask(const pulse_motionlib_t* lib, const pulse_ztask_reset_args_t* args, int64_t num_envs, void* stream);
 
@@ -1124,6 +1136,87 @@ typedef struct {
 } pulse_terrain_spawn_args_t;
 int pulse_reset_terrain(const pulse_motionlib_t* lib, const pulse_ztask_reset_args_t* args, const pulse_terrain_spawn_args_t* spawn,
                         int64_t num_envs, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * AMP demo and replay rings on the device (learning/replay_buffer.py ReplayBuffer; AMPAgent._init_amp_demo_buf, _update_amp_demos,
+ * _store_replay_amp_obs and the buffer samples of train_epoch, phc/learning/amp_agent.py:476-484, :988-1000, :1043-1057), with every
+ * counter on the device so that no call reads anything back to the host.  A ring is `capacity` rows of `row_floats` floats and the
+ * int64 counters ctr[PULSE_RING_CTRS]:
+ *   head, total_count, sample_head   the ReplayBuffer's _head, _total_count, _sample_head;
+ *   perm_key                         the number of _reset_sample_idx calls: the sampling permutation _sample_idx is the keyed Feistel
+ *                                    bijection of [0, capacity) with round keys Philox(seed, 9 * 2^32, perm_key), cycle-walked;
+ *   draws                            the number of fetches / stores (the counter of their Philox draws);
+ *   last_count                       the rows the last replay store kept (scratch of pulse_amp_replay_store).
+ * The Feistel network: the smallest even bit width 2h >= max(2, ceil(log2 m)) over the domain [0, m); four rounds
+ * (L, R) <- (R, L ^ (F(R, k_r) & (2^h - 1))) with F(x, k) = fmix32(x * 0x9E3779B1 ^ k) (MurmurHash3's finaliser), repeated until the
+ * value falls inside [0, m).
+ * pulse_amp_demo_fetch   fetch_amp_obs_demo + build_amp_obs_demo (phc/env/tasks/humanoid_amp.py:215-284) of num_samples rows straight
+ *                        into the ring, then store()'s head / total_count update: per row a clip (inverse CDF of sampling_cdf), t0 by
+ *                        sample_time_interval (the SMPL _sample_time, :376-380), the motion at t0 - k dt for k < num_steps without the
+ *                        ground fix, build_amp_observations_smpl in amp_width 196 / 195 and the upright setting.  24-body SMPL only.
+ * pulse_amp_replay_store _store_replay_amp_obs: once total_count > capacity a Bernoulli(keep_prob) keep mask, the ordered compaction of
+ *                        the kept rows, a random subset of capacity rows (Feistel permutation of the kept count, subset keys) when more
+ *                        survive, then the ring write with wrap and the counter update.
+ * pulse_amp_ring_sample  sample(n): positions sample_head + j mod capacity through the permutation, `% head` while total_count <
+ *                        capacity, `fallback` row j (the agent's own rows) while the ring is empty; only the sample rows j with
+ *                        j mod block < take are gathered (the first `take` rows of every `block`-row minibatch), but sample_head moves by
+ *                        the whole n (and to 0 with a new perm_key once it reaches capacity), as the reference's sample(n) does.
+ * ---------------------------------------------------------------------------------------------- */
+#define PULSE_PLANE_DEMO_CLIP 5
+#define PULSE_PLANE_DEMO_TIME 6
+#define PULSE_PLANE_REPLAY_KEEP 7
+#define PULSE_PLANE_REPLAY_SUBSET 8
+#define PULSE_PLANE_RING_PERM 9
+#define PULSE_RING_HEAD 0
+#define PULSE_RING_TOTAL 1
+#define PULSE_RING_SAMPLE_HEAD 2
+#define PULSE_RING_PERM_KEY 3
+#define PULSE_RING_DRAWS 4
+#define PULSE_RING_LAST_COUNT 5
+#define PULSE_RING_CTRS 8
+
+typedef struct {
+  float* rows;                   /* [capacity, row_floats] */
+  int64_t capacity;              /* buffer_size, 1 .. 2^31 - 1 */
+  int64_t* ctr;                  /* [PULSE_RING_CTRS] device counters, zero for a new ring */
+  uint64_t seed;                 /* Philox key of the ring's draws */
+  int32_t row_floats;            /* num_steps * width */
+  int32_t reserved;
+} pulse_amp_ring_t;
+
+typedef struct {
+  pulse_amp_ring_t ring;
+  const float* sampling_cdf;     /* [num_motions] inclusive fp32 prefix sum of _sampling_batch_prob */
+  int64_t num_samples;           /* rows fetched, <= capacity */
+  int32_t num_steps;             /* numAMPObsSteps, 1 .. 16 */
+  int32_t amp_width;             /* 196 or 195 */
+  int32_t upright;               /* _has_upright_start */
+  float dt;                      /* control dt */
+  int64_t* motion_ids_out;       /* [num_samples] optional: the drawn clips */
+  float* times_out;              /* [num_samples] optional: the drawn t0 */
+} pulse_amp_demo_args_t;
+int pulse_amp_demo_fetch(const pulse_motionlib_t* lib, const pulse_amp_demo_args_t* args, void* stream);
+
+typedef struct {
+  pulse_amp_ring_t ring;
+  const float* src;              /* [num_rows, row_floats] contiguous rows of the horizon (batch_dict['amp_obs']) */
+  int64_t num_rows;              /* < 2^31 */
+  float keep_prob;               /* amp_replay_keep_prob */
+  int32_t reserved;
+  int32_t* kept;                 /* [num_rows] scratch: the kept row ids, ascending */
+  int64_t* src_rows_out;         /* [min(num_rows, capacity)] optional: the source row of the i-th stored row, -1 past the stored count */
+} pulse_amp_store_args_t;
+int pulse_amp_replay_store(const pulse_amp_store_args_t* args, void* stream);
+
+typedef struct {
+  pulse_amp_ring_t ring;
+  int64_t n;                     /* rows of the reference's sample(n); a multiple of block */
+  int64_t block, take;           /* gather sample rows j with j mod block < take, 1 <= take <= block */
+  const float* fallback;         /* [n, row_floats] rows used while total_count == 0 (sample_head then stays), or NULL: zeros */
+  float* out;                    /* [n / block * take, row_floats] */
+  int64_t* ring_rows_out;        /* [n / block * take] optional: the ring row of each gathered row, -1 for a fallback row */
+} pulse_amp_sample_args_t;
+int pulse_amp_ring_sample(const pulse_amp_sample_args_t* args, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Task observation for every observation version / tracked-body subset / number of future samples (SURVEY 8f-4): replaces the

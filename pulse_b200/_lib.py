@@ -122,7 +122,7 @@ class AmpRowArgs(C.Structure):
         ("body_state", C.c_void_p), ("body_env_stride", C.c_int64), ("dof_pos", C.c_void_p), ("dof_vel", C.c_void_p),
         ("dof_env_stride", C.c_int64), ("dof_elem_stride", C.c_int64), ("prev", C.c_void_p), ("ld_prev", C.c_int64),
         ("out", C.c_void_p), ("ld_out", C.c_int64), ("num_steps", C.c_int32), ("reserved", C.c_int32),
-        ("fresh", C.c_void_p), ("fresh_rows", C.c_void_p),
+        ("fresh", C.c_void_p), ("fresh_rows", C.c_void_p), ("amp_width", C.c_int32), ("remove_base_rot", C.c_int32),
     ]
 
 
@@ -225,8 +225,32 @@ class ZTaskResetArgs(C.Structure):
         ("contact_forces", C.c_void_p), ("contact_env_stride", C.c_int64), ("contact_bodies", C.c_int32), ("reserved", C.c_int32),
         ("target_states", C.c_void_p), ("target_env_stride", C.c_int64), ("near_prob", C.c_float), ("near_dist", C.c_float),
         ("tar_dist_min", C.c_float), ("tar_dist_max", C.c_float), ("actor_ids", C.c_void_p), ("tar_actor_ids", C.c_void_p),
-        ("env_list", C.c_void_p), ("actor_list", C.c_void_p), ("tar_actor_list", C.c_void_p), ("count", C.c_void_p),
+        ("env_list", C.c_void_p), ("actor_list", C.c_void_p), ("tar_actor_list", C.c_void_p), ("count", C.c_void_p), ("amp_fresh", C.c_void_p),
     ]
+
+
+PLANE_DEMO_CLIP, PLANE_DEMO_TIME, PLANE_REPLAY_KEEP, PLANE_REPLAY_SUBSET, PLANE_RING_PERM = 5, 6, 7, 8, 9
+RING_HEAD, RING_TOTAL, RING_SAMPLE_HEAD, RING_PERM_KEY, RING_DRAWS, RING_LAST_COUNT, RING_CTRS = 0, 1, 2, 3, 4, 5, 8
+
+
+class AmpRing(C.Structure):
+    _fields_ = [("rows", C.c_void_p), ("capacity", C.c_int64), ("ctr", C.c_void_p), ("seed", C.c_uint64), ("row_floats", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+class AmpDemoArgs(C.Structure):
+    _fields_ = [("ring", AmpRing), ("sampling_cdf", C.c_void_p), ("num_samples", C.c_int64), ("num_steps", C.c_int32), ("amp_width", C.c_int32),
+                ("upright", C.c_int32), ("dt", C.c_float), ("motion_ids_out", C.c_void_p), ("times_out", C.c_void_p)]
+
+
+class AmpStoreArgs(C.Structure):
+    _fields_ = [("ring", AmpRing), ("src", C.c_void_p), ("num_rows", C.c_int64), ("keep_prob", C.c_float), ("reserved", C.c_int32),
+                ("kept", C.c_void_p), ("src_rows_out", C.c_void_p)]
+
+
+class AmpSampleArgs(C.Structure):
+    _fields_ = [("ring", AmpRing), ("n", C.c_int64), ("block", C.c_int64), ("take", C.c_int64), ("fallback", C.c_void_p), ("out", C.c_void_p),
+                ("ring_rows_out", C.c_void_p)]
 
 
 class ZTaskTaskArgs(C.Structure):
@@ -497,6 +521,9 @@ SIGNATURES = {
     "pulse_smplx_speed_obs_list": (C.c_int, [C.POINTER(SmplxSpeedStepArgs), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_smplx_speed_rollout_step": (C.c_int, [C.POINTER(SmplxSpeedStepArgs), C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_reset_ztask_smplx": (C.c_int, [C.c_void_p, C.POINTER(ZTaskResetArgs), C.c_int64, C.c_void_p]),
+    "pulse_amp_demo_fetch": (C.c_int, [C.c_void_p, C.POINTER(AmpDemoArgs), C.c_void_p]),
+    "pulse_amp_replay_store": (C.c_int, [C.POINTER(AmpStoreArgs), C.c_void_p]),
+    "pulse_amp_ring_sample": (C.c_int, [C.POINTER(AmpSampleArgs), C.c_void_p]),
 }
 
 _lib = None

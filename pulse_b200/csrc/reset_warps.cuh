@@ -7,7 +7,7 @@
 // The entry points, argument structs and Philox word layout are documented in include/pulse_b200.h.
 #pragma once
 #include "compact.cuh"
-#include "humanoid_obs.cuh"
+#include "motion_amp.cuh"
 #include "philox.cuh"
 
 namespace pulse {
@@ -34,34 +34,9 @@ __global__ void __launch_bounds__(kCompactThreads) reset_compact_kernel(const pu
     a.env_list[pos] = env;
     if (a.actor_list != nullptr) a.actor_list[pos] = a.actor_ids != nullptr ? a.actor_ids[env] : static_cast<int>(env);
     if (a.tar_actor_list != nullptr) a.tar_actor_list[pos] = a.tar_actor_ids != nullptr ? a.tar_actor_ids[env] : static_cast<int>(env);
+    if (a.amp_fresh != nullptr) a.amp_fresh[env] = 1;
   }
   if (threadIdx.x == 0) *a.count = base;
-}
-
-// sample_motions: the first clip whose inclusive CDF exceeds u * total (a zero-weight clip never does before its predecessor).
-__device__ __forceinline__ long long pick_motion(const float* cdf, long long m, float u) {
-  const float total = cdf[m - 1];
-  float v = __fmul_rn(u, total);
-  if (v >= total) v = nextafterf(total, 0.0f);
-  long long lo = 0, hi = m - 1;
-  while (lo < hi) {
-    const long long mid = (lo + hi) >> 1;
-    if (cdf[mid] > v) hi = mid;
-    else lo = mid + 1;
-  }
-  return lo;
-}
-
-// build_amp_observations_smpl into the warp's staging row, then `width` floats of it to `out`: 196 is the whole row, 195 drops the
-// root height.  A non-upright start takes the heading and root rotation feature of remove_base_rot(q0).
-template <class JointFn, class KeyPosFn>
-__device__ __forceinline__ void store_amp_row(float* out, int width, float* stage, int lane, Vec3 p0, Quat q0, Vec3 v0, Vec3 w0, bool upright,
-                                              JointFn joint, KeyPosFn key_pos) {
-  store_amp_obs(stage, lane, p0, base_rot_removed(q0, upright), v0, w0, joint, key_pos);
-  __syncwarp();
-  const int skip = PULSE_AMP_OBS - width;
-  for (int c = lane; c < width; c += 32) out[c] = stage[skip + c];
-  __syncwarp();
 }
 
 // The work of one warp in body layout L (lib: the layout's MotionLib descriptor).  `adjust(e, lane, r0, off, p, rq, v, rp, rr, rv, rw)`
@@ -81,7 +56,6 @@ __device__ __forceinline__ void reset_warps(const Lib& lib, const pulse_ztask_re
   const long long items = static_cast<long long>(*a.count) * steps;
   const unsigned long long off = a.offset + (a.offset_dev != nullptr ? *a.offset_dev : 0ull);
   const bool upright = a.upright != 0;
-  const float step30 = static_cast<float>(1.0 / 30.0);
   for (long long it = warp0; it < items; it += nwarps) {
     const long long i = it / steps;
     const int k = static_cast<int>(it - i * steps);
@@ -95,7 +69,7 @@ __device__ __forceinline__ void reset_warps(const Lib& lib, const pulse_ztask_re
     float t0 = 0.0f;
     if (a.state_init == PULSE_ZINIT_RANDOM) {   // sample_time_interval: ((phase * motion_len) / curr_fps).long() * curr_fps
       const float ph = a.phase != nullptr ? a.phase[e] : u01(r0.x);
-      t0 = __fmul_rn(__ll2float_rn(static_cast<long long>(__fdiv_rn(__fmul_rn(ph, mlen), step30))), step30);
+      t0 = sample_time_interval(ph, mlen);
     }
     const float t = k == 0 ? t0 : __fadd_rn(t0, __fmul_rn(-a.dt, static_cast<float>(k)));
     long long i0, i1;
@@ -109,19 +83,8 @@ __device__ __forceinline__ void reset_warps(const Lib& lib, const pulse_ztask_re
 
     if constexpr (L::kSmplTerms) {
       if (k > 0) {   // _init_amp_obs_ref: the motion at t0 - k dt as it is, without the ground fix or the pose adjustment
-        const Vec3 p0 = {lerp_rn(r0p[0], r1p[0], b), lerp_rn(r0p[1], r1p[1], b), lerp_rn(r0p[2], r1p[2], b)};
-        const Vec3 v0 = {lerp_rn(r0p[168], r1p[168], b), lerp_rn(r0p[169], r1p[169], b), lerp_rn(r0p[170], r1p[170], b)};
-        const Vec3 w0 = {lerp_rn(r0p[240], r1p[240], b), lerp_rn(r0p[241], r1p[241], b), lerp_rn(r0p[242], r1p[242], b)};
-        const Quat q0 = slerp(ldq4(r0p + 72), ldq4(r1p + 72), b);
-        const auto joint = [&](int jt) {
-          return AmpJoint{quat_exp_map(slerp(ldq4(x0 + 4 * (jt + 1)), ldq4(x1 + 4 * (jt + 1)), b)),
-                          {lerp_rn(x0[96 + 3 * jt], x1[96 + 3 * jt], b), lerp_rn(x0[97 + 3 * jt], x1[97 + 3 * jt], b),
-                           lerp_rn(x0[98 + 3 * jt], x1[98 + 3 * jt], b)}};
-        };
-        const auto key_pos = [&](int kb) {
-          return Vec3{lerp_rn(r0p[3 * kb], r1p[3 * kb], b), lerp_rn(r0p[3 * kb + 1], r1p[3 * kb + 1], b), lerp_rn(r0p[3 * kb + 2], r1p[3 * kb + 2], b)};
-        };
-        store_amp_row(a.amp_obs_buf + (e * a.num_amp_steps + k) * a.amp_width, a.amp_width, stage, lane, p0, q0, v0, w0, upright, joint, key_pos);
+        store_motion_amp_row(b, r0p, r1p, x0, x1, a.amp_obs_buf + (e * a.num_amp_steps + k) * a.amp_width, a.amp_width, stage, lane,
+                             upright);
         continue;
       }
     }

@@ -9,8 +9,10 @@
 //                       experience slice (humanoid_amp.py:622-667 + amp_agent.py:385): 7 056 B read + 7 840 B written per env instead
 //                       of the in-place shift (7 056 + 7 840) followed by a 7 840 + 7 840 B copy.  Envs reset since the last step take
 //                       their previous row from the rows `pulse_reset_ref_state` back-filled (`fresh` flags, cleared here).
+//   amp_row_any_kernel  the same row in the other layouts the resets write: 195 floats (no root height; rows are 780 B, so not
+//                       16-byte units) and / or the remove_base_rot heading of a non-upright start.
 #include "philox.cuh"
-#include "humanoid_obs.cuh"
+#include "motion_amp.cuh"
 #include "value_unnorm.cuh"
 
 namespace pulse {
@@ -100,9 +102,37 @@ __global__ void __launch_bounds__(128) amp_row_kernel(const pulse_amp_row_args_t
     }
     for (int c = lane + 512; c < nvec; c += 32) dst[c] = src[c];   // more than 11 history steps
   }
+  __syncwarp();   // every lane has read the flag before lane 0 clears it
   if (fresh && lane == 0) a.fresh[e] = 0;
   // ---- current observation -------------------------------------------------------------------------------------------------------
   store_amp_obs_sim(out, lane, a, e);
+}
+
+constexpr int kAmpRowWarps = 4;
+
+__global__ void __launch_bounds__(kAmpRowWarps * 32) amp_row_any_kernel(const pulse_amp_row_args_t a, int width, long long n) {
+  __shared__ float stage_all[kAmpRowWarps][PULSE_AMP_OBS];
+  const long long e = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (e >= n) return;
+  float* out = a.out + e * a.ld_out;
+  const bool fresh = a.fresh != nullptr && a.fresh[e] != 0;
+  const float* prev = fresh ? a.fresh_rows + e * (long long)a.num_steps * width : a.prev + e * a.ld_prev;
+  const int hist = (a.num_steps - 1) * width;
+  for (int c = lane; c < hist; c += 32) __stcs(out + width + c, __ldcs(prev + c));
+  __syncwarp();   // every lane has read the flag before lane 0 clears it
+  if (fresh && lane == 0) a.fresh[e] = 0;
+  const float* bs = a.body_state + e * a.body_env_stride;
+  const float* dp = a.dof_pos + e * a.dof_env_stride;
+  const float* dv = a.dof_vel + e * a.dof_env_stride;
+  const long long ds = a.dof_elem_stride;
+  const auto joint = [&](int jt) {
+    return AmpJoint{{dp[(3 * jt + 0) * ds], dp[(3 * jt + 1) * ds], dp[(3 * jt + 2) * ds]},
+                    {dv[(3 * jt + 0) * ds], dv[(3 * jt + 1) * ds], dv[(3 * jt + 2) * ds]}};
+  };
+  const auto key_pos = [&](int kb) { return ldv(bs + kb * PULSE_BODY_STATE_W); };
+  store_amp_row(out, width, stage_all[threadIdx.x >> 5], lane, ldv(bs), ldq(bs + 3), ldv(bs + 7), ldv(bs + 10), a.remove_base_rot == 0, joint,
+                key_pos);
 }
 
 __global__ void bump_counter_kernel(unsigned long long* c, unsigned long long by) { *c += by; }
@@ -150,12 +180,21 @@ extern "C" int pulse_amp_obs_row(const pulse_amp_row_args_t* args, int64_t num_e
   const pulse_amp_row_args_t& a = *args;
   PULSE_REQUIRE(a.body_state && a.dof_pos && a.dof_vel && a.prev && a.out, "pulse_amp_obs_row: null buffer");
   PULSE_REQUIRE(a.num_steps >= 1 && a.num_steps <= 16, "pulse_amp_obs_row: num_steps %d outside [1,16]", a.num_steps);
-  PULSE_REQUIRE(a.ld_prev >= (a.num_steps - 1) * PULSE_AMP_OBS && a.ld_out >= a.num_steps * PULSE_AMP_OBS, "pulse_amp_obs_row: row strides too small");
-  PULSE_REQUIRE(aligned16(a.prev) && aligned16(a.out) && (a.ld_prev % 4) == 0 && (a.ld_out % 4) == 0, "pulse_amp_obs_row: rows must be 16-byte aligned");
+  PULSE_REQUIRE(a.amp_width == 0 || a.amp_width == PULSE_AMP_OBS || a.amp_width == PULSE_AMP_OBS_NO_HEIGHT,
+                "pulse_amp_obs_row: amp_width %d is neither %d nor %d", a.amp_width, PULSE_AMP_OBS, PULSE_AMP_OBS_NO_HEIGHT);
+  const int width = a.amp_width == 0 ? PULSE_AMP_OBS : a.amp_width;
+  PULSE_REQUIRE(a.ld_prev >= (a.num_steps - 1) * width && a.ld_out >= a.num_steps * width, "pulse_amp_obs_row: row strides too small");
   PULSE_REQUIRE(a.prev != a.out, "pulse_amp_obs_row: prev and out must be different experience slices (use pulse_amp_obs for the in-place shift)");
   PULSE_REQUIRE((a.fresh == nullptr) == (a.fresh_rows == nullptr), "pulse_amp_obs_row: fresh flags and fresh_rows go together");
-  PULSE_REQUIRE(a.fresh_rows == nullptr || aligned16(a.fresh_rows), "pulse_amp_obs_row: fresh_rows not 16-byte aligned");
   PULSE_REQUIRE(a.body_env_stride >= PULSE_NUM_BODIES * PULSE_BODY_STATE_W, "pulse_amp_obs_row: body_env_stride too small");
+  if (width != PULSE_AMP_OBS || a.remove_base_rot != 0) {
+    amp_row_any_kernel<<<static_cast<unsigned>((num_envs + kAmpRowWarps - 1) / kAmpRowWarps), kAmpRowWarps * 32, 0,
+                         static_cast<cudaStream_t>(stream)>>>(a, width, (long long)num_envs);
+    PULSE_LAUNCH_OK("amp_row_any_kernel");
+    return PULSE_OK;
+  }
+  PULSE_REQUIRE(aligned16(a.prev) && aligned16(a.out) && (a.ld_prev % 4) == 0 && (a.ld_out % 4) == 0, "pulse_amp_obs_row: rows must be 16-byte aligned");
+  PULSE_REQUIRE(a.fresh_rows == nullptr || aligned16(a.fresh_rows), "pulse_amp_obs_row: fresh_rows not 16-byte aligned");
   const long long threads = num_envs * 32;
   amp_row_kernel<<<static_cast<unsigned>((threads + 127) / 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(a, (long long)num_envs);
   PULSE_LAUNCH_OK("amp_row_kernel");

@@ -65,6 +65,7 @@ extern "C" int pulse_reset_terrain(const pulse_motionlib_t* lib, const pulse_zta
   PULSE_REQUIRE(a.state_init == PULSE_ZINIT_RANDOM, "pulse_reset_terrain: state_init %d, the terrain task always samples the start time (RANDOM)",
                 a.state_init);
   PULSE_REQUIRE(a.amp_obs_buf == nullptr || (a.num_amp_steps >= 1 && a.num_amp_steps <= 16), "pulse_reset_terrain: num_amp_steps outside [1,16]");
+  PULSE_REQUIRE(a.amp_fresh == nullptr || a.amp_obs_buf != nullptr, "pulse_reset_terrain: amp_fresh flags need the back-filled amp_obs_buf");
   PULSE_REQUIRE(a.amp_obs_buf == nullptr || a.amp_width == PULSE_AMP_OBS || a.amp_width == PULSE_AMP_OBS_NO_HEIGHT,
                 "pulse_reset_terrain: amp_width %d is neither %d nor %d", a.amp_width, PULSE_AMP_OBS, PULSE_AMP_OBS_NO_HEIGHT);
   PULSE_REQUIRE(lib->d.aux_rec != nullptr, "pulse_reset_terrain: the MotionLib handle has no aux records (dof_pos / dof_vel)");

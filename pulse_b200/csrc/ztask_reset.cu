@@ -104,6 +104,7 @@ extern "C" int pulse_reset_ztask(const pulse_motionlib_t* lib, const pulse_ztask
   PULSE_REQUIRE(a.pose_mode >= PULSE_ZPOSE_AS_IS && a.pose_mode <= PULSE_ZPOSE_FACE_X, "pulse_reset_ztask: unknown pose_mode %d", a.pose_mode);
   PULSE_REQUIRE(a.state_init == PULSE_ZINIT_RANDOM || a.state_init == PULSE_ZINIT_START, "pulse_reset_ztask: unknown state_init %d", a.state_init);
   PULSE_REQUIRE(a.amp_obs_buf == nullptr || (a.num_amp_steps >= 1 && a.num_amp_steps <= 16), "pulse_reset_ztask: num_amp_steps outside [1,16]");
+  PULSE_REQUIRE(a.amp_fresh == nullptr || a.amp_obs_buf != nullptr, "pulse_reset_ztask: amp_fresh flags need the back-filled amp_obs_buf");
   PULSE_REQUIRE(a.amp_obs_buf == nullptr || a.amp_width == PULSE_AMP_OBS || a.amp_width == PULSE_AMP_OBS_NO_HEIGHT,
                 "pulse_reset_ztask: amp_width %d is neither %d nor %d", a.amp_width, PULSE_AMP_OBS, PULSE_AMP_OBS_NO_HEIGHT);
   PULSE_REQUIRE(lib->d.aux_rec != nullptr, "pulse_reset_ztask: the MotionLib handle has no aux records (dof_pos / dof_vel)");
@@ -150,6 +151,7 @@ extern "C" int pulse_reset_ztask_smplx(const pulse_smplx_motionlib_t* lib, const
   PULSE_REQUIRE(a.contact_forces == nullptr || (a.contact_bodies >= 0 && a.contact_env_stride >= 3 * a.contact_bodies),
                 "pulse_reset_ztask_smplx: bad contact-force strides");
   PULSE_REQUIRE(a.amp_obs_buf == nullptr, "pulse_reset_ztask_smplx: the AMP history back-fill is not served for SMPL-X (amp_obs_buf must be NULL)");
+  PULSE_REQUIRE(a.amp_fresh == nullptr, "pulse_reset_ztask_smplx: no AMP rows for SMPL-X (amp_fresh must be NULL)");
   PULSE_REQUIRE(a.target_states == nullptr, "pulse_reset_ztask_smplx: the SMPL-X reset serves the speed task (target_states must be NULL)");
   PULSE_REQUIRE(a.pose_mode == PULSE_ZPOSE_FACE_X, "pulse_reset_ztask_smplx: pose_mode %d, the speed task's is PULSE_ZPOSE_FACE_X", a.pose_mode);
   PULSE_REQUIRE(a.floor != nullptr && a.floor_len >= lib->d.total_frames, "pulse_reset_ztask_smplx: floor table of %lld frames, the MotionLib has %lld",

@@ -35,7 +35,7 @@ def compute_from_task(task) -> HumanoidImCompute:
     return HumanoidImCompute.from_task(task, track_body_ids=tuple(int(j) for j in task._track_bodies_id), obs_version=obs_v)
 
 
-def check_pieces(comp, policy, vae) -> None:
+def check_pieces(comp, policy, vae, amp=None) -> None:
     """Checks that the tracked-body compute, the latent policy and the frozen VAE belong together; raises PulseError naming the mismatch."""
     who = "ImZStepsB200"
     if not isinstance(comp, HumanoidImCompute) or comp.track is None:
@@ -44,8 +44,11 @@ def check_pieces(comp, policy, vae) -> None:
         raise _lib.PulseError(f"{who}: cycle_motion is not supported (its start-time rewrite of wrapped envs runs on the host)")
     if comp.cfg.use_mean_reset:
         raise _lib.PulseError(f"{who}: use_mean_reset (the im_eval criterion) is an evaluation setting, not a training one")
-    if getattr(policy, "disc", None) is not None:
-        raise _lib.PulseError(f"{who}: the discriminator is not part of this driver (task reward only); build the policy without it")
+    if (getattr(policy, "disc", None) is not None) != (amp is not None):
+        raise _lib.PulseError(f"{who}: a policy with a discriminator needs the AMP part (amp=AmpBuffersB200) and the AMP part a discriminator")
+    if amp is not None and (amp.amp_width != 196 or not amp.upright):
+        raise _lib.PulseError(f"{who}: the reference-state reset back-fills 196-float upright AMP rows, the AMP part has {amp.amp_width} "
+                              f"(upright {amp.upright})")
     if int(policy.obs_size) != comp.obs_size:
         raise _lib.PulseError(f"{who}: the tracked observation has {comp.obs_size} floats, the policy reads {policy.obs_size}")
     if int(vae.S) != SELF_OBS or int(vae.A) != 69:
@@ -84,28 +87,32 @@ class ImZStepsB200(LatentStepsB200):
 
     `comp`: a HumanoidImCompute with `track_body_ids` set (`compute_from_task(task)` builds it from a live task with the settings the
     HumanoidIm mixin reads); its MotionLib serves the reset and the steps.  `policy`: PPOPolicy(obs_size=comp.obs_size,
-    num_actions=vae.E, units=(2048, 1536, 1024, 1024, 512, 512), act="silu", logstd=-1.5) without discriminator (pulse_z_vr.yaml).
+    num_actions=vae.E, units=(2048, 1536, 1024, 1024, 512, 512), act="silu", logstd=-1.5) (pulse_z_vr.yaml).
     `vae`: PulseVAE(with_critic=False) holding the frozen prior, decoder and the checkpoint's obs_rms.  `sim`: the simulator's and the
     task's tensors, read and written in place through their strides: body_state, root_states, dof_pos, dof_vel, progress_buf,
     motion_ids (`_sampled_motion_ids`), motion_start_times, motion_start_offset (`_motion_start_times_offset`), global_offset;
     dof_force with power_reward; optional contact_forces (cleared for the reset envs) and actor_ids.
 
-    Out of scope: the discriminator (pulse_z_vr.yaml still trains it with disc_coef 5 although disc_reward_w is 0; leaving it out does
-    not change the reward, but it removes the discriminator's gradients from the shared gradient-norm clip, so the reset is called
-    without an AMP buffer); the fut_tracks windows, observation versions 1/2/3/8/9, non-upright starts, zero_out_far and occlusion;
+    With the AMP part (`amp`, an AmpBuffersB200 of 196-float upright rows over the comp's MotionLib, given exactly when the policy has a
+    discriminator) the reset back-fills the AMP history through pulse_reset_ref_state's AMP path and `train_epoch()` trains the
+    discriminator inside the shared gradient-norm clip, as pulse_z_vr.yaml does (LatentStepsB200).
+
+    Out of scope: the fut_tracks windows, observation versions 1/2/3/8/9, non-upright starts, zero_out_far and occlusion;
     multi-GPU; the smplx humanoid; an agent mixin (INTEGRATION.md wires the hooks).  The IMAmpAgent evaluation pass is `evaluate`."""
 
     def __init__(self, comp: HumanoidImCompute, policy, vae, sim: dict, horizon: int = 32, pd_offset: Optional[torch.Tensor] = None,
                  pd_scale: Optional[torch.Tensor] = None, pd_freeze: Optional[torch.Tensor] = None, use_graphs: bool = True,
-                 gamma: float = 0.99, tau: float = 0.95, reset_seed: int = 0):
-        check_pieces(comp, policy, vae)
+                 gamma: float = 0.99, tau: float = 0.95, reset_seed: int = 0, amp=None, task_reward_w: float = 1.0,
+                 disc_reward_w: float = 0.0):
+        check_pieces(comp, policy, vae, amp)
         keys = SIM_KEYS + (("dof_force",) if comp.cfg.power_reward else ())
         missing = [k for k in keys if sim.get(k) is None]
         if missing:
             raise _lib.PulseError(f"ImZStepsB200: sim lacks {missing}")
         self.n = int(sim["progress_buf"].shape[0])
         self.comp = comp
-        self._setup(comp, comp, policy, vae, sim, horizon, comp.obs_size, pd_offset, pd_scale, pd_freeze, use_graphs, gamma, tau, reset_seed)
+        self._setup(comp, comp, policy, vae, sim, horizon, comp.obs_size, pd_offset, pd_scale, pd_freeze, use_graphs, gamma, tau, reset_seed,
+                    amp, task_reward_w, disc_reward_w)
 
     # ------------------------------------------------------------------ the task's pieces of one step
     def _state(self) -> dict:
@@ -120,7 +127,8 @@ class ImZStepsB200(LatentStepsB200):
             motion_ids=s["motion_ids"], motion_start_times=s["motion_start_times"], motion_start_offset=s["motion_start_offset"],
             global_offset=s["global_offset"], progress_buf=s["progress_buf"], root_states=s["root_states"], dof_pos=s["dof_pos"],
             dof_vel=s["dof_vel"], rigid_body_state=s["body_state"], reset_buf=self.reset_buf, contact_forces=s.get("contact_forces"),
-            actor_ids=s.get("actor_ids"), seed=self.reset_seed, offset=t, offset_dev=self.policy.rng_offset)
+            actor_ids=s.get("actor_ids"), seed=self.reset_seed, offset=t, offset_dev=self.policy.rng_offset,
+            amp_obs_buf=self.amp_init if self.amp is not None else None, amp_fresh=self.amp_fresh if self.amp is not None else None)
 
     def _reset_obs(self, t: int) -> None:
         """`_compute_observations(env_ids)` of the reset envs into obses[:, t] (HumanoidIm's `_reset_task` does nothing)."""
@@ -143,6 +151,7 @@ class ImZStepsB200(LatentStepsB200):
         self.comp.step(flags=_lib.STEP_OBS, obs_buf=self.obs_carry, **self._state())
         self.reset_buf.zero_()
         self.terminate_buf.zero_()
+        self._amp_start()
 
     def evaluate(self, dataset, physics=None, auto_pmcp: bool = False, auto_pmcp_soft: bool = False, **kw):
         """`IMAmpAgent.eval` (im_amp.py:136-242) of this policy over every clip of `dataset` (a MotionDatasetB200) on this driver's

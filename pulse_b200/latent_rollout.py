@@ -31,6 +31,17 @@ class LatentStepsB200(GraphRunner):
     `finish()` then computes GAE, normalised advantages and value-normalised returns from the task reward alone (task_reward_w 1,
     disc_reward_w 0) and `train_epoch()` runs the PPO update.
 
+    The AMP part (opt-in: `amp`, an AmpBuffersB200, given exactly when the policy has a discriminator).  The driver then keeps the
+    horizon's AMP rows `amp_obs[n, T, steps * width]` and the reset's back-filled history `amp_init[n, steps, width]` with its fresh
+    flags; after the step kernel of every step, on main, `pulse_amp_obs_row` writes amp_obs[:, t] = [current row | the first steps - 1
+    rows of amp_obs[:, t-1]] (of the back-filled rows for envs reset at step t: _init_amp_obs + _update_hist_amp_obs,
+    humanoid_amp.py:519-563, :622-630).  `finish()` mixes task_reward_w * r + disc_reward_w * disc.rewards(amp_obs) (the discriminator
+    forward pass is skipped at disc_reward_w 0); `train_epoch()` fetches amp_batch_size new demo rows, draws the demo and replay samples
+    of the whole horizon (only the first amp_minibatch_size rows of each minibatch are gathered), passes amp = (amp_obs rows, replay
+    rows, demo rows) at each minibatch's row offset to `train_minibatch` -- the discriminator's gradients share the actor / critic
+    gradient-norm clip -- and stores the horizon's rows into the replay ring after the last mini-epoch; all of it graph-captured.
+    Memory at 8192 envs, T = 32, 10 x 196 floats: amp_obs 2.06 GB, each 200 000-row ring 1.57 GB, each gathered sample 0.51 GB.
+
     The experience buffers are env-major (`obses[n, T, W]`, `actions[n, T, E]`, `mus[n, T, E]`, `neglogp[n, T]`; `adv[n*T]`, `ret[n*T]`), so
     a minibatch is a contiguous row range; `values`, `next_values` [T, n, 1], `rewards`, `dones` [T, n] are time-major as GAE reads them.
 
@@ -44,14 +55,16 @@ class LatentStepsB200(GraphRunner):
        P (prior mean, decoder operand); the observation of the reset envs overwrites rows of obses[:, t+1] that B's normalise reads (main
        waits for the event B records after it); the step kernel(t+1) rewrites `terminate_buf` that B's value_post reads (main waits for B);
        B starts after the step kernel(t).  A and B use separate critic operands and workspaces (slot 0 / slot 1).  The reset does not
-       clear `terminate_buf`: the step kernel rewrites it for every env each step and nothing reads it in between.
+       clear `terminate_buf`: the step kernel rewrites it for every env each step and nothing reads it in between.  The AMP row of step
+       t runs on main after the step kernel(t): reset(t+1) rewrites the body state and the fresh flags it reads, and main's order keeps
+       it before.
        With `physics` / `refresh` hooks the steps run as graph segments between the hook calls (reset | act | post), each with the same
        forks joined inside the segment.  `use_graphs=False` runs the same entry points on one stream in the order above.
        No ATen elementwise op, boolean-mask index or host synchronisation is inside the loop."""
 
     def _setup(self, task, reset, policy, vae, sim: dict, horizon: int, obs_width: int, pd_offset: Optional[torch.Tensor],
                pd_scale: Optional[torch.Tensor], pd_freeze: Optional[torch.Tensor], use_graphs: bool, gamma: float, tau: float,
-               reset_seed: int) -> None:
+               reset_seed: int, amp=None, task_reward_w: float = 1.0, disc_reward_w: float = 0.0) -> None:
         """The buffers and state every driver shares; the subclass calls it after its checks."""
         self.task, self.reset, self.policy, self.vae, self.sim, self.T = task, reset, policy, vae, sim, int(horizon)
         self.dev = policy.device
@@ -79,6 +92,17 @@ class LatentStepsB200(GraphRunner):
         self.reset_ws = None
         self.z_actions = None          # the decoder's output of the last step, fp32 [n, A] (a reused workspace)
         self._streams = None
+        self.amp, self.task_w, self.disc_w = amp, float(task_reward_w), float(disc_reward_w)
+        if amp is None and (self.task_w != 1.0 or self.disc_w != 0.0):
+            raise _lib.PulseError("task_reward_w / disc_reward_w mix in the discriminator reward: they need the AMP part (amp=AmpBuffersB200)")
+        if amp is not None:
+            if T < 2:
+                raise _lib.PulseError("the AMP part needs a horizon of at least 2 steps (each AMP row shifts the previous step's row)")
+            if policy.disc.size != amp.row_floats:
+                raise _lib.PulseError(f"the discriminator reads {policy.disc.size} floats, the AMP rows have {amp.num_steps} x {amp.amp_width}")
+            self.amp_obs = z(n, T, amp.row_floats)
+            self.amp_init, self.amp_fresh = z(n, amp.num_steps, amp.amp_width), z(n, dtype=torch.int32)
+            self.amp_x, self._amp_bufs = None, {}
 
     # ------------------------------------------------------------------ the task's pieces (subclass)
     def _reset(self, t: int) -> None:
@@ -128,6 +152,36 @@ class LatentStepsB200(GraphRunner):
         self.z_actions = dec = vae.dec.forward(dec_in)
         self._pre_physics(dec, t)
 
+    def _amp_row(self, t: int) -> None:
+        """The AMP row of step t (humanoid_amp.py:194-210, :622-667; amp_agent.py:385) into amp_obs[:, t]."""
+        s, amp = self.sim, self.amp
+        prev = self.amp_obs[:, t - 1] if t > 0 else self.amp_obs[:, self.T - 1]
+        out = self.amp_obs[:, t]
+        a = _lib.AmpRowArgs(body_state=s["body_state"].data_ptr(), body_env_stride=s["body_state"].stride(0), dof_pos=s["dof_pos"].data_ptr(),
+                            dof_vel=s["dof_vel"].data_ptr(), dof_env_stride=s["dof_pos"].stride(0), dof_elem_stride=s["dof_pos"].stride(1),
+                            prev=prev.data_ptr(), ld_prev=prev.stride(0), out=out.data_ptr(), ld_out=out.stride(0), num_steps=amp.num_steps,
+                            fresh=self.amp_fresh.data_ptr(), fresh_rows=self.amp_init.data_ptr(), amp_width=amp.amp_width,
+                            remove_base_rot=int(not amp.upright))
+        self._launch("pulse_amp_obs_row", C.byref(a), self.n)
+
+    def _amp_start(self) -> None:
+        """The AMP history of the initial state, for `first_observation`: the current AMP row in every history row of every env
+        (_init_amp_obs_default, humanoid_amp.py:530-533), so that the first horizon's rows carry no zero history.  The reference builds
+        the start-up history through its state init; with Random / Start it takes the history from the motion instead."""
+        if self.amp is None:
+            return
+        W = self.amp.amp_width
+        self._amp_row(self.T - 1)                                    # amp_obs[:, T-1, :W] = the current row (history from amp_obs[:, T-2])
+        self.amp_init.copy_(self.amp_obs[:, self.T - 1, :W].unsqueeze(1).expand_as(self.amp_init))
+        self.amp_obs[:, self.T - 1].copy_(self.amp_init.view(self.n, -1))
+        self.amp_fresh.zero_()
+
+    def _step(self, t: int) -> None:
+        """The step kernel(t), then the AMP row of step t."""
+        self._env_step(t)
+        if self.amp is not None:
+            self._amp_row(t)
+
     def _next_obs(self, t: int) -> torch.Tensor:
         return self.obses[:, t + 1] if t + 1 < self.T else self.obs_carry
 
@@ -152,7 +206,7 @@ class LatentStepsB200(GraphRunner):
             self._act(t)
             if self.physics is not None:
                 self.physics(t)
-            self._env_step(t)
+            self._step(t)
             self._next_values(t)
 
     def _whole_overlapped(self) -> None:
@@ -173,6 +227,8 @@ class LatentStepsB200(GraphRunner):
             with torch.cuda.stream(B):
                 norm_done = torch.cuda.Event()
                 self._next_values(t, after_normalize=lambda ev=norm_done: ev.record(B))
+            if self.amp is not None:
+                self._amp_row(t)                                     # on main, beside B's next values, before reset(t+1)
         main.wait_stream(B)
 
     def _act_segment(self, t: int) -> None:
@@ -180,7 +236,7 @@ class LatentStepsB200(GraphRunner):
         self._act(t, *self._sides()[:2])
 
     def _post_segment(self, t: int) -> None:
-        self._env_step(t)
+        self._step(t)
         self._next_values(t)
 
     def play_steps(self) -> None:
@@ -204,19 +260,55 @@ class LatentStepsB200(GraphRunner):
 
     # ------------------------------------------------------------------ after the horizon
     def finish(self) -> None:
-        """GAE + returns, advantage normalisation and value / return normalisation (`rollout.finish_returns`) from the task reward alone:
-        task_reward_w 1, disc_reward_w 0 (`_combine_rewards`, amp_agent.py:1011-1025)."""
-        finish_returns(self.policy, self.dones, self.values, self.rewards.unsqueeze(-1), self.next_values, self.adv, self.ret, self.gamma, self.tau)
+        """GAE + returns, advantage normalisation and value / return normalisation (`rollout.finish_returns`) of the mixed reward
+        task_reward_w * r + disc_reward_w * disc_r (`_combine_rewards`, amp_agent.py:1011-1025); without the AMP part the task reward
+        alone (task_reward_w 1, disc_reward_w 0)."""
+        mb_rewards = self.rewards.unsqueeze(-1)
+        if self.amp is not None:
+            n, T = self.n, self.T
+            if self.task_w != 1.0:
+                mb_rewards = self.task_w * mb_rewards
+            if self.disc_w != 0.0:                                   # disc_reward_w 0 adds 0 x a finite reward: the pass is skipped
+                if self.amp_x is None:
+                    from .nets import pad_k
+                    self.amp_x = torch.zeros(n * T, pad_k(self.amp.row_floats), device=self.dev, dtype=torch.bfloat16)
+                disc_r = self.policy.disc.rewards(self.amp_obs.view(n * T, -1), self.amp_x)      # env-major [n*T, 1]
+                mb_rewards = mb_rewards + self.disc_w * disc_r.view(n, T).t().unsqueeze(-1)
+        finish_returns(self.policy, self.dones, self.values, mb_rewards, self.next_values, self.adv, self.ret, self.gamma, self.tau)
+
+    def _amp_batches(self, mb: int):
+        """The gathered demo / replay samples of one epoch: [rows / mb * take, steps * width] each (a reused workspace)."""
+        rows, amp = self.n * self.T, self.amp
+        take = min(amp.minibatch_size, mb)
+        if mb not in self._amp_bufs:
+            z = lambda: torch.zeros(rows // mb * take, amp.row_floats, device=self.dev)
+            self._amp_bufs[mb] = (z(), z())
+        return take, self._amp_bufs[mb]
+
+    def _amp_prelude(self, mb: int) -> None:
+        """`_update_amp_demos`, then the demo sample and the replay sample (or the agent's rows) of train_epoch (amp_agent.py:476-484)."""
+        amp, rows = self.amp, self.n * self.T
+        _, (demo, replay) = self._amp_batches(mb)
+        amp.update_demos()
+        amp.sample(amp.demo, rows, mb, demo)
+        amp.sample(amp.replay, rows, mb, replay, fallback=self.amp_obs.view(rows, -1))
+
+    def _amp_store(self) -> None:
+        self.amp.store_replay(self.amp_obs.view(self.n * self.T, -1))
 
     def _update_mb(self, i: int, mb: int) -> None:
         r0, r1 = i * mb, (i + 1) * mb
         rows = self.n * self.T
+        amp = None
+        if self.amp is not None:                             # amp_agent.py:621-628: the first amp_minibatch_size rows of each batch
+            take, (demo, replay) = self._amp_batches(mb)
+            amp = (self.amp_obs.view(rows, -1)[r0:r0 + take], replay[i * take:(i + 1) * take], demo[i * take:(i + 1) * take])
         self.policy.train_minibatch(self.obses.view(rows, -1)[r0:r1], self.actions.view(rows, -1)[r0:r1], self.neglogp.view(rows)[r0:r1],
-                                    self.adv[r0:r1], self.ret[r0:r1], old_mu=self.mus.view(rows, -1)[r0:r1])
+                                    self.adv[r0:r1], self.ret[r0:r1], old_mu=self.mus.view(rows, -1)[r0:r1], amp=amp)
 
     def train_epoch(self, mini_epochs: int = 6, minibatch: int = 16384) -> torch.Tensor:
-        """The PPO update of one epoch (`train_epoch` -> `calc_gradients`, amp_agent.py:462-548, :605-760, without the discriminator
-        term): `mini_epochs` passes over the horizon's experience in contiguous minibatches of min(minibatch, n*T) rows, one
+        """The PPO update of one epoch (`train_epoch` -> `calc_gradients`, amp_agent.py:462-548, :605-760; the discriminator term with
+        the AMP part, see the class docstring): `mini_epochs` passes over the horizon's experience in contiguous minibatches of min(minibatch, n*T) rows, one
         `train_minibatch` each with old_mu = mus; every minibatch index is one CUDA graph.  Returns the policy's stats tensor,
         accumulated over the epoch (cleared at its start)."""
         rows = self.n * self.T
@@ -224,7 +316,11 @@ class LatentStepsB200(GraphRunner):
         if mb <= 0 or rows % mb:
             raise _lib.PulseError(f"minibatch {minibatch} must divide the {rows} rows of a horizon")
         self.policy.reset_stats()
+        if self.amp is not None:
+            self._run(("amp_prelude", mb), self._amp_prelude, mb)
         for _ in range(mini_epochs):
             for i in range(rows // mb):
                 self._run(("update", i, mb), self._update_mb, i, mb)
+        if self.amp is not None:
+            self._run(("amp_store",), self._amp_store)       # _store_replay_amp_obs after the update (amp_agent.py:539)
         return self.policy.stats

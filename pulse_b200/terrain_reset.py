@@ -69,17 +69,17 @@ class TerrainResetB200(ZTaskResetB200):
                    contact_forces: Optional[torch.Tensor] = None, amp_obs_buf: Optional[torch.Tensor] = None,
                    actor_ids: Optional[torch.Tensor] = None, motion_ids: Optional[torch.Tensor] = None, motion_u: Optional[torch.Tensor] = None,
                    phase: Optional[torch.Tensor] = None, loc_ids: Optional[torch.Tensor] = None, seed: int = 0, offset: int = 0,
-                   offset_dev: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
+                   offset_dev: Optional[torch.Tensor] = None, amp_fresh: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
         """`pulse_reset_terrain` for the envs of `reset_buf` (mask) or the ascending `env_ids` (int64 list): the arguments of
         `ZTaskResetB200.reset_envs` (no target actor), plus `loc_ids` int64 [N], the injected walkable-table index per env (the
-        reference's `np.random.randint(0, num_samples)`), or None: Philox word z of (seed, env, offset [+ *offset_dev]).  Returns the
+        reference's `np.random.randint(0, num_samples)`), or None: Philox word z of (seed, env, offset [+ *offset_dev]); `amp_fresh` as there.  Returns the
         workspace {'env_list', 'actor_list', 'count', 'loc_ids'} (device; loc_ids holds the location index of each reset env)."""
         N = int(progress_buf.shape[0])
         a, ws = self._args(root_states=root_states, dof_pos=dof_pos, dof_vel=dof_vel, rigid_body_state=rigid_body_state, progress_buf=progress_buf,
                            sampled_motion_ids=sampled_motion_ids, motion_start_times=motion_start_times, reset_buf=reset_buf, env_ids=env_ids,
                            terminate_buf=terminate_buf, contact_forces=contact_forces, amp_obs_buf=amp_obs_buf, actor_ids=actor_ids,
                            target_states=None, tar_actor_ids=None, motion_ids=motion_ids, motion_u=motion_u, phase=phase, strike_u=None,
-                           seed=seed, offset=offset, offset_dev=offset_dev)
+                           seed=seed, offset=offset, offset_dev=offset_dev, amp_fresh=amp_fresh)
         s = _lib.TerrainSpawnArgs()
         self.terrain.fill(s)
         s.center_points, s.num_center_points = self.center_points.data_ptr(), int(self.center_points.shape[0])

@@ -29,7 +29,7 @@ def _same_heightfield(a, b) -> bool:
     return a.heightfield.data_ptr() == b.heightfield.data_ptr() or torch.equal(a.heightfield, b.heightfield.to(a.heightfield.device))
 
 
-def check_pieces(task, reset, policy, vae) -> None:
+def check_pieces(task, reset, policy, vae, amp=None) -> None:
     """Checks that the step object, the reset, the sept policy and the frozen VAE belong together; raises PulseError naming the mismatch."""
     who = "TerrainStepsB200"
     if not isinstance(task, PedestrianTerrainTaskB200):
@@ -42,8 +42,11 @@ def check_pieces(task, reset, policy, vae) -> None:
         raise _lib.PulseError(f"{who}: the reset and the task sample different heightfields")
     if not isinstance(policy, SeptPolicy):
         raise _lib.PulseError(f"{who}: policy must be a SeptPolicy (the amp_sept network of pulse_z_terrain.yaml)")
-    if getattr(policy, "disc", None) is not None:
-        raise _lib.PulseError(f"{who}: the discriminator is not part of this driver (task reward only); build the policy without it")
+    if (getattr(policy, "disc", None) is not None) != (amp is not None):
+        raise _lib.PulseError(f"{who}: a policy with a discriminator needs the AMP part (amp=AmpBuffersB200) and the AMP part a discriminator")
+    if amp is not None and (amp.amp_width != reset.amp_width or amp.upright != reset.upright):
+        raise _lib.PulseError(f"{who}: the AMP part writes {amp.amp_width}-float rows (upright {amp.upright}), the reset {reset.amp_width}-float "
+                              f"rows (upright {reset.upright})")
     W = int(task.get_obs_size())
     if int(policy.S) + int(policy.task_in) != W:
         raise _lib.PulseError(f"{who}: the task writes {W} observation floats, the policy reads {policy.S} + {policy.task_in}")
@@ -95,21 +98,24 @@ class TerrainStepsB200(LatentStepsB200):
     `task`: a PedestrianTerrainTaskB200 on a heightfield; its traj_verts are the waypoints the steps read and the resets rewrite, and the
     caller provides the initial ones (e.g. `task.reset_task` over all envs) before `first_observation()`.  `reset`: the
     TerrainResetB200 over the same heightfield (same sizes, scales and cells, compared once at construction: the task and the reset
-    may hold separate uploads of the map, as two `from_reference` calls make them).  `policy`: SeptPolicy(num_actions=vae.E, with_disc=False, ...) whose self + task
+    may hold separate uploads of the map, as two `from_reference` calls make them).  `policy`: SeptPolicy(num_actions=vae.E, ...) whose self + task
     observation is the task's (358 + 1044 = 1402 floats for env_pulse_terrain.yaml).  `vae`: PulseVAE(with_critic=False) holding the
     frozen prior, decoder and the checkpoint's obs_rms.  `sim`: the simulator's tensors, read and written in place through their
     strides: body_state, root_states, dof_pos, dof_vel, progress_buf, sampled_motion_ids, motion_start_times (the terrain reset's
     clip / start-time buffers); contact_forces with early termination; dof_force with power_reward; optional actor_ids.
 
-    Out of scope: the discriminator (pulse_z_terrain.yaml still trains it with disc_coef 5 although its reward weight is 0; leaving it out
-    does not change the reward, but it removes the discriminator's gradients from the shared gradient-norm clip, so the reset is called
-    without an AMP buffer); multi-GPU; group observations and the velocity map; mesh terrain; Default / Hybrid state init; an agent
+    With the AMP part (`amp`, an AmpBuffersB200 of the reset's layout, 196 floats for env_pulse_terrain.yaml, given exactly when the
+    policy has a discriminator) the reset back-fills the AMP history and `train_epoch()` trains the discriminator inside the shared
+    gradient-norm clip, as pulse_z_terrain.yaml does (LatentStepsB200).
+
+    Out of scope: multi-GPU; group observations and the velocity map; mesh terrain; Default / Hybrid state init; an agent
     mixin (INTEGRATION.md wires the hooks)."""
 
     def __init__(self, task, reset, policy, vae, sim: dict, horizon: int = 32, pd_offset: Optional[torch.Tensor] = None,
                  pd_scale: Optional[torch.Tensor] = None, pd_freeze: Optional[torch.Tensor] = None, use_graphs: bool = True,
-                 gamma: float = 0.99, tau: float = 0.95, reset_seed: int = 0):
-        check_pieces(task, reset, policy, vae)
+                 gamma: float = 0.99, tau: float = 0.95, reset_seed: int = 0, amp=None, task_reward_w: float = 1.0,
+                 disc_reward_w: float = 0.0):
+        check_pieces(task, reset, policy, vae, amp)
         keys = SIM_KEYS + (("contact_forces",) if task.enable_early_termination else ()) + (("dof_force",) if task.power_reward else ())
         missing = [k for k in keys if sim.get(k) is None]
         if missing:
@@ -118,7 +124,7 @@ class TerrainStepsB200(LatentStepsB200):
         if n != task.num_envs:
             raise _lib.PulseError(f"TerrainStepsB200: sim has {n} envs, the task {task.num_envs}")
         self._setup(task, reset, policy, vae, sim, horizon, task.get_obs_size(), pd_offset, pd_scale, pd_freeze, use_graphs, gamma, tau,
-                    reset_seed)
+                    reset_seed, amp, task_reward_w, disc_reward_w)
 
     # ------------------------------------------------------------------ the task's pieces of one step
     def _step_args(self, flags: int, obs: torch.Tensor, rew: torch.Tensor):
@@ -140,8 +146,9 @@ class TerrainStepsB200(LatentStepsB200):
         self.reset_ws = self.reset.reset_envs(
             root_states=s["root_states"], dof_pos=s["dof_pos"], dof_vel=s["dof_vel"], rigid_body_state=s["body_state"],
             progress_buf=s["progress_buf"], sampled_motion_ids=s["sampled_motion_ids"], motion_start_times=s["motion_start_times"],
-            reset_buf=self.reset_buf, contact_forces=s.get("contact_forces"), amp_obs_buf=None, actor_ids=s.get("actor_ids"),
-            seed=self.reset_seed, offset=t, offset_dev=self.policy.rng_offset)
+            reset_buf=self.reset_buf, contact_forces=s.get("contact_forces"), amp_obs_buf=self.amp_init if self.amp is not None else None,
+            actor_ids=s.get("actor_ids"), seed=self.reset_seed, offset=t, offset_dev=self.policy.rng_offset,
+            amp_fresh=self.amp_fresh if self.amp is not None else None)
 
     def _reset_obs(self, t: int) -> None:
         """`_compute_observations(env_ids)` of the reset envs into obses[:, t], then `_reset_task` (humanoid_amp_task.py:66-76)."""
@@ -167,3 +174,4 @@ class TerrainStepsB200(LatentStepsB200):
         self._launch("pulse_terrain_step", C.byref(a), self.n)
         self.reset_buf.zero_()
         self.terminate_buf.zero_()
+        self._amp_start()

@@ -103,18 +103,19 @@ class ZTaskResetB200:
                    tar_actor_ids: Optional[torch.Tensor] = None, motion_ids: Optional[torch.Tensor] = None,
                    motion_u: Optional[torch.Tensor] = None, phase: Optional[torch.Tensor] = None,
                    strike_u: Optional[torch.Tensor] = None, seed: int = 0, offset: int = 0,
-                   offset_dev: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
+                   offset_dev: Optional[torch.Tensor] = None, amp_fresh: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
         """`pulse_reset_ztask` for the envs of `reset_buf` (mask) or `env_ids` (int64 list): clip and start time, ground fix, the task's
         pose adjustment, the simulator views written in place, `_sampled_motion_ids` / `_motion_start_times`, counters and contact forces
         cleared, the strike target (kind "strike": `target_states` is the [N, 13] view of the target actors) and the AMP history
         [N, steps, 195 | 196].  `env_ids` must be ascending (what `nonzero` returns): an id out of range or not above its predecessor
         is skipped.  Injected draws are per ENV: `motion_ids` int64 [N] (the clips themselves) or `motion_u` [N] (uniforms turned into
-        clips through the sampling CDF), `phase` [N], `strike_u` [N, 4]; None -> Philox on (seed, env, offset [+ *offset_dev]).  Returns the workspace {'env_list', 'actor_list', 'tar_actor_list', 'count'} (device)."""
+        clips through the sampling CDF), `phase` [N], `strike_u` [N, 4]; None -> Philox on (seed, env, offset [+ *offset_dev]).  `amp_fresh`
+        int32 [N] (with amp_obs_buf): set to 1 for every reset env, for `pulse_amp_obs_row`.  Returns the workspace {'env_list', 'actor_list', 'tar_actor_list', 'count'} (device)."""
         a, ws = self._args(root_states=root_states, dof_pos=dof_pos, dof_vel=dof_vel, rigid_body_state=rigid_body_state, progress_buf=progress_buf,
                            sampled_motion_ids=sampled_motion_ids, motion_start_times=motion_start_times, reset_buf=reset_buf, env_ids=env_ids,
                            terminate_buf=terminate_buf, contact_forces=contact_forces, amp_obs_buf=amp_obs_buf, actor_ids=actor_ids,
                            target_states=target_states, tar_actor_ids=tar_actor_ids, motion_ids=motion_ids, motion_u=motion_u, phase=phase,
-                           strike_u=strike_u, seed=seed, offset=offset, offset_dev=offset_dev)
+                           strike_u=strike_u, seed=seed, offset=offset, offset_dev=offset_dev, amp_fresh=amp_fresh)
         fn, handle = ("pulse_reset_ztask_smplx", self.motion_lib.smplx_handle) if self.smplx else ("pulse_reset_ztask", self.motion_lib.handle)
         with torch.cuda.device(self.device):
             _lib.check(getattr(self.lib, fn)(handle, C.byref(a), int(progress_buf.shape[0]), _lib.current_stream(self.device)), fn)
@@ -122,7 +123,7 @@ class ZTaskResetB200:
 
     def _args(self, *, root_states, dof_pos, dof_vel, rigid_body_state, progress_buf, sampled_motion_ids, motion_start_times, reset_buf, env_ids,
               terminate_buf, contact_forces, amp_obs_buf, actor_ids, target_states, tar_actor_ids, motion_ids, motion_u, phase, strike_u, seed,
-              offset, offset_dev):
+              offset, offset_dev, amp_fresh=None):
         """The checked `pulse_ztask_reset_args_t` of a `reset_envs` call, and the workspace it writes."""
         N = int(progress_buf.shape[0])
         dev = self.device
@@ -185,6 +186,10 @@ class ZTaskResetB200:
             if amp_obs_buf.dtype != torch.float32 or amp_obs_buf.device != dev:
                 raise _lib.PulseError(f"amp_obs_buf must be float32 on {dev}")
             a.amp_obs_buf, a.num_amp_steps, a.amp_width = amp_obs_buf.data_ptr(), int(amp_obs_buf.shape[1]), self.amp_width
+        if amp_fresh is not None:
+            if amp_obs_buf is None or amp_fresh.dtype != torch.int32 or amp_fresh.shape != (N,) or not amp_fresh.is_contiguous() or amp_fresh.device != dev:
+                raise _lib.PulseError(f"amp_fresh must be contiguous int32 [{N}] on {dev}, given with amp_obs_buf")
+            a.amp_fresh = amp_fresh.data_ptr()
         for name, t, dt_ in (("sampled_motion_ids", sampled_motion_ids, torch.int64), ("motion_start_times", motion_start_times, torch.float32),
                              ("progress_buf", progress_buf, torch.int64)):
             if t.dtype != dt_ or not t.is_contiguous() or t.shape[0] != N or t.device != dev:

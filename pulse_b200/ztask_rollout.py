@@ -21,7 +21,7 @@ SIM_KEYS = ("body_state", "root_states", "dof_pos", "dof_vel", "progress_buf", "
 STRIKE_KEYS = ("target_states", "tar_contact_forces")
 
 
-def check_pieces(task, reset, policy, vae) -> str:
+def check_pieces(task, reset, policy, vae, amp=None) -> str:
     """The task kind ("reach" / "speed" / "strike") after checking that the step object, the reset, the latent policy and the frozen
     VAE belong together; raises PulseError otherwise.  SMPL: observations of 361 / 361 / 373 floats, a 358 -> 69 decoder.  SMPL-X
     (SmplxSpeedTaskB200, PULSE-X): the speed task's 781 floats, a 778 -> 153 decoder and a 48-dimensional latent (env_pulsex_amp.yaml)."""
@@ -43,8 +43,15 @@ def check_pieces(task, reset, policy, vae) -> str:
         raise _lib.PulseError(f"ZTaskStepsB200: the decoder must map the {S}-float self observation to {A} dof targets, not {vae.S} -> {vae.A}")
     if E is not None and int(vae.E) != E:
         raise _lib.PulseError(f"ZTaskStepsB200: the {layout} latent has {E} dimensions (embedding_size), the VAE's {vae.E}")
-    if getattr(policy, "disc", None) is not None:
-        raise _lib.PulseError("ZTaskStepsB200: the discriminator is not part of this driver (task reward only); build the policy without it")
+    if (getattr(policy, "disc", None) is not None) != (amp is not None):
+        raise _lib.PulseError("ZTaskStepsB200: a policy with a discriminator needs the AMP part (amp=AmpBuffersB200) and the AMP part a "
+                              "discriminator")
+    if amp is not None:
+        if layout == "smplx":
+            raise _lib.PulseError("ZTaskStepsB200: no AMP part (and no discriminator) for SMPL-X: there is no 52-body AMP layout")
+        if amp.amp_width != reset.amp_width or amp.upright != reset.upright:
+            raise _lib.PulseError(f"ZTaskStepsB200: the AMP part writes {amp.amp_width}-float rows (upright {amp.upright}), the reset "
+                                  f"{reset.amp_width}-float rows (upright {reset.upright})")
     return kind
 
 
@@ -55,11 +62,13 @@ class ZTaskStepsB200(LatentStepsB200):
             `reset_task` (reach, speed);
          5. `pulse_ztask_pre_physics`: PD targets into pd_tar, prev_root_pos (speed, strike), `_update_task` of the due envs (reach, speed);
          7. the rollout step kernel (`pulse_reach_rollout_step` / `pulse_ztask_rollout_step`).
-    `finish()` uses the task reward alone (task_reward_w 1, disc_reward_w 0, pulse_z_task.yaml:90-91).
+    `finish()` uses the task reward alone (task_reward_w 1, disc_reward_w 0, pulse_z_task.yaml:90-91).  With the AMP part (`amp`, an
+    AmpBuffersB200 of the reset's amp_width and upright setting: 195 floats for env_pulse_amp.yaml) the reset also back-fills the AMP
+    history, the driver keeps the horizon's AMP rows and `train_epoch()` trains the discriminator (disc_coef 5) inside the shared
+    gradient-norm clip, as pulse_z_task.yaml does (LatentStepsB200); task_reward_w / disc_reward_w then mix the rewards.
 
     `task`: the ReachTaskB200 / SpeedTaskB200 / StrikeTaskB200 whose targets, change steps and termination settings the steps use.
-    `reset`: the ZTaskResetB200 of the same kind.  `policy`: PPOPolicy(obs_size=task.obs_size, num_actions=vae.E, ...) without
-    discriminator.  `vae`: PulseVAE(with_critic=False) holding the frozen prior, decoder and the checkpoint's obs_rms.  `sim`: the
+    `reset`: the ZTaskResetB200 of the same kind.  `policy`: PPOPolicy(obs_size=task.obs_size, num_actions=vae.E, ...).  `vae`: PulseVAE(with_critic=False) holding the frozen prior, decoder and the checkpoint's obs_rms.  `sim`: the
     simulator's tensors, read and written in place through their strides: body_state, root_states, dof_pos, dof_vel, progress_buf,
     sampled_motion_ids, motion_start_times; optional contact_forces, actor_ids, dof_force (the speed task's power term); strike:
     target_states, tar_contact_forces and optional tar_actor_ids.
@@ -68,15 +77,17 @@ class ZTaskStepsB200(LatentStepsB200):
     `reset` a ZTaskResetB200 over a 52-body MotionLib, `policy` PPOPolicy(obs_size=781, num_actions=48), `vae` PulseVAE(self_obs_size=778,
     num_actions=153, latent=48); the sim views hold >= 52 bodies and 153 dofs, and `dof_force` is refused (no power term).
 
-    Out of scope: the discriminator (the reference still trains it here with disc_coef 5 although disc_reward_w is 0; leaving it out does
-    not change the reward, but it removes the discriminator's gradients from the shared gradient-norm clip, so the reset is called
-    without an AMP buffer); multi-GPU; the smplx humanoid's reach and strike tasks; Default / Hybrid state init; the power_usage_reward
+    `policy` may carry a discriminator exactly when `amp` is given (PPOPolicy(..., with_disc=True, amp_obs_size=10 * amp_width)); the
+    SMPL-X speed task takes neither (no 52-body AMP layout).
+
+    Out of scope: multi-GPU; the smplx humanoid's reach and strike tasks; Default / Hybrid state init; the power_usage_reward
     terms the step kernels exclude."""
 
     def __init__(self, task, reset, policy, vae, sim: dict, horizon: int = 32, pd_offset: Optional[torch.Tensor] = None,
                  pd_scale: Optional[torch.Tensor] = None, pd_freeze: Optional[torch.Tensor] = None, use_graphs: bool = True,
-                 gamma: float = 0.99, tau: float = 0.95, reset_seed: int = 0):
-        self.kind = check_pieces(task, reset, policy, vae)
+                 gamma: float = 0.99, tau: float = 0.95, reset_seed: int = 0, amp=None, task_reward_w: float = 1.0,
+                 disc_reward_w: float = 0.0):
+        self.kind = check_pieces(task, reset, policy, vae, amp)
         self.layout = getattr(task, "layout", "smpl")
         missing = [k for k in SIM_KEYS + (STRIKE_KEYS if self.kind == "strike" else ()) if k not in sim]
         if missing:
@@ -86,7 +97,8 @@ class ZTaskStepsB200(LatentStepsB200):
         n = self.n = int(sim["progress_buf"].shape[0])
         if n != task.num_envs:
             raise _lib.PulseError(f"ZTaskStepsB200: sim has {n} envs, the task {task.num_envs}")
-        self._setup(task, reset, policy, vae, sim, horizon, task.obs_size, pd_offset, pd_scale, pd_freeze, use_graphs, gamma, tau, reset_seed)
+        self._setup(task, reset, policy, vae, sim, horizon, task.obs_size, pd_offset, pd_scale, pd_freeze, use_graphs, gamma, tau, reset_seed,
+                    amp, task_reward_w, disc_reward_w)
 
     # ------------------------------------------------------------------ the pieces of one step
     def _step_args(self, obs: torch.Tensor, rew: torch.Tensor):
@@ -124,9 +136,10 @@ class ZTaskStepsB200(LatentStepsB200):
         self.reset_ws = self.reset.reset_envs(
             root_states=s["root_states"], dof_pos=s["dof_pos"], dof_vel=s["dof_vel"], rigid_body_state=s["body_state"],
             progress_buf=s["progress_buf"], sampled_motion_ids=s["sampled_motion_ids"], motion_start_times=s["motion_start_times"],
-            reset_buf=self.reset_buf, contact_forces=s.get("contact_forces"), amp_obs_buf=None, actor_ids=s.get("actor_ids"),
-            target_states=s["target_states"] if strike else None, tar_actor_ids=s.get("tar_actor_ids") if strike else None,
-            seed=self.reset_seed, offset=t, offset_dev=self.policy.rng_offset)
+            reset_buf=self.reset_buf, contact_forces=s.get("contact_forces"), amp_obs_buf=self.amp_init if self.amp is not None else None,
+            actor_ids=s.get("actor_ids"), target_states=s["target_states"] if strike else None,
+            tar_actor_ids=s.get("tar_actor_ids") if strike else None, seed=self.reset_seed, offset=t, offset_dev=self.policy.rng_offset,
+            amp_fresh=self.amp_fresh if self.amp is not None else None)
 
     def _reset_obs(self, t: int) -> None:
         """`_compute_observations(env_ids)` of the reset envs into obses[:, t], then `_reset_task` (humanoid_amp_task.py:66-76)."""
@@ -168,3 +181,4 @@ class ZTaskStepsB200(LatentStepsB200):
         self._launch("pulse_reach_step" if self.kind == "reach" else _ENTRIES[self.layout][0], C.byref(a), self.n)
         self.reset_buf.zero_()
         self.terminate_buf.zero_()
+        self._amp_start()
