@@ -821,7 +821,7 @@ typedef struct {
   int32_t pose_mode;             /* PULSE_ZPOSE_* */
   int32_t upright;               /* _has_upright_start (FACE_X heading and the AMP rotation features) */
   int32_t state_init;            /* PULSE_ZINIT_* */
-  int32_t amp_width;             /* 196 or 195 */
+  int32_t amp_width;             /* 196 or 195 (SMPL-X: 466 or 465) */
   int32_t num_amp_steps;         /* numAMPObsSteps; 0 with amp_obs_buf NULL */
   float dt;                      /* control dt */
   float* amp_obs_buf;            /* [N, num_amp_steps, amp_width] or NULL */
@@ -948,6 +948,13 @@ int pulse_ztask_rollout_step(const pulse_ztask_step_args_t* args, float* dones, 
 #define PULSE_SMPLX_SPEED_OBS 781    /* + compute_speed_observations (humanoid_speed.py:310-325)      */
 #define PULSE_SMPLX_FRAME_REC 676    /* packed per-frame record: pos156 | rot208 | vel156 | angvel156 */
 #define PULSE_SMPLX_AUX_REC 364      /* packed per-frame record: lrs208 | dvs153 | pad3             */
+/* The AMP observation of the SMPL-X humanoid (build_amp_observations_smpl, humanoid_amp.py:924-969, env_pulsex_amp.yaml): dof_subset
+ * drops only L_Toe and R_Toe (humanoid.py:404-421), so 49 of the 51 joints are kept; key bodies R_Ankle, L_Ankle, R_Wrist, L_Wrist
+ * = bodies 7, 3, 36, 17.  [h 1 | root rot 6 | root vel 3 | root ang vel 3 | 49 x six(dof) | 147 dof vel | 4 x key pos 3], all in
+ * the heading frame of remove_base_rot(root_rot) (has_upright_start False); 465 without the root height (ampRootHeightObs False,
+ * the env_pulsex_amp.yaml width, 10 x 465 = 4650 floats per discriminator row). */
+#define PULSE_SMPLX_AMP_OBS 466
+#define PULSE_SMPLX_AMP_OBS_NO_HEIGHT 465
 
 /* MotionLib tables of the SMPL-X humanoid (MotionLibSMPL loaded with smplx_humanoid.xml, motion_lib_base.py:287-316), packed into
  * the two records above by one kernel.  The handle is its own type: SMPL-X tables never reach an SMPL entry point. */
@@ -1004,12 +1011,20 @@ int pulse_smplx_speed_obs_list(const pulse_smplx_speed_step_args_t* args, const 
 int pulse_smplx_speed_rollout_step(const pulse_smplx_speed_step_args_t* args, float* dones, int64_t num_envs, void* stream);
 
 /* The reference-state reset of pulse_reset_ztask for the SMPL-X speed task, no host synchronisation: the compaction, then one warp per
- * reset env: clip and start-time draws, the 52-body gather, the SMPL ground fix from the per-frame floor table, the FACE_X pose
- * adjustment (HumanoidSpeed._sample_ref_state, humanoid_speed.py:251-270, heading of remove_base_rot(root_rot) when !upright) and the
- * scatter into the root, [N, >= 52, 13] rigid-body and [N, 153] dof views, counters and contact forces.  The argument struct is
- * pulse_reset_ztask's with pose_mode PULSE_ZPOSE_FACE_X; the AMP history back-fill (amp_obs_buf) and the strike target (target_states)
- * are refused.  _reset_task follows through pulse_ztask_reset_task, the PD targets through pulse_ztask_pre_physics (dofs 153). */
+ * (reset env, AMP history step k): clip and start-time draws, the 52-body gather, the SMPL ground fix from the per-frame floor table,
+ * the FACE_X pose adjustment (HumanoidSpeed._sample_ref_state, humanoid_speed.py:251-270, heading of remove_base_rot(root_rot) when
+ * !upright) and the scatter into the root, [N, >= 52, 13] rigid-body and [N, 153] dof views, counters and contact forces.  The argument
+ * struct is pulse_reset_ztask's with pose_mode PULSE_ZPOSE_FACE_X; the strike target (target_states) is refused.  With amp_obs_buf
+ * [N, num_amp_steps, amp_width] (amp_width PULSE_SMPLX_AMP_OBS or PULSE_SMPLX_AMP_OBS_NO_HEIGHT, num_amp_steps 1..16) the AMP history
+ * is back-filled as in pulse_reset_ztask: row 0 from the state just written, rows k >= 1 from the unadjusted motion at t0 - k dt; the
+ * state outputs are those of the same call without it.  _reset_task follows through pulse_ztask_reset_task, the PD targets through
+ * pulse_ztask_pre_physics (dofs 153). */
 int pulse_reset_ztask_smplx(const pulse_smplx_motionlib_t* lib, const pulse_ztask_reset_args_t* args, int64_t num_envs, void* stream);
+
+/* pulse_amp_obs_row for the SMPL-X humanoid: the AMP row [current W | first (steps-1)*W floats of the previous row] of every env from
+ * [N, >= 52, 13] body views and [N, 153] dof views, W = amp_width PULSE_SMPLX_AMP_OBS or PULSE_SMPLX_AMP_OBS_NO_HEIGHT (0 is refused),
+ * with the heading of remove_base_rot(q0) (remove_base_rot must be 1); fresh envs take their history from fresh_rows, as there. */
+int pulse_smplx_amp_obs_row(const pulse_amp_row_args_t* args, int64_t num_envs, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Pedestrian terrain task HumanoidPedestrianTerrain(Z) (phc/env/tasks/humanoid_pedestrian_terrain.py): post_physics_step in one launch,
@@ -1153,7 +1168,9 @@ int pulse_reset_terrain(const pulse_motionlib_t* lib, const pulse_ztask_reset_ar
  * pulse_amp_demo_fetch   fetch_amp_obs_demo + build_amp_obs_demo (phc/env/tasks/humanoid_amp.py:215-284) of num_samples rows straight
  *                        into the ring, then store()'s head / total_count update: per row a clip (inverse CDF of sampling_cdf), t0 by
  *                        sample_time_interval (the SMPL _sample_time, :376-380), the motion at t0 - k dt for k < num_steps without the
- *                        ground fix, build_amp_observations_smpl in amp_width 196 / 195 and the upright setting.  24-body SMPL only.
+ *                        ground fix, build_amp_observations_smpl in amp_width 196 / 195 and the upright setting.  24-body SMPL.
+ * pulse_smplx_amp_demo_fetch  the same over the SMPL-X tables: amp_width PULSE_SMPLX_AMP_OBS / PULSE_SMPLX_AMP_OBS_NO_HEIGHT, upright 0;
+ *                        the same Philox planes, so clips and start times are pulse_amp_demo_fetch's word for word.
  * pulse_amp_replay_store _store_replay_amp_obs: once total_count > capacity a Bernoulli(keep_prob) keep mask, the ordered compaction of
  *                        the kept rows, a random subset of capacity rows (Feistel permutation of the kept count, subset keys) when more
  *                        survive, then the ring write with wrap and the counter update.
@@ -1189,13 +1206,14 @@ typedef struct {
   const float* sampling_cdf;     /* [num_motions] inclusive fp32 prefix sum of _sampling_batch_prob */
   int64_t num_samples;           /* rows fetched, <= capacity */
   int32_t num_steps;             /* numAMPObsSteps, 1 .. 16 */
-  int32_t amp_width;             /* 196 or 195 */
+  int32_t amp_width;             /* 196 or 195 (SMPL-X: 466 or 465) */
   int32_t upright;               /* _has_upright_start */
   float dt;                      /* control dt */
   int64_t* motion_ids_out;       /* [num_samples] optional: the drawn clips */
   float* times_out;              /* [num_samples] optional: the drawn t0 */
 } pulse_amp_demo_args_t;
 int pulse_amp_demo_fetch(const pulse_motionlib_t* lib, const pulse_amp_demo_args_t* args, void* stream);
+int pulse_smplx_amp_demo_fetch(const pulse_smplx_motionlib_t* lib, const pulse_amp_demo_args_t* args, void* stream);
 
 typedef struct {
   pulse_amp_ring_t ring;

@@ -307,6 +307,7 @@ class SmplxSpeedStepArgs(C.Structure):
 
 
 SMPLX_BODIES, SMPLX_DOF, SMPLX_SELF_OBS, SMPLX_SPEED_OBS = 52, 153, 778, 781
+SMPLX_AMP_OBS, SMPLX_AMP_OBS_NO_HEIGHT = 466, 465       # PULSE_SMPLX_AMP_OBS(_NO_HEIGHT): the SMPL-X AMP row, with / without root height
 
 
 # Philox index planes of the latent tasks' draws (include/pulse_b200.h): index = env + plane
@@ -521,7 +522,9 @@ SIGNATURES = {
     "pulse_smplx_speed_obs_list": (C.c_int, [C.POINTER(SmplxSpeedStepArgs), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_smplx_speed_rollout_step": (C.c_int, [C.POINTER(SmplxSpeedStepArgs), C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_reset_ztask_smplx": (C.c_int, [C.c_void_p, C.POINTER(ZTaskResetArgs), C.c_int64, C.c_void_p]),
+    "pulse_smplx_amp_obs_row": (C.c_int, [C.POINTER(AmpRowArgs), C.c_int64, C.c_void_p]),
     "pulse_amp_demo_fetch": (C.c_int, [C.c_void_p, C.POINTER(AmpDemoArgs), C.c_void_p]),
+    "pulse_smplx_amp_demo_fetch": (C.c_int, [C.c_void_p, C.POINTER(AmpDemoArgs), C.c_void_p]),
     "pulse_amp_replay_store": (C.c_int, [C.POINTER(AmpStoreArgs), C.c_void_p]),
     "pulse_amp_ring_sample": (C.c_int, [C.POINTER(AmpSampleArgs), C.c_void_p]),
 }

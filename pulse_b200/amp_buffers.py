@@ -11,6 +11,10 @@ import torch
 
 from . import _lib
 
+# the AMP row widths per body layout: with the root height, without it (ampRootHeightObs)
+AMP_WIDTHS = {"smpl": (196, 195), "smplx": (_lib.SMPLX_AMP_OBS, _lib.SMPLX_AMP_OBS_NO_HEIGHT)}
+_DEMO_FETCH = {"smpl": "pulse_amp_demo_fetch", "smplx": "pulse_smplx_amp_demo_fetch"}
+
 
 class AmpRing:
     """One ReplayBuffer of `capacity` AMP rows of `row_floats` floats, with its device counters."""
@@ -32,19 +36,24 @@ class AmpRing:
 class AmpBuffersB200:
     """The demo ring filled from the MotionLib and the replay ring of the policy's own AMP rows.
 
-    `motion_lib`: the MotionLibB200 the demo rows come from (24-body SMPL); `sampling_cdf` its clip CDF (default: the MotionLib's).
-    `num_steps` x `amp_width` (196, or 195 without the root height) and `upright` are the env's AMP layout, `dt` its control step.
-    The sizes and the keep probability are the learning config's amp_obs_demo_buffer_size, amp_replay_buffer_size, amp_batch_size,
-    amp_replay_keep_prob and amp_minibatch_size.  Memory: capacity * num_steps * amp_width * 4 bytes per ring (1.57 GB for 200 000 rows
-    of 10 x 196 floats)."""
+    `motion_lib`: the MotionLibB200 the demo rows come from; `sampling_cdf` its clip CDF (default: the MotionLib's).  `num_steps` x
+    `amp_width` and `upright` are the env's AMP layout, `dt` its control step: a 24-body SMPL MotionLib takes 196 floats, or 195
+    without the root height, upright or not; a 52-body SMPL-X one (PULSE-X, env_pulsex_amp.yaml) takes 466 or 465 and upright=False
+    (`pulse_smplx_amp_demo_fetch`).  The sizes and the keep probability are the learning config's amp_obs_demo_buffer_size,
+    amp_replay_buffer_size, amp_batch_size, amp_replay_keep_prob and amp_minibatch_size.  Memory: capacity * num_steps * amp_width * 4
+    bytes per ring (1.57 GB for 200 000 rows of 10 x 196 floats, 3.72 GB for 200 000 rows of 10 x 465)."""
 
     def __init__(self, motion_lib, *, num_steps: int = 10, amp_width: int = 196, upright: bool = True, dt: float = float(torch.tensor(1.0 / 60.0, dtype=torch.float32) * 2),
                  demo_buffer_size: int = 200000, replay_buffer_size: int = 200000, batch_size: int = 512, keep_prob: float = 0.01,
                  minibatch_size: int = 4096, seed: int = 0, sampling_cdf: Optional[torch.Tensor] = None):
-        if amp_width not in (195, 196):
-            raise _lib.PulseError(f"amp_width {amp_width}: the AMP rows are 196 floats, or 195 without the root height")
-        if getattr(motion_lib, "smplx", False):
-            raise _lib.PulseError("the AMP demo fetch serves the 24-body SMPL MotionLib (no SMPL-X AMP layout)")
+        self.smplx = bool(getattr(motion_lib, "smplx", False))
+        self.layout = "smplx" if self.smplx else "smpl"
+        widths = AMP_WIDTHS[self.layout]
+        if amp_width not in widths:
+            raise _lib.PulseError(f"amp_width {amp_width}: the {self.layout} AMP rows are {widths[0]} floats, or {widths[1]} without the root "
+                                  f"height")
+        if self.smplx and upright:
+            raise _lib.PulseError("the SMPL-X AMP rows take upright=False (env_pulsex_amp.yaml: has_upright_start False)")
         if not 1 <= batch_size <= demo_buffer_size:
             raise _lib.PulseError(f"amp_batch_size {batch_size} must lie in [1, amp_obs_demo_buffer_size]")
         self.motion_lib, self.device = motion_lib, motion_lib._device
@@ -68,14 +77,16 @@ class AmpBuffersB200:
     # ------------------------------------------------------------------ demo ring
     def fetch_demos(self, num_samples: Optional[int] = None, motion_ids_out: Optional[torch.Tensor] = None,
                     times_out: Optional[torch.Tensor] = None) -> None:
-        """`_amp_obs_demo_buffer.store(fetch_amp_obs_demo(num_samples))` in one call (`pulse_amp_demo_fetch`); the optional outputs receive
-        the drawn clips and start times."""
+        """`_amp_obs_demo_buffer.store(fetch_amp_obs_demo(num_samples))` in one call (`pulse_amp_demo_fetch`, `pulse_smplx_amp_demo_fetch`
+        for SMPL-X); the optional outputs receive the drawn clips and start times."""
         n = self.batch_size if num_samples is None else int(num_samples)
         a = _lib.AmpDemoArgs(ring=self.demo.desc(), sampling_cdf=self.cdf().data_ptr(), num_samples=n, num_steps=self.num_steps,
                              amp_width=self.amp_width, upright=int(self.upright), dt=self.dt, motion_ids_out=_lib.ptr(motion_ids_out),
                              times_out=_lib.ptr(times_out))
+        fn = _DEMO_FETCH[self.layout]
+        handle = self.motion_lib.smplx_handle if self.smplx else self.motion_lib.handle
         with torch.cuda.device(self.device):
-            _lib.check(self.lib.pulse_amp_demo_fetch(self.motion_lib.handle, C.byref(a), self._stream()), "pulse_amp_demo_fetch")
+            _lib.check(getattr(self.lib, fn)(handle, C.byref(a), self._stream()), fn)
 
     def init_demo(self) -> None:
         """`_init_amp_demo_buf`: ceil(buffer_size / amp_batch_size) fetches of amp_batch_size rows, wrapping as the ring does."""

@@ -1,6 +1,7 @@
 // The AMP demo and replay rings (learning/replay_buffer.py ReplayBuffer, AMPAgent._update_amp_demos / _store_replay_amp_obs and the
 // buffer samples of train_epoch, phc/learning/amp_agent.py:476-484, :988-1057) on device-side counters:
-//   demo_fetch_kernel    one warp per (row, history step): clip and t0 draws, the motion at t0 - k dt, the AMP row straight into the ring;
+//   demo_fetch_kernel    one warp per (row, history step): clip and t0 draws, the motion at t0 - k dt, the AMP row straight into the ring
+//                        (SMPL, and SMPL-X through pulse_smplx_amp_demo_fetch);
 //   keep_compact_kernel  one CTA: the Bernoulli keep mask (once total_count > capacity) and the ordered compaction of the kept rows;
 //   ring_store_kernel    one warp per stored row: the kept row (or the subset's pick of it) into the ring at head, with wrap;
 //   ring_sample_kernel   one warp per gathered row: the permuted ring position (or the fallback row);
@@ -61,8 +62,9 @@ __device__ __forceinline__ void copy_row(float* __restrict__ dst, const float* _
 }
 
 // ---- demo fetch -------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kRingWarps * 32) demo_fetch_kernel(const pulse_motionlib_desc_t lib, const pulse_amp_demo_args_t a) {
-  __shared__ float stage_all[kRingWarps][PULSE_AMP_OBS];
+template <class L, class Desc>
+__global__ void __launch_bounds__(kRingWarps * 32) demo_fetch_kernel(const Desc lib, const pulse_amp_demo_args_t a) {
+  __shared__ float stage_all[kRingWarps][L::kAmpObs];
   float* stage = stage_all[threadIdx.x >> 5];
   const int lane = threadIdx.x & 31;
   const long long items = a.num_samples * a.num_steps;
@@ -89,9 +91,9 @@ __global__ void __launch_bounds__(kRingWarps * 32) demo_fetch_kernel(const pulse
     frame_blend_rn(t, mlen, lib.num_frames[mid], lib.dt[mid], i0, i1, b);
     const long long f0 = i0 + lib.length_starts[mid], f1 = i1 + lib.length_starts[mid];
     const long long slot = (head + i) % a.ring.capacity;
-    store_motion_amp_row(b, lib.frame_rec + f0 * PULSE_FRAME_REC, lib.frame_rec + f1 * PULSE_FRAME_REC, lib.aux_rec + f0 * PULSE_AUX_REC,
-                         lib.aux_rec + f1 * PULSE_AUX_REC, a.ring.rows + slot * a.ring.row_floats + k * a.amp_width, a.amp_width, stage, lane,
-                         a.upright != 0);
+    store_motion_amp_row<L>(b, lib.frame_rec + f0 * L::kFrameRec, lib.frame_rec + f1 * L::kFrameRec, lib.aux_rec + f0 * L::kAuxRec,
+                            lib.aux_rec + f1 * L::kAuxRec, a.ring.rows + slot * a.ring.row_floats + k * a.amp_width, a.amp_width, stage, lane,
+                            a.upright != 0);
   }
 }
 
@@ -185,30 +187,43 @@ int check_ring(const pulse_amp_ring_t& r, const char* who) {
   return PULSE_OK;
 }
 
+// The checks of a demo fetch over a MotionLib descriptor `d` whose AMP rows are `full` floats (`full - 1` without the root height),
+// then the fetch kernel in layout L and store()'s counter update.
+template <class L, class Desc>
+int demo_fetch(const Desc& d, const pulse_amp_demo_args_t& a, void* stream, const char* who) {
+  if (const int s = check_ring(a.ring, who)) return s;
+  constexpr int full = L::kAmpObs;
+  PULSE_REQUIRE(a.sampling_cdf != nullptr && d.num_motions >= 1, "%s: null sampling_cdf", who);
+  PULSE_REQUIRE(d.aux_rec != nullptr, "%s: the MotionLib handle has no aux records (dof_pos / dof_vel)", who);
+  PULSE_REQUIRE(a.num_steps >= 1 && a.num_steps <= 16, "%s: num_steps %d outside [1,16]", who, a.num_steps);
+  PULSE_REQUIRE(a.amp_width == full || a.amp_width == full - 1, "%s: amp_width %d is neither %d nor %d", who, a.amp_width, full, full - 1);
+  PULSE_REQUIRE(L::kUpright || a.upright == 0, "%s: the SMPL-X rows take the heading of remove_base_rot(q0) (upright 0)", who);
+  PULSE_REQUIRE(a.ring.row_floats == a.num_steps * a.amp_width, "%s: ring rows of %d floats, the demo rows have %d", who,
+                a.ring.row_floats, a.num_steps * a.amp_width);
+  PULSE_REQUIRE(a.num_samples >= 0 && a.num_samples <= a.ring.capacity, "%s: num_samples %lld outside [0, capacity]", who,
+                (long long)a.num_samples);
+  if (a.num_samples == 0) return PULSE_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  demo_fetch_kernel<L><<<grid_for(a.num_samples * a.num_steps, kRingWarps), kRingWarps * 32, 0, st>>>(d, a);
+  PULSE_LAUNCH_OK("demo_fetch_kernel");
+  ring_store_done_kernel<<<1, 1, 0, st>>>(reinterpret_cast<long long*>(a.ring.ctr), (long long)a.ring.capacity, (long long)a.num_samples);
+  PULSE_LAUNCH_OK("ring_store_done_kernel");
+  return PULSE_OK;
+}
+
 }  // namespace
 }  // namespace pulse
 
 extern "C" int pulse_amp_demo_fetch(const pulse_motionlib_t* lib, const pulse_amp_demo_args_t* args, void* stream) {
   using namespace pulse;
   PULSE_REQUIRE(lib != nullptr && args != nullptr, "pulse_amp_demo_fetch: null lib/args");
-  const pulse_amp_demo_args_t& a = *args;
-  if (const int s = check_ring(a.ring, "pulse_amp_demo_fetch")) return s;
-  PULSE_REQUIRE(a.sampling_cdf != nullptr && lib->d.num_motions >= 1, "pulse_amp_demo_fetch: null sampling_cdf");
-  PULSE_REQUIRE(lib->d.aux_rec != nullptr, "pulse_amp_demo_fetch: the MotionLib handle has no aux records (dof_pos / dof_vel)");
-  PULSE_REQUIRE(a.num_steps >= 1 && a.num_steps <= 16, "pulse_amp_demo_fetch: num_steps %d outside [1,16]", a.num_steps);
-  PULSE_REQUIRE(a.amp_width == PULSE_AMP_OBS || a.amp_width == PULSE_AMP_OBS_NO_HEIGHT, "pulse_amp_demo_fetch: amp_width %d is neither %d nor %d",
-                a.amp_width, PULSE_AMP_OBS, PULSE_AMP_OBS_NO_HEIGHT);
-  PULSE_REQUIRE(a.ring.row_floats == a.num_steps * a.amp_width, "pulse_amp_demo_fetch: ring rows of %d floats, the demo rows have %d",
-                a.ring.row_floats, a.num_steps * a.amp_width);
-  PULSE_REQUIRE(a.num_samples >= 0 && a.num_samples <= a.ring.capacity, "pulse_amp_demo_fetch: num_samples %lld outside [0, capacity]",
-                (long long)a.num_samples);
-  if (a.num_samples == 0) return PULSE_OK;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  demo_fetch_kernel<<<grid_for(a.num_samples * a.num_steps, kRingWarps), kRingWarps * 32, 0, st>>>(lib->d, a);
-  PULSE_LAUNCH_OK("demo_fetch_kernel");
-  ring_store_done_kernel<<<1, 1, 0, st>>>(reinterpret_cast<long long*>(a.ring.ctr), (long long)a.ring.capacity, (long long)a.num_samples);
-  PULSE_LAUNCH_OK("ring_store_done_kernel");
-  return PULSE_OK;
+  return demo_fetch<SmplLayout>(lib->d, *args, stream, "pulse_amp_demo_fetch");
+}
+
+extern "C" int pulse_smplx_amp_demo_fetch(const pulse_smplx_motionlib_t* lib, const pulse_amp_demo_args_t* args, void* stream) {
+  using namespace pulse;
+  PULSE_REQUIRE(lib != nullptr && args != nullptr, "pulse_smplx_amp_demo_fetch: null lib/args");
+  return demo_fetch<SmplxLayout>(lib->d, *args, stream, "pulse_smplx_amp_demo_fetch");
 }
 
 extern "C" int pulse_amp_replay_store(const pulse_amp_store_args_t* args, void* stream) {

@@ -5,22 +5,44 @@
 
 namespace pulse {
 
-// The body layouts the latent-task step and reset code is instantiated for.  B bodies give a MotionLib frame record
+namespace {  // __constant__ tables are per module; one copy in every translation unit that builds AMP rows
+// kept joints (joint = body - 1), dropping L_Toe(3) R_Toe(7) L_Hand(17) R_Hand(22): humanoid.py:397,417-421
+__constant__ int c_kept_joint[19] = {0, 1, 2, 4, 5, 6, 8, 9, 10, 11, 12, 13, 14, 15, 16, 18, 19, 20, 21};
+__constant__ int c_key_body[4] = {7, 3, 22, 17};  // R_Ankle, L_Ankle, R_Wrist, L_Wrist (env_im.yaml:36)
+// SMPL-X: joints 0..50 without L_Toe(3) R_Toe(7) (humanoid.py:404-421, no hand joints dropped); key bodies R_Ankle, L_Ankle,
+// R_Wrist, L_Wrist in SMPLH_MUJOCO_NAMES order (env_pulsex_amp.yaml key_bodies)
+__constant__ int c_smplx_kept_joint[49] = {0,  1,  2,  4,  5,  6,  8,  9,  10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26,
+                                           27, 28, 29, 30, 31, 32, 33, 34, 35, 36, 37, 38, 39, 40, 41, 42, 43, 44, 45, 46, 47, 48, 49, 50};
+__constant__ int c_smplx_key_body[4] = {7, 3, 36, 17};
+}  // namespace
+
+// The body layouts the latent-task step, reset and AMP code is instantiated for.  B bodies give a MotionLib frame record
 // pos 3B | rot 4B | vel 3B | angvel 3B, an aux record lrs 4B | dvs 3(B - 1) | pad, and a self observation of 1 + 3(B - 1) + 6B + 3B + 3B
 // floats.  kUpright: the step's self observation takes the heading of the root rotation itself (has_upright_start), otherwise
-// of remove_base_rot(root).  kSmplTerms: the terms only the SMPL path serves (strike, the power term, the AMP history rows).
+// of remove_base_rot(root).  kSmplTerms: the task terms only the SMPL path serves (strike, the power term).  The AMP observation
+// (build_amp_observations_smpl with dof_subset) keeps kAmpJoints joints, kept_joint(i) for i < kAmpJoints, and the four key bodies
+// key_body(i): kAmpObs = 1 + 6 + 3 + 3 + 9 kAmpJoints + 12 floats with the root height.
 struct SmplLayout {
   static constexpr int kBodies = PULSE_NUM_BODIES, kDofs = PULSE_NUM_DOF, kSelfObs = PULSE_SELF_OBS;
   static constexpr int kFrameRec = PULSE_FRAME_REC, kAuxRec = PULSE_AUX_REC;
+  static constexpr int kAmpJoints = 19, kAmpObs = PULSE_AMP_OBS;
   static constexpr bool kUpright = true, kSmplTerms = true;
   using StepArgs = pulse_ztask_step_args_t;
+  __device__ static __forceinline__ int kept_joint(int i) { return c_kept_joint[i]; }
+  __device__ static __forceinline__ int key_body(int i) { return c_key_body[i]; }
 };
 struct SmplxLayout {
   static constexpr int kBodies = PULSE_SMPLX_BODIES, kDofs = PULSE_SMPLX_DOF, kSelfObs = PULSE_SMPLX_SELF_OBS;
   static constexpr int kFrameRec = PULSE_SMPLX_FRAME_REC, kAuxRec = PULSE_SMPLX_AUX_REC;
+  static constexpr int kAmpJoints = 49, kAmpObs = PULSE_SMPLX_AMP_OBS;
   static constexpr bool kUpright = false, kSmplTerms = false;
   using StepArgs = pulse_smplx_speed_step_args_t;
+  __device__ static __forceinline__ int kept_joint(int i) { return c_smplx_kept_joint[i]; }
+  __device__ static __forceinline__ int key_body(int i) { return c_smplx_key_body[i]; }
 };
+static_assert(13 + 9 * SmplLayout::kAmpJoints + 12 == PULSE_AMP_OBS, "SMPL AMP observation");
+static_assert(13 + 9 * SmplxLayout::kAmpJoints + 12 == PULSE_SMPLX_AMP_OBS, "SMPL-X AMP observation");
+static_assert(PULSE_SMPLX_AMP_OBS - 1 == PULSE_SMPLX_AMP_OBS_NO_HEIGHT, "SMPL-X AMP observation without the root height");
 static_assert(3 * PULSE_SMPLX_BODIES + 4 * PULSE_SMPLX_BODIES + 6 * PULSE_SMPLX_BODIES == PULSE_SMPLX_FRAME_REC, "SMPL-X frame record");
 static_assert(4 * PULSE_SMPLX_BODIES + PULSE_SMPLX_DOF <= PULSE_SMPLX_AUX_REC && PULSE_SMPLX_AUX_REC % 4 == 0, "SMPL-X aux record");
 static_assert(1 + 3 * (PULSE_SMPLX_BODIES - 1) + 12 * PULSE_SMPLX_BODIES == PULSE_SMPLX_SELF_OBS, "SMPL-X self observation");
@@ -39,23 +61,21 @@ __device__ __forceinline__ void store_self_obs(float* o, int j, Vec3 p, Vec3 p_r
   stv(o + 12 * B - 2 + 3 * j, yaw_rot(yr, w));
 }
 
-namespace {  // __constant__ tables are per module; one copy in every translation unit that builds AMP rows
-// kept joints (joint = body - 1), dropping L_Toe(3) R_Toe(7) L_Hand(17) R_Hand(22): humanoid.py:397,417-421
-__constant__ int c_kept_joint[19] = {0, 1, 2, 4, 5, 6, 8, 9, 10, 11, 12, 13, 14, 15, 16, 18, 19, 20, 21};
-__constant__ int c_key_body[4] = {7, 3, 22, 17};  // R_Ankle, L_Ankle, R_Wrist, L_Wrist (env_im.yaml:36)
-}  // namespace
-
 struct AmpJoint {
   Vec3 exp_map;  // the joint's local rotation
   Vec3 vel;      // its three dof velocities
 };
 
-// build_amp_observations_smpl (humanoid_amp.py:924-969) with dof_to_obs_smpl (humanoid.py:1436-1446): one warp writes the 196-float
-// AMP observation [h | six(hinv q0) | R v0 | R w0 | 19 x six(dof) | 57 dof velocities | 4 x R(key - p0)] of the root state
-// (p0, q0, v0, w0).  Lane 0 writes the root features, lanes 0..18 the kept joints, lanes 19..22 the key bodies.  joint(jt) returns
-// joint jt's AmpJoint, key_pos(kb) key body kb's world position.
-template <class JointFn, class KeyPosFn>
+// build_amp_observations_smpl (humanoid_amp.py:924-969) with dof_to_obs_smpl (humanoid.py:1436-1446) in body layout L: one warp writes
+// the L::kAmpObs-float AMP observation [h | six(hinv q0) | R v0 | R w0 | J x six(dof) | 3J dof velocities | 4 x R(key - p0)] of the
+// root state (p0, q0, v0, w0), J = L::kAmpJoints (196 floats for SMPL, 466 for SMPL-X).  Lane 0 writes the root features, lane l the
+// kept joints l, l + 32, ... below J, and the four lanes after the last joint lane of the last pass the key bodies (SMPL: joints on
+// lanes 0..18, key bodies on 19..22; SMPL-X: joints on 0..31 and 0..16, key bodies on 17..20).  joint(jt) returns joint jt's AmpJoint,
+// key_pos(kb) key body kb's world position.
+template <class L = SmplLayout, class JointFn, class KeyPosFn>
 __device__ __forceinline__ void store_amp_obs(float* o, int lane, Vec3 p0, Quat q0, Vec3 v0, Vec3 w0, JointFn joint, KeyPosFn key_pos) {
+  constexpr int kJ = L::kAmpJoints, kPasses = (kJ + 31) / 32, kKey0 = kJ - 32 * (kPasses - 1);
+  static_assert(kKey0 + 4 <= 32, "the key bodies share the last pass's warp");
   float hs, hc;
   heading_half(q0, hs, hc);
   const Quat h_inv = {0.0f, 0.0f, -hs, hc};
@@ -66,18 +86,22 @@ __device__ __forceinline__ void store_amp_obs(float* o, int lane, Vec3 p0, Quat 
     stv(o + 7, yaw_rot(yr, v0));
     stv(o + 10, yaw_rot(yr, w0));
   }
-  if (lane < 19) {
-    const AmpJoint jt = joint(c_kept_joint[lane]);
-    qsix(exp_map_quat(jt.exp_map), o + 13 + 6 * lane);
-    stv(o + 127 + 3 * lane, jt.vel);
-  } else if (lane < 23) {
-    stv(o + 184 + 3 * (lane - 19), yaw_rot(yr, key_pos(c_key_body[lane - 19]) - p0));
+#pragma unroll 1
+  for (int s = 0; s < kPasses; ++s) {   // not unrolled: two SMPL-X passes unrolled keep registers live across the sincos slow path
+    const int i = lane + 32 * s;
+    if (i < kJ) {
+      const AmpJoint jt = joint(L::kept_joint(i));
+      qsix(exp_map_quat(jt.exp_map), o + 13 + 6 * i);
+      stv(o + 13 + 6 * kJ + 3 * i, jt.vel);
+    } else if (s == kPasses - 1 && lane < kKey0 + 4) {
+      stv(o + 13 + 9 * kJ + 3 * (lane - kKey0), yaw_rot(yr, key_pos(L::key_body(lane - kKey0)) - p0));
+    }
   }
 }
 
 // store_amp_obs from the simulator state of env e: the root and key bodies from body_state ([pos | quat | vel | ang vel] per body),
 // the joints from the dof position / velocity views.
-template <class Args>
+template <class L = SmplLayout, class Args>
 __device__ __forceinline__ void store_amp_obs_sim(float* o, int lane, const Args& a, long long e) {
   const float* bs = a.body_state + e * a.body_env_stride;
   const float* dp = a.dof_pos + e * a.dof_env_stride;
@@ -88,7 +112,7 @@ __device__ __forceinline__ void store_amp_obs_sim(float* o, int lane, const Args
                     {dv[(3 * jt + 0) * ds], dv[(3 * jt + 1) * ds], dv[(3 * jt + 2) * ds]}};
   };
   const auto key_pos = [&](int kb) { return ldv(bs + kb * PULSE_BODY_STATE_W); };
-  store_amp_obs(o, lane, ldv(bs), ldq(bs + 3), ldv(bs + 7), ldv(bs + 10), joint, key_pos);
+  store_amp_obs<L>(o, lane, ldv(bs), ldq(bs + 3), ldv(bs + 7), ldv(bs + 10), joint, key_pos);
 }
 
 // The fall test of compute_humanoid_reset (humanoid.py:1573-1608) for body lane j of env e: `contact` when a body that may not

@@ -3,7 +3,7 @@
 //                         the humanoid and target actor lists and a device-side count;
 //   reset_warps           one warp per (reset env, AMP history step k), for a body layout (SMPL, SMPL-X): clip and start-time
 //                         draws, MotionLib gather, SMPL ground fix from the per-frame floor table, the caller's adjustment of the root
-//                         and bodies, the scatter into the simulator's views, counters and the AMP rows (195- or 196-float layout).
+//                         and bodies, the scatter into the simulator's views, counters and the AMP rows (195 / 196 floats for SMPL, 465 / 466 for SMPL-X).
 // The entry points, argument structs and Philox word layout are documented in include/pulse_b200.h.
 #pragma once
 #include "compact.cuh"
@@ -43,7 +43,7 @@ __global__ void __launch_bounds__(kCompactThreads) reset_compact_kernel(const pu
 // runs after the ground fix once per body a lane holds (lane l holds bodies l and l + 32 where the layout has them): (p, rq, v) are
 // that body's position, rotation and velocity, (rp, rr, rv, rw) the root's in every lane; a lane's second call gets its own copy of the
 // root, so the root is adjusted once.  r0 is Philox block (seed, e, off) when a draw is not injected or `more_draws` is set, zero
-// otherwise.  What it leaves is what _set_env_state writes.  The AMP history rows are SMPL's (L::kSmplTerms).
+// otherwise.  What it leaves is what _set_env_state writes.  The AMP history rows are layout L's (`stage`: L::kAmpObs floats).
 template <class L, class Lib, class Adjust>
 __device__ __forceinline__ void reset_warps(const Lib& lib, const pulse_ztask_reset_args_t& a, bool more_draws, float* stage,
                                             const Adjust& adjust) {
@@ -81,12 +81,10 @@ __device__ __forceinline__ void reset_warps(const Lib& lib, const pulse_ztask_re
     const float* x0 = lib.aux_rec + f0 * L::kAuxRec;
     const float* x1 = lib.aux_rec + f1 * L::kAuxRec;
 
-    if constexpr (L::kSmplTerms) {
-      if (k > 0) {   // _init_amp_obs_ref: the motion at t0 - k dt as it is, without the ground fix or the pose adjustment
-        store_motion_amp_row(b, r0p, r1p, x0, x1, a.amp_obs_buf + (e * a.num_amp_steps + k) * a.amp_width, a.amp_width, stage, lane,
-                             upright);
-        continue;
-      }
+    if (k > 0) {   // _init_amp_obs_ref: the motion at t0 - k dt as it is, without the ground fix or the pose adjustment
+      store_motion_amp_row<L>(b, r0p, r1p, x0, x1, a.amp_obs_buf + (e * a.num_amp_steps + k) * a.amp_width, a.amp_width, stage, lane,
+                              upright);
+      continue;
     }
 
     // ---- the reset state: lane l holds bodies l (slot 0) and l + 32 (slot 1) -------------------------------------------------------
@@ -145,22 +143,20 @@ __device__ __forceinline__ void reset_warps(const Lib& lib, const pulse_ztask_re
       if (a.reset_buf != nullptr) a.reset_buf[e] = 0;
       if (a.terminate_buf != nullptr) a.terminate_buf[e] = 0;
     }
-    if constexpr (L::kSmplTerms) {
-      if (a.amp_obs_buf == nullptr) continue;
-      // row 0: _compute_amp_observations(env_ids) of the rigid bodies and dofs just written
-      __syncwarp();
-      const float* bs = a.rigid_body_state + e * a.body_env_stride;
-      const float* dp = a.dof_pos + e * a.dof_env_stride;
-      const float* dv = a.dof_vel + e * a.dof_env_stride;
-      const long long ds = a.dof_elem_stride;
-      const auto joint = [&](int jt) {
-        return AmpJoint{{dp[(3 * jt + 0) * ds], dp[(3 * jt + 1) * ds], dp[(3 * jt + 2) * ds]},
-                        {dv[(3 * jt + 0) * ds], dv[(3 * jt + 1) * ds], dv[(3 * jt + 2) * ds]}};
-      };
-      const auto key_pos = [&](int kb) { return ldv(bs + kb * PULSE_BODY_STATE_W); };
-      store_amp_row(a.amp_obs_buf + e * a.num_amp_steps * a.amp_width, a.amp_width, stage, lane, ldv(bs), ldq(bs + 3), ldv(bs + 7), ldv(bs + 10),
-                    upright, joint, key_pos);
-    }
+    if (a.amp_obs_buf == nullptr) continue;
+    // row 0: _compute_amp_observations(env_ids) of the rigid bodies and dofs just written
+    __syncwarp();
+    const float* bs = a.rigid_body_state + e * a.body_env_stride;
+    const float* dp = a.dof_pos + e * a.dof_env_stride;
+    const float* dv = a.dof_vel + e * a.dof_env_stride;
+    const long long ds = a.dof_elem_stride;
+    const auto joint = [&](int jt) {
+      return AmpJoint{{dp[(3 * jt + 0) * ds], dp[(3 * jt + 1) * ds], dp[(3 * jt + 2) * ds]},
+                      {dv[(3 * jt + 0) * ds], dv[(3 * jt + 1) * ds], dv[(3 * jt + 2) * ds]}};
+    };
+    const auto key_pos = [&](int kb) { return ldv(bs + kb * PULSE_BODY_STATE_W); };
+    store_amp_row<L>(a.amp_obs_buf + e * a.num_amp_steps * a.amp_width, a.amp_width, stage, lane, ldv(bs), ldq(bs + 3), ldv(bs + 7), ldv(bs + 10),
+                     upright, joint, key_pos);
   }
 }
 

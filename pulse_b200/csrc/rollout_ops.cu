@@ -10,7 +10,8 @@
 //                       of the in-place shift (7 056 + 7 840) followed by a 7 840 + 7 840 B copy.  Envs reset since the last step take
 //                       their previous row from the rows `pulse_reset_ref_state` back-filled (`fresh` flags, cleared here).
 //   amp_row_any_kernel  the same row in the other layouts the resets write: 195 floats (no root height; rows are 780 B, so not
-//                       16-byte units) and / or the remove_base_rot heading of a non-upright start.
+//                       16-byte units) and / or the remove_base_rot heading of a non-upright start; instantiated for SMPL-X
+//                       (pulse_smplx_amp_obs_row, 466 / 465 floats, not 16-byte units either).
 #include "philox.cuh"
 #include "motion_amp.cuh"
 #include "value_unnorm.cuh"
@@ -110,8 +111,9 @@ __global__ void __launch_bounds__(128) amp_row_kernel(const pulse_amp_row_args_t
 
 constexpr int kAmpRowWarps = 4;
 
+template <class L>
 __global__ void __launch_bounds__(kAmpRowWarps * 32) amp_row_any_kernel(const pulse_amp_row_args_t a, int width, long long n) {
-  __shared__ float stage_all[kAmpRowWarps][PULSE_AMP_OBS];
+  __shared__ float stage_all[kAmpRowWarps][L::kAmpObs];
   const long long e = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (e >= n) return;
@@ -131,8 +133,8 @@ __global__ void __launch_bounds__(kAmpRowWarps * 32) amp_row_any_kernel(const pu
                     {dv[(3 * jt + 0) * ds], dv[(3 * jt + 1) * ds], dv[(3 * jt + 2) * ds]}};
   };
   const auto key_pos = [&](int kb) { return ldv(bs + kb * PULSE_BODY_STATE_W); };
-  store_amp_row(out, width, stage_all[threadIdx.x >> 5], lane, ldv(bs), ldq(bs + 3), ldv(bs + 7), ldv(bs + 10), a.remove_base_rot == 0, joint,
-                key_pos);
+  store_amp_row<L>(out, width, stage_all[threadIdx.x >> 5], lane, ldv(bs), ldq(bs + 3), ldv(bs + 7), ldv(bs + 10), a.remove_base_rot == 0, joint,
+                   key_pos);
 }
 
 __global__ void bump_counter_kernel(unsigned long long* c, unsigned long long by) { *c += by; }
@@ -188,8 +190,8 @@ extern "C" int pulse_amp_obs_row(const pulse_amp_row_args_t* args, int64_t num_e
   PULSE_REQUIRE((a.fresh == nullptr) == (a.fresh_rows == nullptr), "pulse_amp_obs_row: fresh flags and fresh_rows go together");
   PULSE_REQUIRE(a.body_env_stride >= PULSE_NUM_BODIES * PULSE_BODY_STATE_W, "pulse_amp_obs_row: body_env_stride too small");
   if (width != PULSE_AMP_OBS || a.remove_base_rot != 0) {
-    amp_row_any_kernel<<<static_cast<unsigned>((num_envs + kAmpRowWarps - 1) / kAmpRowWarps), kAmpRowWarps * 32, 0,
-                         static_cast<cudaStream_t>(stream)>>>(a, width, (long long)num_envs);
+    amp_row_any_kernel<SmplLayout><<<static_cast<unsigned>((num_envs + kAmpRowWarps - 1) / kAmpRowWarps), kAmpRowWarps * 32, 0,
+                                     static_cast<cudaStream_t>(stream)>>>(a, width, (long long)num_envs);
     PULSE_LAUNCH_OK("amp_row_any_kernel");
     return PULSE_OK;
   }
@@ -198,6 +200,29 @@ extern "C" int pulse_amp_obs_row(const pulse_amp_row_args_t* args, int64_t num_e
   const long long threads = num_envs * 32;
   amp_row_kernel<<<static_cast<unsigned>((threads + 127) / 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(a, (long long)num_envs);
   PULSE_LAUNCH_OK("amp_row_kernel");
+  return PULSE_OK;
+}
+
+extern "C" int pulse_smplx_amp_obs_row(const pulse_amp_row_args_t* args, int64_t num_envs, void* stream) {
+  using namespace pulse;
+  PULSE_REQUIRE(args != nullptr, "pulse_smplx_amp_obs_row: null args");
+  PULSE_REQUIRE(num_envs >= 0, "pulse_smplx_amp_obs_row: negative num_envs");
+  if (num_envs == 0) return PULSE_OK;
+  const pulse_amp_row_args_t& a = *args;
+  PULSE_REQUIRE(a.body_state && a.dof_pos && a.dof_vel && a.prev && a.out, "pulse_smplx_amp_obs_row: null buffer");
+  PULSE_REQUIRE(a.num_steps >= 1 && a.num_steps <= 16, "pulse_smplx_amp_obs_row: num_steps %d outside [1,16]", a.num_steps);
+  PULSE_REQUIRE(a.amp_width == PULSE_SMPLX_AMP_OBS || a.amp_width == PULSE_SMPLX_AMP_OBS_NO_HEIGHT,
+                "pulse_smplx_amp_obs_row: amp_width %d is neither %d nor %d", a.amp_width, PULSE_SMPLX_AMP_OBS, PULSE_SMPLX_AMP_OBS_NO_HEIGHT);
+  PULSE_REQUIRE(a.remove_base_rot == 1, "pulse_smplx_amp_obs_row: the SMPL-X rows take the heading of remove_base_rot(q0) (remove_base_rot 1)");
+  const int width = a.amp_width;
+  PULSE_REQUIRE(a.ld_prev >= (a.num_steps - 1) * width && a.ld_out >= a.num_steps * width, "pulse_smplx_amp_obs_row: row strides too small");
+  PULSE_REQUIRE(a.prev != a.out, "pulse_smplx_amp_obs_row: prev and out must be different experience slices");
+  PULSE_REQUIRE((a.fresh == nullptr) == (a.fresh_rows == nullptr), "pulse_smplx_amp_obs_row: fresh flags and fresh_rows go together");
+  PULSE_REQUIRE(a.body_env_stride >= PULSE_SMPLX_BODIES * PULSE_BODY_STATE_W, "pulse_smplx_amp_obs_row: body_env_stride too small");
+  PULSE_REQUIRE(a.dof_elem_stride >= 1 && a.dof_env_stride >= PULSE_SMPLX_DOF * a.dof_elem_stride, "pulse_smplx_amp_obs_row: dof strides too small");
+  amp_row_any_kernel<SmplxLayout><<<static_cast<unsigned>((num_envs + kAmpRowWarps - 1) / kAmpRowWarps), kAmpRowWarps * 32, 0,
+                                    static_cast<cudaStream_t>(stream)>>>(a, width, (long long)num_envs);
+  PULSE_LAUNCH_OK("amp_row_any_kernel<SmplxLayout>");
   return PULSE_OK;
 }
 

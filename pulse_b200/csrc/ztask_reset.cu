@@ -5,7 +5,8 @@
 //                         gather, SMPL ground fix, _set_env_state, counters, AMP rows) with the task's pose adjustment and the strike
 //                         target;
 //   ztask_task_kernel     (pulse_ztask_reset_task) the reach / speed _reset_task over the same list, after the observation.
-// pulse_reset_ztask_smplx runs the first two for the SMPL-X speed task: ztask_reset_kernel<SmplxLayout>, without AMP rows or target.
+// pulse_reset_ztask_smplx runs the first two for the SMPL-X speed task: ztask_reset_kernel<SmplxLayout>, with the 465- / 466-float AMP
+// rows and without a strike target.
 // The entry points, argument structs and Philox word layout are documented in include/pulse_b200.h.
 #include "reset_warps.cuh"
 
@@ -17,7 +18,7 @@ constexpr unsigned long long kTaskStream = 2ull << 32;     // Philox index e + 2
 
 template <class L, class Lib>
 __global__ void __launch_bounds__(kResetWarps * 32) ztask_reset_kernel(const Lib lib, const pulse_ztask_reset_args_t a) {
-  __shared__ float stage_all[kResetWarps][L::kSmplTerms ? PULSE_AMP_OBS : 1];
+  __shared__ float stage_all[kResetWarps][L::kAmpObs];
   const bool upright = a.upright != 0;
   const auto adjust = [&](long long e, int lane, const Philox4& r0, unsigned long long off, Vec3& p, Quat& rq, Vec3& v, Vec3& rp, Quat& rr,
                           Vec3& rv, Vec3& rw) {
@@ -150,8 +151,12 @@ extern "C" int pulse_reset_ztask_smplx(const pulse_smplx_motionlib_t* lib, const
                 a.body_env_stride >= PULSE_SMPLX_BODIES * PULSE_BODY_STATE_W, "pulse_reset_ztask_smplx: bad root / dof / rigid-body strides");
   PULSE_REQUIRE(a.contact_forces == nullptr || (a.contact_bodies >= 0 && a.contact_env_stride >= 3 * a.contact_bodies),
                 "pulse_reset_ztask_smplx: bad contact-force strides");
-  PULSE_REQUIRE(a.amp_obs_buf == nullptr, "pulse_reset_ztask_smplx: the AMP history back-fill is not served for SMPL-X (amp_obs_buf must be NULL)");
-  PULSE_REQUIRE(a.amp_fresh == nullptr, "pulse_reset_ztask_smplx: no AMP rows for SMPL-X (amp_fresh must be NULL)");
+  PULSE_REQUIRE(a.amp_obs_buf == nullptr || (a.num_amp_steps >= 1 && a.num_amp_steps <= 16),
+                "pulse_reset_ztask_smplx: the AMP history back-fill takes num_amp_steps in [1,16], not %d", a.num_amp_steps);
+  PULSE_REQUIRE(a.amp_obs_buf == nullptr || a.amp_width == PULSE_SMPLX_AMP_OBS || a.amp_width == PULSE_SMPLX_AMP_OBS_NO_HEIGHT,
+                "pulse_reset_ztask_smplx: AMP amp_width %d is neither %d nor %d (the SMPL-X rows)", a.amp_width, PULSE_SMPLX_AMP_OBS,
+                PULSE_SMPLX_AMP_OBS_NO_HEIGHT);
+  PULSE_REQUIRE(a.amp_fresh == nullptr || a.amp_obs_buf != nullptr, "pulse_reset_ztask_smplx: amp_fresh flags need the back-filled AMP amp_obs_buf");
   PULSE_REQUIRE(a.target_states == nullptr, "pulse_reset_ztask_smplx: the SMPL-X reset serves the speed task (target_states must be NULL)");
   PULSE_REQUIRE(a.pose_mode == PULSE_ZPOSE_FACE_X, "pulse_reset_ztask_smplx: pose_mode %d, the speed task's is PULSE_ZPOSE_FACE_X", a.pose_mode);
   PULSE_REQUIRE(a.floor != nullptr && a.floor_len >= lib->d.total_frames, "pulse_reset_ztask_smplx: floor table of %lld frames, the MotionLib has %lld",
@@ -162,7 +167,7 @@ extern "C" int pulse_reset_ztask_smplx(const pulse_smplx_motionlib_t* lib, const
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   reset_compact_kernel<<<1, kCompactThreads, 0, st>>>(a, (long long)num_envs);
   PULSE_LAUNCH_OK("reset_compact_kernel");
-  const long long upper = a.env_ids_in != nullptr ? a.num_ids : num_envs;
+  const long long upper = (a.env_ids_in != nullptr ? a.num_ids : num_envs) * (a.amp_obs_buf != nullptr ? a.num_amp_steps : 1);
   ztask_reset_kernel<SmplxLayout><<<grid_for(upper, kResetWarps), kResetWarps * 32, 0, st>>>(lib->d, a);
   PULSE_LAUNCH_OK("ztask_reset_kernel<SmplxLayout>");
   return PULSE_OK;

@@ -10,6 +10,9 @@ import torch
 from . import _lib
 from .rollout import GraphRunner, finish_returns
 
+# the AMP row entry point per body layout (AmpBuffersB200.layout)
+_AMP_ROW = {"smpl": "pulse_amp_obs_row", "smplx": "pulse_smplx_amp_obs_row"}
+
 
 class LatentStepsB200(GraphRunner):
     """One horizon of a latent-space task per `play_steps()`.  A subclass supplies the task's pieces of a step:
@@ -40,7 +43,9 @@ class LatentStepsB200(GraphRunner):
     of the whole horizon (only the first amp_minibatch_size rows of each minibatch are gathered), passes amp = (amp_obs rows, replay
     rows, demo rows) at each minibatch's row offset to `train_minibatch` -- the discriminator's gradients share the actor / critic
     gradient-norm clip -- and stores the horizon's rows into the replay ring after the last mini-epoch; all of it graph-captured.
-    Memory at 8192 envs, T = 32, 10 x 196 floats: amp_obs 2.06 GB, each 200 000-row ring 1.57 GB, each gathered sample 0.51 GB.
+    Memory at 8192 envs, T = 32, 10 x 196 floats: amp_obs 2.06 GB, each 200 000-row ring 1.57 GB, each gathered sample 0.51 GB.  With
+    the SMPL-X rows (10 x 465 floats): amp_obs n * 32 * 4650 * 4 B (0.91 GB at 1536 envs, 4.9 GB at 8192), the bf16 discriminator
+    operand n * 32 * 4672 * 2 B (0.46 GB, 2.4 GB), each 200 000-row ring 3.72 GB.
 
     The experience buffers are env-major (`obses[n, T, W]`, `actions[n, T, E]`, `mus[n, T, E]`, `neglogp[n, T]`; `adv[n*T]`, `ret[n*T]`), so
     a minibatch is a contiguous row range; `values`, `next_values` [T, n, 1], `rewards`, `dones` [T, n] are time-major as GAE reads them.
@@ -153,7 +158,7 @@ class LatentStepsB200(GraphRunner):
         self._pre_physics(dec, t)
 
     def _amp_row(self, t: int) -> None:
-        """The AMP row of step t (humanoid_amp.py:194-210, :622-667; amp_agent.py:385) into amp_obs[:, t]."""
+        """The AMP row of step t (humanoid_amp.py:194-210, :622-667; amp_agent.py:385) into amp_obs[:, t], by the AMP part's body layout."""
         s, amp = self.sim, self.amp
         prev = self.amp_obs[:, t - 1] if t > 0 else self.amp_obs[:, self.T - 1]
         out = self.amp_obs[:, t]
@@ -162,7 +167,7 @@ class LatentStepsB200(GraphRunner):
                             prev=prev.data_ptr(), ld_prev=prev.stride(0), out=out.data_ptr(), ld_out=out.stride(0), num_steps=amp.num_steps,
                             fresh=self.amp_fresh.data_ptr(), fresh_rows=self.amp_init.data_ptr(), amp_width=amp.amp_width,
                             remove_base_rot=int(not amp.upright))
-        self._launch("pulse_amp_obs_row", C.byref(a), self.n)
+        self._launch(_AMP_ROW[amp.layout], C.byref(a), self.n)
 
     def _amp_start(self) -> None:
         """The AMP history of the initial state, for `first_observation`: the current AMP row in every history row of every env

@@ -20,6 +20,7 @@ from . import _lib
 from .motion_lib import MotionLibB200
 
 AMP_WIDTHS = (196, 195)
+SMPLX_AMP_WIDTHS = (_lib.SMPLX_AMP_OBS, _lib.SMPLX_AMP_OBS_NO_HEIGHT)
 _POSE = {"reach": _lib.ZPOSE_ROOT_XY_ZERO, "strike": _lib.ZPOSE_ROOT_XY_ZERO, "speed": _lib.ZPOSE_FACE_X}
 _INIT = {"Random": _lib.ZINIT_RANDOM, "Start": _lib.ZINIT_START}
 
@@ -53,8 +54,8 @@ class ZTaskResetB200:
     196- or 195-float AMP rows (ampRootHeightObs, False in env_pulse_amp.yaml).
 
     A 52-body MotionLib (SMPL-X, PULSE-X) serves the speed task through `pulse_reset_ztask_smplx`: views of >= 52 bodies and 153 dofs,
-    `upright` False as in env_pulsex_amp.yaml (True is refused: the SMPL-X step takes the non-upright heading), no AMP history
-    (`amp_obs_buf`) and no discriminator."""
+    `upright` False as in env_pulsex_amp.yaml (True is refused: the SMPL-X step takes the non-upright heading), and the AMP history
+    in the SMPL-X rows: 466 floats, or 465 without the root height (`amp_root_height_obs`)."""
 
     def __init__(self, kind: str, motion_lib: MotionLibB200, floor: torch.Tensor, *, upright: bool = True, state_init: str = "Random",
                  amp_root_height_obs: bool = False, dt: float = float(torch.tensor(1.0 / 60.0, dtype=torch.float32) * 2),
@@ -80,7 +81,7 @@ class ZTaskResetB200:
             raise _lib.PulseError(f"floor table has {floor.shape[0]} frames, the MotionLib {motion_lib.gts.shape[0]}")
         self.floor = floor.contiguous()
         self.upright, self.state_init, self.dt = bool(upright), state_init, float(dt)
-        self.amp_width = 196 if amp_root_height_obs else 195
+        self.amp_width = (SMPLX_AMP_WIDTHS if self.smplx else AMP_WIDTHS)[0 if amp_root_height_obs else 1]
         self.strike = (float(near_prob), float(near_dist), float(tar_dist_min), float(tar_dist_max))
         self.reach = (float(reach_dist_max), float(tar_height_min), float(tar_height_max))
         self.speed = (float(tar_speed_min), float(tar_speed_max))
@@ -135,8 +136,6 @@ class ZTaskResetB200:
                 raise _lib.PulseError(f"{name} must be a {dtype} view on {dev} with {N} rows, {what}")
 
         B, D = self.bodies, self.dofs
-        if self.smplx and amp_obs_buf is not None:
-            raise _lib.PulseError("the SMPL-X reset has no AMP history back-fill (amp_obs_buf must be None)")
         view(rigid_body_state, "rigid_body_state", torch.float32, rigid_body_state.dim() == 3 and rigid_body_state.shape[1] >= B,
              rigid_body_state.stride(1) == 13 and rigid_body_state.stride(2) == 1, f"[N, B >= {B}, 13] with row stride 13")
         view(root_states, "root_states", torch.float32, root_states.dim() == 2 and root_states.shape[1] >= 13, root_states.stride(1) == 1,
@@ -182,7 +181,7 @@ class ZTaskResetB200:
         a.pose_mode, a.upright, a.state_init, a.dt = self.pose_mode, int(self.upright), self.init_code, self.dt
         if amp_obs_buf is not None:
             if not amp_obs_buf.is_contiguous() or amp_obs_buf.dim() != 3 or amp_obs_buf.shape[0] != N or amp_obs_buf.shape[-1] != self.amp_width:
-                raise _lib.PulseError(f"amp_obs_buf must be contiguous [N, steps, {self.amp_width}]")
+                raise _lib.PulseError(f"amp_obs_buf must be contiguous [N, steps, {self.amp_width}] (the reset's AMP rows)")
             if amp_obs_buf.dtype != torch.float32 or amp_obs_buf.device != dev:
                 raise _lib.PulseError(f"amp_obs_buf must be float32 on {dev}")
             a.amp_obs_buf, a.num_amp_steps, a.amp_width = amp_obs_buf.data_ptr(), int(amp_obs_buf.shape[1]), self.amp_width
@@ -276,17 +275,31 @@ _KEY_BODY_IDS = (7, 3, 22, 17)                                                  
 _DOF_SUBSET = tuple(k for k in range(69) if (k // 3) not in (3, 7, 17, 22))        # humanoid.py:397,417-421
 
 
+# SMPL-X (smplx_humanoid.yaml, env_pulsex_amp.yaml): R_Ankle, L_Ankle, R_Wrist, L_Wrist in SMPLH_MUJOCO_NAMES order, and the dofs of
+# joints 0..50 without L_Toe (3) and R_Toe (7) (humanoid.py:404-421): 147 of 153
+SMPLX_KEY_BODY_IDS = (7, 3, 36, 17)
+SMPLX_DOF_SUBSET = tuple(k for k in range(153) if (k // 3) not in (3, 7))
+
+
+def check_amp_layout(task, who: str, smplx: bool = False) -> None:
+    """Refuses, naming the option, a task whose AMP observation the device rows do not build: amp_obs_v other than 1, other key bodies
+    (_key_body_ids) or another dof_subset than the layout's (SMPL: `_KEY_BODY_IDS` / `_DOF_SUBSET`; SMPL-X: `SMPLX_KEY_BODY_IDS` /
+    `SMPLX_DOF_SUBSET`).  A PULSE-X integration calls it with smplx=True on its HumanoidSpeedZ task before wiring the AMP part."""
+    keys, subset, dropped = (SMPLX_KEY_BODY_IDS, SMPLX_DOF_SUBSET, "toes") if smplx else (_KEY_BODY_IDS, _DOF_SUBSET, "toes and hands")
+    if int(getattr(task, "amp_obs_v", 1)) != 1:
+        raise _lib.PulseError(f"{who}: amp_obs_v {task.amp_obs_v}, the device AMP rows are amp_obs_v 1")
+    if tuple(int(i) for i in task._key_body_ids.tolist()) != keys:
+        raise _lib.PulseError(f"{who}: keyBodies (_key_body_ids) other than R_Ankle, L_Ankle, R_Wrist, L_Wrist {keys}")
+    if not getattr(task, "_has_dof_subset", False) or tuple(int(i) for i in task.dof_subset.tolist()) != subset:
+        raise _lib.PulseError(f"{who}: a dof_subset (_has_dof_subset) other than the one without {dropped}")
+
+
 def smpl_reset_tables(task, ml, who: str):
     """The checks shared by the device resets' mixins and what they build once per MotionLib load: the task's MotionLib as a
     `MotionLibB200` and the floor table of its one body shape.  Refuses, naming the option, what the device reset does not serve."""
     if getattr(task, "humanoid_type", None) != "smpl":
         raise _lib.PulseError(f"{who}: humanoid_type {getattr(task, 'humanoid_type', None)!r}, the device reset serves 'smpl'")
-    if int(getattr(task, "amp_obs_v", 1)) != 1:
-        raise _lib.PulseError(f"{who}: amp_obs_v {task.amp_obs_v}, the device AMP rows are amp_obs_v 1")
-    if tuple(int(i) for i in task._key_body_ids.tolist()) != _KEY_BODY_IDS:
-        raise _lib.PulseError(f"{who}: keyBodies (_key_body_ids) other than R_Ankle, L_Ankle, R_Wrist, L_Wrist")
-    if not getattr(task, "_has_dof_subset", False) or tuple(int(i) for i in task.dof_subset.tolist()) != _DOF_SUBSET:
-        raise _lib.PulseError(f"{who}: a dof_subset (_has_dof_subset) other than the one without toes and hands")
+    check_amp_layout(task, who)
     shapes = task.humanoid_shapes
     if bool((shapes != shapes[0:1]).any()):              # once per MotionLib load: one host read
         raise _lib.PulseError(f"{who}: shape variation (humanoid_shapes rows differ); the floor table is per shape")

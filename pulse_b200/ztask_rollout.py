@@ -47,8 +47,6 @@ def check_pieces(task, reset, policy, vae, amp=None) -> str:
         raise _lib.PulseError("ZTaskStepsB200: a policy with a discriminator needs the AMP part (amp=AmpBuffersB200) and the AMP part a "
                               "discriminator")
     if amp is not None:
-        if layout == "smplx":
-            raise _lib.PulseError("ZTaskStepsB200: no AMP part (and no discriminator) for SMPL-X: there is no 52-body AMP layout")
         if amp.amp_width != reset.amp_width or amp.upright != reset.upright:
             raise _lib.PulseError(f"ZTaskStepsB200: the AMP part writes {amp.amp_width}-float rows (upright {amp.upright}), the reset "
                                   f"{reset.amp_width}-float rows (upright {reset.upright})")
@@ -77,8 +75,10 @@ class ZTaskStepsB200(LatentStepsB200):
     `reset` a ZTaskResetB200 over a 52-body MotionLib, `policy` PPOPolicy(obs_size=781, num_actions=48), `vae` PulseVAE(self_obs_size=778,
     num_actions=153, latent=48); the sim views hold >= 52 bodies and 153 dofs, and `dof_force` is refused (no power term).
 
-    `policy` may carry a discriminator exactly when `amp` is given (PPOPolicy(..., with_disc=True, amp_obs_size=10 * amp_width)); the
-    SMPL-X speed task takes neither (no 52-body AMP layout).
+    `policy` may carry a discriminator exactly when `amp` is given (PPOPolicy(..., with_disc=True, amp_obs_size=10 * amp_width)).  For
+    the SMPL-X speed task that is AmpBuffersB200(ml, amp_width=465, upright=False, ...) over the same 52-body MotionLib, a reset of
+    amp_root_height_obs False and PPOPolicy(obs_size=781, num_actions=48, units=(2048, 1024, 512), act="silu", with_disc=True,
+    amp_obs_size=4650).
 
     Out of scope: multi-GPU; the smplx humanoid's reach and strike tasks; Default / Hybrid state init; the power_usage_reward
     terms the step kernels exclude."""

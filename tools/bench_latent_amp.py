@@ -9,9 +9,16 @@ MotionLib and simulator state, no physics); the discriminator arm swaps in the s
 (1024-512 ReLU, disc_coef 5) and an AmpBuffersB200 of the learning configs' sizes (200 000-row rings, amp_batch_size 512,
 amp_minibatch_size 4096, keep probability 0.01), disc_reward_w 0.
 
+The smplx-speed task is the PULSE-X speed driver of tools/bench_smplx_speed.py (52 bodies, 48 latent dimensions) with 10 x 465-float
+AMP rows (env_pulsex_amp.yaml) and a 4650-wide discriminator input; for it a last line times `pulse_smplx_amp_obs_row` alone at
+--row-envs envs (device events around --row-reps back-to-back launches, median of 5 samples, one L2 flush before each) beside the bytes
+one env-step moves as computed from the shapes.
+
   python tools/bench_latent_amp.py --task speed --envs 1536 8192
   python tools/bench_latent_amp.py --task vr --envs 3072
+  python tools/bench_latent_amp.py --task smplx-speed --envs 1536 8192
 """
+import ctypes as C
 import argparse
 import json
 import os
@@ -23,6 +30,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from tools import bench_imz_rollout as bimz          # noqa: E402
+from tools import bench_smplx_speed as bsx           # noqa: E402
 from tools import bench_terrain_rollout as bter      # noqa: E402
 from tools import bench_ztask_rollout as bzt         # noqa: E402
 
@@ -41,6 +49,8 @@ def build(task, n, dev, use_graphs, disc, terrain=None):
         d0 = bter.build(n, dev, use_graphs, *terrain)
     elif task == "vr":
         d0 = bimz.build(n, dev, use_graphs)
+    elif task == "smplx-speed":
+        d0 = bsx.build(n, dev, use_graphs)
     else:
         d0 = bzt.build(task, n, dev, use_graphs)
     if not disc:
@@ -57,20 +67,62 @@ def build(task, n, dev, use_graphs, disc, terrain=None):
             pol = SeptPolicy(num_actions=32, with_disc=True, amp_obs_size=amp.row_floats, device=dev, seed=0)
             d = TerrainStepsB200(d0.task, d0.reset, pol, d0.vae, d0.sim, amp=amp, **kw)
         else:
-            pol = PPOPolicy(obs_size=d0.task.obs_size, num_actions=32, units=bzt.UNITS, act="silu", device=dev, seed=0, with_disc=True,
-                            amp_obs_size=amp.row_floats)
+            pol = PPOPolicy(obs_size=d0.task.obs_size, num_actions=bsx.LATENT if task == "smplx-speed" else 32, units=bzt.UNITS, act="silu",
+                            device=dev, seed=0, with_disc=True, amp_obs_size=amp.row_floats)
             d = ZTaskStepsB200(d0.task, d0.reset, pol, d0.vae, d0.sim, amp=amp, **kw)
     d.first_observation()
     return d
 
 
+def row_bytes(width=465, steps=10):
+    """Bytes one env-step of pulse_smplx_amp_obs_row moves, from the shapes: reads the (steps - 1) history rows, the root's 13 body floats,
+    the 4 key bodies' positions and the 49 kept joints' 147 dof positions and velocities; writes the steps x width row."""
+    rd = {"history": (steps - 1) * width * 4, "state": (13 + 4 * 3 + 2 * 147) * 4}
+    wr = {"row": steps * width * 4}
+    return rd, wr
+
+
+def time_row(n, reps, dev, flush):
+    """pulse_smplx_amp_obs_row alone: microseconds per launch (median of 5 samples of `reps` launches) and the shapes' bytes."""
+    from pulse_b200 import _lib
+    lib = _lib.load()
+    s = bsx.sim_state(n, dev, 7)
+    W = 465
+    prev, out = torch.randn(n, 10 * W, device=dev), torch.zeros(n, 10 * W, device=dev)
+    a = _lib.AmpRowArgs(body_state=s["body_state"].data_ptr(), body_env_stride=s["body_state"].stride(0), dof_pos=s["dof_pos"].data_ptr(),
+                        dof_vel=s["dof_vel"].data_ptr(), dof_env_stride=s["dof_pos"].stride(0), dof_elem_stride=s["dof_pos"].stride(1),
+                        prev=prev.data_ptr(), ld_prev=10 * W, out=out.data_ptr(), ld_out=10 * W, num_steps=10, amp_width=W, remove_base_rot=1)
+    st = _lib.current_stream(dev)
+    for _ in range(10):
+        _lib.check(lib.pulse_smplx_amp_obs_row(C.byref(a), n, st), "pulse_smplx_amp_obs_row")
+    times = []
+    for _ in range(5):
+        flush.zero_()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            _lib.check(lib.pulse_smplx_amp_obs_row(C.byref(a), n, st), "pulse_smplx_amp_obs_row")
+        e1.record()
+        torch.cuda.synchronize()
+        times.append(e0.elapsed_time(e1) * 1e3 / reps)
+    rd, wr = row_bytes(W)
+    per_env = sum(rd.values()) + sum(wr.values())
+    us = sorted(times)[len(times) // 2]
+    return {"workload": "pulse_smplx_amp_obs_row alone: %d envs, 10 x %d floats, %d back-to-back launches per sample, median of 5 samples"
+                        % (n, W, reps), "envs": n, "kernel_us": round(us, 2), "kernel_us_samples": [round(t, 2) for t in times],
+            "bytes_per_env_step": {"read": rd, "write": wr, "total": per_env}, "MB_per_launch": round(per_env * n / 1e6, 1),
+            "achieved_GB_per_s": round(per_env * n / (us * 1e-6) / 1e9, 1)}
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--task", choices=("reach", "speed", "strike", "terrain", "vr"), default="speed")
+    ap.add_argument("--task", choices=("reach", "speed", "strike", "terrain", "vr", "smplx-speed"), default="speed")
     ap.add_argument("--envs", type=int, nargs="+", default=[1536, 8192])
     ap.add_argument("--iters", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--amp-reps", type=int, default=10)
+    ap.add_argument("--row-envs", type=int, default=16384)
+    ap.add_argument("--row-reps", type=int, default=200)
     args = ap.parse_args()
     if args.iters < 3:
         raise SystemExit("at least three timed iterations")
@@ -126,6 +178,9 @@ def main():
                 del d
             out["disc" if disc else "no_disc"] = arms
         print(json.dumps(out), flush=True)
+    if args.task == "smplx-speed":
+        torch.cuda.empty_cache()
+        print(json.dumps(dict(time_row(args.row_envs, args.row_reps, dev, flush), gpu=info)), flush=True)
 
 
 if __name__ == "__main__":
