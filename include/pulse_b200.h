@@ -1010,6 +1010,41 @@ int pulse_smplx_speed_obs_list(const pulse_smplx_speed_step_args_t* args, const 
 /* progress_buf += 1, the step, dones[e] = float(reset_buf[e]), as pulse_ztask_rollout_step. */
 int pulse_smplx_speed_rollout_step(const pulse_smplx_speed_step_args_t* args, float* dones, int64_t num_envs, void* stream);
 
+/* Post-physics step of the SMPL-X reach and strike tasks (HumanoidReachZ / HumanoidStrikeZ with robot=smplx_humanoid): the self
+ * observation of pulse_smplx_speed_step (the heading of remove_base_rot(root_rot)), then the task observation in the heading of the
+ * RAW root rotation, the reward and the reset, as the SMPL steps compute them:
+ *   PULSE_ZTASK_REACH   compute_location_observations / compute_reach_reward (humanoid_reach.py:224-250), reward
+ *                       exp(-4 ||tar_pos - p[reach_body_id]||^2); compute_humanoid_reset (humanoid.py:1573-1608).  obs 778 + 3.
+ *   PULSE_ZTASK_STRIKE  compute_strike_observations / compute_strike_reward (humanoid_strike.py:270-328), the strike variant of
+ *                       compute_humanoid_reset (:330-375): also fails when the target is pushed (> 50 N in x or y) while a body in
+ *                       neither contact_body_mask nor strike_body_mask presses harder than 50 N, over all 52 bodies.  obs 778 + 15.
+ * Body sets are 64-bit masks (SMPL-X body ids go up to 51; bits 52..63 must be clear).  Neither task has a power term. */
+#define PULSE_SMPLX_REACH_OBS 781    /* 778 + compute_location_observations 3 */
+#define PULSE_SMPLX_STRIKE_OBS 793   /* 778 + compute_strike_observations 15  */
+typedef struct {
+  int32_t kind, enable_early_termination;                  /* PULSE_ZTASK_REACH or PULSE_ZTASK_STRIKE */
+  const float* body_state; int64_t body_env_stride;        /* [N, >=52, 13] pos quat(xyzw) linvel angvel */
+  const float* contact_forces; int64_t contact_env_stride; /* [N, >=52, 3] or NULL */
+  const float* termination_heights;                        /* [52] */
+  uint64_t contact_body_mask;                              /* bit j: body j may touch the ground (_contact_body_ids) */
+  uint64_t strike_body_mask;                               /* strike: bit j: body j may hit the target (_strike_body_ids) */
+  int32_t reach_body_id; int32_t reserved;                 /* reach: [0, 52) */
+  const int64_t* progress_buf; int64_t max_episode_length;
+  const float* tar_pos;                                    /* reach: [N, 3] */
+  const float* prev_root_pos; float dt; float reserved2;   /* strike: [N, 3] root position before the physics step */
+  const float* target_states; int64_t target_env_stride;   /* strike: [N, 13] view of the target actor's root state */
+  const float* tar_contact_forces; int64_t tar_contact_env_stride;   /* strike: [N, 3] view */
+  float* obs_buf; int64_t obs_stride;                      /* [N, >= 781 (reach) / 793 (strike)] */
+  float* rew_buf;                                          /* [N] */
+  int64_t* reset_buf; int64_t* terminate_buf;              /* [N] */
+} pulse_smplx_target_step_args_t;
+int pulse_smplx_target_step(const pulse_smplx_target_step_args_t* args, int64_t num_envs, void* stream);
+/* The observation rows of the envs env_list[0 .. *count), as pulse_ztask_obs_list. */
+int pulse_smplx_target_obs_list(const pulse_smplx_target_step_args_t* args, const int64_t* env_list, const int32_t* count, int64_t num_envs,
+                                void* stream);
+/* progress_buf += 1, the step, dones[e] = float(reset_buf[e]), as pulse_ztask_rollout_step. */
+int pulse_smplx_target_rollout_step(const pulse_smplx_target_step_args_t* args, float* dones, int64_t num_envs, void* stream);
+
 /* The reference-state reset of pulse_reset_ztask for the SMPL-X speed task, no host synchronisation: the compaction, then one warp per
  * (reset env, AMP history step k): clip and start-time draws, the 52-body gather, the SMPL ground fix from the per-frame floor table,
  * the FACE_X pose adjustment (HumanoidSpeed._sample_ref_state, humanoid_speed.py:251-270, heading of remove_base_rot(root_rot) when
@@ -1020,6 +1055,12 @@ int pulse_smplx_speed_rollout_step(const pulse_smplx_speed_step_args_t* args, fl
  * state outputs are those of the same call without it.  _reset_task follows through pulse_ztask_reset_task, the PD targets through
  * pulse_ztask_pre_physics (dofs 153). */
 int pulse_reset_ztask_smplx(const pulse_smplx_motionlib_t* lib, const pulse_ztask_reset_args_t* args, int64_t num_envs, void* stream);
+
+/* The reference-state reset of pulse_reset_ztask_smplx for the SMPL-X reach and strike tasks: the same launches and checks, with
+ * pose_mode PULSE_ZPOSE_ROOT_XY_ZERO (humanoid_reach.py:46-48, humanoid_strike.py:147-150; any other mode is refused).  target_states
+ * is NULL for reach and the [N, 13] target view for strike, which receives _reset_target (humanoid_strike.py:124-145) around the new
+ * root as in pulse_reset_ztask, with the same draws.  _reset_task of the reach task follows through pulse_ztask_reset_task. */
+int pulse_reset_smplx_target(const pulse_smplx_motionlib_t* lib, const pulse_ztask_reset_args_t* args, int64_t num_envs, void* stream);
 
 /* pulse_amp_obs_row for the SMPL-X humanoid: the AMP row [current W | first (steps-1)*W floats of the previous row] of every env from
  * [N, >= 52, 13] body views and [N, 153] dof views, W = amp_width PULSE_SMPLX_AMP_OBS or PULSE_SMPLX_AMP_OBS_NO_HEIGHT (0 is refused),

@@ -306,7 +306,19 @@ class SmplxSpeedStepArgs(C.Structure):
     ]
 
 
+class SmplxTargetStepArgs(C.Structure):
+    _fields_ = [
+        ("kind", C.c_int32), ("enable_early_termination", C.c_int32), ("body_state", C.c_void_p), ("body_env_stride", C.c_int64),
+        ("contact_forces", C.c_void_p), ("contact_env_stride", C.c_int64), ("termination_heights", C.c_void_p), ("contact_body_mask", C.c_uint64),
+        ("strike_body_mask", C.c_uint64), ("reach_body_id", C.c_int32), ("reserved", C.c_int32), ("progress_buf", C.c_void_p),
+        ("max_episode_length", C.c_int64), ("tar_pos", C.c_void_p), ("prev_root_pos", C.c_void_p), ("dt", C.c_float), ("reserved2", C.c_float),
+        ("target_states", C.c_void_p), ("target_env_stride", C.c_int64), ("tar_contact_forces", C.c_void_p), ("tar_contact_env_stride", C.c_int64),
+        ("obs_buf", C.c_void_p), ("obs_stride", C.c_int64), ("rew_buf", C.c_void_p), ("reset_buf", C.c_void_p), ("terminate_buf", C.c_void_p),
+    ]
+
+
 SMPLX_BODIES, SMPLX_DOF, SMPLX_SELF_OBS, SMPLX_SPEED_OBS = 52, 153, 778, 781
+SMPLX_REACH_OBS, SMPLX_STRIKE_OBS = 781, 793          # PULSE_SMPLX_REACH_OBS / PULSE_SMPLX_STRIKE_OBS: 778 + 3 / + 15
 SMPLX_AMP_OBS, SMPLX_AMP_OBS_NO_HEIGHT = 466, 465       # PULSE_SMPLX_AMP_OBS(_NO_HEIGHT): the SMPL-X AMP row, with / without root height
 
 
@@ -522,6 +534,10 @@ SIGNATURES = {
     "pulse_smplx_speed_obs_list": (C.c_int, [C.POINTER(SmplxSpeedStepArgs), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_smplx_speed_rollout_step": (C.c_int, [C.POINTER(SmplxSpeedStepArgs), C.c_void_p, C.c_int64, C.c_void_p]),
     "pulse_reset_ztask_smplx": (C.c_int, [C.c_void_p, C.POINTER(ZTaskResetArgs), C.c_int64, C.c_void_p]),
+    "pulse_smplx_target_step": (C.c_int, [C.POINTER(SmplxTargetStepArgs), C.c_int64, C.c_void_p]),
+    "pulse_smplx_target_obs_list": (C.c_int, [C.POINTER(SmplxTargetStepArgs), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "pulse_smplx_target_rollout_step": (C.c_int, [C.POINTER(SmplxTargetStepArgs), C.c_void_p, C.c_int64, C.c_void_p]),
+    "pulse_reset_smplx_target": (C.c_int, [C.c_void_p, C.POINTER(ZTaskResetArgs), C.c_int64, C.c_void_p]),
     "pulse_smplx_amp_obs_row": (C.c_int, [C.POINTER(AmpRowArgs), C.c_int64, C.c_void_p]),
     "pulse_amp_demo_fetch": (C.c_int, [C.c_void_p, C.POINTER(AmpDemoArgs), C.c_void_p]),
     "pulse_smplx_amp_demo_fetch": (C.c_int, [C.c_void_p, C.POINTER(AmpDemoArgs), C.c_void_p]),

@@ -19,14 +19,16 @@ __constant__ int c_smplx_key_body[4] = {7, 3, 36, 17};
 // The body layouts the latent-task step, reset and AMP code is instantiated for.  B bodies give a MotionLib frame record
 // pos 3B | rot 4B | vel 3B | angvel 3B, an aux record lrs 4B | dvs 3(B - 1) | pad, and a self observation of 1 + 3(B - 1) + 6B + 3B + 3B
 // floats.  kUpright: the step's self observation takes the heading of the root rotation itself (has_upright_start), otherwise
-// of remove_base_rot(root).  kSmplTerms: the task terms only the SMPL path serves (strike, the power term).  The AMP observation
+// of remove_base_rot(root).  kTasks: bit k set when the step serves task kind k (PULSE_ZTASK_*) through StepArgs.kind, or through
+// the layout alone when it serves one kind; kPower: the speed task's power term.  The AMP observation
 // (build_amp_observations_smpl with dof_subset) keeps kAmpJoints joints, kept_joint(i) for i < kAmpJoints, and the four key bodies
 // key_body(i): kAmpObs = 1 + 6 + 3 + 3 + 9 kAmpJoints + 12 floats with the root height.
 struct SmplLayout {
   static constexpr int kBodies = PULSE_NUM_BODIES, kDofs = PULSE_NUM_DOF, kSelfObs = PULSE_SELF_OBS;
   static constexpr int kFrameRec = PULSE_FRAME_REC, kAuxRec = PULSE_AUX_REC;
   static constexpr int kAmpJoints = 19, kAmpObs = PULSE_AMP_OBS;
-  static constexpr bool kUpright = true, kSmplTerms = true;
+  static constexpr bool kUpright = true, kPower = true;
+  static constexpr unsigned kTasks = (1u << PULSE_ZTASK_SPEED) | (1u << PULSE_ZTASK_STRIKE);
   using StepArgs = pulse_ztask_step_args_t;
   __device__ static __forceinline__ int kept_joint(int i) { return c_kept_joint[i]; }
   __device__ static __forceinline__ int key_body(int i) { return c_key_body[i]; }
@@ -35,10 +37,16 @@ struct SmplxLayout {
   static constexpr int kBodies = PULSE_SMPLX_BODIES, kDofs = PULSE_SMPLX_DOF, kSelfObs = PULSE_SMPLX_SELF_OBS;
   static constexpr int kFrameRec = PULSE_SMPLX_FRAME_REC, kAuxRec = PULSE_SMPLX_AUX_REC;
   static constexpr int kAmpJoints = 49, kAmpObs = PULSE_SMPLX_AMP_OBS;
-  static constexpr bool kUpright = false, kSmplTerms = false;
+  static constexpr bool kUpright = false, kPower = false;
+  static constexpr unsigned kTasks = 1u << PULSE_ZTASK_SPEED;
   using StepArgs = pulse_smplx_speed_step_args_t;
   __device__ static __forceinline__ int kept_joint(int i) { return c_smplx_kept_joint[i]; }
   __device__ static __forceinline__ int key_body(int i) { return c_smplx_key_body[i]; }
+};
+// The SMPL-X reach and strike steps: SmplxLayout's geometry with their own argument struct.
+struct SmplxTargetLayout : SmplxLayout {
+  static constexpr unsigned kTasks = (1u << PULSE_ZTASK_REACH) | (1u << PULSE_ZTASK_STRIKE);
+  using StepArgs = pulse_smplx_target_step_args_t;
 };
 static_assert(13 + 9 * SmplLayout::kAmpJoints + 12 == PULSE_AMP_OBS, "SMPL AMP observation");
 static_assert(13 + 9 * SmplxLayout::kAmpJoints + 12 == PULSE_SMPLX_AMP_OBS, "SMPL-X AMP observation");

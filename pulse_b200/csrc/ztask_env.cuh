@@ -1,4 +1,5 @@
-// One env of the latent-space tasks' post-physics step (reach; speed / strike; the SMPL-X speed task), one warp per env, lane = body:
+// One env of the latent-space tasks' post-physics step (reach; speed / strike; the SMPL-X speed, reach and strike tasks), one warp per
+// env, lane = body:
 // self observation, task observation, reward and reset.  Shared by the step and list-observation kernels (ztask_step.cu) and by the rollout step kernels that
 // write into experience-buffer slices (ztask_rollout.cu), so all of them produce the same rows bit for bit.
 #pragma once
@@ -54,12 +55,16 @@ __device__ __forceinline__ void reach_env(const pulse_reach_step_args_t& a, long
   }
 }
 
-// One env of the speed / strike step in body layout L (SmplLayout: speed and strike; SmplxLayout: speed).  kObsOnly: the observation
-// alone.  Lane l holds bodies l and l + 32 (the second only where the layout has more than 32 bodies).
-template <class L>
-__device__ __forceinline__ bool ztask_is_speed(const typename L::StepArgs& a) {
-  if constexpr (L::kSmplTerms) return a.kind == PULSE_ZTASK_SPEED;
-  else return true;
+// One env of the speed / strike step in body layout L (SmplLayout: speed and strike; SmplxLayout: speed; SmplxTargetLayout: reach and
+// strike).  kObsOnly: the observation alone.  Lane l holds bodies l and l + 32 (the second only where the layout has more than 32 bodies).
+// ztask_is<L, K>: whether env work takes task kind K's branch -- a constant where the layout serves K alone or not at all.
+template <class L, int K>
+constexpr bool kServes = (L::kTasks >> K) & 1u;
+template <class L, int K>
+__device__ __forceinline__ bool ztask_is(const typename L::StepArgs& a) {
+  if constexpr (!kServes<L, K>) return false;
+  else if constexpr (L::kTasks == (1u << K)) return true;
+  else return a.kind == K;
 }
 
 template <class L, bool kObsOnly>
@@ -99,7 +104,7 @@ __device__ __forceinline__ void ztask_env(const typename L::StepArgs& a, long lo
     const FallFlags fall = fall_flags(a, e, j, body, p[s].z);
     contact = contact || fall.contact;
     height = height || fall.height;
-    if constexpr (L::kSmplTerms) {
+    if constexpr (kServes<L, PULSE_ZTASK_STRIKE>) {
       // strike: a body that is neither a ground-contact body nor a strike body pressing harder than 50 N (humanoid_strike.py:356-364)
       if (a.enable_early_termination && body && a.contact_forces != nullptr && !(((a.contact_body_mask | a.strike_body_mask) >> j) & 1u)) {
         const float* cf = a.contact_forces + e * a.contact_env_stride + j * 3;
@@ -110,35 +115,62 @@ __device__ __forceinline__ void ztask_env(const typename L::StepArgs& a, long lo
   const bool any_contact = __any_sync(kFull, contact), any_height = __any_sync(kFull, height);
   bool any_hard = false;
   float power = 0.0f;
-  if constexpr (L::kSmplTerms) {
-    any_hard = __any_sync(kFull, hard_contact);
+  if constexpr (kServes<L, PULSE_ZTASK_STRIKE>) any_hard = __any_sync(kFull, hard_contact);
+  if constexpr (L::kPower) {
     // power term of the speed task: -c * sum |tau * qdot|, zero for progress <= 3 (humanoid_speed.py:215-222)
     power = a.kind == PULSE_ZTASK_SPEED && a.dof_force != nullptr ? dof_power(a, e, lane) : 0.0f;
   }
+  // reach: the reach body's position, broadcast from its slot and lane (a shuffle every lane takes part in)
+  Vec3 p_reach = {0.0f, 0.0f, 0.0f};
+  if constexpr (kServes<L, PULSE_ZTASK_REACH> && !kObsOnly) {
+    if (ztask_is<L, PULSE_ZTASK_REACH>(a)) {
+      const int rs = a.reach_body_id >> 5, rl = a.reach_body_id & 31;
+      Vec3 src = p[0];
+#pragma unroll
+      for (int s = 1; s < kSlots; ++s)
+        if (s == rs) src = p[s];
+      p_reach = {__shfl_sync(kFull, src.x, rl), __shfl_sync(kFull, src.y, rl), __shfl_sync(kFull, src.z, rl)};
+    }
+  }
   if (lane == 0) {
     const long long prog = a.progress_buf[e];
-    const float* pr = a.prev_root_pos + 3 * e;
-    const float vx = (p_root.x - pr[0]) / a.dt, vy = (p_root.y - pr[1]) / a.dt;   // root_vel = delta_root_pos / dt
+    float vx = 0.0f, vy = 0.0f;
+    if (!ztask_is<L, PULSE_ZTASK_REACH>(a)) {   // the reach task has no prev_root_pos
+      const float* pr = a.prev_root_pos + 3 * e;
+      vx = (p_root.x - pr[0]) / a.dt;                                              // root_vel = delta_root_pos / dt
+      vy = (p_root.y - pr[1]) / a.dt;
+    }
     float* t = o + L::kSelfObs;
     bool failed = any_contact && any_height;
-    if (ztask_is_speed<L>(a)) {
-      // observation: heading-frame x axis (first two components) and the target speed (:310-325)
-      const Vec3 d = yaw_rot(yr, Vec3{1.0f, 0.0f, 0.0f});
-      const float ts = a.tar_speed[e];
-      t[0] = d.x; t[1] = d.y; t[2] = ts;
-      if constexpr (kObsOnly) return;
-      const float err = ts - vx;
-      float rew = expf(-0.25f * (err * err + 0.1f * vy * vy));                    // :327-343
-      if (a.reward_raw != nullptr) a.reward_raw[e * a.raw_stride] = rew;
-      if constexpr (L::kSmplTerms) {
-        if (a.dof_force != nullptr) {
-          const float pw = prog <= 3 ? 0.0f : -a.power_coefficient * power;
-          rew += pw;
-          if (a.reward_raw != nullptr) a.reward_raw[e * a.raw_stride + 1] = pw;
+    if (ztask_is<L, PULSE_ZTASK_SPEED>(a)) {
+      if constexpr (kServes<L, PULSE_ZTASK_SPEED>) {
+        // observation: heading-frame x axis (first two components) and the target speed (:310-325)
+        const Vec3 d = yaw_rot(yr, Vec3{1.0f, 0.0f, 0.0f});
+        const float ts = a.tar_speed[e];
+        t[0] = d.x; t[1] = d.y; t[2] = ts;
+        if constexpr (kObsOnly) return;
+        const float err = ts - vx;
+        float rew = expf(-0.25f * (err * err + 0.1f * vy * vy));                    // :327-343
+        if (a.reward_raw != nullptr) a.reward_raw[e * a.raw_stride] = rew;
+        if constexpr (L::kPower) {
+          if (a.dof_force != nullptr) {
+            const float pw = prog <= 3 ? 0.0f : -a.power_coefficient * power;
+            rew += pw;
+            if (a.reward_raw != nullptr) a.reward_raw[e * a.raw_stride + 1] = pw;
+          }
         }
+        a.rew_buf[e] = rew;
       }
-      a.rew_buf[e] = rew;
-    } else if constexpr (L::kSmplTerms) {
+    } else if (ztask_is<L, PULSE_ZTASK_REACH>(a)) {
+      if constexpr (kServes<L, PULSE_ZTASK_REACH>) {
+        const Vec3 tar = {a.tar_pos[3 * e], a.tar_pos[3 * e + 1], a.tar_pos[3 * e + 2]};
+        const Vec3 lt = yaw_rot(yr, tar - p_root);  // compute_location_observations (humanoid_reach.py:224-236)
+        t[0] = lt.x; t[1] = lt.y; t[2] = lt.z;
+        if constexpr (kObsOnly) return;
+        const Vec3 d = tar - p_reach;               // compute_reach_reward (:238-250)
+        a.rew_buf[e] = expf(-4.0f * (d.x * d.x + d.y * d.y + d.z * d.z));
+      }
+    } else if constexpr (kServes<L, PULSE_ZTASK_STRIKE>) {
       const float* ts = a.target_states + e * a.target_env_stride;
       const Vec3 tp = {ts[0], ts[1], ts[2]};
       const Quat tq = {ts[3], ts[4], ts[5], ts[6]};

@@ -6,7 +6,8 @@
 //                         target;
 //   ztask_task_kernel     (pulse_ztask_reset_task) the reach / speed _reset_task over the same list, after the observation.
 // pulse_reset_ztask_smplx runs the first two for the SMPL-X speed task: ztask_reset_kernel<SmplxLayout>, with the 465- / 466-float AMP
-// rows and without a strike target.
+// rows and without a strike target; pulse_reset_smplx_target runs the same kernel for the SMPL-X reach and strike tasks (root xy zeroed,
+// the strike target placed around it).
 // The entry points, argument structs and Philox word layout are documented in include/pulse_b200.h.
 #include "reset_warps.cuh"
 
@@ -136,33 +137,33 @@ extern "C" int pulse_ztask_reset_task(const pulse_ztask_task_args_t* args, int64
   return PULSE_OK;
 }
 
-extern "C" int pulse_reset_ztask_smplx(const pulse_smplx_motionlib_t* lib, const pulse_ztask_reset_args_t* args, int64_t num_envs, void* stream) {
-  using namespace pulse;
-  PULSE_REQUIRE(lib != nullptr && args != nullptr, "pulse_reset_ztask_smplx: null lib/args");
+namespace pulse {
+namespace {
+// The checks pulse_reset_ztask_smplx and pulse_reset_smplx_target share (`who` prefixes the messages), then their two launches.
+int reset_smplx(const pulse_smplx_motionlib_t* lib, const pulse_ztask_reset_args_t* args, int64_t num_envs, void* stream, const char* who) {
+  PULSE_REQUIRE(lib != nullptr && args != nullptr, "%s: null lib/args", who);
   const pulse_ztask_reset_args_t& a = *args;
-  PULSE_REQUIRE(num_envs >= 0 && num_envs < (1ll << 31), "pulse_reset_ztask_smplx: num_envs %lld outside [0, 2^31)", (long long)num_envs);
-  PULSE_REQUIRE(a.reset_buf != nullptr || a.env_ids_in != nullptr, "pulse_reset_ztask_smplx: neither a reset mask nor an env id list");
-  PULSE_REQUIRE(a.env_ids_in == nullptr || (a.num_ids >= 0 && a.num_ids <= num_envs), "pulse_reset_ztask_smplx: num_ids %lld outside [0, %lld]",
+  PULSE_REQUIRE(num_envs >= 0 && num_envs < (1ll << 31), "%s: num_envs %lld outside [0, 2^31)", who, (long long)num_envs);
+  PULSE_REQUIRE(a.reset_buf != nullptr || a.env_ids_in != nullptr, "%s: neither a reset mask nor an env id list", who);
+  PULSE_REQUIRE(a.env_ids_in == nullptr || (a.num_ids >= 0 && a.num_ids <= num_envs), "%s: num_ids %lld outside [0, %lld]", who,
                 (long long)a.num_ids, (long long)num_envs);
-  PULSE_REQUIRE(a.env_list != nullptr && a.count != nullptr, "pulse_reset_ztask_smplx: env_list / count outputs are required");
-  PULSE_REQUIRE(a.sampled_motion_ids && a.motion_start_times && a.progress_buf, "pulse_reset_ztask_smplx: null task buffer");
-  PULSE_REQUIRE(a.root_states && a.dof_pos && a.dof_vel && a.rigid_body_state, "pulse_reset_ztask_smplx: null simulator tensor");
+  PULSE_REQUIRE(a.env_list != nullptr && a.count != nullptr, "%s: env_list / count outputs are required", who);
+  PULSE_REQUIRE(a.sampled_motion_ids && a.motion_start_times && a.progress_buf, "%s: null task buffer", who);
+  PULSE_REQUIRE(a.root_states && a.dof_pos && a.dof_vel && a.rigid_body_state, "%s: null simulator tensor", who);
   PULSE_REQUIRE(a.root_env_stride >= PULSE_BODY_STATE_W && a.dof_elem_stride >= 1 && a.dof_env_stride >= PULSE_SMPLX_DOF * a.dof_elem_stride &&
-                a.body_env_stride >= PULSE_SMPLX_BODIES * PULSE_BODY_STATE_W, "pulse_reset_ztask_smplx: bad root / dof / rigid-body strides");
+                a.body_env_stride >= PULSE_SMPLX_BODIES * PULSE_BODY_STATE_W, "%s: bad root / dof / rigid-body strides", who);
   PULSE_REQUIRE(a.contact_forces == nullptr || (a.contact_bodies >= 0 && a.contact_env_stride >= 3 * a.contact_bodies),
-                "pulse_reset_ztask_smplx: bad contact-force strides");
+                "%s: bad contact-force strides", who);
   PULSE_REQUIRE(a.amp_obs_buf == nullptr || (a.num_amp_steps >= 1 && a.num_amp_steps <= 16),
-                "pulse_reset_ztask_smplx: the AMP history back-fill takes num_amp_steps in [1,16], not %d", a.num_amp_steps);
+                "%s: the AMP history back-fill takes num_amp_steps in [1,16], not %d", who, a.num_amp_steps);
   PULSE_REQUIRE(a.amp_obs_buf == nullptr || a.amp_width == PULSE_SMPLX_AMP_OBS || a.amp_width == PULSE_SMPLX_AMP_OBS_NO_HEIGHT,
-                "pulse_reset_ztask_smplx: AMP amp_width %d is neither %d nor %d (the SMPL-X rows)", a.amp_width, PULSE_SMPLX_AMP_OBS,
+                "%s: AMP amp_width %d is neither %d nor %d (the SMPL-X rows)", who, a.amp_width, PULSE_SMPLX_AMP_OBS,
                 PULSE_SMPLX_AMP_OBS_NO_HEIGHT);
-  PULSE_REQUIRE(a.amp_fresh == nullptr || a.amp_obs_buf != nullptr, "pulse_reset_ztask_smplx: amp_fresh flags need the back-filled AMP amp_obs_buf");
-  PULSE_REQUIRE(a.target_states == nullptr, "pulse_reset_ztask_smplx: the SMPL-X reset serves the speed task (target_states must be NULL)");
-  PULSE_REQUIRE(a.pose_mode == PULSE_ZPOSE_FACE_X, "pulse_reset_ztask_smplx: pose_mode %d, the speed task's is PULSE_ZPOSE_FACE_X", a.pose_mode);
-  PULSE_REQUIRE(a.floor != nullptr && a.floor_len >= lib->d.total_frames, "pulse_reset_ztask_smplx: floor table of %lld frames, the MotionLib has %lld",
+  PULSE_REQUIRE(a.amp_fresh == nullptr || a.amp_obs_buf != nullptr, "%s: amp_fresh flags need the back-filled AMP amp_obs_buf", who);
+  PULSE_REQUIRE(a.floor != nullptr && a.floor_len >= lib->d.total_frames, "%s: floor table of %lld frames, the MotionLib has %lld", who,
                 (long long)a.floor_len, (long long)lib->d.total_frames);
-  PULSE_REQUIRE(a.motion_ids_in != nullptr || a.sampling_cdf != nullptr, "pulse_reset_ztask_smplx: null sampling_cdf (needed to draw the clips)");
-  PULSE_REQUIRE(a.state_init == PULSE_ZINIT_RANDOM || a.state_init == PULSE_ZINIT_START, "pulse_reset_ztask_smplx: unknown state_init %d", a.state_init);
+  PULSE_REQUIRE(a.motion_ids_in != nullptr || a.sampling_cdf != nullptr, "%s: null sampling_cdf (needed to draw the clips)", who);
+  PULSE_REQUIRE(a.state_init == PULSE_ZINIT_RANDOM || a.state_init == PULSE_ZINIT_START, "%s: unknown state_init %d", who, a.state_init);
   if (num_envs == 0) return PULSE_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   reset_compact_kernel<<<1, kCompactThreads, 0, st>>>(a, (long long)num_envs);
@@ -171,4 +172,25 @@ extern "C" int pulse_reset_ztask_smplx(const pulse_smplx_motionlib_t* lib, const
   ztask_reset_kernel<SmplxLayout><<<grid_for(upper, kResetWarps), kResetWarps * 32, 0, st>>>(lib->d, a);
   PULSE_LAUNCH_OK("ztask_reset_kernel<SmplxLayout>");
   return PULSE_OK;
+}
+}  // namespace
+}  // namespace pulse
+
+extern "C" int pulse_reset_ztask_smplx(const pulse_smplx_motionlib_t* lib, const pulse_ztask_reset_args_t* args, int64_t num_envs, void* stream) {
+  using namespace pulse;
+  PULSE_REQUIRE(args != nullptr, "pulse_reset_ztask_smplx: null lib/args");
+  PULSE_REQUIRE(args->target_states == nullptr, "pulse_reset_ztask_smplx: the SMPL-X reset serves the speed task (target_states must be NULL)");
+  PULSE_REQUIRE(args->pose_mode == PULSE_ZPOSE_FACE_X, "pulse_reset_ztask_smplx: pose_mode %d, the speed task's is PULSE_ZPOSE_FACE_X",
+                args->pose_mode);
+  return reset_smplx(lib, args, num_envs, stream, "pulse_reset_ztask_smplx");
+}
+
+extern "C" int pulse_reset_smplx_target(const pulse_smplx_motionlib_t* lib, const pulse_ztask_reset_args_t* args, int64_t num_envs, void* stream) {
+  using namespace pulse;
+  PULSE_REQUIRE(args != nullptr, "pulse_reset_smplx_target: null lib/args");
+  PULSE_REQUIRE(args->pose_mode == PULSE_ZPOSE_ROOT_XY_ZERO, "pulse_reset_smplx_target: pose_mode %d, the reach and strike tasks' is "
+                "PULSE_ZPOSE_ROOT_XY_ZERO", args->pose_mode);
+  PULSE_REQUIRE(args->target_states == nullptr || args->target_env_stride >= PULSE_BODY_STATE_W,
+                "pulse_reset_smplx_target: bad target_states stride");
+  return reset_smplx(lib, args, num_envs, stream, "pulse_reset_smplx_target");
 }

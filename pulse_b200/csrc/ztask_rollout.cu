@@ -6,7 +6,8 @@
 //                             made here (Philox index plane e + 3 * 2^32);
 //   reach_rollout_kernel /    progress_buf += 1, then the per-env step code of ztask_env.cuh into the next step's observation slice and
 //   ztask_rollout_kernel      the step's reward row, then dones = float(reset); ztask_rollout_kernel<SmplxLayout> is the SMPL-X
-//                             speed task's (pulse_smplx_speed_rollout_step).
+//                             speed task's (pulse_smplx_speed_rollout_step), ztask_rollout_kernel<SmplxTargetLayout> the SMPL-X
+//                             reach and strike tasks' (pulse_smplx_target_rollout_step).
 // The entry points, argument structs and the Philox word layout are documented in include/pulse_b200.h.
 #include <cuda_bf16.h>
 
@@ -212,5 +213,20 @@ extern "C" int pulse_smplx_speed_rollout_step(const pulse_smplx_speed_step_args_
   PULSE_REQUIRE(num_envs > 0, "pulse_smplx_speed_rollout_step: num_envs must be positive");
   ztask_rollout_kernel<SmplxLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(*args, dones, (long long)num_envs);
   PULSE_LAUNCH_OK("ztask_rollout_kernel<SmplxLayout>");
+  return PULSE_OK;
+}
+
+namespace pulse {
+int check_smplx_target_args(const pulse_smplx_target_step_args_t* args, bool step, const char* who);   // ztask_step.cu
+}  // namespace pulse
+
+extern "C" int pulse_smplx_target_rollout_step(const pulse_smplx_target_step_args_t* args, float* dones, int64_t num_envs, void* stream) {
+  using namespace pulse;
+  const int st = check_smplx_target_args(args, true, "pulse_smplx_target_rollout_step");
+  if (st != PULSE_OK) return st;
+  PULSE_REQUIRE(dones != nullptr, "pulse_smplx_target_rollout_step: null dones");
+  PULSE_REQUIRE(num_envs > 0, "pulse_smplx_target_rollout_step: num_envs must be positive");
+  ztask_rollout_kernel<SmplxTargetLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(*args, dones, (long long)num_envs);
+  PULSE_LAUNCH_OK("ztask_rollout_kernel<SmplxTargetLayout>");
   return PULSE_OK;
 }

@@ -8,6 +8,8 @@
 //           reset = the strike variant of compute_humanoid_reset  :330-375
 //   smplx speed  the speed step above for the 52-body SMPL-X humanoid (env_pulsex_amp.yaml): the same per-env code instantiated for
 //           SmplxLayout, the self observation in the heading of remove_base_rot(root) (has_upright_start False)
+//   smplx reach / strike  the reach and strike steps above for the same humanoid (pulse_smplx_target_step): the per-env code
+//           instantiated for SmplxTargetLayout, the reach body broadcast from its slot (body id / 32) and lane (body id % 32)
 // The per-env device code is ztask_env.cuh's, shared with the rollout step kernels of ztask_rollout.cu.
 #include "ztask_env.cuh"
 
@@ -180,5 +182,63 @@ extern "C" int pulse_smplx_speed_obs_list(const pulse_smplx_speed_step_args_t* a
   ztask_obs_list_kernel<SmplxLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       *args, reinterpret_cast<const long long*>(env_list), count);
   PULSE_LAUNCH_OK("ztask_obs_list_kernel<SmplxLayout>");
+  return PULSE_OK;
+}
+
+namespace pulse {
+// The checks of the SMPL-X reach / strike step's arguments shared by its three entry points (`who` prefixes the messages).
+int check_smplx_target_args(const pulse_smplx_target_step_args_t* args, bool step, const char* who) {
+  PULSE_REQUIRE(args != nullptr, "%s: null args", who);
+  const pulse_smplx_target_step_args_t& a = *args;
+  PULSE_REQUIRE(a.kind == PULSE_ZTASK_REACH || a.kind == PULSE_ZTASK_STRIKE, "%s: task kind %d, this step serves PULSE_ZTASK_REACH and "
+                "PULSE_ZTASK_STRIKE", who, a.kind);
+  const bool reach = a.kind == PULSE_ZTASK_REACH;
+  PULSE_REQUIRE(a.body_state && a.obs_buf, "%s: null body_state / obs_buf", who);
+  PULSE_REQUIRE(a.body_env_stride >= PULSE_SMPLX_BODIES * PULSE_BODY_STATE_W, "%s: body_env_stride %lld < %d", who,
+                (long long)a.body_env_stride, PULSE_SMPLX_BODIES * PULSE_BODY_STATE_W);
+  const int width = reach ? PULSE_SMPLX_REACH_OBS : PULSE_SMPLX_STRIKE_OBS;
+  PULSE_REQUIRE(a.obs_stride >= width, "%s: obs_stride %lld < %d", who, (long long)a.obs_stride, width);
+  PULSE_REQUIRE(!reach || a.tar_pos != nullptr, "%s: the reach task needs tar_pos", who);
+  PULSE_REQUIRE(reach || (a.target_states != nullptr && a.target_env_stride >= PULSE_BODY_STATE_W), "%s: the strike task needs "
+                "target_states with target_env_stride >= 13", who);
+  if (!step) return PULSE_OK;
+  PULSE_REQUIRE(a.progress_buf && a.rew_buf && a.reset_buf && a.terminate_buf, "%s: null buffer", who);
+  PULSE_REQUIRE(!a.enable_early_termination || a.termination_heights != nullptr, "%s: termination_heights required", who);
+  PULSE_REQUIRE(a.contact_forces == nullptr || a.contact_env_stride >= PULSE_SMPLX_BODIES * 3, "%s: contact_env_stride %lld < %d", who,
+                (long long)a.contact_env_stride, PULSE_SMPLX_BODIES * 3);
+  PULSE_REQUIRE(((a.contact_body_mask | a.strike_body_mask) >> PULSE_SMPLX_BODIES) == 0, "%s: contact_body_mask / strike_body_mask "
+                "set bits at or above %d", who, PULSE_SMPLX_BODIES);
+  if (reach) {
+    PULSE_REQUIRE(a.reach_body_id >= 0 && a.reach_body_id < PULSE_SMPLX_BODIES, "%s: reach_body_id %d outside [0, %d)", who, a.reach_body_id,
+                  PULSE_SMPLX_BODIES);
+  } else {
+    PULSE_REQUIRE(a.tar_contact_forces != nullptr, "%s: the strike task needs tar_contact_forces", who);
+    PULSE_REQUIRE(a.prev_root_pos != nullptr, "%s: the strike task needs prev_root_pos", who);
+    PULSE_REQUIRE(a.dt > 0.0f, "%s: dt must be positive", who);
+  }
+  return PULSE_OK;
+}
+}  // namespace pulse
+
+extern "C" int pulse_smplx_target_step(const pulse_smplx_target_step_args_t* args, int64_t num_envs, void* stream) {
+  using namespace pulse;
+  const int st = check_smplx_target_args(args, true, "pulse_smplx_target_step");
+  if (st != PULSE_OK) return st;
+  PULSE_REQUIRE(num_envs > 0, "pulse_smplx_target_step: num_envs must be positive");
+  ztask_step_kernel<SmplxTargetLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(*args, (long long)num_envs);
+  PULSE_LAUNCH_OK("ztask_step_kernel<SmplxTargetLayout>");
+  return PULSE_OK;
+}
+
+extern "C" int pulse_smplx_target_obs_list(const pulse_smplx_target_step_args_t* args, const int64_t* env_list, const int32_t* count,
+                                           int64_t num_envs, void* stream) {
+  using namespace pulse;
+  const int st = check_smplx_target_args(args, false, "pulse_smplx_target_obs_list");
+  if (st != PULSE_OK) return st;
+  PULSE_REQUIRE(env_list && count && num_envs >= 0, "pulse_smplx_target_obs_list: null env_list / count or negative num_envs");
+  if (num_envs == 0) return PULSE_OK;
+  ztask_obs_list_kernel<SmplxTargetLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      *args, reinterpret_cast<const long long*>(env_list), count);
+  PULSE_LAUNCH_OK("ztask_obs_list_kernel<SmplxTargetLayout>");
   return PULSE_OK;
 }

@@ -55,7 +55,10 @@ class ZTaskResetB200:
 
     A 52-body MotionLib (SMPL-X, PULSE-X) serves the speed task through `pulse_reset_ztask_smplx`: views of >= 52 bodies and 153 dofs,
     `upright` False as in env_pulsex_amp.yaml (True is refused: the SMPL-X step takes the non-upright heading), and the AMP history
-    in the SMPL-X rows: 466 floats, or 465 without the root height (`amp_root_height_obs`)."""
+    in the SMPL-X rows: 466 floats, or 465 without the root height (`amp_root_height_obs`).  SMPL-X reach and strike go through the
+    subclass SmplxTargetResetB200."""
+    # the tasks a 52-body MotionLib serves here, and their entry point (SmplxTargetResetB200 sets both)
+    smplx_kinds, smplx_entry = ("speed",), "pulse_reset_ztask_smplx"
 
     def __init__(self, kind: str, motion_lib: MotionLibB200, floor: torch.Tensor, *, upright: bool = True, state_init: str = "Random",
                  amp_root_height_obs: bool = False, dt: float = float(torch.tensor(1.0 / 60.0, dtype=torch.float32) * 2),
@@ -68,8 +71,8 @@ class ZTaskResetB200:
             raise _lib.PulseError(f"state_init {state_init!r}: the device reset serves Random and Start")
         self.kind, self.motion_lib, self.device = kind, motion_lib, motion_lib._device
         self.smplx = bool(getattr(motion_lib, "smplx", False))
-        if self.smplx and kind != "speed":
-            raise _lib.PulseError(f"the SMPL-X reset serves the speed task, not {kind!r}")
+        if self.smplx and kind not in self.smplx_kinds:
+            raise _lib.PulseError(f"the SMPL-X {type(self).__name__} serves {' and '.join(self.smplx_kinds)}, not {kind!r}")
         if self.smplx and upright:
             raise _lib.PulseError("the SMPL-X reset takes upright=False (env_pulsex_amp.yaml: has_upright_start False), the heading its "
                                   "step kernel uses")
@@ -117,7 +120,7 @@ class ZTaskResetB200:
                            terminate_buf=terminate_buf, contact_forces=contact_forces, amp_obs_buf=amp_obs_buf, actor_ids=actor_ids,
                            target_states=target_states, tar_actor_ids=tar_actor_ids, motion_ids=motion_ids, motion_u=motion_u, phase=phase,
                            strike_u=strike_u, seed=seed, offset=offset, offset_dev=offset_dev, amp_fresh=amp_fresh)
-        fn, handle = ("pulse_reset_ztask_smplx", self.motion_lib.smplx_handle) if self.smplx else ("pulse_reset_ztask", self.motion_lib.handle)
+        fn, handle = (self.smplx_entry, self.motion_lib.smplx_handle) if self.smplx else ("pulse_reset_ztask", self.motion_lib.handle)
         with torch.cuda.device(self.device):
             _lib.check(getattr(self.lib, fn)(handle, C.byref(a), int(progress_buf.shape[0]), _lib.current_stream(self.device)), fn)
         return ws
@@ -269,6 +272,20 @@ class ZTaskResetB200:
             t.offset_dev = offset_dev.data_ptr()
         with torch.cuda.device(self.device):
             _lib.check(self.lib.pulse_ztask_reset_task(C.byref(t), N, _lib.current_stream(self.device)), "pulse_ztask_reset_task")
+
+
+class SmplxTargetResetB200(ZTaskResetB200):
+    """The reset of the SMPL-X reach and strike tasks (PULSE-X) over a 52-body MotionLib, through `pulse_reset_smplx_target`: the
+    reference-state reset of ZTaskResetB200 with the root's xy zeroed (humanoid_reach.py:46-48, humanoid_strike.py:147-150), the strike
+    target placed around it (`target_states`), the AMP back-fill in the SMPL-X rows, and reach's `reset_task`.  `upright=True` is
+    refused.  It is a subclass rather than a wider ZTaskResetB200 so that ZTaskResetB200 keeps its contract: over SMPL-X tables it
+    serves the speed task and refuses the others."""
+    smplx_kinds, smplx_entry = ("reach", "strike"), "pulse_reset_smplx_target"
+
+    def __init__(self, kind: str, motion_lib: MotionLibB200, floor: torch.Tensor, **kw):
+        if not getattr(motion_lib, "smplx", False):
+            raise _lib.PulseError("SmplxTargetResetB200 takes a 52-body (SMPL-X) MotionLib; ZTaskResetB200 serves the SMPL one")
+        super().__init__(kind, motion_lib, floor, **kw)
 
 
 _KEY_BODY_IDS = (7, 3, 22, 17)                                                     # env_im.yaml / env_pulse_amp.yaml key bodies

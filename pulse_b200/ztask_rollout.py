@@ -11,12 +11,18 @@ from . import _lib
 from .latent_rollout import LatentStepsB200
 
 _KINDS = {_lib.ZTASK_REACH: "reach", _lib.ZTASK_SPEED: "speed", _lib.ZTASK_STRIKE: "strike"}
-_WIDTHS = {"reach": 361, "speed": 361, "strike": 373}
-# per body layout: (observation width of the speed task, self observation -> dof targets of the decoder, latent size or None = any)
-_LAYOUTS = {"smpl": (None, 358, 69, None), "smplx": (_lib.SMPLX_SPEED_OBS, _lib.SMPLX_SELF_OBS, _lib.SMPLX_DOF, 48)}
-# the step's entry points per body layout: (step, list observation, rollout step) of the speed / strike tasks
-_ENTRIES = {"smpl": ("pulse_ztask_step", "pulse_ztask_obs_list", "pulse_ztask_rollout_step"),
-            "smplx": ("pulse_smplx_speed_step", "pulse_smplx_speed_obs_list", "pulse_smplx_speed_rollout_step")}
+# the observation width per (body layout, task kind)
+_WIDTHS = {("smpl", "reach"): 361, ("smpl", "speed"): 361, ("smpl", "strike"): 373, ("smplx", "reach"): _lib.SMPLX_REACH_OBS,
+           ("smplx", "speed"): _lib.SMPLX_SPEED_OBS, ("smplx", "strike"): _lib.SMPLX_STRIKE_OBS}
+# per body layout: (self observation -> dof targets of the decoder, latent size or None = any)
+_LAYOUTS = {"smpl": (358, 69, None), "smplx": (_lib.SMPLX_SELF_OBS, _lib.SMPLX_DOF, 48)}
+# the step's entry points per (body layout, task kind): (step, list observation, rollout step)
+_REACH = ("pulse_reach_step", "pulse_reach_obs_list", "pulse_reach_rollout_step")
+_ZTASK = ("pulse_ztask_step", "pulse_ztask_obs_list", "pulse_ztask_rollout_step")
+_SMPLX_TARGET = ("pulse_smplx_target_step", "pulse_smplx_target_obs_list", "pulse_smplx_target_rollout_step")
+_ENTRIES = {("smpl", "reach"): _REACH, ("smpl", "speed"): _ZTASK, ("smpl", "strike"): _ZTASK,
+            ("smplx", "speed"): ("pulse_smplx_speed_step", "pulse_smplx_speed_obs_list", "pulse_smplx_speed_rollout_step"),
+            ("smplx", "reach"): _SMPLX_TARGET, ("smplx", "strike"): _SMPLX_TARGET}
 SIM_KEYS = ("body_state", "root_states", "dof_pos", "dof_vel", "progress_buf", "sampled_motion_ids", "motion_start_times")
 STRIKE_KEYS = ("target_states", "tar_contact_forces")
 
@@ -24,17 +30,19 @@ STRIKE_KEYS = ("target_states", "tar_contact_forces")
 def check_pieces(task, reset, policy, vae, amp=None) -> str:
     """The task kind ("reach" / "speed" / "strike") after checking that the step object, the reset, the latent policy and the frozen
     VAE belong together; raises PulseError otherwise.  SMPL: observations of 361 / 361 / 373 floats, a 358 -> 69 decoder.  SMPL-X
-    (SmplxSpeedTaskB200, PULSE-X): the speed task's 781 floats, a 778 -> 153 decoder and a 48-dimensional latent (env_pulsex_amp.yaml)."""
+    (SmplxReachTaskB200 / SmplxSpeedTaskB200 / SmplxStrikeTaskB200, PULSE-X): 781 / 781 / 793 floats, a 778 -> 153 decoder and a
+    48-dimensional latent (env_pulsex_amp.yaml)."""
     kind = _KINDS.get(getattr(task, "kind", None))
     if kind is None:
-        raise _lib.PulseError("ZTaskStepsB200: task must be a ReachTaskB200, SpeedTaskB200, StrikeTaskB200 or SmplxSpeedTaskB200")
+        raise _lib.PulseError("ZTaskStepsB200: task must be a ReachTaskB200, SpeedTaskB200, StrikeTaskB200 or one of their SMPL-X "
+                              "counterparts (SmplxReachTaskB200, SmplxSpeedTaskB200, SmplxStrikeTaskB200)")
     if getattr(reset, "kind", None) != kind:
         raise _lib.PulseError(f"ZTaskStepsB200: the reset serves {getattr(reset, 'kind', None)!r}, the task is {kind!r}")
     layout = getattr(task, "layout", "smpl")
     if bool(getattr(reset, "smplx", False)) != (layout == "smplx"):
         raise _lib.PulseError(f"ZTaskStepsB200: the task is {layout}, the reset's MotionLib has {getattr(reset, 'bodies', 24)} bodies")
-    W, S, A, E = _LAYOUTS[layout]
-    W = W or _WIDTHS[kind]
+    S, A, E = _LAYOUTS[layout]
+    W = _WIDTHS[(layout, kind)]
     if int(task.obs_size) != W or int(policy.obs_size) != W:
         raise _lib.PulseError(f"ZTaskStepsB200: the {layout} {kind} observation has {W} floats, the task writes {task.obs_size} and the policy reads {policy.obs_size}")
     if int(policy.A) != int(vae.E):
@@ -59,7 +67,8 @@ class ZTaskStepsB200(LatentStepsB200):
          1. reset of the done envs (`ZTaskResetB200.reset_envs`), then the list observation of the reset envs into obses[:, t], then
             `reset_task` (reach, speed);
          5. `pulse_ztask_pre_physics`: PD targets into pd_tar, prev_root_pos (speed, strike), `_update_task` of the due envs (reach, speed);
-         7. the rollout step kernel (`pulse_reach_rollout_step` / `pulse_ztask_rollout_step`).
+         7. the rollout step kernel (`pulse_reach_rollout_step` / `pulse_ztask_rollout_step`, SMPL-X: `pulse_smplx_speed_rollout_step` /
+            `pulse_smplx_target_rollout_step`).
     `finish()` uses the task reward alone (task_reward_w 1, disc_reward_w 0, pulse_z_task.yaml:90-91).  With the AMP part (`amp`, an
     AmpBuffersB200 of the reset's amp_width and upright setting: 195 floats for env_pulse_amp.yaml) the reset also back-fills the AMP
     history, the driver keeps the horizon's AMP rows and `train_epoch()` trains the discriminator (disc_coef 5) inside the shared
@@ -80,8 +89,10 @@ class ZTaskStepsB200(LatentStepsB200):
     amp_root_height_obs False and PPOPolicy(obs_size=781, num_actions=48, units=(2048, 1024, 512), act="silu", with_disc=True,
     amp_obs_size=4650).
 
-    Out of scope: multi-GPU; the smplx humanoid's reach and strike tasks; Default / Hybrid state init; the power_usage_reward
-    terms the step kernels exclude."""
+    The PULSE-X reach and strike tasks take the same pieces with a SmplxReachTaskB200 / SmplxStrikeTaskB200 (obs_size 781 / 793), a
+    SmplxTargetResetB200 of the same kind over the 52-body MotionLib, and the same decoder, latent and AMP part.
+
+    Out of scope: multi-GPU; Default / Hybrid state init; the power_usage_reward terms the step kernels exclude."""
 
     def __init__(self, task, reset, policy, vae, sim: dict, horizon: int = 32, pd_offset: Optional[torch.Tensor] = None,
                  pd_scale: Optional[torch.Tensor] = None, pd_freeze: Optional[torch.Tensor] = None, use_graphs: bool = True,
@@ -93,7 +104,7 @@ class ZTaskStepsB200(LatentStepsB200):
         if missing:
             raise _lib.PulseError(f"ZTaskStepsB200: sim lacks {missing}")
         if self.layout == "smplx" and sim.get("dof_force") is not None:
-            raise _lib.PulseError("ZTaskStepsB200: sim['dof_force'] given, but the SMPL-X speed step has no power term")
+            raise _lib.PulseError("ZTaskStepsB200: sim['dof_force'] given, but the SMPL-X steps have no power term")
         n = self.n = int(sim["progress_buf"].shape[0])
         if n != task.num_envs:
             raise _lib.PulseError(f"ZTaskStepsB200: sim has {n} envs, the task {task.num_envs}")
@@ -104,21 +115,20 @@ class ZTaskStepsB200(LatentStepsB200):
     def _step_args(self, obs: torch.Tensor, rew: torch.Tensor):
         """The task's step arguments with the outputs pointed at experience slices and the driver's reset / terminate words."""
         s, task = self.sim, self.task
-        if self.kind == "reach":
+        if self.kind == "reach" and self.layout == "smpl":
             a = task._step_args(s["body_state"], s["progress_buf"], s.get("contact_forces"))
         else:
             a = task._args(s["body_state"], s["progress_buf"], s.get("contact_forces"))
-        if self.kind != "reach" and self.layout == "smpl":
-            if self.kind == "speed":
-                a.tar_speed = task._tar_speed.data_ptr()
-                if task.power_reward:
-                    if s.get("dof_force") is None:
-                        raise _lib.PulseError("the speed task's power_reward needs sim['dof_force']")
-                    a.dof_force, a.dof_force_stride, a.power_coefficient = s["dof_force"].data_ptr(), s["dof_force"].stride(0), task.power_coefficient
-                    a.dof_vel, a.dof_env_stride, a.dof_elem_stride = s["dof_vel"].data_ptr(), s["dof_vel"].stride(0), s["dof_vel"].stride(1)
-            else:
-                a.target_states, a.target_env_stride = s["target_states"].data_ptr(), s["target_states"].stride(0)
-                a.tar_contact_forces, a.tar_contact_env_stride = s["tar_contact_forces"].data_ptr(), s["tar_contact_forces"].stride(0)
+        if self.kind == "speed" and self.layout == "smpl":
+            a.tar_speed = task._tar_speed.data_ptr()
+            if task.power_reward:
+                if s.get("dof_force") is None:
+                    raise _lib.PulseError("the speed task's power_reward needs sim['dof_force']")
+                a.dof_force, a.dof_force_stride, a.power_coefficient = s["dof_force"].data_ptr(), s["dof_force"].stride(0), task.power_coefficient
+                a.dof_vel, a.dof_env_stride, a.dof_elem_stride = s["dof_vel"].data_ptr(), s["dof_vel"].stride(0), s["dof_vel"].stride(1)
+        elif self.kind == "strike":
+            a.target_states, a.target_env_stride = s["target_states"].data_ptr(), s["target_states"].stride(0)
+            a.tar_contact_forces, a.tar_contact_env_stride = s["tar_contact_forces"].data_ptr(), s["tar_contact_forces"].stride(0)
         a.obs_buf, a.obs_stride, a.rew_buf = obs.data_ptr(), obs.stride(0), rew.data_ptr()
         a.reset_buf, a.terminate_buf = self.reset_buf.data_ptr(), self.terminate_buf.data_ptr()
         return a
@@ -145,7 +155,7 @@ class ZTaskStepsB200(LatentStepsB200):
         """`_compute_observations(env_ids)` of the reset envs into obses[:, t], then `_reset_task` (humanoid_amp_task.py:66-76)."""
         ws = self.reset_ws
         a = self._step_args(self.obses[:, t], self.rewards[t])
-        self._launch("pulse_reach_obs_list" if self.kind == "reach" else _ENTRIES[self.layout][1], C.byref(a), ws["env_list"].data_ptr(),
+        self._launch(_ENTRIES[(self.layout, self.kind)][1], C.byref(a), ws["env_list"].data_ptr(),
                      ws["count"].data_ptr(), self.n)
         if self.kind != "strike":
             self.reset.reset_task(progress_buf=self.sim["progress_buf"], seed=self.reset_seed, offset=t, offset_dev=self.policy.rng_offset,
@@ -173,12 +183,12 @@ class ZTaskStepsB200(LatentStepsB200):
     def _env_step(self, t: int) -> None:
         """post_physics_step (humanoid.py:1315-1346): one fused launch."""
         a = self._step_args(self._next_obs(t), self.rewards[t])
-        self._launch("pulse_reach_rollout_step" if self.kind == "reach" else _ENTRIES[self.layout][2], C.byref(a), self.dones[t].data_ptr(), self.n)
+        self._launch(_ENTRIES[(self.layout, self.kind)][2], C.byref(a), self.dones[t].data_ptr(), self.n)
 
     def first_observation(self) -> None:
         """Observation of the initial state (Humanoid.reset -> _compute_observations at start-up): fills `obs_carry`."""
         a = self._step_args(self.obs_carry, self.rewards[0])
-        self._launch("pulse_reach_step" if self.kind == "reach" else _ENTRIES[self.layout][0], C.byref(a), self.n)
+        self._launch(_ENTRIES[(self.layout, self.kind)][0], C.byref(a), self.n)
         self.reset_buf.zero_()
         self.terminate_buf.zero_()
         self._amp_start()

@@ -2,7 +2,8 @@
 (phc/env/tasks/humanoid_speed.py, humanoid_strike.py) for the post-physics path -- reward, reset, observation in ONE launch
 (`pulse_ztask_step`) -- and the task-state updates (`_update_task` / `_reset_task`).  Like the reach task (pulse_b200/reach.py) the policy
 acts in the frozen PULSE latent space (`PulseVAE.compute_z_actions`); Isaac Gym keeps the physics and owns the state tensors.
-`SmplxSpeedTaskB200` is the speed task of PULSE-X on the 52-body SMPL-X humanoid (`pulse_smplx_speed_step`).
+`SmplxSpeedTaskB200` is the speed task of PULSE-X on the 52-body SMPL-X humanoid (`pulse_smplx_speed_step`); `SmplxReachTaskB200` and
+`SmplxStrikeTaskB200` are its reach and strike tasks (`pulse_smplx_target_step`).
 """
 import ctypes as C
 import math
@@ -11,7 +12,7 @@ from typing import Optional, Sequence
 import torch
 
 from . import _lib
-from .reach import SMPL_BODY_NAMES
+from .reach import SMPL_BODY_NAMES, ReachTaskB200
 
 SPEED_OBS, STRIKE_OBS = 361, 373      # 358 self observation + 3 / + 15
 
@@ -241,3 +242,160 @@ class SmplxSpeedTaskB200:
         with torch.cuda.device(self.device):
             _lib.check(self.lib.pulse_smplx_speed_obs_list(C.byref(a), env_list.data_ptr(), count.data_ptr(), self.num_envs,
                                                            _lib.current_stream(self.device)), "pulse_smplx_speed_obs_list")
+
+
+def _smplx_body_mask(who: str, name: str, ids: Sequence[int]) -> int:
+    B = _lib.SMPLX_BODIES
+    ids = [int(i) for i in ids]
+    if any(i < 0 or i >= B for i in ids):
+        raise _lib.PulseError(f"{who}: {name} {ids} outside [0, {B})")
+    return sum(1 << i for i in set(ids))
+
+
+class _SmplxTargetTask:
+    """The state and launches the SMPL-X reach and strike step objects share (`pulse_smplx_target_step` and its list observation)."""
+    kind, obs_size, layout = 0, 0, "smplx"
+
+    def __init__(self, who: str, num_envs: int, device, contact_body_ids, max_episode_length: int, enable_early_termination: bool,
+                 termination_height: float, power_reward: bool, power_usage_reward: bool):
+        if power_reward or power_usage_reward:
+            raise _lib.PulseError(f"{who}: power_reward / power_usage_reward are not served for SMPL-X (env_pulsex_amp.yaml has both off)")
+        self.who = who
+        self.contact_body_mask = _smplx_body_mask(who, "contact_body_ids", contact_body_ids)
+        self.strike_body_mask, self.reach_body_id = 0, 0
+        self.device, self.num_envs = torch.device(device), int(num_envs)
+        self.max_episode_length, self.enable_early_termination = int(max_episode_length), bool(enable_early_termination)
+        self.power_reward = False
+        dev, n = self.device, self.num_envs
+        self.termination_heights = torch.full((_lib.SMPLX_BODIES,), termination_height, device=dev)
+        self.obs_buf = torch.zeros(n, self.obs_size, device=dev)
+        self.rew_buf = torch.zeros(n, device=dev)
+        self.reset_buf = torch.zeros(n, dtype=torch.int64, device=dev)
+        self._terminate_buf = torch.zeros(n, dtype=torch.int64, device=dev)
+        self.lib = _lib.load()
+
+    def _args(self, rigid_body_state, progress_buf, contact_forces):
+        """The step arguments without the task's target views (the strike task adds them)."""
+        B = _lib.SMPLX_BODIES
+        if rigid_body_state.dim() != 3 or rigid_body_state.shape[1] < B or rigid_body_state.stride(1) != 13 or rigid_body_state.stride(2) != 1:
+            raise _lib.PulseError(f"rigid_body_state must be a [N, B>={B}, 13] view with row stride 13")
+        if contact_forces is not None and (contact_forces.dim() != 3 or contact_forces.shape[1] < B or contact_forces.stride(1) != 3
+                                           or contact_forces.stride(2) != 1):
+            raise _lib.PulseError(f"contact_forces must be a [N, B>={B}, 3] view with contiguous bodies")
+        return _lib.SmplxTargetStepArgs(
+            kind=self.kind, enable_early_termination=int(self.enable_early_termination), body_state=rigid_body_state.data_ptr(),
+            body_env_stride=rigid_body_state.stride(0), contact_forces=contact_forces.data_ptr() if contact_forces is not None else None,
+            contact_env_stride=contact_forces.stride(0) if contact_forces is not None else 0, termination_heights=self.termination_heights.data_ptr(),
+            contact_body_mask=self.contact_body_mask, strike_body_mask=self.strike_body_mask, reach_body_id=self.reach_body_id,
+            progress_buf=progress_buf.data_ptr(), max_episode_length=self.max_episode_length, obs_buf=self.obs_buf.data_ptr(),
+            obs_stride=self.obs_buf.stride(0), rew_buf=self.rew_buf.data_ptr(), reset_buf=self.reset_buf.data_ptr(),
+            terminate_buf=self._terminate_buf.data_ptr())
+
+    def _launch(self, a, dof_force) -> None:
+        if dof_force is not None:
+            raise _lib.PulseError(f"{self.who}: dof_force given, but the SMPL-X {_KIND_NAMES[self.kind]} step has no power term")
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.pulse_smplx_target_step(C.byref(a), self.num_envs, _lib.current_stream(self.device)), "pulse_smplx_target_step")
+
+    def _launch_list(self, a, env_list: torch.Tensor, count: torch.Tensor) -> None:
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.pulse_smplx_target_obs_list(C.byref(a), env_list.data_ptr(), count.data_ptr(), self.num_envs,
+                                                            _lib.current_stream(self.device)), "pulse_smplx_target_obs_list")
+
+
+_KIND_NAMES = {_lib.ZTASK_REACH: "reach", _lib.ZTASK_STRIKE: "strike"}
+
+
+class SmplxReachTaskB200(_SmplxTargetTask):
+    """HumanoidReach(Z) for the 52-body SMPL-X humanoid of PULSE-X (`env.task=HumanoidReachZ env=env_pulsex_amp robot=smplx_humanoid`):
+    the post-physics step `pulse_smplx_target_step` and `_update_task`, with what ReachTaskB200 carries.  The self observation takes the
+    heading of remove_base_rot(root_rot), the target offset that of the raw root rotation, as the reference does; obs = [self 778 | 3].
+    Bodies are indices in the simulator's body order (SMPLH_MUJOCO_NAMES): `reach_body_id` is `_reach_body_id`, `contact_body_ids` the
+    task's `_contact_body_ids`.  The SMPL-X humanoid has no R_Hand body; its right arm is R_Elbow 35, R_Wrist 36 and the finger bodies
+    37-51.  power_reward / power_usage_reward are refused, as is a `dof_force`."""
+    kind, obs_size = _lib.ZTASK_REACH, _lib.SMPLX_REACH_OBS
+
+    def __init__(self, num_envs: int, device="cuda:0", *, reach_body_id: int, contact_body_ids: Sequence[int], tar_change_steps_min: int = 100,
+                 tar_change_steps_max: int = 200, tar_dist_max: float = 1.0, tar_height_min: float = 0.5, tar_height_max: float = 1.5,
+                 max_episode_length: int = 300, enable_early_termination: bool = True, termination_height: float = 0.15,
+                 power_reward: bool = False, power_usage_reward: bool = False):
+        _smplx_body_mask("SmplxReachTaskB200", "reach_body_id", [reach_body_id])
+        super().__init__("SmplxReachTaskB200", num_envs, device, contact_body_ids, max_episode_length, enable_early_termination,
+                         termination_height, power_reward, power_usage_reward)
+        self.reach_body_id = int(reach_body_id)
+        self.tar_change_steps_min, self.tar_change_steps_max = tar_change_steps_min, tar_change_steps_max
+        self.tar_dist_max, self.tar_height_min, self.tar_height_max = tar_dist_max, tar_height_min, tar_height_max
+        dev, n = self.device, self.num_envs
+        self._tar_pos = torch.zeros(n, 3, device=dev)
+        self._tar_change_steps = torch.zeros(n, dtype=torch.int64, device=dev)
+        self._rand = torch.zeros(n, 3, device=dev)
+        self._steps = torch.zeros(n, dtype=torch.int64, device=dev)
+
+    def get_task_obs_size(self) -> int:
+        return 3
+
+    update_task = ReachTaskB200.update_task     # pulse_reach_update_task does not depend on the body layout
+
+    def _args(self, rigid_body_state, progress_buf, contact_forces):
+        a = super()._args(rigid_body_state, progress_buf, contact_forces)
+        a.tar_pos = self._tar_pos.data_ptr()
+        return a
+
+    def post_physics_step(self, rigid_body_state: torch.Tensor, progress_buf: torch.Tensor, contact_forces: Optional[torch.Tensor] = None,
+                          dof_force: Optional[torch.Tensor] = None) -> None:
+        """compute_reach_reward + compute_humanoid_reset + the observation in one launch."""
+        self._launch(self._args(rigid_body_state, progress_buf, contact_forces), dof_force)
+
+    def observe_list(self, rigid_body_state: torch.Tensor, env_list: torch.Tensor, count: torch.Tensor, progress_buf: torch.Tensor,
+                     contact_forces: Optional[torch.Tensor] = None) -> None:
+        """_compute_observations(env_ids) for the envs env_list[0 .. *count): post_physics_step's rows for them, nothing else."""
+        self._launch_list(self._args(rigid_body_state, progress_buf, contact_forces), env_list, count)
+
+
+class SmplxStrikeTaskB200(_SmplxTargetTask):
+    """HumanoidStrike(Z) for the 52-body SMPL-X humanoid of PULSE-X (`env.task=HumanoidStrikeZ env=env_pulsex_amp robot=smplx_humanoid`):
+    the post-physics step `pulse_smplx_target_step`, with what StrikeTaskB200 carries.  obs = [self 778 | 15], the target in the heading
+    of the raw root rotation.  `strike_body_ids` is `_strike_body_ids`, `contact_body_ids` `_contact_body_ids`, both indices in the
+    simulator's body order (SMPL-X has no R_Hand; the right arm is R_Elbow 35, R_Wrist 36 and the finger bodies 37-51).  The early
+    termination's pushing body is any body outside both sets pressing harder than 50 N, over all 52 bodies.  power_reward /
+    power_usage_reward are refused, as is a `dof_force`."""
+    kind, obs_size = _lib.ZTASK_STRIKE, _lib.SMPLX_STRIKE_OBS
+
+    def __init__(self, num_envs: int, device="cuda:0", *, strike_body_ids: Sequence[int], contact_body_ids: Sequence[int],
+                 tar_dist_min: float = 0.5, tar_dist_max: float = 10.0, near_dist: float = 1.5, near_prob: float = 0.5,
+                 max_episode_length: int = 300, enable_early_termination: bool = True, termination_height: float = 0.15, dt: float = 1.0 / 30.0,
+                 power_reward: bool = False, power_usage_reward: bool = False):
+        strike_mask = _smplx_body_mask("SmplxStrikeTaskB200", "strike_body_ids", strike_body_ids)
+        super().__init__("SmplxStrikeTaskB200", num_envs, device, contact_body_ids, max_episode_length, enable_early_termination,
+                         termination_height, power_reward, power_usage_reward)
+        self.strike_body_mask, self.dt = strike_mask, float(dt)
+        self._tar_dist_min, self._tar_dist_max, self._near_dist, self._near_prob = tar_dist_min, tar_dist_max, near_dist, near_prob
+        self._prev_root_pos = torch.zeros(self.num_envs, 3, device=self.device)
+
+    def get_task_obs_size(self) -> int:
+        return 15
+
+    pre_physics_step = _ZTaskBase.pre_physics_step
+    reset_target = StrikeTaskB200.reset_target
+
+    def _args(self, rigid_body_state, progress_buf, contact_forces):
+        a = super()._args(rigid_body_state, progress_buf, contact_forces)
+        a.prev_root_pos, a.dt = self._prev_root_pos.data_ptr(), self.dt
+        return a
+
+    def post_physics_step(self, rigid_body_state: torch.Tensor, progress_buf: torch.Tensor, target_states: torch.Tensor,
+                          tar_contact_forces: torch.Tensor, contact_forces: Optional[torch.Tensor] = None,
+                          dof_force: Optional[torch.Tensor] = None) -> None:
+        """compute_strike_reward + the strike compute_humanoid_reset + the observation in one launch.  target_states [N, 13] and
+        tar_contact_forces [N, 3] are views of the simulator tensors, read through their env strides."""
+        a = self._args(rigid_body_state, progress_buf, contact_forces)
+        a.target_states, a.target_env_stride = target_states.data_ptr(), target_states.stride(0)
+        a.tar_contact_forces, a.tar_contact_env_stride = tar_contact_forces.data_ptr(), tar_contact_forces.stride(0)
+        self._launch(a, dof_force)
+
+    def observe_list(self, rigid_body_state: torch.Tensor, env_list: torch.Tensor, count: torch.Tensor, progress_buf: torch.Tensor,
+                     target_states: torch.Tensor, contact_forces: Optional[torch.Tensor] = None) -> None:
+        """_compute_observations(env_ids) for the envs env_list[0 .. *count): post_physics_step's rows for them, nothing else."""
+        a = self._args(rigid_body_state, progress_buf, contact_forces)
+        a.target_states, a.target_env_stride = target_states.data_ptr(), target_states.stride(0)
+        self._launch_list(a, env_list, count)

@@ -1,7 +1,9 @@
 #!/usr/bin/env python
 """The PULSE-X speed task on the device (HumanoidSpeedZ, robot=smplx_humanoid, env_pulsex_amp.yaml): full training iterations of the
 52-body SMPL-X humanoid through `ZTaskStepsB200`, measured as tools/bench_ztask_rollout.py measures the SMPL latent tasks, and the step
-kernel alone.
+kernel alone.  --task reach / strike measures the PULSE-X reach or strike task the same way (HumanoidReachZ / HumanoidStrikeZ, reach
+body R_Wrist 36, strike bodies R_Elbow, R_Wrist and the right index finger's base 35, 36, 37), and times `pulse_smplx_target_step`
+alternated sample by sample with `pulse_smplx_speed_step` in the same call, so the two rates compare.
 
   iteration  one horizon (device resets inside it, latent policy 2048-1024-512 SiLU over 48 latent dimensions, frozen prior + 778 -> 153
              decoder of the PULSE-X VAE's shapes with random weights, pre-physics and step kernels; no physics), then `finish` and the
@@ -15,7 +17,7 @@ kernel alone.
 
 One JSON line per measurement, with the card name, power limit and maximum SM clock read in the same call.  Needs a CUDA device.
 
-  python tools/bench_smplx_speed.py [--envs 1536 8192] [--iters 5] [--warmup 2] [--step-envs 16384] [--step-reps 200]
+  python tools/bench_smplx_speed.py [--task speed|reach|strike] [--envs 1536 8192] [--iters 5] [--warmup 2] [--step-envs 16384] [--step-reps 200]
 """
 import argparse
 import ctypes as C
@@ -60,36 +62,68 @@ def sim_state(n, dev, seed):
                 motion_start_times=torch.zeros(n, device=dev))
 
 
-def build(n, dev, use_graphs):
+REACH_BODY, STRIKE_IDS = 36, (35, 36, 37)
+
+
+def make_task(kind, n, dev):
+    from pulse_b200.ztasks import SmplxReachTaskB200, SmplxSpeedTaskB200, SmplxStrikeTaskB200
+    if kind == "reach":
+        return SmplxReachTaskB200(n, device=dev, reach_body_id=REACH_BODY, contact_body_ids=CONTACT_IDS)
+    if kind == "strike":
+        return SmplxStrikeTaskB200(n, device=dev, strike_body_ids=STRIKE_IDS, contact_body_ids=CONTACT_IDS)
+    return SmplxSpeedTaskB200(n, device=dev, contact_body_ids=CONTACT_IDS)
+
+
+def with_target(s, n, dev):
+    """The strike task's target views: body 53 of an [N, 54, 13] rigid-body tensor's contact rows and an [N, 2, 13] actor root tensor."""
+    g = torch.Generator(device=dev).manual_seed(400)
+    roots = torch.randn(n, 2, 13, device=dev, generator=g)
+    roots[:, 1, 3:7] = torch.nn.functional.normalize(roots[:, 1, 3:7], dim=-1)
+    s["target_states"], s["tar_contact_forces"] = roots[:, 1], s["contact_forces"][:, B]
+    return s
+
+
+def build(n, dev, use_graphs, kind="speed"):
     from pulse_b200.motion_lib import MotionLibB200
     from pulse_b200.ppo import PPOPolicy
     from pulse_b200.vae import PulseVAE
-    from pulse_b200.ztask_reset import ZTaskResetB200
+    from pulse_b200.ztask_reset import SmplxTargetResetB200, ZTaskResetB200
     from pulse_b200.ztask_rollout import ZTaskStepsB200
-    from pulse_b200.ztasks import SmplxSpeedTaskB200
     ml = MotionLibB200.from_tables(tables(256, dev, 100))
     g = torch.Generator(device=dev).manual_seed(300)
     floor = -0.9 + 0.05 * torch.rand(ml.gts.shape[0], device=dev, generator=g)            # stand-in for the ground table
-    task = SmplxSpeedTaskB200(n, device=dev, contact_body_ids=CONTACT_IDS)
+    task = make_task(kind, n, dev)
     policy = PPOPolicy(obs_size=task.obs_size, num_actions=LATENT, units=UNITS, act="silu", device=dev, seed=0)
     vae = PulseVAE(self_obs_size=778, num_actions=D, latent=LATENT, device=dev, with_critic=False)
-    drv = ZTaskStepsB200(task, ZTaskResetB200("speed", ml, floor, upright=False), policy, vae, sim_state(n, dev, 200), horizon=HORIZON,
-                         use_graphs=use_graphs, reset_seed=1)
+    reset = ZTaskResetB200("speed", ml, floor, upright=False) if kind == "speed" else SmplxTargetResetB200(kind, ml, floor, upright=False)
+    sim = sim_state(n, dev, 200)
+    if kind == "strike":
+        sim = with_target(sim, n, dev)
+    drv = ZTaskStepsB200(task, reset, policy, vae, sim, horizon=HORIZON, use_graphs=use_graphs, reset_seed=1)
     drv.first_observation()
     return drv
 
 
-def step_bytes():
+def step_bytes(kind="speed"):
     """Bytes one env-step of pulse_smplx_speed_step moves, from the shapes: reads the 52 x 13 body floats, 52 x 3 contact floats, the
     52 termination heights (cached across envs: not counted), progress, prev_root_pos and tar_speed; writes the 781-float observation
-    row, reward, reward_raw, reset and terminate."""
+    row, reward, reward_raw, reset and terminate.  Reach reads tar_pos instead of prev_root_pos / tar_speed and writes no reward_raw;
+    strike reads prev_root_pos, the 13-float target state and its 3-float contact force, and writes a 793-float row."""
     rd = {"body_state": B * 13 * 4, "contact_forces": B * 3 * 4, "progress/prev_root/tar_speed": 8 + 12 + 4}
     wr = {"obs_row": 781 * 4, "rew/reward_raw": 8, "reset/terminate": 16}
+    if kind == "reach":
+        rd, wr = dict(rd), dict(wr)
+        del rd["progress/prev_root/tar_speed"], wr["rew/reward_raw"]
+        rd["progress/tar_pos"], wr["rew"] = 8 + 12, 4
+    elif kind == "strike":
+        rd = {"body_state": B * 13 * 4, "contact_forces": B * 3 * 4, "progress/prev_root": 8 + 12, "target_state": 13 * 4, "tar_contact": 3 * 4}
+        wr = {"obs_row": 793 * 4, "rew": 4, "reset/terminate": 16}
     return rd, wr
 
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--task", choices=("speed", "reach", "strike"), default="speed")
     ap.add_argument("--envs", type=int, nargs="+", default=[1536, 8192])
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
@@ -115,7 +149,7 @@ def main():
         return s, e
 
     for n in args.envs:
-        arms = {"graph": build(n, dev, True), "eager": build(n, dev, False)}
+        arms = {"graph": build(n, dev, True, args.task), "eager": build(n, dev, False, args.task)}
         mb = min(MINIBATCH, n * HORIZON)
         update = lambda d: (d.finish(), d.train_epoch(mini_epochs=MINI_EPOCHS, minibatch=mb))
         ev = {a: {"horizon": [], "update": []} for a in arms}
@@ -134,9 +168,9 @@ def main():
         arms["eager"].play_steps()
         torch.cuda.synchronize()
         launches = (lib.pulse_launch_count() - c0) / HORIZON
-        out = {"workload": "PULSE-X speed task iteration (HumanoidSpeedZ, smplx_humanoid, 52 bodies, 153 dofs): %d envs, horizon %d, latent "
+        out = {"workload": "PULSE-X %s task iteration (Humanoid%sZ, smplx_humanoid, 52 bodies, 153 dofs): %d envs, horizon %d, latent "
                            "policy %s SiLU over %d dims, frozen prior + 778->153 decoder, task reward only, %d mini-epochs of %d rows, no physics"
-                           % (n, HORIZON, "-".join(map(str, UNITS)), LATENT, MINI_EPOCHS, mb),
+                           % (args.task, args.task.capitalize(), n, HORIZON, "-".join(map(str, UNITS)), LATENT, MINI_EPOCHS, mb),
                "gpu": info, "envs": n, "iters": args.iters, "warmup": args.warmup, "launches_per_step": round(launches, 2)}
         for a in arms:
             ms = {k: [s.elapsed_time(e) for s, e in v] for k, v in ev[a].items()}
@@ -150,32 +184,46 @@ def main():
         del arms
         torch.cuda.empty_cache()
 
-    # the step kernel alone
-    from pulse_b200.ztasks import SmplxSpeedTaskB200
+    # the step kernel alone; with --task reach / strike the target step and the speed step, alternated sample by sample
     n = args.step_envs
-    task = SmplxSpeedTaskB200(n, device=dev, contact_body_ids=CONTACT_IDS)
+    kinds = ["speed"] if args.task == "speed" else [args.task, "speed"]
     s = sim_state(n, dev, 7)
-    a = task._args(s["body_state"], s["progress_buf"], s["contact_forces"])
+    if args.task == "strike":
+        s = with_target(s, n, dev)
     st = _lib.current_stream(dev)
-    for _ in range(10):
-        _lib.check(lib.pulse_smplx_speed_step(C.byref(a), n, st), "pulse_smplx_speed_step")
-    times = []
+    calls = {}
+    for kind in kinds:
+        task = make_task(kind, n, dev)
+        a = task._args(s["body_state"], s["progress_buf"], s["contact_forces"])
+        if kind == "strike":
+            a.target_states, a.target_env_stride = s["target_states"].data_ptr(), s["target_states"].stride(0)
+            a.tar_contact_forces, a.tar_contact_env_stride = s["tar_contact_forces"].data_ptr(), s["tar_contact_forces"].stride(0)
+        fn = "pulse_smplx_speed_step" if kind == "speed" else "pulse_smplx_target_step"
+        calls[kind] = (fn, getattr(lib, fn), a, task)
+    for fn, f, a, _ in calls.values():
+        for _ in range(10):
+            _lib.check(f(C.byref(a), n, st), fn)
+    times = {k: [] for k in kinds}
     for _ in range(5):
-        flush.zero_()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(args.step_reps):
-            _lib.check(lib.pulse_smplx_speed_step(C.byref(a), n, st), "pulse_smplx_speed_step")
-        e1.record()
-        torch.cuda.synchronize()
-        times.append(e0.elapsed_time(e1) * 1e3 / args.step_reps)
-    rd, wr = step_bytes()
-    per_env = sum(rd.values()) + sum(wr.values())
-    us = sorted(times)[len(times) // 2]
-    print(json.dumps({"workload": "pulse_smplx_speed_step alone: %d envs, %d back-to-back launches per sample, median of 5 samples" % (n, args.step_reps),
-                      "gpu": info, "envs": n, "kernel_us": round(us, 2), "kernel_us_samples": [round(t, 2) for t in times],
-                      "bytes_per_env_step": {"read": rd, "write": wr, "total": per_env},
-                      "achieved_GB_per_s": round(per_env * n / (us * 1e-6) / 1e9, 1)}), flush=True)
+        for kind in kinds:
+            fn, f, a, _ = calls[kind]
+            flush.zero_()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(args.step_reps):
+                _lib.check(f(C.byref(a), n, st), fn)
+            e1.record()
+            torch.cuda.synchronize()
+            times[kind].append(e0.elapsed_time(e1) * 1e3 / args.step_reps)
+    for kind in kinds:
+        rd, wr = step_bytes(kind)
+        per_env = sum(rd.values()) + sum(wr.values())
+        us = sorted(times[kind])[len(times[kind]) // 2]
+        name = calls[kind][0] + ("" if kind == "speed" else " (%s)" % kind)
+        print(json.dumps({"workload": "%s alone: %d envs, %d back-to-back launches per sample, median of 5 samples" % (name, n, args.step_reps),
+                          "gpu": info, "envs": n, "kernel_us": round(us, 2), "kernel_us_samples": [round(t, 2) for t in times[kind]],
+                          "bytes_per_env_step": {"read": rd, "write": wr, "total": per_env},
+                          "achieved_GB_per_s": round(per_env * n / (us * 1e-6) / 1e9, 1)}), flush=True)
 
 
 if __name__ == "__main__":
