@@ -24,6 +24,36 @@ height field) and recomputes each output in float64:
   height must then equal that cell's min(h1, h2) vscale exactly.  The center height (a mean over the 3 x 3 center points) is checked
   against the interval its reachable cells give; those points are multiples of the cell size, so their edge share is limited by
   reset_fp64.EDGE_MAX as in the spawn reset.
+
+The imitation step (im_step.cu: im_step_kernel, both the 934-float row and the tracked row) and the general task observation
+(task_obs.cu) have their own references, im_step_ref and task_obs_ref:
+
+* planner, exact: t_rew = motion_time_rn(prog), t_obs = motion_time_rn(prog + 1 - rec) (three fp32 roundings in the reference's order),
+  the frame rows and blend of oracle.pulse_oracle.frame_blend (pinned to frame_blend_rn by tests/test_gpu_motion_fp64.py), the
+  pass_time mask, progress_rw under PULSE_STEP_ADVANCE and the getup pull-back, fdones_out.  The blend is an exact operand of every
+  later link, as in motion_fp64.query_ref.
+* reference pose at t_rew and t_obs: query_ref on the tables plus global_offset -- lerps for position and velocities, slerp candidates
+  for the rotations, slerp + exponential map candidates for ref_dof_pos (the aux records of the observation rows, joints 1..23).
+* reward: the position / velocity / angular-velocity sums sum_j |r_j - x_j|^2 carry the lerp bound through the squares (2 |d| td + td^2),
+  sq3's three roundings and the 24 roundings of the column sum; the mean's fp32 constant 1 / 72 (or 1 / 24) is off by at most u32
+  relative and its product rounds once; k * e rounds once; expf is exp_neg's 2 ulp.  The rotation error is the angle of
+  r.q (x) conj(q): 2 acos(w) wrapped past fp32(pi) as oracle.pulse_oracle.wrap_angle wraps it, with acos conditioned by
+  motion_fp64._acos_err near w = +-1 and the s <= 1e-5 zero branch; w is known within r.q's slerp bound times |q|_1 plus the 8-product
+  rounding (qmul8_err).  Every branch the bound allows (every allowed slerp candidate, then zero / plain / wrapped angle) gives a
+  theta^2 interval; the body's term is that union, so the reward has one value and one bound, and rows where the slerp candidates
+  differ (reset_fp64.primary) are counted, their share limited.  The power term is sum |tau qdot| (dof_power: 69 products, 2 adds
+  per body thread and the 24-term column sum), zero at prog <= 3.  reward = sum w_i r_i + power within 5 u32 of its terms.
+* reset: the per-body decision dist > termination_distances[j] is taken from an fp32 restatement in the kernel's pinned order
+  (lerp_rn, the __fadd_rn offset, __fsub_rn, norm3_rn's two fused multiply-adds and the correctly rounded root), which makes it exact;
+  the mean criterion sums those distances in body order and divides by popc(mask).  The float64 distance is a second link: the
+  restatement must lie within its bound, and every row whose distances all lie outside their bound of the threshold must take the
+  float64 decision; the share of rows that do not is limited.  prog > 1, early termination, cycle recovery and getup recovery are exact.
+* observation at t_obs: self_obs_ref (upright), and the six pieces of the v6 task block, each its own link -- yaw_apply of r.p - p,
+  r.v - v, r.w - w and r.p - p_root, six_ref of H^-1 (r.q (x) conj q) H (yaw_qmul, then yaw_qmul_right) and of H^-1 r.q.  Rows whose
+  heading is ill-conditioned or whose r.q may take two slerp branches pass any rotation-dependent value; their share is limited.
+* task_obs_ref: the same pieces from the fp32 ref_* arrays the kernel read (exact operands), the heading of body 0 through
+  base_rot_removed(upright), in every version's layout (flat over (t, j) for 1, 2, 3; per sample for 6, 7, 8, 9), v8's R rv / R rw,
+  v9's root-velocity pair from tracked body 0, and v2's dof difference, which is one fp32 rounding of the float64 difference: exact.
 """
 import math
 from typing import Dict, List, Optional
@@ -123,11 +153,13 @@ def check_self(rep: Optional[Report], tag: str, obs: torch.Tensor, ref: Dict[str
 
 
 # ------------------------------------------------------------------------------------------------------------------ the latent tasks
-def _dof_power(dof_force, dof_vel):
+def dof_power(dof_force, dof_vel, adds: int = 8):
+    """sum |f v| over the 69 dofs and its bound: the products (one rounding each), then `adds` roundings along the deepest chain of
+    the kernel's sum -- 3 lane-local adds and 5 shuffle levels in the latent-task steps; 2 adds per body thread and the 24-term
+    column sum in the imitation step."""
     t = (f64(dof_force)[:, :NUM_DOF] * f64(dof_vel)[:, :NUM_DOF]).abs()
     s = t.sum(-1)
-    # products (one rounding each), then at most 3 lane-local adds and 5 shuffle levels
-    return s, 10 * U32 * s
+    return s, (adds + 2) * U32 * s
 
 
 def _root_vel(root, prev, dt):
@@ -136,7 +168,7 @@ def _root_vel(root, prev, dt):
     return v, 2 * U32 * v.abs()
 
 
-def _exp_neg(a, ta):
+def exp_neg(a, ta):
     """expf(-a) for a >= 0 known within ta, and its bound (expf: 2 ulp; below fp32's smallest normal number the result may be a
     subnormal or 0)."""
     e = torch.exp(-a)
@@ -225,12 +257,12 @@ def ztask_ref(kind: int, B: int, inp: Dict[str, torch.Tensor], obs_only: bool = 
         vy, tvy = v[:, 1], tv[:, 1]
         a = 0.25 * (err * err + 0.1 * vy * vy)
         ta = 0.25 * (2 * err.abs() * terr + terr * terr + 0.1 * (2 * vy.abs() * tvy + tvy * tvy)) + 5 * U32 * a
-        rew, trew = _exp_neg(a, ta)
+        rew, trew = exp_neg(a, ta)
         out["raw0"] = (rew[:, None], trew[:, None])
         pw, tpw = torch.zeros(n, dtype=torch.float64), torch.zeros(n, dtype=torch.float64)
         if inp.get("dof_force") is not None:
             c = f32r(inp["power_c"])
-            s, ts_ = _dof_power(inp["dof_force"], inp["dof_vel"])
+            s, ts_ = dof_power(inp["dof_force"], inp["dof_vel"])
             live = prog > 3
             pw = torch.where(live, -c * s, pw)
             tpw = torch.where(live, c * ts_ + U32 * c * s, tpw)
@@ -243,7 +275,7 @@ def ztask_ref(kind: int, B: int, inp: Dict[str, torch.Tensor], obs_only: bool = 
         s = (d * d).sum(-1)
         a = 4 * s
         ta = 4 * ((2 * d.abs() * td + td * td).sum(-1) + 4 * U32 * s)
-        rew, trew = _exp_neg(a, ta)
+        rew, trew = exp_neg(a, ta)
         out["reward"] = [(rew[:, None], trew[:, None], ones)]
     else:
         ts = f64(inp["target"])
@@ -275,7 +307,7 @@ def ztask_ref(kind: int, B: int, inp: Dict[str, torch.Tensor], obs_only: bool = 
         npos_sure = zero_ds | (ds + tds <= 0)
         verr = torch.clamp(1 - ds, min=0.0)
         tverr = tds + U32 * verr
-        vel_r, tvel = _exp_neg(4 * verr * verr, 4 * (2 * verr * tverr + tverr * tverr) + 3 * U32 * 4 * verr * verr)
+        vel_r, tvel = exp_neg(4 * verr * verr, 4 * (2 * verr * tverr + tverr * tverr) + 3 * U32 * 4 * verr * verr)
         cands = [(torch.ones(n, 1, dtype=torch.float64), torch.zeros(n, 1, dtype=torch.float64), ~ge_sure)]
         for vr, tvr, ok in ((vel_r, tvel, ~npos_sure), (torch.zeros_like(vel_r), torch.zeros_like(tvel), ~pos_sure)):
             r = 0.6 * rot_r + 0.4 * vr
@@ -444,11 +476,11 @@ def terrain_ref(inp: Dict[str, object], flags: int) -> Dict[str, object]:
         td = ttar[:, :2] + U32 * d.abs()
         err = (d * d).sum(-1)
         terr = (2 * d.abs() * td + td * td).sum(-1) + 2 * U32 * err
-        loc, tloc = _exp_neg(2 * err, 2 * terr + U32 * 2 * err)
+        loc, tloc = exp_neg(2 * err, 2 * terr + U32 * 2 * err)
         power, tpow = torch.zeros(n, dtype=torch.float64), torch.zeros(n, dtype=torch.float64)
         if inp.get("dof_force") is not None:
             c = f32r(inp["power_c"])
-            s, ts_ = _dof_power(inp["dof_force"], inp["dof_vel"])
+            s, ts_ = dof_power(inp["dof_force"], inp["dof_vel"])
             power, tpow = -c * s, c * ts_ + U32 * c * s
         one, zero = torch.ones_like(loc), torch.zeros_like(loc)
         if inp["fuzzy"]:
@@ -575,3 +607,413 @@ def check_terrain(rep: Optional[Report], tag: str, flags: int, got: Dict[str, to
         mf.check_branches(rep, f"{tag} heights", hobs[..., None], ref["heights"], built=None if built is None else built[:, None])
         rf.limit_share(rep, f"{tag} heights cell edge", ref["heights edge"], None if built is None else built[:, None])
         rf.limit_share(rep, f"{tag} heights center height cell edge", ref["ref edge"], built, amb_max=rf.EDGE_MAX)
+
+
+# ------------------------------------------------------------------------------------------------------------------ imitation step
+IM_SELF, IM_TASK = 358, 576
+REW, RST, OBS, ADVANCE = 1, 2, 4, 8
+IM_PIECES = (("dp", 3), ("drot", 6), ("dv", 3), ("dw", 3), ("lp", 3), ("lrot", 6))     # the v6 task block, block-major over the bodies
+EXP_EPS = 1e-5
+
+
+def motion_time32(prog: torch.Tensor, dt: float, start: torch.Tensor, off: torch.Tensor) -> torch.Tensor:
+    """motion_time_rn: fp32(progress) * dt + start + offset, three fp32 roundings (torch rounds each CPU float32 operation)."""
+    return (prog.long().float() * torch.tensor(dt, dtype=torch.float32) + start.float()) + off.float()
+
+
+def fma32(a: torch.Tensor, b: torch.Tensor, c: torch.Tensor) -> torch.Tensor:
+    """fmaf of fp32 tensors, rounded once: a * b is exact in float64; the float64 sum's own rounding error e is recovered exactly
+    (two-sum) and decides the one case where rounding twice differs from rounding once -- a float64 sum exactly halfway between two
+    fp32 numbers."""
+    p = a.double() * b.double()
+    cc = c.double()
+    s = p + cc
+    bb = s - p
+    e = (p - (s - bb)) + (cc - bb)
+    r = s.float()
+    other = torch.nextafter(r, torch.where(s > r.double(), torch.full_like(r, math.inf), torch.full_like(r, -math.inf)))
+    half = (s == 0.5 * (r.double() + other.double())) & (e != 0) & (s != r.double())
+    up = torch.where(e > 0, torch.maximum(r, other), torch.minimum(r, other))
+    return torch.where(half, up, r)
+
+
+def lerp_rn32(p0: torch.Tensor, p1: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """lerp_rn: ((1 - b) p0) + (b p1), every operation rounded on its own."""
+    return (1.0 - b) * p0 + b * p1
+
+
+def reset_dist32(p0, p1, b, goff, pos) -> torch.Tensor:
+    """The kernel's termination distance in its pinned fp32 order: r.p = lerp_rn + __fadd_rn offset, __fsub_rn, norm3_rn =
+    sqrt(fma(z, z, fma(y, y, x x))).  p0 / p1 [n, B, 3] the frame rows, b [n, 1, 1] the blend, goff [n, 1, 3], pos [n, B, 3]."""
+    rp = lerp_rn32(p0.float(), p1.float(), b.float()) + goff.float()
+    d = pos.float() - rp
+    x, y, z = d.unbind(-1)
+    return torch.sqrt(fma32(z, z, fma32(y, y, x * x)))
+
+
+def yaw_qmul_right(hs, hc, dth, q, tq):
+    """qmul(q, (0, 0, hs, hc)) -- the right multiply by the forward heading that closes H^-1 (x) q (x) H -- in float64 with its bound,
+    as reset_fp64.yaw_qmul: pairwise mixing, |q| dth / 2, the 8-product rounding."""
+    h = torch.stack([torch.zeros_like(hs), torch.zeros_like(hs), hs, hc], -1).expand(q.shape)
+    out = mf.qmul(q, h)
+    pair = torch.stack([tq[..., 0] + tq[..., 1], tq[..., 0] + tq[..., 1], tq[..., 2] + tq[..., 3], tq[..., 2] + tq[..., 3]], -1)
+    return out, pair + (0.5 * q.norm(dim=-1) * dth.expand(q.shape[:-1]))[..., None] + mf.qmul8_err(q, h)
+
+
+def rel_rot(rq, trq, q):
+    """r.q (x) conj(q) of fp32 simulator quaternions q in float64, with its bound: r.q's bound times |q|_1 per component, and the
+    8-product rounding."""
+    qc = mf.qconj(q)
+    return mf.qmul(rq, qc), (trq.amax(-1) * q.abs().sum(-1))[..., None] + mf.qmul8_err(rq, qc)
+
+
+def angle_cands(w: torch.Tensor, dw: torch.Tensor) -> List[mf.Cand]:
+    """quat_angle (quat_to_angle_axis's angle) of a quaternion whose w is known within dw: candidates [..., 1] for the s <= 1e-5 zero,
+    2 acos(w), and 2 acos(w) - 2 pi past fp32(pi), with motion_fp64.expmap_cands' conditioning (acosf 2 ulp, the wrap's fp32 2 pi)."""
+    s2 = 1.0 - w * w
+    ds2 = 2 * w.abs() * dw + dw * dw + 2 * U32
+    s_lo = torch.sqrt(torch.clamp(s2 - ds2, min=0.0)) * (1 - U32)
+    s_hi = torch.sqrt(torch.clamp(s2 + ds2, min=0.0)) * (1 + U32)
+    live = s_hi > EXP_EPS * (1 - U32)
+    wc = torch.clamp(w, -1.0, 1.0)
+    ang = 2.0 * torch.acos(wc)
+    e_ang = 2 * mf._acos_err(wc, dw) + 4 * U32 * ang
+    zero = torch.zeros_like(w)[..., None]
+    out: List[mf.Cand] = [(zero, zero, s_lo <= EXP_EPS * (1 + U32))]
+    out.append((ang[..., None], e_ang[..., None], live & (ang - e_ang < mf.PI32)))
+    wa = ang - 2 * math.pi
+    out.append((wa[..., None], (e_ang + abs(mf.TWO_PI32 - 2 * math.pi) + U32 * wa.abs())[..., None], live & (ang + e_ang >= math.pi)))
+    return out
+
+
+def _sq_interval(cands: List[mf.Cand]):
+    """The union over the allowed candidates of [(|a| - t)^2, (|a| + t)^2] (one more rounding for the fp32 square): (mid, half-width)."""
+    lo = hi = None
+    for v, t, ok in cands:
+        a, e = v[..., 0].abs(), t[..., 0]
+        l, h = torch.clamp(a - e, min=0.0) ** 2 * (1 - U32), (a + e) ** 2 * (1 + U32)
+        l = torch.where(ok, l, torch.full_like(l, math.inf))
+        h = torch.where(ok, h, torch.full_like(h, -math.inf))
+        lo, hi = (l, h) if lo is None else (torch.minimum(lo, l), torch.maximum(hi, h))
+    return 0.5 * (lo + hi), 0.5 * (hi - lo)
+
+
+def _sum_sq(d, td):
+    """sum over bodies of |d_j|^2 for fp32 differences d [n, B, 3] known within td: the squares (2 |d| td + td^2), sq3's three
+    roundings, and the B roundings of the column's running sum."""
+    sq = (d * d).sum(-1)
+    S = sq.sum(-1)
+    return S, ((2 * d.abs() * td + td * td).sum(-1) + 3 * U32 * sq).sum(-1) + d.shape[1] * U32 * S
+
+
+def _mean_exp(S, tS, cnt: int, k: float):
+    """expf(-k (S * fp32(1 / cnt))) against exp(-k S / cnt): the constant's rounding (u32 relative), the two products, exp_neg."""
+    c, kk = f32r(1.0 / cnt), f32r(k)
+    e = S / cnt
+    te = tS * c + abs(c - 1.0 / cnt) * S + U32 * e
+    a = kk * e
+    return exp_neg(a, kk * te + U32 * a)
+
+
+def im_pose(tb, ids, t32, goff):
+    """query_ref at fp32 times t32 with oracle.pulse_oracle.frame_blend's blend as the exact operand, plus the global frame rows.
+    A clip of one frame has length 0, and at time 0 the phase is 0 / 0: frame_blend_rn's fmaxf / fminf take the NaN to phase 0, where
+    the float reference would index with NaN.  Such a clip's rows are 0 and 0 whatever its length, so it is queried with length 1."""
+    from oracle import pulse_oracle as po
+    tb = {k: v for k, v in tb.items() if k != "motion_aa"}
+    tb["lengths"] = torch.where(tb["lengths"] == 0, torch.ones_like(tb["lengths"]), tb["lengths"])
+    i0, i1, b = po.frame_blend(t32, tb["lengths"][ids], tb["num_frames"][ids], tb["dt"][ids])
+    q = mf.query_ref(tb, ids, t32, b, goff)
+    q["f0"], q["f1"] = i0 + tb["length_starts"][ids], i1 + tb["length_starts"][ids]
+    return q
+
+
+def im_step_ref(tb, inp: Dict[str, object], cfg) -> Dict[str, object]:
+    """One pulse_im_step launch on the envs of inp (CPU): body [n, 24, 13], progress (as read) [n], motion_ids, start, offset [n],
+    goff [n, 3], cycle [n] int32 or None, recovery [n] int32 or None, dof_force / dof_vel [n, 69] or None, term [24] fp32, mask (int),
+    flags (PULSE_STEP_* bits, ADVANCE included).  cfg: an ImConfig (dt, reward_specs, power_coefficient, enable_early_termination,
+    cycle_motion, max_episode_length, use_mean_reset).  tb: the float32 tables as a dict.
+    Returns the exact planner outputs ("pass_time", "progress", "reset", "terminate", "fdones"), the reward links, the fp64 reset links,
+    the observation pieces ("self", "task" {piece: (ref [n, 24, w], tol)}, "obs ill"), the side buffers and the four-row count."""
+    flags = int(inp["flags"])
+    do_rew, do_reset, do_obs = bool(flags & REW), bool(flags & RST), bool(flags & OBS)
+    need_t = do_rew or do_reset
+    body = inp["body"].float()[:, :24]
+    b64 = f64(body)
+    n = body.shape[0]
+    ids = inp["motion_ids"].long()
+    prog = inp["progress"].long() + (1 if flags & ADVANCE else 0)
+    rec = torch.zeros(n, dtype=torch.bool)
+    if do_reset and inp.get("recovery") is not None:
+        rec = inp["recovery"].int() > 0
+    start, off, goff = inp["start"].float(), inp["offset"].float(), inp["goff"].float()
+    t_rew = motion_time32(prog, cfg.dt, start, off)
+    t_obs = motion_time32(prog + 1 - rec.long(), cfg.dt, start, off)
+    mlen = tb["lengths"][ids].float()
+    out: Dict[str, object] = {"t_rew": t_rew, "t_obs": t_obs}
+    pos, rot, vel, ang = b64[..., 0:3], b64[..., 3:7], b64[..., 7:10], b64[..., 10:13]
+    amb_rows = torch.zeros(n, dtype=torch.bool)
+    if need_t:
+        q1 = im_pose(tb, ids, t_rew, goff)
+        out["pass_time"] = (t_rew >= mlen).to(torch.uint8)
+    if do_obs:
+        q2 = im_pose(tb, ids, t_obs, goff)
+    if need_t and do_obs:
+        rows = torch.stack([q1["f0"], q1["f1"], q2["f0"], q2["f1"]], 1)
+        srt = rows.sort(1).values
+        out["four"] = int(((srt[:, 1:] != srt[:, :-1]).sum(1) == 3).sum())
+    # progress counter: the planner's advance, the recovering env's pull-back
+    progress = inp["progress"].long().clone()
+    if flags & ADVANCE:
+        progress = torch.where(rec, progress, prog)
+    progress = torch.where(rec, prog - 1, progress)
+    out["progress"] = progress
+
+    if do_rew:
+        spec = cfg.reward_specs
+        rp, trp = q1["rg_pos"]
+        d = rp - pos
+        S, tS = _sum_sq(d, trp + U32 * d.abs())
+        r_pos = _mean_exp(S, tS, 72, spec["k_pos"])
+        raw = [r_pos]
+        for key, x in (("body_vel", vel), ("body_ang_vel", ang)):
+            v, tv = q1[key]
+            d = v - x
+            raw.append(_mean_exp(*_sum_sq(d, tv + U32 * d.abs()), 72, spec["k_vel" if key == "body_vel" else "k_ang_vel"]))
+        # rotation: the union of theta^2 over every allowed slerp candidate and angle branch
+        mids, halves = [], []
+        th_c: List[mf.Cand] = []
+        for v, t, ok in q1["rb_rot"]:
+            dq, tdq = rel_rot(v, t, rot)
+            th_c += [(a, ta, ok & oa) for a, ta, oa in angle_cands(dq[..., 3], tdq[..., 3])]
+        mid, half = _sq_interval(th_c)
+        Sr = mid.sum(-1)
+        r_rot = _mean_exp(Sr, half.sum(-1) + 24 * U32 * (mid + half).sum(-1), 24, spec["k_rot"])
+        _, _, slerp_amb = rf.primary(q1["rb_rot"])
+        out["rot amb"] = slerp_amb.any(-1)
+        amb_rows |= out["rot amb"]
+        raw = [raw[0], r_rot, raw[1], raw[2]]
+        w = [f32r(spec[k]) for k in ("w_pos", "w_rot", "w_vel", "w_ang_vel")]
+        tot = sum(wi * r for wi, (r, _) in zip(w, raw))
+        ttot = sum(wi * t for wi, (_, t) in zip(w, raw)) + 5 * U32 * sum(wi * r.abs() for wi, (r, _) in zip(w, raw))
+        power = None
+        if inp.get("dof_force") is not None:
+            c = f32r(cfg.power_coefficient)
+            s, ts_ = dof_power(inp["dof_force"], inp["dof_vel"], adds=2 + 23)
+            live = prog > 3
+            pw = torch.where(live, -c * s, torch.zeros_like(s))
+            tpw = torch.where(live, c * ts_ + U32 * c * s, torch.zeros_like(s))
+            power = (pw, tpw)
+            tot = tot + pw
+            ttot = ttot + tpw + 5 * U32 * pw.abs()
+        out["raw"] = raw + ([power] if power is not None else [])
+        out["reward"] = (tot, ttot + U32 * tot.abs())
+
+    if do_reset:
+        mask = int(inp["mask"])
+        bits = torch.tensor([(mask >> j) & 1 for j in range(24)], dtype=torch.bool)
+        term = inp["term"].float()
+        fr = tb["gts"]
+        d32 = reset_dist32(fr[q1["f0"]], fr[q1["f1"]], q1["blend"][:, None, None], goff[:, None, :], body[..., 0:3])
+        rp, trp = q1["rg_pos"]
+        dd = pos - rp
+        d64 = dd.norm(dim=-1)
+        td64 = (trp + U32 * dd.abs()).norm(dim=-1) + 3 * U32 * d64
+        out["dist"] = (d32, d64, td64)
+        cnt = bin(mask & 0xFFFFFF).count("1")
+        first = (mask & -mask).bit_length() - 1
+        if cfg.use_mean_reset:
+            m32 = torch.zeros(n, dtype=torch.float32)
+            for j in range(24):
+                m32 = m32 + torch.where(bits[j], d32[:, j], torch.zeros_like(m32))
+            fell = m32 / torch.tensor(float(cnt), dtype=torch.float32) > term[first]
+            md = (d64 * bits).sum(-1) / cnt
+            tmd = ((td64 * bits).sum(-1) + 24 * U32 * (d64 * bits).sum(-1)) / cnt + U32 * md
+            t0 = float(term[first])
+            fell_lo, fell_hi = md - tmd > t0, md + tmd > t0
+        else:
+            fell = ((d32 > term[None]) & bits[None]).any(-1)
+            fell_lo = ((d64 - td64 > f64(term)[None]) & bits[None]).any(-1)
+            fell_hi = ((d64 + td64 > f64(term)[None]) & bits[None]).any(-1)
+        pass_time = (prog >= int(cfg.max_episode_length) - 1) if cfg.cycle_motion else (t_rew >= mlen)
+        cyc = inp["cycle"].int() if inp.get("cycle") is not None else torch.zeros(n, dtype=torch.int32)
+        hold = (~pass_time & (cyc > 0)) | rec
+        live = (prog > 1) & bool(cfg.enable_early_termination) & ~hold
+
+        def decide(f):
+            t = (f & live).long()
+            return torch.where(hold, torch.zeros_like(t), torch.where(pass_time, torch.ones_like(t), t)), t
+
+        out["reset"], out["terminate"] = decide(fell)
+        out["term_lo"], out["term_hi"] = decide(fell_lo)[1], decide(fell_hi)[1]
+        out["fdones"] = out["reset"].float()
+
+    if do_obs:
+        out["self"] = self_obs_ref(body, True)
+        hd = heading(rot[:, 0], True)
+        hs, hc, dth = _h(hd, 1)
+        rp, trp = q2["rg_pos"]
+        rv, trv = q2["body_vel"]
+        rw, trw = q2["body_ang_vel"]
+        rq, trq, amb2 = rf.primary(q2["rb_rot"])
+        rel = lambda a, ta, b_: (a - b_, ta + U32 * (a - b_).abs())
+        task = {"dp": yaw_apply(hs, hc, dth, *rel(rp, trp, pos)),
+                "dv": yaw_apply(hs, hc, dth, *rel(rv, trv, vel)),
+                "dw": yaw_apply(hs, hc, dth, *rel(rw, trw, ang)),
+                "lp": yaw_apply(hs, hc, dth, *rel(rp, trp, pos[:, 0:1].expand_as(pos)))}
+        dq, tdq = rel_rot(rq, trq, rot)
+        task["drot"] = rf.six_ref(*yaw_qmul_right(hs, hc, dth, *rf.yaw_qmul(hs, hc, dth, dq, tdq)))
+        task["lrot"] = rf.six_ref(*rf.yaw_qmul(hs, hc, dth, rq, trq))
+        out["task"] = task
+        out["obs ill"] = hd[3] | amb2.any(-1)
+        amb_rows |= out["obs ill"]
+        out["ref_body_pos"], out["ref_body_vel"] = q2["rg_pos"], q2["body_vel"]
+        out["ref_body_rot"], out["ref_dof_pos"] = q2["rb_rot"], q2["dof_pos"]
+    out["amb"] = amb_rows
+    return out
+
+
+def im_task_block(ref: Dict[str, object], track: Optional[tuple] = None):
+    """The task block of the row as (ref, tol) [n, width] plus {piece: (first column, last column)}: the 576-float v6 block, or the
+    tracked block of track = (version, ids), whose columns humanoid_im.track_columns selects from the v6 block."""
+    from pulse_b200.humanoid_im import TRACK_BLOCKS, track_columns
+    n = ref["task"]["dp"][0].shape[0]
+    full = torch.cat([ref["task"][k][0].reshape(n, -1) for k, _ in IM_PIECES], 1)
+    tol = torch.cat([loose(ref["task"][k][1], ref["obs ill"]).reshape(n, -1) for k, _ in IM_PIECES], 1)
+    widths = dict(IM_PIECES)
+    if track is None:
+        cols, names, K = torch.arange(IM_TASK), [k for k, _ in IM_PIECES], 24
+    else:
+        version, tids = track
+        cols, K = track_columns(version, tids), len(tids)
+        at = {24 * sum(wd for _, wd in IM_PIECES[:i]): k for i, (k, _) in enumerate(IM_PIECES)}     # v6 offset -> piece
+        names = [at[off] for off, _ in TRACK_BLOCKS[version]]
+    spans, c0 = {}, 0
+    for k in names:
+        spans[k] = (c0, c0 + widths[k] * K)
+        c0 += widths[k] * K
+    return full[:, cols], tol[:, cols], spans
+
+
+def check_im_step(rep: Optional[Report], tag: str, got: Dict[str, torch.Tensor], ref: Dict[str, object], flags: int,
+                  track: Optional[tuple] = None, built: Optional[torch.Tensor] = None) -> None:
+    """A step's outputs on the envs of the reference (CPU tensors: obs [n, >= width], self_obs [n, 358] or None, rew [n], raw
+    [n, >= 4] or None, reset / terminate int64, pass_time uint8, progress int64, fdones float or None, ref_body_* / ref_dof_pos or
+    None) against im_step_ref, link by link."""
+    if flags & (REW | RST):
+        check_exact(rep, f"{tag} pass_time", got["pass_time"], ref["pass_time"])
+    if got.get("progress") is not None:
+        check_exact(rep, f"{tag} progress", got["progress"], ref["progress"])
+    if flags & REW:
+        names = ("pos", "rot", "vel", "ang vel", "power")
+        if got.get("raw") is not None:
+            for c, (r, t) in enumerate(ref["raw"]):
+                check(rep, f"{tag} reward raw {names[c]}", got["raw"][:, c], r, t)
+        check(rep, f"{tag} reward", got["rew"], *ref["reward"])
+        rf.limit_share(rep, f"{tag} reward rot slerp branch", ref["rot amb"], built)
+    if flags & RST:
+        d32, d64, td64 = ref["dist"]
+        check(rep, f"{tag} reset distance (fp32 restatement)", d32, d64, td64)
+        term = got["terminate"].long()
+        wrong = (term != ref["term_lo"]) & (term != ref["term_hi"])
+        rep is not None and rep.add(f"{tag} terminate (fp64 decided)", float(wrong.any()))
+        if wrong.any():
+            k = int(torch.nonzero(wrong)[0])
+            raise BoundError(f"{tag} terminate (fp64 decided): {int(wrong.sum())} rows contradict the float64 distances, first env {k}: "
+                             f"got {int(term[k])}, allowed {int(ref['term_lo'][k])} / {int(ref['term_hi'][k])}")
+        rf.limit_share(rep, f"{tag} terminate within the distance bound", ref["term_lo"] != ref["term_hi"], built)
+        check_exact(rep, f"{tag} terminate", term, ref["terminate"])
+        check_exact(rep, f"{tag} reset", got["reset"], ref["reset"])
+        if got.get("fdones") is not None:
+            check_exact(rep, f"{tag} fdones", got["fdones"], ref["fdones"])
+    if flags & OBS:
+        obs = got["obs"]
+        check_self(rep, tag, obs[:, :IM_SELF], ref["self"], built)
+        if got.get("self_obs") is not None:
+            check_exact(rep, f"{tag} self_obs_buf = obs[:, :358]", got["self_obs"], obs[:, :IM_SELF])
+        r, t, spans = im_task_block(ref, track)
+        for k, (a, b) in spans.items():
+            check(rep, f"{tag} task {k}", obs[:, IM_SELF + a:IM_SELF + b], r[:, a:b], t[:, a:b])
+        rf.limit_share(rep, f"{tag} task heading / slerp branch", ref["obs ill"], built)
+        if got.get("ref_body_pos") is not None:
+            check(rep, f"{tag} ref body pos", got["ref_body_pos"], *ref["ref_body_pos"])
+            check(rep, f"{tag} ref body vel", got["ref_body_vel"], *ref["ref_body_vel"])
+            bb = None if built is None else built[:, None]
+            mf.check_branches(rep, f"{tag} ref body rot", got["ref_body_rot"], ref["ref_body_rot"], built=bb)
+            mf.check_branches(rep, f"{tag} ref dof pos", got["ref_dof_pos"].reshape(-1, 23, 3), ref["ref_dof_pos"], built=bb)
+
+
+# ------------------------------------------------------------------------------------------------------------------ task observation
+# (piece, width, columns per unit of J, constant) in each version's layout; "flat" layouts index items it = t J + j over all samples,
+# "per_t" layouts repeat the pieces per sample with a stride of the listed total
+TASK_LAYOUT = {
+    1: ("flat", [("dp", 3, 0, 0), ("drot", 6, 3, 0), ("dv", 3, 9, 0), ("dw", 3, 12, 0)]),
+    2: ("flat", [("dp", 3, 0, 0), ("drot", 6, 3, 0), ("dv", 3, 9, 0), ("dw", 3, 12, 0)]),
+    3: ("flat", [("dp", 3, 0, 0), ("drot", 6, 3, 0)]),
+    6: ("per_t", [("dp", 3, 0, 0), ("drot", 6, 3, 0), ("dv", 3, 9, 0), ("dw", 3, 12, 0), ("lp", 3, 15, 0), ("lrot", 6, 18, 0)]),
+    7: ("per_t", [("dp", 3, 0, 0), ("dv", 3, 3, 0), ("lp", 3, 6, 0)]),
+    8: ("per_t", [("dp", 3, 0, 0), ("drot", 6, 3, 0), ("dv", 3, 9, 0), ("dw", 3, 12, 0), ("lp", 3, 15, 0), ("lrot", 6, 18, 0),
+                  ("lv", 3, 24, 0), ("lw", 3, 27, 0)]),
+    9: ("per_t", [("dp", 3, 0, 0), ("drot", 6, 3, 0), ("lp", 3, 9, 6), ("lrot", 6, 12, 6)]),
+}
+
+
+def task_obs_size(version: int, J: int, T: int) -> int:
+    return {1: 15 * T * J, 2: 15 * J + 3 * (J - 1), 3: 9 * T * J, 6: 24 * T * J, 7: 9 * T * J, 8: 30 * J, 9: T * (18 * J + 6)}[version]
+
+
+def task_obs_ref(version: int, T: int, track_ids, upright: bool, body, ref_pos, ref_rot, ref_vel, ref_ang, dof_pos=None,
+                 ref_dof=None) -> Dict[str, object]:
+    """pulse_im_task_obs on the fp32 arrays it read: body [n, 24, 13], ref_* [n T, 24, .] (row e T + t), dof_pos / ref_dof [n, 69].
+    Returns {"links": [(name, columns [k], ref [n, k], tol [n, k])], "exact": [(name, columns, ref)], "ill": rows, "size"}."""
+    b = f64(body)[:, :24]
+    n = b.shape[0]
+    ids = torch.as_tensor(list(track_ids), dtype=torch.long)
+    J = len(ids)
+    hd = heading(b[:, 0, 3:7], upright)
+    hs, hc, dth = _h(hd, 2)
+    g = lambda x, w: f64(x).reshape(n, T, 24, w)[:, :, ids]
+    rp, rq, rv, rw = g(ref_pos, 3), g(ref_rot, 4), g(ref_vel, 3), g(ref_ang, 3)
+    bt = b[:, ids][:, None]
+    p, q, v, w = (bt[..., a:c].expand(n, T, J, c - a) for a, c in ((0, 3), (3, 7), (7, 10), (10, 13)))
+    p_root = b[:, 0, 0:3][:, None, None].expand_as(p)
+    diff = lambda a, c: yaw_apply(hs, hc, dth, a - c, U32 * (a - c).abs())
+    pieces = {"dp": diff(rp, p), "dv": diff(rv, v), "dw": diff(rw, w), "lp": diff(rp, p_root),
+              "lv": yaw_apply(hs, hc, dth, rv, torch.zeros_like(rv)), "lw": yaw_apply(hs, hc, dth, rw, torch.zeros_like(rw))}
+    if version != 7:
+        dq, tdq = rel_rot(rq, torch.zeros_like(rq), q)
+        pieces["drot"] = rf.six_ref(*yaw_qmul_right(hs, hc, dth, *rf.yaw_qmul(hs, hc, dth, dq, tdq)))
+        pieces["lrot"] = rf.six_ref(*rf.yaw_qmul(hs, hc, dth, rq, torch.zeros_like(rq)))
+    kind, plist = TASK_LAYOUT[version]
+    stride = {6: 24 * J, 7: 9 * J, 8: 30 * J, 9: 18 * J + 6}.get(version, 0)
+    tt = torch.arange(T)[:, None, None]
+    jj = torch.arange(J)[None, :, None]
+    links = []
+    for name, wd, cj, c0 in plist:
+        cc = torch.arange(wd)[None, None, :]
+        if kind == "flat":
+            cols = cj * T * J + wd * (tt * J + jj) + cc
+        else:
+            cols = tt * stride + cj * J + c0 + wd * jj + cc
+        r, t = pieces[name]
+        links.append((name, cols.reshape(-1), r.reshape(n, -1), loose(t, hd[3]).reshape(n, -1)))
+    if version == 9:                                    # root = tracked body 0: its velocity pair once per sample
+        for name, key, c0 in (("root dv", "dv", 9 * J), ("root dw", "dw", 9 * J + 3)):
+            r, t = pieces[key]
+            cols = torch.arange(T)[:, None] * stride + c0 + torch.arange(3)[None, :]
+            links.append((name, cols.reshape(-1), r[:, :, 0].reshape(n, -1), loose(t[:, :, 0], hd[3]).reshape(n, -1)))
+    exact = []
+    if version == 2:
+        d0 = (3 * (ids[1:] - 1))[:, None] + torch.arange(3)[None, :]
+        want = r32(f64(ref_dof)[:, d0.reshape(-1)] - f64(dof_pos)[:, d0.reshape(-1)])
+        exact.append(("dof", 15 * J + torch.arange(3 * (J - 1)), want))
+    return {"links": links, "exact": exact, "ill": hd[3], "size": task_obs_size(version, J, T)}
+
+
+def check_task_obs(rep: Optional[Report], tag: str, obs: torch.Tensor, ref: Dict[str, object], built: Optional[torch.Tensor] = None) -> None:
+    """pulse_im_task_obs rows [n, >= size] against task_obs_ref, one link per piece."""
+    for name, cols, r, t in ref["links"]:
+        check(rep, f"{tag} {name}", obs[:, cols], r, t)
+    for name, cols, want in ref["exact"]:
+        check_exact(rep, f"{tag} {name}", obs[:, cols], want)
+    rf.limit_share(rep, f"{tag} heading", ref["ill"], built)
