@@ -33,6 +33,12 @@ struct SmplLayout {
   __device__ static __forceinline__ int kept_joint(int i) { return c_kept_joint[i]; }
   __device__ static __forceinline__ int key_body(int i) { return c_key_body[i]; }
 };
+// The SMPL reach step: SmplLayout's geometry with the reach task's argument struct.
+struct SmplReachLayout : SmplLayout {
+  static constexpr bool kPower = false;
+  static constexpr unsigned kTasks = 1u << PULSE_ZTASK_REACH;
+  using StepArgs = pulse_reach_step_args_t;
+};
 struct SmplxLayout {
   static constexpr int kBodies = PULSE_SMPLX_BODIES, kDofs = PULSE_SMPLX_DOF, kSelfObs = PULSE_SMPLX_SELF_OBS;
   static constexpr int kFrameRec = PULSE_SMPLX_FRAME_REC, kAuxRec = PULSE_SMPLX_AUX_REC;
@@ -59,7 +65,7 @@ static_assert(1 + 3 * (PULSE_SMPLX_BODIES - 1) + 12 * PULSE_SMPLX_BODIES == PULS
 // self observation of B bodies [root height | (B-1) x position | B x six-D rotation | B x velocity | B x angular velocity] (358 floats
 // for SMPL), all in the heading frame.  The heights p.z and p_root.z are taken from the task's reference (the ground, or the
 // terrain's center height); (hs, hc) is the heading's half-angle sine / cosine and yr = make_yaw of the inverse heading.  The
-// imitation and reach step kernels write the same layout inline (see im_step.cu).
+// imitation step kernel writes the same layout inline (see im_step.cu).
 template <int B = PULSE_NUM_BODIES>
 __device__ __forceinline__ void store_self_obs(float* o, int j, Vec3 p, Vec3 p_root, Quat q, Vec3 v, Vec3 w, float hs, float hc, Yaw yr) {
   if (j == 0) o[0] = p_root.z;

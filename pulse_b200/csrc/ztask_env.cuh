@@ -1,62 +1,13 @@
-// One env of the latent-space tasks' post-physics step (reach; speed / strike; the SMPL-X speed, reach and strike tasks), one warp per
-// env, lane = body:
-// self observation, task observation, reward and reset.  Shared by the step and list-observation kernels (ztask_step.cu) and by the rollout step kernels that
-// write into experience-buffer slices (ztask_rollout.cu), so all of them produce the same rows bit for bit.
+// One env of the latent-space tasks' post-physics step (the SMPL reach, speed and strike tasks; the SMPL-X speed, reach and strike
+// tasks), one warp per env, lane = body: self observation, task observation, reward and reset.  ztask_kernel (ztask_step.cu) runs it
+// in its step, list-observation and rollout modes, so all of them produce the same rows bit for bit.
 #pragma once
 #include "humanoid_obs.cuh"
 
 namespace pulse {
 
-// One env of the reach step.  kObsOnly: the observation alone (the reset envs' _compute_observations(env_ids)).
-template <bool kObsOnly>
-__device__ __forceinline__ void reach_env(const pulse_reach_step_args_t& a, long long e, int lane) {
-  const int j = lane;
-  const bool body = j < PULSE_NUM_BODIES;
-  const float* bs = a.body_state + e * a.body_env_stride + (body ? j : 0) * 13;
-  Vec3 p = {bs[0], bs[1], bs[2]}, v = {bs[7], bs[8], bs[9]}, w = {bs[10], bs[11], bs[12]};
-  Quat q = {bs[3], bs[4], bs[5], bs[6]};
-  const Vec3 p_root = {__shfl_sync(kFull, p.x, 0), __shfl_sync(kFull, p.y, 0), __shfl_sync(kFull, p.z, 0)};
-  const Quat q_root = {__shfl_sync(kFull, q.x, 0), __shfl_sync(kFull, q.y, 0), __shfl_sync(kFull, q.z, 0), __shfl_sync(kFull, q.w, 0)};
-  float hs, hc;
-  heading_half(q_root, hs, hc);
-  const Yaw yr = make_yaw(Quat{0.0f, 0.0f, -hs, hc});
-  float* o = a.obs_buf + e * a.obs_stride;
-  if (body) {  // store_self_obs's layout written out, for the reason given in im_step.cu
-    if (j == 0) o[0] = p_root.z;
-    else {
-      const Vec3 lp = yaw_rot(yr, p - p_root);
-      o[1 + 3 * (j - 1)] = lp.x; o[2 + 3 * (j - 1)] = lp.y; o[3 + 3 * (j - 1)] = lp.z;
-    }
-    float six[6];
-    qsix(yaw_mul_left(-hs, hc, q), six);
-#pragma unroll
-    for (int i = 0; i < 6; ++i) o[70 + 6 * j + i] = six[i];
-    const Vec3 lv = yaw_rot(yr, v), lw = yaw_rot(yr, w);
-    o[214 + 3 * j] = lv.x; o[215 + 3 * j] = lv.y; o[216 + 3 * j] = lv.z;
-    o[286 + 3 * j] = lw.x; o[287 + 3 * j] = lw.y; o[288 + 3 * j] = lw.z;
-  }
-  const Vec3 tar = {a.tar_pos[3 * e], a.tar_pos[3 * e + 1], a.tar_pos[3 * e + 2]};
-  const FallFlags fall = fall_flags(a, e, j, body, p.z);
-  const bool any_contact = __any_sync(kFull, fall.contact), any_height = __any_sync(kFull, fall.height);
-  // the reach body's position, broadcast
-  const int rb = a.reach_body_id;
-  const Vec3 pr = {__shfl_sync(kFull, p.x, rb), __shfl_sync(kFull, p.y, rb), __shfl_sync(kFull, p.z, rb)};
-  if (lane == 0) {
-    const Vec3 lt = yaw_rot(yr, tar - p_root);  // compute_location_observations (humanoid_reach.py:224-236)
-    o[PULSE_SELF_OBS + 0] = lt.x; o[PULSE_SELF_OBS + 1] = lt.y; o[PULSE_SELF_OBS + 2] = lt.z;
-    if constexpr (!kObsOnly) {
-      const Vec3 d = tar - pr;                  // compute_reach_reward (:238-250)
-      a.rew_buf[e] = expf(-4.0f * (d.x * d.x + d.y * d.y + d.z * d.z));
-      const long long prog = a.progress_buf[e];
-      const long long term = (any_contact && any_height && prog > 1) ? 1 : 0;
-      a.terminate_buf[e] = term;
-      a.reset_buf[e] = prog >= a.max_episode_length - 1 ? 1 : term;
-    }
-  }
-}
-
-// One env of the speed / strike step in body layout L (SmplLayout: speed and strike; SmplxLayout: speed; SmplxTargetLayout: reach and
-// strike).  kObsOnly: the observation alone.  Lane l holds bodies l and l + 32 (the second only where the layout has more than 32 bodies).
+// One env of the step in body layout L (SmplReachLayout: reach; SmplLayout: speed and strike; SmplxLayout: speed; SmplxTargetLayout:
+// reach and strike).  kObsOnly: the observation alone.  Lane l holds bodies l and l + 32 (the second only where the layout has more than 32 bodies).
 // ztask_is<L, K>: whether env work takes task kind K's branch -- a constant where the layout serves K alone or not at all.
 template <class L, int K>
 constexpr bool kServes = (L::kTasks >> K) & 1u;
@@ -133,12 +84,14 @@ __device__ __forceinline__ void ztask_env(const typename L::StepArgs& a, long lo
     }
   }
   if (lane == 0) {
-    const long long prog = a.progress_buf[e];
+    const long long prog = kObsOnly ? 0 : a.progress_buf[e];
     float vx = 0.0f, vy = 0.0f;
-    if (!ztask_is<L, PULSE_ZTASK_REACH>(a)) {   // the reach task has no prev_root_pos
-      const float* pr = a.prev_root_pos + 3 * e;
-      vx = (p_root.x - pr[0]) / a.dt;                                              // root_vel = delta_root_pos / dt
-      vy = (p_root.y - pr[1]) / a.dt;
+    if constexpr (!kObsOnly && L::kTasks != (1u << PULSE_ZTASK_REACH)) {   // the SMPL reach struct has no prev_root_pos and no dt
+      if (!ztask_is<L, PULSE_ZTASK_REACH>(a)) {
+        const float* pr = a.prev_root_pos + 3 * e;
+        vx = (p_root.x - pr[0]) / a.dt;                                            // root_vel = delta_root_pos / dt
+        vy = (p_root.y - pr[1]) / a.dt;
+      }
     }
     float* t = o + L::kSelfObs;
     bool failed = any_contact && any_height;
@@ -200,6 +153,7 @@ __device__ __forceinline__ void ztask_env(const typename L::StepArgs& a, long lo
       const bool tar_contact = fabsf(tc[0]) > 50.0f || fabsf(tc[1]) > 50.0f;
       failed = failed || (a.enable_early_termination && tar_contact && any_hard);
     }
+    // fall_flags raises no flag without early termination, so for reach and speed the first term only restates `failed`
     const long long term = (a.enable_early_termination && failed && prog > 1) ? 1 : 0;
     a.terminate_buf[e] = term;
     a.reset_buf[e] = prog >= a.max_episode_length - 1 ? 1 : term;

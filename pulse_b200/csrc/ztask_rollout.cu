@@ -3,17 +3,15 @@
 //   latent_post_kernel        the latent policy's sampling (policy_post_kernel's draws and arithmetic), neglogp, the de-normalised value
 //                             and z = prior_mu + a_z as bf16 into the decoder operand: pulse_policy_post + pulse_vae_reparam in one launch;
 //   ztask_pre_physics_kernel  PD targets from the decoder output, prev_root_pos, and _update_task of the due envs with draws injected or
-//                             made here (Philox index plane e + 3 * 2^32);
-//   reach_rollout_kernel /    progress_buf += 1, then the per-env step code of ztask_env.cuh into the next step's observation slice and
-//   ztask_rollout_kernel      the step's reward row, then dones = float(reset); ztask_rollout_kernel<SmplxLayout> is the SMPL-X
-//                             speed task's (pulse_smplx_speed_rollout_step), ztask_rollout_kernel<SmplxTargetLayout> the SMPL-X
-//                             reach and strike tasks' (pulse_smplx_target_rollout_step).
+//                             made here (Philox index plane e + 3 * 2^32).
+// The rollout step kernels (progress_buf += 1, the step into the experience-buffer slices, dones = float(reset)) are ztask_step.cu's
+// ztask_kernel in its rollout mode.
 // The entry points, argument structs and the Philox word layout are documented in include/pulse_b200.h.
 #include <cuda_bf16.h>
 
 #include "philox.cuh"
+#include "pulse_common.cuh"
 #include "value_unnorm.cuh"
-#include "ztask_env.cuh"
 
 namespace pulse {
 namespace {
@@ -92,28 +90,6 @@ __global__ void __launch_bounds__(256) ztask_pre_physics_kernel(const pulse_ztas
   }
 }
 
-// progress_buf += 1 (humanoid.py:1317) by the lane that reads it back in the per-env code, then the step, then the done flag.
-__global__ void __launch_bounds__(256) reach_rollout_kernel(const pulse_reach_step_args_t a, float* __restrict__ dones, long long n) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  long long* progress = const_cast<long long*>(reinterpret_cast<const long long*>(a.progress_buf));
-  for (long long e = blockIdx.x * 8ll + warp; e < n; e += 8ll * gridDim.x) {
-    if (lane == 0) progress[e] += 1;
-    reach_env<false>(a, e, lane);
-    if (lane == 0) dones[e] = static_cast<float>(a.reset_buf[e]);
-  }
-}
-
-template <class L>
-__global__ void __launch_bounds__(256) ztask_rollout_kernel(const typename L::StepArgs a, float* __restrict__ dones, long long n) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  long long* progress = const_cast<long long*>(reinterpret_cast<const long long*>(a.progress_buf));
-  for (long long e = blockIdx.x * 8ll + warp; e < n; e += 8ll * gridDim.x) {
-    if (lane == 0) progress[e] += 1;
-    ztask_env<L, false>(a, e, lane);
-    if (lane == 0) dones[e] = static_cast<float>(a.reset_buf[e]);
-  }
-}
-
 }  // namespace
 }  // namespace pulse
 
@@ -157,76 +133,5 @@ extern "C" int pulse_ztask_pre_physics(const pulse_ztask_pre_physics_args_t* arg
   if (num_envs == 0) return PULSE_OK;
   ztask_pre_physics_kernel<<<grid_for(num_envs * a.dofs, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, (long long)num_envs);
   PULSE_LAUNCH_OK("ztask_pre_physics_kernel");
-  return PULSE_OK;
-}
-
-extern "C" int pulse_reach_rollout_step(const pulse_reach_step_args_t* args, float* dones, int64_t num_envs, void* stream) {
-  using namespace pulse;
-  PULSE_REQUIRE(args && dones, "pulse_reach_rollout_step: null args / dones");
-  const pulse_reach_step_args_t& a = *args;
-  PULSE_REQUIRE(a.body_state && a.tar_pos && a.progress_buf && a.obs_buf && a.rew_buf && a.reset_buf && a.terminate_buf,
-                "pulse_reach_rollout_step: null buffer");
-  PULSE_REQUIRE(num_envs > 0 && a.body_env_stride >= 24 * 13 && a.obs_stride >= PULSE_REACH_OBS, "pulse_reach_rollout_step: bad strides");
-  PULSE_REQUIRE(a.reach_body_id >= 0 && a.reach_body_id < 24, "pulse_reach_rollout_step: reach_body_id out of range");
-  PULSE_REQUIRE(!a.enable_early_termination || a.termination_heights != nullptr, "pulse_reach_rollout_step: termination_heights required");
-  PULSE_REQUIRE(a.contact_forces == nullptr || a.contact_env_stride >= 24 * 3, "pulse_reach_rollout_step: bad contact stride");
-  reach_rollout_kernel<<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, dones, (long long)num_envs);
-  PULSE_LAUNCH_OK("reach_rollout_kernel");
-  return PULSE_OK;
-}
-
-extern "C" int pulse_ztask_rollout_step(const pulse_ztask_step_args_t* args, float* dones, int64_t num_envs, void* stream) {
-  using namespace pulse;
-  PULSE_REQUIRE(args && dones, "pulse_ztask_rollout_step: null args / dones");
-  const pulse_ztask_step_args_t& a = *args;
-  PULSE_REQUIRE(a.kind == PULSE_ZTASK_SPEED || a.kind == PULSE_ZTASK_STRIKE, "pulse_ztask_rollout_step: unknown task kind %d", a.kind);
-  PULSE_REQUIRE(num_envs > 0, "pulse_ztask_rollout_step: num_envs must be positive");
-  PULSE_REQUIRE(a.body_state && a.progress_buf && a.prev_root_pos && a.obs_buf && a.rew_buf && a.reset_buf && a.terminate_buf,
-                "pulse_ztask_rollout_step: null buffer");
-  PULSE_REQUIRE(a.dt > 0.0f, "pulse_ztask_rollout_step: dt must be positive");
-  PULSE_REQUIRE(a.body_env_stride >= 24 * 13, "pulse_ztask_rollout_step: body_env_stride %lld < 312", (long long)a.body_env_stride);
-  PULSE_REQUIRE(!a.enable_early_termination || a.termination_heights != nullptr, "pulse_ztask_rollout_step: termination_heights required");
-  PULSE_REQUIRE(a.contact_forces == nullptr || a.contact_env_stride >= 24 * 3, "pulse_ztask_rollout_step: bad contact stride");
-  if (a.kind == PULSE_ZTASK_SPEED) {
-    PULSE_REQUIRE(a.tar_speed != nullptr, "pulse_ztask_rollout_step: speed task needs tar_speed");
-    PULSE_REQUIRE(a.obs_stride >= PULSE_SPEED_OBS, "pulse_ztask_rollout_step: obs_stride %lld < %d", (long long)a.obs_stride, PULSE_SPEED_OBS);
-    PULSE_REQUIRE(a.dof_force == nullptr || (a.dof_vel != nullptr && a.dof_elem_stride >= 1), "pulse_ztask_rollout_step: power term needs dof_vel");
-    PULSE_REQUIRE(a.reward_raw == nullptr || a.raw_stride >= (a.dof_force ? 2 : 1), "pulse_ztask_rollout_step: raw_stride too small");
-  } else {
-    PULSE_REQUIRE(a.target_states && a.tar_contact_forces, "pulse_ztask_rollout_step: strike task needs target_states and tar_contact_forces");
-    PULSE_REQUIRE(a.obs_stride >= PULSE_STRIKE_OBS, "pulse_ztask_rollout_step: obs_stride %lld < %d", (long long)a.obs_stride, PULSE_STRIKE_OBS);
-  }
-  ztask_rollout_kernel<SmplLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, dones, (long long)num_envs);
-  PULSE_LAUNCH_OK("ztask_rollout_kernel");
-  return PULSE_OK;
-}
-
-namespace pulse {
-int check_smplx_speed_args(const pulse_smplx_speed_step_args_t* args, bool step, const char* who);   // ztask_step.cu
-}  // namespace pulse
-
-extern "C" int pulse_smplx_speed_rollout_step(const pulse_smplx_speed_step_args_t* args, float* dones, int64_t num_envs, void* stream) {
-  using namespace pulse;
-  const int st = check_smplx_speed_args(args, true, "pulse_smplx_speed_rollout_step");
-  if (st != PULSE_OK) return st;
-  PULSE_REQUIRE(dones != nullptr, "pulse_smplx_speed_rollout_step: null dones");
-  PULSE_REQUIRE(num_envs > 0, "pulse_smplx_speed_rollout_step: num_envs must be positive");
-  ztask_rollout_kernel<SmplxLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(*args, dones, (long long)num_envs);
-  PULSE_LAUNCH_OK("ztask_rollout_kernel<SmplxLayout>");
-  return PULSE_OK;
-}
-
-namespace pulse {
-int check_smplx_target_args(const pulse_smplx_target_step_args_t* args, bool step, const char* who);   // ztask_step.cu
-}  // namespace pulse
-
-extern "C" int pulse_smplx_target_rollout_step(const pulse_smplx_target_step_args_t* args, float* dones, int64_t num_envs, void* stream) {
-  using namespace pulse;
-  const int st = check_smplx_target_args(args, true, "pulse_smplx_target_rollout_step");
-  if (st != PULSE_OK) return st;
-  PULSE_REQUIRE(dones != nullptr, "pulse_smplx_target_rollout_step: null dones");
-  PULSE_REQUIRE(num_envs > 0, "pulse_smplx_target_rollout_step: num_envs must be positive");
-  ztask_rollout_kernel<SmplxTargetLayout><<<grid_for(num_envs, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(*args, dones, (long long)num_envs);
-  PULSE_LAUNCH_OK("ztask_rollout_kernel<SmplxTargetLayout>");
   return PULSE_OK;
 }

@@ -16,13 +16,6 @@ _WIDTHS = {("smpl", "reach"): 361, ("smpl", "speed"): 361, ("smpl", "strike"): 3
            ("smplx", "speed"): _lib.SMPLX_SPEED_OBS, ("smplx", "strike"): _lib.SMPLX_STRIKE_OBS}
 # per body layout: (self observation -> dof targets of the decoder, latent size or None = any)
 _LAYOUTS = {"smpl": (358, 69, None), "smplx": (_lib.SMPLX_SELF_OBS, _lib.SMPLX_DOF, 48)}
-# the step's entry points per (body layout, task kind): (step, list observation, rollout step)
-_REACH = ("pulse_reach_step", "pulse_reach_obs_list", "pulse_reach_rollout_step")
-_ZTASK = ("pulse_ztask_step", "pulse_ztask_obs_list", "pulse_ztask_rollout_step")
-_SMPLX_TARGET = ("pulse_smplx_target_step", "pulse_smplx_target_obs_list", "pulse_smplx_target_rollout_step")
-_ENTRIES = {("smpl", "reach"): _REACH, ("smpl", "speed"): _ZTASK, ("smpl", "strike"): _ZTASK,
-            ("smplx", "speed"): ("pulse_smplx_speed_step", "pulse_smplx_speed_obs_list", "pulse_smplx_speed_rollout_step"),
-            ("smplx", "reach"): _SMPLX_TARGET, ("smplx", "strike"): _SMPLX_TARGET}
 SIM_KEYS = ("body_state", "root_states", "dof_pos", "dof_vel", "progress_buf", "sampled_motion_ids", "motion_start_times")
 STRIKE_KEYS = ("target_states", "tar_contact_forces")
 
@@ -115,20 +108,11 @@ class ZTaskStepsB200(LatentStepsB200):
     def _step_args(self, obs: torch.Tensor, rew: torch.Tensor):
         """The task's step arguments with the outputs pointed at experience slices and the driver's reset / terminate words."""
         s, task = self.sim, self.task
-        if self.kind == "reach" and self.layout == "smpl":
-            a = task._step_args(s["body_state"], s["progress_buf"], s.get("contact_forces"))
-        else:
-            a = task._args(s["body_state"], s["progress_buf"], s.get("contact_forces"))
-        if self.kind == "speed" and self.layout == "smpl":
-            a.tar_speed = task._tar_speed.data_ptr()
-            if task.power_reward:
-                if s.get("dof_force") is None:
-                    raise _lib.PulseError("the speed task's power_reward needs sim['dof_force']")
-                a.dof_force, a.dof_force_stride, a.power_coefficient = s["dof_force"].data_ptr(), s["dof_force"].stride(0), task.power_coefficient
-                a.dof_vel, a.dof_env_stride, a.dof_elem_stride = s["dof_vel"].data_ptr(), s["dof_vel"].stride(0), s["dof_vel"].stride(1)
+        a = task._args(s["body_state"], s["progress_buf"], s.get("contact_forces"))
+        if self.kind == "speed":
+            task._power_args(a, s.get("dof_force"), s.get("dof_vel"))
         elif self.kind == "strike":
-            a.target_states, a.target_env_stride = s["target_states"].data_ptr(), s["target_states"].stride(0)
-            a.tar_contact_forces, a.tar_contact_env_stride = s["tar_contact_forces"].data_ptr(), s["tar_contact_forces"].stride(0)
+            task._target_args(a, s["target_states"], s["tar_contact_forces"])
         a.obs_buf, a.obs_stride, a.rew_buf = obs.data_ptr(), obs.stride(0), rew.data_ptr()
         a.reset_buf, a.terminate_buf = self.reset_buf.data_ptr(), self.terminate_buf.data_ptr()
         return a
@@ -155,7 +139,7 @@ class ZTaskStepsB200(LatentStepsB200):
         """`_compute_observations(env_ids)` of the reset envs into obses[:, t], then `_reset_task` (humanoid_amp_task.py:66-76)."""
         ws = self.reset_ws
         a = self._step_args(self.obses[:, t], self.rewards[t])
-        self._launch(_ENTRIES[(self.layout, self.kind)][1], C.byref(a), ws["env_list"].data_ptr(),
+        self._launch(self.task.entries[1], C.byref(a), ws["env_list"].data_ptr(),
                      ws["count"].data_ptr(), self.n)
         if self.kind != "strike":
             self.reset.reset_task(progress_buf=self.sim["progress_buf"], seed=self.reset_seed, offset=t, offset_dev=self.policy.rng_offset,
@@ -183,12 +167,12 @@ class ZTaskStepsB200(LatentStepsB200):
     def _env_step(self, t: int) -> None:
         """post_physics_step (humanoid.py:1315-1346): one fused launch."""
         a = self._step_args(self._next_obs(t), self.rewards[t])
-        self._launch(_ENTRIES[(self.layout, self.kind)][2], C.byref(a), self.dones[t].data_ptr(), self.n)
+        self._launch(self.task.entries[2], C.byref(a), self.dones[t].data_ptr(), self.n)
 
     def first_observation(self) -> None:
         """Observation of the initial state (Humanoid.reset -> _compute_observations at start-up): fills `obs_carry`."""
         a = self._step_args(self.obs_carry, self.rewards[0])
-        self._launch(_ENTRIES[(self.layout, self.kind)][0], C.byref(a), self.n)
+        self._launch(self.task.entries[0], C.byref(a), self.n)
         self.reset_buf.zero_()
         self.terminate_buf.zero_()
         self._amp_start()

@@ -1,5 +1,5 @@
-"""Teacher-forced float64 references of the task step kernels (ztask_env.cuh: reach_env and ztask_env<SmplLayout | SmplxLayout |
-SmplxTargetLayout>; terrain.cu: terrain_env; ztask_step.cu: reach_update_task_kernel; amp_obs.cu), each output with an element-wise
+"""Teacher-forced float64 references of the task step kernels (ztask_env.cuh: ztask_env<SmplReachLayout | SmplLayout |
+SmplxLayout | SmplxTargetLayout>; terrain.cu: terrain_env; ztask_step.cu: reach_update_task_kernel; amp_obs.cu), each output with an element-wise
 bound derived from the fp32 operations its kernel performs (the style of tests/fp64_ref.py and tests/reset_fp64.py, whose comparators,
 heading and rotation references are reused).
 
@@ -185,7 +185,7 @@ def rot_err_orders(tq: torch.Tensor) -> torch.Tensor:
 
 
 def ztask_ref(kind: int, B: int, inp: Dict[str, torch.Tensor], obs_only: bool = False) -> Dict[str, object]:
-    """One latent-task step (reach_env for B = 24 and kind REACH, ztask_env otherwise) on inputs `inp` (CPU tensors):
+    """One latent-task step (ztask_env in the layout of B and kind) on inputs `inp` (CPU tensors):
       body [n, B, 13], progress [n], and as the kind needs: contact [n, B, 3] (or None), term_h [B], contact_mask, strike_mask (ints),
       early (bool), max_len, prev [n, 3], dt, tar_speed [n], dof_force / dof_vel [n, 69] (or None), power_c, tar_pos [n, 3], reach_id,
       target [n, 13], tar_contact [n, 3].

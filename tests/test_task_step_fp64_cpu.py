@@ -1,6 +1,6 @@
 """The task steps' float64 references (tests/step_fp64.py) have teeth: a float32 CPU simulation of each step kernel passes every link,
 and a simulation with one defect fails the link it breaks with BoundError naming it.  The simulations restate the arithmetic of
-ztask_env.cuh (reach_env, ztask_env for the SMPL, SMPL-X speed and SMPL-X reach / strike layouts) and terrain.cu / terrain_height.cuh
+ztask_env.cuh (ztask_env for the SMPL reach, SMPL speed / strike, SMPL-X speed and SMPL-X reach / strike layouts) and terrain.cu / terrain_height.cuh
 (terrain_env, whose _rn intrinsics are the round-to-nearest float32 operations torch performs on the CPU) in float32 torch operations.
 The input generators (with the built edge envs) are shared with tests/test_gpu_task_step_fp64.py."""
 import math
@@ -161,7 +161,7 @@ def self_obs32(body, upright, zshift=None):
 
 
 def sim_ztask(kind: int, B: int, inp, mut=None):
-    """ztask_env<L> / reach_env in float32: {"obs", "rew", "raw", "reset", "terminate"}."""
+    """ztask_env<L> in float32: {"obs", "rew", "raw", "reset", "terminate"}."""
     body = inp["body"].float()[:, :B]
     n = body.shape[0]
     root, rq = body[:, 0, 0:3], body[:, 0, 3:7]
