@@ -213,7 +213,8 @@ int pulse_amp_obs(const pulse_amp_obs_args_t* args, int64_t num_envs, void* stre
  *   pulse_policy_post   get_action_values' sampling (common_agent.py:262-288; ModelA2CContinuousLogStd [rl_games]): action = mu +
  *                       exp(logstd) * eps, neglogp, de-normalised value (running_mean_std.py:84-87), optional PD targets
  *                       (Humanoid._action_to_pd_targets, humanoid.py:1392-1394).  eps: injected, or Philox4x32-10(seed,
- *                       row, *rng_offset + rng_step) drawn in the kernel (a device-side offset keeps CUDA-graph replays fresh).
+ *                       row, *rng_offset + rng_step) drawn in the kernel (a device-side offset keeps CUDA-graph replays fresh;
+ *                       the index layout per row is listed with the other Philox planes below).  1 <= num_actions <= 256.
  *   pulse_value_post    next_values = unnormalise(critic(next obs)) * (1 - terminated)   (amp_agent.py:396-398)
  *   pulse_amp_obs_row   AMP observation row of this step = [current W | first (steps-1)*W floats of the previous row], written
  *                       into its experience slice (humanoid_amp.py:622-667 + amp_agent.py:385); W = amp_width (196 by default, 195
@@ -511,7 +512,7 @@ int pulse_gaussian_sample(const float* mu, int64_t ld_mu, const float* eps, cons
  *   a = max(-A r, -A clip(r, 1-e, 1+e)), r = exp(old_neglogp - neglogp);  c = (ret - v)^2;
  *   b = sum(clamp_min(mu-1,0)^2 + clamp_max(mu+1,0)^2);  loss = mean(a) + critic_coef*mean(c) + bounds_coef*mean(b).
  * Outputs: dmu bf16 [rows, ld_dmu] (+ transposed [A_pad, ld_t]), dvalue bf16 [rows, ld_dv] (+ transposed),
- * stats[0..5] fp64 accumulators: sum a, sum c, sum b, sum kl, clipped count, sum neglogp (caller zeroes). */
+ * stats[0..5] fp64 accumulators: sum a, sum c, sum b, sum kl, clipped count, sum neglogp (caller zeroes).  1 <= num_actions <= 256. */
 typedef struct {
   const float* mu; int64_t ld_mu;       /* [rows, A] network output */
   const float* value; int64_t ld_value; /* [rows, 1] */
@@ -795,6 +796,11 @@ int pulse_ztask_obs_list(const pulse_ztask_step_args_t* args, const int64_t* env
  *   index 8 * 2^32     x, y, z, w: Feistel round keys of the subset      counter ctr[PULSE_RING_DRAWS]
  *   index 9 * 2^32     x, y, z, w: Feistel round keys of the sampling permutation   counter ctr[PULSE_RING_PERM_KEY]
  * pulse_reset_terrain reads index e as above, with word z as the spawn location (w unused).
+ * pulse_policy_post keys its action noise by the policy's own seed, counter *rng_offset + rng_step, one block per action pair
+ * p = k / 2 of row r (words x, y: actions 2p, 2p + 1 by Box-Muller; z, w unused):
+ *   num_actions <= 128        index r * 64 + p    (p < 64)
+ *   128 < num_actions <= 256  index r * 128 + p   (p < 128; the SMPL-X dof-space policy, 153 actions)
+ * so the blocks of two rows never overlap at either width.
  * ---------------------------------------------------------------------------------------------- */
 #define PULSE_ZTASK_REACH 3
 #define PULSE_ZPOSE_AS_IS 0

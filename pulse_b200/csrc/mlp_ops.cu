@@ -188,6 +188,8 @@ __global__ void __launch_bounds__(128) gaussian_sample_kernel(const float* __res
 }
 
 // ---- PPO losses + gradients w.r.t. mu / value ---------------------------------------------------------------------
+// kPer actions per lane: 4 for A <= 128, 8 for A <= 256 (the SMPL-X dof-space policy's 153)
+template <int kPer>
 __global__ void __launch_bounds__(256) ppo_loss_kernel(const pulse_ppo_loss_args_t a, long long rows) {
   // Warps stride over the rows (a few rows each on a one-wave grid): the per-action constants are computed once per lane, the loss
   // statistics stay in registers until ONE set of fp64 atomics per block (six per 128-thread block serialise on six addresses).
@@ -195,7 +197,6 @@ __global__ void __launch_bounds__(256) ppo_loss_kernel(const pulse_ppo_loss_args
   const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
   __shared__ double s_stats[8][6];
   const int A = a.num_actions;
-  constexpr int kPer = 4;                       // actions per lane: A <= 128
   float sg[kPer], inv_sg2[kPer], lsum = 0.0f;
 #pragma unroll
   for (int q = 0; q < kPer; ++q) {
@@ -825,10 +826,17 @@ extern "C" int pulse_ppo_loss(const pulse_ppo_loss_args_t* args, int64_t rows, v
   PULSE_REQUIRE(args != nullptr && rows > 0, "pulse_ppo_loss: bad argument");
   const pulse_ppo_loss_args_t& a = *args;
   PULSE_REQUIRE(a.mu && a.value && a.actions && a.old_neglogp && a.advantages && a.returns && a.logstd, "pulse_ppo_loss: null input");
-  PULSE_REQUIRE(a.num_actions > 0 && a.num_actions <= 128, "pulse_ppo_loss: num_actions outside [1,128]");
+  PULSE_REQUIRE(a.num_actions > 0 && a.num_actions <= 256, "pulse_ppo_loss: num_actions %d outside [1,256]", a.num_actions);
+  PULSE_REQUIRE(a.ld_mu >= a.num_actions && a.ld_value >= 1 && (a.dmu == nullptr || a.ld_dmu >= a.num_actions),
+                "pulse_ppo_loss: leading dimensions too small");
   // 8 warps per block, one row per warp at a time; 8 blocks per SM are all resident (2048 threads per SM)
-  ppo_loss_kernel<<<grid_for(rows, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, rows);
-  PULSE_LAUNCH_OK("ppo_loss_kernel");
+  if (a.num_actions <= 128) {
+    ppo_loss_kernel<4><<<grid_for(rows, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, rows);
+    PULSE_LAUNCH_OK("ppo_loss_kernel<4>");
+  } else {
+    ppo_loss_kernel<8><<<grid_for(rows, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(a, rows);
+    PULSE_LAUNCH_OK("ppo_loss_kernel<8>");
+  }
   return PULSE_OK;
 }
 

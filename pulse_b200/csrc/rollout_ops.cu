@@ -25,6 +25,8 @@ __global__ void __launch_bounds__(128) policy_post_kernel(const pulse_policy_pos
   if (row >= rows) return;
   const int A = a.num_actions;
   const unsigned long long off = a.rng_offset != nullptr ? *a.rng_offset + a.rng_step : a.rng_step;
+  // Philox indices per row: 64 (pairs p < 64) up to 128 actions, 128 above, so no two rows share a block (pulse_b200.h)
+  const unsigned long long row_blocks = A <= 128 ? 64ull : 128ull;
   float acc = 0.0f, ls = 0.0f;
   // lanes take PAIRS of actions (2*lane + 64*i): one Philox call yields four words = two Box-Muller pairs
   for (int i = 0; 2 * lane + 64 * i < A; ++i) {
@@ -34,7 +36,7 @@ __global__ void __launch_bounds__(128) policy_post_kernel(const pulse_policy_pos
       e0 = a.eps[row * a.ld_eps + k0];
       e1 = k0 + 1 < A ? a.eps[row * a.ld_eps + k0 + 1] : 0.0f;
     } else {
-      const Philox4 r = philox4x32_10(a.seed, static_cast<unsigned long long>(row) * 64ull + static_cast<unsigned long long>(lane + 32 * i), off);
+      const Philox4 r = philox4x32_10(a.seed, static_cast<unsigned long long>(row) * row_blocks + static_cast<unsigned long long>(lane + 32 * i), off);
       box_muller(r.x, r.y, e0, e1);
     }
 #pragma unroll
@@ -149,7 +151,7 @@ extern "C" int pulse_policy_post(const pulse_policy_post_args_t* args, int64_t r
   if (rows == 0) return PULSE_OK;
   const pulse_policy_post_args_t& a = *args;
   PULSE_REQUIRE(a.mu && a.logstd && a.actions && a.neglogp, "pulse_policy_post: null mu / logstd / actions / neglogp");
-  PULSE_REQUIRE(a.num_actions >= 1 && a.num_actions <= 128, "pulse_policy_post: num_actions %d outside [1,128]", a.num_actions);
+  PULSE_REQUIRE(a.num_actions >= 1 && a.num_actions <= 256, "pulse_policy_post: num_actions %d outside [1,256]", a.num_actions);
   PULSE_REQUIRE(a.ld_mu >= a.num_actions && a.ld_actions >= a.num_actions && a.ld_neglogp >= 1, "pulse_policy_post: leading dimensions too small");
   PULSE_REQUIRE(a.eps == nullptr || a.ld_eps >= a.num_actions, "pulse_policy_post: ld_eps too small");
   PULSE_REQUIRE(a.mus_out == nullptr || a.ld_mus >= a.num_actions, "pulse_policy_post: ld_mus too small");

@@ -31,6 +31,9 @@ class LatentStepsB200(GraphRunner):
     the decoder MLP on [clamp(norm(s), +-5) | z] (HumanoidZ.compute_z_actions); `_pre_physics`; the caller's `physics(t)` hook;
     `_env_step(t)`; next_values[t] = critic(obses[:, t+1]) (1 - terminate) on the critic's second operand slot.
     S and A are the VAE's self-observation width and dof count (358 and 69 for SMPL, 778 and 153 for SMPL-X), E its latent size.
+    With `vae=None` the driver runs the non-latent task trained by PPO from scratch (learning=ppo): the policy acts in the A dofs
+    (E = A), `get_action_values` is the heads and `pulse_policy_post` (actions, neglogp, de-normalised value), and `_pre_physics`
+    takes the sampled actions themselves; there is no prior, `pulse_latent_post`, decoder or side P.
     `finish()` then computes GAE, normalised advantages and value-normalised returns from the task reward alone (task_reward_w 1,
     disc_reward_w 0) and `train_epoch()` runs the PPO update.
 
@@ -75,7 +78,10 @@ class LatentStepsB200(GraphRunner):
         self.dev = policy.device
         self.lib = _lib.load()
         n = self.n
-        T, W, E, A, dev = self.T, int(obs_width), vae.E, vae.A, self.dev
+        # the policy acts in the latent (E) with a VAE, in the dof space (A) without one
+        E, A = (vae.E, vae.A) if vae is not None else (policy.A, policy.A)
+        T, W, dev = self.T, int(obs_width), self.dev
+        self.dofs = A
         z = lambda *s, **k: torch.zeros(*s, device=dev, **k)
         self.obses, self.obs_carry = z(n, T, W), z(n, W)
         self.actions, self.mus, self.neglogp = z(n, T, E), z(n, T, E), z(n, T)
@@ -95,7 +101,7 @@ class LatentStepsB200(GraphRunner):
         self.physics: Optional[Callable[[int], None]] = None           # physics(t): between the pre-physics work and the step kernel
         self.refresh: Optional[Callable[[int, dict], None]] = None     # refresh(t, ws): after the reset, before the reset envs' observation
         self.reset_ws = None
-        self.z_actions = None          # the decoder's output of the last step, fp32 [n, A] (a reused workspace)
+        self.z_actions = None          # the decoder's output of the last step, fp32 [n, A] (a reused workspace); None without a VAE
         self._streams = None
         self.amp, self.task_w, self.disc_w = amp, float(task_reward_w), float(disc_reward_w)
         if amp is None and (self.task_w != 1.0 or self.disc_w != 0.0):
@@ -131,9 +137,16 @@ class LatentStepsB200(GraphRunner):
             _lib.check(getattr(self.lib, name)(*args, _lib.current_stream(self.dev)), name)
 
     def _act(self, t: int, side_a=None, side_p=None) -> None:
-        """get_action_values (amp_agent.py:359-378), HumanoidZ.compute_z_actions (humanoid_z.py:75-155) and the task's pre-physics work."""
+        """get_action_values (amp_agent.py:359-378), HumanoidZ.compute_z_actions (humanoid_z.py:75-155) and the task's pre-physics work.
+        Without a VAE (the dof-space baseline): the heads, `pulse_policy_post` (sample, neglogp, value) and the pre-physics work on the
+        sampled actions, which are the dof actions (Humanoid.step -> pre_physics_step)."""
         pol, vae, n = self.policy, self.vae, self.n
         obs, mus = self.obses[:, t], self.mus[:, t]
+        actions, neglogp, values = self.actions[:, t], self.neglogp[:, t], self.values[t]
+        if vae is None:
+            pol.act_into(obs, actions=actions, neglogp=neglogp, mus=mus, values=values, rng_step=t, side=side_a)
+            self._pre_physics(actions, t)
+            return
         main = torch.cuda.current_stream(self.dev)
         if side_p is not None:
             side_p.wait_stream(main)
@@ -144,7 +157,6 @@ class LatentStepsB200(GraphRunner):
         value = pol.heads_into(obs, mus=mus, side=side_a)
         if side_p is not None:
             main.wait_stream(side_p)
-        actions, neglogp, values = self.actions[:, t], self.neglogp[:, t], self.values[t]
         rms = pol.value_rms
         a = _lib.LatentPostArgs(mu=mus.data_ptr(), ld_mu=mus.stride(0), logstd=pol.logstd.data_ptr(), seed=pol.rng_seed,
                                 rng_offset=pol.rng_offset.data_ptr(), rng_step=t, latent=vae.E, actions=actions.data_ptr(),
@@ -196,8 +208,10 @@ class LatentStepsB200(GraphRunner):
                                        after_normalize=after_normalize)
 
     def _sides(self):
+        """(A, P, B); no side P without a VAE (there is no prior to run)."""
         if self._streams is None:
-            self._streams = tuple(torch.cuda.Stream(self.dev) for _ in range(3))
+            mk = lambda: torch.cuda.Stream(self.dev)
+            self._streams = (mk(), mk() if self.vae is not None else None, mk())
         return self._streams
 
     # ------------------------------------------------------------------ schedules

@@ -24,7 +24,8 @@ def check_pieces(task, reset, policy, vae, amp=None) -> str:
     """The task kind ("reach" / "speed" / "strike") after checking that the step object, the reset, the latent policy and the frozen
     VAE belong together; raises PulseError otherwise.  SMPL: observations of 361 / 361 / 373 floats, a 358 -> 69 decoder.  SMPL-X
     (SmplxReachTaskB200 / SmplxSpeedTaskB200 / SmplxStrikeTaskB200, PULSE-X): 781 / 781 / 793 floats, a 778 -> 153 decoder and a
-    48-dimensional latent (env_pulsex_amp.yaml)."""
+    48-dimensional latent (env_pulsex_amp.yaml).  `vae=None`: the dof-space baseline (learning=ppo), whose policy acts in the
+    layout's 69 / 153 dofs."""
     kind = _KINDS.get(getattr(task, "kind", None))
     if kind is None:
         raise _lib.PulseError("ZTaskStepsB200: task must be a ReachTaskB200, SpeedTaskB200, StrikeTaskB200 or one of their SMPL-X "
@@ -38,12 +39,20 @@ def check_pieces(task, reset, policy, vae, amp=None) -> str:
     W = _WIDTHS[(layout, kind)]
     if int(task.obs_size) != W or int(policy.obs_size) != W:
         raise _lib.PulseError(f"ZTaskStepsB200: the {layout} {kind} observation has {W} floats, the task writes {task.obs_size} and the policy reads {policy.obs_size}")
-    if int(policy.A) != int(vae.E):
-        raise _lib.PulseError(f"ZTaskStepsB200: the policy acts in {policy.A} dimensions, the VAE's latent has {vae.E}")
-    if int(vae.S) != S or int(vae.A) != A:
-        raise _lib.PulseError(f"ZTaskStepsB200: the decoder must map the {S}-float self observation to {A} dof targets, not {vae.S} -> {vae.A}")
-    if E is not None and int(vae.E) != E:
-        raise _lib.PulseError(f"ZTaskStepsB200: the {layout} latent has {E} dimensions (embedding_size), the VAE's {vae.E}")
+    if vae is None:
+        if int(policy.A) != A:
+            raise _lib.PulseError(f"ZTaskStepsB200: without a VAE the policy acts in the {layout} humanoid's {A} dofs, not in {policy.A} "
+                                  f"dimensions (a latent-space policy needs its VAE)")
+    else:
+        if int(policy.A) == A:
+            raise _lib.PulseError(f"ZTaskStepsB200: the policy acts in the {layout} humanoid's {A} dofs, but a VAE was given (the "
+                                  f"dof-space baseline takes vae=None)")
+        if int(policy.A) != int(vae.E):
+            raise _lib.PulseError(f"ZTaskStepsB200: the policy acts in {policy.A} dimensions, the VAE's latent has {vae.E}")
+        if int(vae.S) != S or int(vae.A) != A:
+            raise _lib.PulseError(f"ZTaskStepsB200: the decoder must map the {S}-float self observation to {A} dof targets, not {vae.S} -> {vae.A}")
+        if E is not None and int(vae.E) != E:
+            raise _lib.PulseError(f"ZTaskStepsB200: the {layout} latent has {E} dimensions (embedding_size), the VAE's {vae.E}")
     if (getattr(policy, "disc", None) is not None) != (amp is not None):
         raise _lib.PulseError("ZTaskStepsB200: a policy with a discriminator needs the AMP part (amp=AmpBuffersB200) and the AMP part a "
                               "discriminator")
@@ -84,6 +93,15 @@ class ZTaskStepsB200(LatentStepsB200):
 
     The PULSE-X reach and strike tasks take the same pieces with a SmplxReachTaskB200 / SmplxStrikeTaskB200 (obs_size 781 / 793), a
     SmplxTargetResetB200 of the same kind over the 52-body MotionLib, and the same decoder, latent and AMP part.
+
+    The PPO baseline (`HumanoidReach` / `HumanoidSpeed` / `HumanoidStrike` under learning=ppo, the same task trained from scratch):
+    `vae=None` and a policy that acts in the dofs, PPOPolicy(obs_size=task.obs_size, num_actions=69 (SMPL) or 153 (SMPL-X),
+    units=(2048, 1024, 512), act="silu", logstd=-2.9) (ppo.yaml).  A step is then `heads_into` (critic beside actor on side A),
+    `pulse_policy_post` into actions[:, t], neglogp[:, t] and values[t], and `pulse_ztask_pre_physics` on actions[:, t]: no prior,
+    latent post-processing or decoder, and no side P.  `actions` and `mus` are [n, T, dofs].  The reset, observations, step kernel,
+    next values, AMP part, `finish` and `train_epoch` are those of the latent driver.  The actor head writes its 153-float rows of
+    `mus` straight into the strided slice mus[:, t]: the forward epilogue stores fp32 rows with 16-byte stores only when the row
+    stride is a multiple of 4 floats and element-wise otherwise, so every horizon T is accepted without padding.
 
     Out of scope: multi-GPU; Default / Hybrid state init; the power_usage_reward terms the step kernels exclude."""
 
@@ -146,9 +164,10 @@ class ZTaskStepsB200(LatentStepsB200):
                                   **self._task_kw())
 
     def _pre_physics(self, dec: torch.Tensor, t: int, rand: Optional[torch.Tensor] = None, steps: Optional[torch.Tensor] = None) -> None:
-        """`pulse_ztask_pre_physics` on the decoder output `dec` [n, dofs]; `rand` / `steps` inject the `_update_task` draws per env."""
+        """`pulse_ztask_pre_physics` on the decoder output `dec` [n, dofs] (without a VAE: the sampled actions); `rand` / `steps` inject
+        the `_update_task` draws per env."""
         s, task, kind = self.sim, self.task, self.kind
-        p = _lib.ZTaskPrePhysicsArgs(kind=task.kind, dofs=self.vae.A, action=dec.data_ptr(), ld_action=dec.stride(0), pd_offset=self.pd[0].data_ptr(),
+        p = _lib.ZTaskPrePhysicsArgs(kind=task.kind, dofs=self.dofs, action=dec.data_ptr(), ld_action=dec.stride(0), pd_offset=self.pd[0].data_ptr(),
                                      pd_scale=self.pd[1].data_ptr(), freeze=_lib.ptr(self.pd_freeze), pd_out=self.pd_tar.data_ptr(),
                                      ld_pd=self.pd_tar.stride(0), progress_buf=s["progress_buf"].data_ptr(), seed=self.reset_seed, offset=t,
                                      offset_dev=self.policy.rng_offset.data_ptr(), rand=_lib.ptr(rand), steps_in=_lib.ptr(steps))

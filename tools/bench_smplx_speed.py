@@ -9,7 +9,10 @@ alternated sample by sample with `pulse_smplx_speed_step` in the same call, so t
              decoder of the PULSE-X VAE's shapes with random weights, pre-physics and step kernels; no physics), then `finish` and the
              PPO update (6 mini-epochs of 16384-row minibatches), on synthetic 52-body MotionLib tables and simulator state.  Two arms
              alternated iteration by iteration: graph (as shipped) and eager (use_graphs=False).  Milliseconds per horizon and update
-             from device events after --warmup, with an L2 flush before each timed region, over --iters iterations.
+             from device events after --warmup, with an L2 flush before each timed region, over --iters iterations.  --policy direct
+             measures the PPO baseline instead (HumanoidSpeed / HumanoidReach / HumanoidStrike under learning=ppo: ZTaskStepsB200 with
+             vae=None, the same network acting in the 153 dofs, no prior or decoder); --policy both alternates the latent and the direct
+             drivers' arms iteration by iteration, on MotionLib tables and simulator state built from the same seeds.
   step       `pulse_smplx_speed_step` alone at --step-envs envs: device events around --step-reps back-to-back launches (one L2
              flush before each sample), beside the bytes one env-step reads and writes as computed from the shapes (52 x 13 body
              floats, 52 x 3 contact floats, the 781-float observation row, and the per-env scalars).  At 16384 envs a launch touches
@@ -17,7 +20,7 @@ alternated sample by sample with `pulse_smplx_speed_step` in the same call, so t
 
 One JSON line per measurement, with the card name, power limit and maximum SM clock read in the same call.  Needs a CUDA device.
 
-  python tools/bench_smplx_speed.py [--task speed|reach|strike] [--envs 1536 8192] [--iters 5] [--warmup 2] [--step-envs 16384] [--step-reps 200]
+  python tools/bench_smplx_speed.py [--task speed|reach|strike] [--policy latent|direct|both] [--envs 1536 8192] [--iters 5] [--warmup 2] [--step-envs 16384] [--step-reps 200]
 """
 import argparse
 import ctypes as C
@@ -30,7 +33,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from tools.bench_ztask_rollout import HORIZON, MINI_EPOCHS, MINIBATCH, UNITS, gpu_info   # noqa: E402
+from tools.bench_ztask_rollout import HORIZON, MINI_EPOCHS, MINIBATCH, POLICIES, UNITS, gpu_info   # noqa: E402
 
 B, D, LATENT = 52, 153, 48
 CONTACT_IDS = (7, 3, 8, 4)          # R_Ankle, L_Ankle, R_Toe, L_Toe in the SMPLH_MUJOCO_NAMES order
@@ -83,7 +86,7 @@ def with_target(s, n, dev):
     return s
 
 
-def build(n, dev, use_graphs, kind="speed"):
+def build(n, dev, use_graphs, kind="speed", policy="latent"):
     from pulse_b200.motion_lib import MotionLibB200
     from pulse_b200.ppo import PPOPolicy
     from pulse_b200.vae import PulseVAE
@@ -93,13 +96,16 @@ def build(n, dev, use_graphs, kind="speed"):
     g = torch.Generator(device=dev).manual_seed(300)
     floor = -0.9 + 0.05 * torch.rand(ml.gts.shape[0], device=dev, generator=g)            # stand-in for the ground table
     task = make_task(kind, n, dev)
-    policy = PPOPolicy(obs_size=task.obs_size, num_actions=LATENT, units=UNITS, act="silu", device=dev, seed=0)
-    vae = PulseVAE(self_obs_size=778, num_actions=D, latent=LATENT, device=dev, with_critic=False)
+    if policy == "direct":                                                                  # ppo.yaml: the policy writes the 153 dof targets
+        pol, vae = PPOPolicy(obs_size=task.obs_size, num_actions=D, units=UNITS, act="silu", logstd=-2.9, device=dev, seed=0), None
+    else:
+        pol = PPOPolicy(obs_size=task.obs_size, num_actions=LATENT, units=UNITS, act="silu", device=dev, seed=0)
+        vae = PulseVAE(self_obs_size=778, num_actions=D, latent=LATENT, device=dev, with_critic=False)
     reset = ZTaskResetB200("speed", ml, floor, upright=False) if kind == "speed" else SmplxTargetResetB200(kind, ml, floor, upright=False)
     sim = sim_state(n, dev, 200)
     if kind == "strike":
         sim = with_target(sim, n, dev)
-    drv = ZTaskStepsB200(task, reset, policy, vae, sim, horizon=HORIZON, use_graphs=use_graphs, reset_seed=1)
+    drv = ZTaskStepsB200(task, reset, pol, vae, sim, horizon=HORIZON, use_graphs=use_graphs, reset_seed=1)
     drv.first_observation()
     return drv
 
@@ -124,6 +130,7 @@ def step_bytes(kind="speed"):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--task", choices=("speed", "reach", "strike"), default="speed")
+    ap.add_argument("--policy", choices=tuple(POLICIES), default="latent")
     ap.add_argument("--envs", type=int, nargs="+", default=[1536, 8192])
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
@@ -149,7 +156,8 @@ def main():
         return s, e
 
     for n in args.envs:
-        arms = {"graph": build(n, dev, True, args.task), "eager": build(n, dev, False, args.task)}
+        pols = POLICIES[args.policy]
+        arms = {(pol, mode): build(n, dev, mode == "graph", args.task, pol) for pol in pols for mode in ("graph", "eager")}
         mb = min(MINIBATCH, n * HORIZON)
         update = lambda d: (d.finish(), d.train_epoch(mini_epochs=MINI_EPOCHS, minibatch=mb))
         ev = {a: {"horizon": [], "update": []} for a in arms}
@@ -164,23 +172,32 @@ def main():
                     ev[a]["update"].append(u)
                     resets[a] += float(done)
         torch.cuda.synchronize()
-        c0 = lib.pulse_launch_count()
-        arms["eager"].play_steps()
-        torch.cuda.synchronize()
-        launches = (lib.pulse_launch_count() - c0) / HORIZON
-        out = {"workload": "PULSE-X %s task iteration (Humanoid%sZ, smplx_humanoid, 52 bodies, 153 dofs): %d envs, horizon %d, latent "
-                           "policy %s SiLU over %d dims, frozen prior + 778->153 decoder, task reward only, %d mini-epochs of %d rows, no physics"
-                           % (args.task, args.task.capitalize(), n, HORIZON, "-".join(map(str, UNITS)), LATENT, MINI_EPOCHS, mb),
-               "gpu": info, "envs": n, "iters": args.iters, "warmup": args.warmup, "launches_per_step": round(launches, 2)}
-        for a in arms:
-            ms = {k: [s.elapsed_time(e) for s, e in v] for k, v in ev[a].items()}
-            mean = {k: sum(v) / len(v) for k, v in ms.items()}
-            out[a] = {"horizon_ms": round(mean["horizon"], 3), "horizon_ms_min_max": [round(min(ms["horizon"]), 3), round(max(ms["horizon"]), 3)],
-                      "update_ms": round(mean["update"], 3), "update_ms_min_max": [round(min(ms["update"]), 3), round(max(ms["update"]), 3)],
-                      "rollout_env_steps_per_s": round(n * HORIZON / (mean["horizon"] * 1e-3), 1),
-                      "iteration_env_steps_per_s": round(n * HORIZON / ((mean["horizon"] + mean["update"]) * 1e-3), 1),
-                      "resets_per_horizon": round(resets[a] / args.iters, 1)}
-        print(json.dumps(out), flush=True)
+        launches = {}
+        for pol in pols:
+            c0 = lib.pulse_launch_count()
+            arms[(pol, "eager")].play_steps()
+            torch.cuda.synchronize()
+            launches[pol] = (lib.pulse_launch_count() - c0) / HORIZON
+        for pol in pols:
+            what = ("PULSE-X %s task iteration (Humanoid%sZ, smplx_humanoid, 52 bodies, 153 dofs): %d envs, horizon %d, latent policy %s SiLU "
+                    "over %d dims, frozen prior + 778->153 decoder" if pol == "latent" else
+                    "PPO baseline %s task iteration (Humanoid%s, smplx_humanoid, 52 bodies, ppo.yaml): %d envs, horizon %d, policy %s SiLU "
+                    "over the %d dofs, no prior or decoder")
+            out = {"workload": (what + ", task reward only, %d mini-epochs of %d rows, no physics")
+                               % (args.task, args.task.capitalize(), n, HORIZON, "-".join(map(str, UNITS)), LATENT if pol == "latent" else D,
+                                  MINI_EPOCHS, mb),
+                   "gpu": info, "envs": n, "iters": args.iters, "warmup": args.warmup, "policy": pol,
+                   "launches_per_step": round(launches[pol], 2)}
+            for mode in ("graph", "eager"):
+                a = (pol, mode)
+                ms = {k: [s.elapsed_time(e) for s, e in v] for k, v in ev[a].items()}
+                mean = {k: sum(v) / len(v) for k, v in ms.items()}
+                out[mode] = {"horizon_ms": round(mean["horizon"], 3), "horizon_ms_min_max": [round(min(ms["horizon"]), 3), round(max(ms["horizon"]), 3)],
+                             "update_ms": round(mean["update"], 3), "update_ms_min_max": [round(min(ms["update"]), 3), round(max(ms["update"]), 3)],
+                             "rollout_env_steps_per_s": round(n * HORIZON / (mean["horizon"] * 1e-3), 1),
+                             "iteration_env_steps_per_s": round(n * HORIZON / ((mean["horizon"] + mean["update"]) * 1e-3), 1),
+                             "resets_per_horizon": round(resets[a] / args.iters, 1)}
+            print(json.dumps(out), flush=True)
         del arms
         torch.cuda.empty_cache()
 

@@ -8,13 +8,17 @@ progress counters are spread over the episode length, so envs reset in every hor
 Two arms, alternated iteration by iteration in the same call so both see the same conditions:
   graph   the driver as shipped: the horizon is one CUDA graph over four streams, one graph per update minibatch
   eager   the same entry points with use_graphs=False: one stream, every launch issued from the host
+--policy picks the policy: latent (the default, above), direct (the PPO baseline HumanoidReach / HumanoidSpeed / HumanoidStrike under
+learning=ppo: ZTaskStepsB200 with vae=None, the same 2048-1024-512 SiLU network acting in the 69 dofs with sigma exp(-2.9), no prior
+or decoder), or both (the latent and the direct drivers' graph and eager arms alternated iteration by iteration, on MotionLib tables
+and simulator state built from the same seeds).  One JSON line per size and policy.
 
 Per size, one JSON line: the card name, power limit and maximum SM clock read in the same call; per arm the launches per step
 (`pulse_launch_count` over one eager horizon / T; the graph arm replays the launches it captured, fork and join included), the
 milliseconds per horizon and per update (device events; mean, min and max over --iters iterations after --warmup, with an L2 flush
 before each timed region) and the env-steps/s of the rollout and of the full iteration.  Needs a CUDA device: there is no fallback.
 
-  python tools/bench_ztask_rollout.py [--kind reach|speed|strike] [--envs 1024 8192] [--iters 5] [--warmup 2]
+  python tools/bench_ztask_rollout.py [--kind reach|speed|strike] [--policy latent|direct|both] [--envs 1024 8192] [--iters 5] [--warmup 2]
 """
 import argparse
 import json
@@ -28,7 +32,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 HORIZON, MINIBATCH, MINI_EPOCHS = 32, 16384, 6
-UNITS = (2048, 1024, 512)          # pulse_z_task.yaml:27-28
+UNITS = (2048, 1024, 512)          # pulse_z_task.yaml:27-28 and ppo.yaml
+POLICIES = {"latent": ("latent",), "direct": ("direct",), "both": ("latent", "direct")}
 
 
 def gpu_info():
@@ -37,7 +42,7 @@ def gpu_info():
     return out.splitlines()[0] if out else "unknown"
 
 
-def build(kind, n, dev, use_graphs):
+def build(kind, n, dev, use_graphs, policy="latent"):
     from pulse_b200.motion_lib import MotionLibB200
     from pulse_b200.ppo import PPOPolicy
     from pulse_b200.reach import ReachTaskB200
@@ -63,9 +68,12 @@ def build(kind, n, dev, use_graphs):
     if kind == "strike":
         sim.update(target_states=root[:, 1], tar_contact_forces=torch.zeros(n, 3, device=dev), tar_actor_ids=sim["actor_ids"] + 1)
     task = {"reach": ReachTaskB200, "speed": SpeedTaskB200, "strike": StrikeTaskB200}[kind](n, device=dev)
-    policy = PPOPolicy(obs_size=task.obs_size, num_actions=32, units=UNITS, act="silu", device=dev, seed=0)
-    vae = PulseVAE(device=dev, with_critic=False)                                           # the frozen prior + decoder
-    drv = ZTaskStepsB200(task, ZTaskResetB200(kind, ml, floor), policy, vae, sim, horizon=HORIZON, use_graphs=use_graphs, reset_seed=1)
+    if policy == "direct":                                                                  # ppo.yaml: the policy writes the 69 dof targets
+        pol, vae = PPOPolicy(obs_size=task.obs_size, num_actions=69, units=UNITS, act="silu", logstd=-2.9, device=dev, seed=0), None
+    else:
+        pol = PPOPolicy(obs_size=task.obs_size, num_actions=32, units=UNITS, act="silu", device=dev, seed=0)
+        vae = PulseVAE(device=dev, with_critic=False)                                       # the frozen prior + decoder
+    drv = ZTaskStepsB200(task, ZTaskResetB200(kind, ml, floor), pol, vae, sim, horizon=HORIZON, use_graphs=use_graphs, reset_seed=1)
     drv.first_observation()
     return drv
 
@@ -73,6 +81,7 @@ def build(kind, n, dev, use_graphs):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--kind", choices=("reach", "speed", "strike"), default="reach")
+    ap.add_argument("--policy", choices=tuple(POLICIES), default="latent")
     ap.add_argument("--envs", type=int, nargs="+", default=[1024, 8192])
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
@@ -96,7 +105,8 @@ def main():
         return s, e
 
     for n in args.envs:
-        arms = {"graph": build(args.kind, n, dev, True), "eager": build(args.kind, n, dev, False)}
+        pols = POLICIES[args.policy]
+        arms = {(pol, mode): build(args.kind, n, dev, mode == "graph", pol) for pol in pols for mode in ("graph", "eager")}
         mb = min(MINIBATCH, n * HORIZON)
         update = lambda d: (d.finish(), d.train_epoch(mini_epochs=MINI_EPOCHS, minibatch=mb))
         ev = {a: {"horizon": [], "update": []} for a in arms}
@@ -111,23 +121,30 @@ def main():
                     ev[a]["update"].append(u)
                     resets[a] += float(done)
         torch.cuda.synchronize()
-        c0 = lib.pulse_launch_count()
-        arms["eager"].play_steps()
-        torch.cuda.synchronize()
-        launches = (lib.pulse_launch_count() - c0) / HORIZON
-        out = {"workload": "latent-space %s task iteration (Humanoid%sZ, pulse_z_task.yaml): %d envs, horizon %d, latent policy %s SiLU, frozen "
-                           "prior + decoder, task reward only, %d mini-epochs of %d rows, no physics, no discriminator"
-                           % (args.kind, args.kind.capitalize(), n, HORIZON, "-".join(map(str, UNITS)), MINI_EPOCHS, mb),
-               "gpu": info, "kind": args.kind, "envs": n, "iters": args.iters, "warmup": args.warmup, "launches_per_step": round(launches, 2)}
-        for a in arms:
-            ms = {k: [s.elapsed_time(e) for s, e in v] for k, v in ev[a].items()}
-            mean = {k: sum(v) / len(v) for k, v in ms.items()}
-            out[a] = {"horizon_ms": round(mean["horizon"], 3), "horizon_ms_min_max": [round(min(ms["horizon"]), 3), round(max(ms["horizon"]), 3)],
-                      "update_ms": round(mean["update"], 3), "update_ms_min_max": [round(min(ms["update"]), 3), round(max(ms["update"]), 3)],
-                      "rollout_env_steps_per_s": round(n * HORIZON / (mean["horizon"] * 1e-3), 1),
-                      "iteration_env_steps_per_s": round(n * HORIZON / ((mean["horizon"] + mean["update"]) * 1e-3), 1),
-                      "resets_per_horizon": round(resets[a] / args.iters, 1)}
-        print(json.dumps(out), flush=True)
+        launches = {}
+        for pol in pols:
+            c0 = lib.pulse_launch_count()
+            arms[(pol, "eager")].play_steps()
+            torch.cuda.synchronize()
+            launches[pol] = (lib.pulse_launch_count() - c0) / HORIZON
+        for pol in pols:
+            what = ("latent-space %s task iteration (Humanoid%sZ, pulse_z_task.yaml): %d envs, horizon %d, latent policy %s SiLU, frozen prior + decoder"
+                    if pol == "latent" else
+                    "PPO baseline %s task iteration (Humanoid%s, ppo.yaml): %d envs, horizon %d, policy %s SiLU over the 69 dofs, no prior or decoder")
+            out = {"workload": (what + ", task reward only, %d mini-epochs of %d rows, no physics, no discriminator")
+                               % (args.kind, args.kind.capitalize(), n, HORIZON, "-".join(map(str, UNITS)), MINI_EPOCHS, mb),
+                   "gpu": info, "kind": args.kind, "envs": n, "iters": args.iters, "warmup": args.warmup, "policy": pol,
+                   "launches_per_step": round(launches[pol], 2)}
+            for mode in ("graph", "eager"):
+                a = (pol, mode)
+                ms = {k: [s.elapsed_time(e) for s, e in v] for k, v in ev[a].items()}
+                mean = {k: sum(v) / len(v) for k, v in ms.items()}
+                out[mode] = {"horizon_ms": round(mean["horizon"], 3), "horizon_ms_min_max": [round(min(ms["horizon"]), 3), round(max(ms["horizon"]), 3)],
+                             "update_ms": round(mean["update"], 3), "update_ms_min_max": [round(min(ms["update"]), 3), round(max(ms["update"]), 3)],
+                             "rollout_env_steps_per_s": round(n * HORIZON / (mean["horizon"] * 1e-3), 1),
+                             "iteration_env_steps_per_s": round(n * HORIZON / ((mean["horizon"] + mean["update"]) * 1e-3), 1),
+                             "resets_per_horizon": round(resets[a] / args.iters, 1)}
+            print(json.dumps(out), flush=True)
         del arms
         torch.cuda.empty_cache()
 
