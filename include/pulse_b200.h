@@ -442,8 +442,12 @@ int pulse_gemm_bf16(const void* a, int64_t lda, const void* b, int64_t ldb, int6
 int pulse_gemm_num_splits(int64_t k, int32_t split_k);
 /* The GEMM's shape rule alone: the output tile width (128 or 256) it picks for an m x n x k GEMM with split_k on `sms` SMs.  A launch
  * takes the wide tile only for forward / ReLU-dgrad GEMMs with a K-major A and bf16-only outputs without a pre-activation, and never
- * under PULSE_GEMM_BN=128 or PULSE_GEMM_STAGES=4.  pulse_gemm_last_tile_n: the width the last GEMM launch took (0 before the first). */
+ * under PULSE_GEMM_BN=128 or PULSE_GEMM_STAGES=4.  pulse_gemm_last_launch: the kernel the last GEMM launch from the host took, as
+ * out[6] = {epilogue mode (0 generic, 1 forward, 2 ReLU dgrad, 3 weight gradient, 4 general-gate dgrad), ring depth, tile width,
+ * tma_out (0 staged epilogue, 1 bulk tensor stores / reductions, 2 register-resident fp32 slabs), splits, grid}; zeros before the
+ * first.  pulse_gemm_last_tile_n: its tile width alone (0 before the first launch). */
 int pulse_gemm_tile_n(int64_t m, int64_t n, int64_t k, int32_t split_k, int32_t sms);
+int pulse_gemm_last_launch(int32_t* out);
 int pulse_gemm_last_tile_n(void);
 
 /* ------------------------------------------------------------------------------------------------

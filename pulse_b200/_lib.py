@@ -461,6 +461,7 @@ SIGNATURES = {
                                   C.POINTER(GemmEpilogue), C.c_int32, C.c_uint32, C.c_void_p]),
     "pulse_gemm_num_splits": (C.c_int, [C.c_int64, C.c_int32]),
     "pulse_gemm_tile_n": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32]),
+    "pulse_gemm_last_launch": (C.c_int, [C.POINTER(C.c_int32)]),
     "pulse_gemm_last_tile_n": (C.c_int, []),
     "pulse_normalize_to_bf16": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                           C.c_void_p, C.c_int64, C.c_float, C.c_void_p]),
@@ -571,6 +572,16 @@ def check(status, what):
     if status != 0:
         msg = load().pulse_last_error().decode("utf-8", "replace")
         raise PulseError(f"{what} failed with status {status}: {msg}")
+
+
+GEMM_LAUNCH_FIELDS = ("mode", "stages", "tile_n", "tma_out", "splits", "grid")
+
+
+def gemm_last_launch() -> dict:
+    """The kernel the last GEMM launch from the host took (pulse_gemm_last_launch), by field name; all 0 before the first."""
+    out = (C.c_int32 * len(GEMM_LAUNCH_FIELDS))()
+    check(load().pulse_gemm_last_launch(out), "pulse_gemm_last_launch")
+    return dict(zip(GEMM_LAUNCH_FIELDS, out))
 
 
 def ptr(t):

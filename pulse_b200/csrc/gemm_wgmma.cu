@@ -420,9 +420,10 @@ bool make_map_slabs(CUtensorMap* map, const float* base, long long splits, long 
   return fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
-// the reduction path needs 16-byte aligned rows; otherwise the kernel falls back to fp32 atomics
-bool tma_reduce_ok(const pulse_gemm_epilogue_t& ep) {
-  return ep.out_f32 != nullptr && ep.accumulate && (ep.ldf % 4) == 0 && (reinterpret_cast<uintptr_t>(ep.out_f32) % 16) == 0;
+// the reduction path needs 16-byte aligned rows and N a multiple of 4: the bulk tensor reduction clips the column tail in whole
+// 16-byte units, so at N = 69 it would add (zeros) into columns 69..71, outside the output.  Otherwise the kernel uses fp32 atomics.
+bool tma_reduce_ok(const pulse_gemm_epilogue_t& ep, long long n) {
+  return ep.out_f32 != nullptr && ep.accumulate && (n % 4) == 0 && (ep.ldf % 4) == 0 && (reinterpret_cast<uintptr_t>(ep.out_f32) % 16) == 0;
 }
 bool tma_rows_ok(const void* base, long long ld) { return (ld % 8) == 0 && (reinterpret_cast<uintptr_t>(base) % 16) == 0; }
 
@@ -441,7 +442,7 @@ int epilogue_maps(int mode, const pulse_gemm_epilogue_t& ep, long long m, long l
   memset(map_p, 0, sizeof(*map_p));
   *tma_out = 0;
   if (mode == kModeWgrad) {
-    if (!tma_reduce_ok(ep)) return PULSE_OK;
+    if (!tma_reduce_ok(ep, n)) return PULSE_OK;
     if (!make_map_c(map_c, ep.out_f32, m, n, ep.ldf)) {
       set_error("pulse_gemm_bf16: cuTensorMapEncodeTiled failed for the fp32 output");
       return PULSE_ERR_CUDA;
@@ -512,7 +513,8 @@ bool narrow_forced() {
   const char* e = getenv("PULSE_GEMM_BN");
   return e != nullptr && atoi(e) == kNarrowBN;
 }
-int g_last_tile_n = 0;   // tile width of the last GEMM launch issued from the host (pulse_gemm_last_tile_n)
+// the last GEMM launch issued from the host (pulse_gemm_last_launch): mode, ring depth, tile width, tma_out, splits, grid
+int g_last_launch[6] = {};
 
 // sets the kernel's dynamic shared-memory size once per instantiation and checks it against the device's opt-in limit
 template <typename Kernel>
@@ -560,7 +562,8 @@ int launch_gemm_ring(const CUtensorMap& map_a, const CUtensorMap& map_b, const C
   cfg.numAttrs = na;
   PULSE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_bf16_kernel<A_MN, B_MN, MODE, S, BN>, map_a, map_b, map_c, map_p, ep, m, n, k, kb_per_split, splits, tma_out));
   PULSE_LAUNCH_OK("gemm_bf16_kernel");
-  g_last_tile_n = BN;
+  const int launch[6] = {MODE, S, BN, tma_out, splits, static_cast<int>(grid)};
+  memcpy(g_last_launch, launch, sizeof(launch));
   return PULSE_OK;
 }
 
@@ -601,7 +604,8 @@ int epilogue_mode(const pulse_gemm_epilogue_t* ep) {
   const bool want_accum = ep->accumulate != 0;
   if (!want_dgrad && !want_accum) return kModeFwd;
   if (!want_fwd && !want_accum) return (ep->gate && ep->gate_mode != PULSE_ACT_RELU) ? kModeDgradVec : kModeDgrad;
-  if (!want_fwd && !want_dgrad && !ep->out) return kModeWgrad;
+  // the weight-gradient epilogue adds the raw accumulator (bulk reductions of the staged tile, or atomics): no alpha
+  if (!want_fwd && !want_dgrad && !ep->out && ep->alpha == 1.0f) return kModeWgrad;
   return kModeGeneric;
 }
 
@@ -622,15 +626,24 @@ extern "C" int pulse_gemm_num_splits(int64_t k, int32_t split_k) {
 }
 
 // the shape rule alone (gemm_tile_n): the width it picks for an m x n x k GEMM with split_k on `sms` SMs.  A launch takes it only where a
-// wide instantiation applies (see launch_gemm); pulse_gemm_last_tile_n reports what a launch took.
+// wide instantiation applies (see launch_gemm); pulse_gemm_last_launch reports what a launch took.
 extern "C" int pulse_gemm_tile_n(int64_t m, int64_t n, int64_t k, int32_t split_k, int32_t sms) {
   const int num_kb = static_cast<int>((k + 63) / 64);
   const int splits = pulse_gemm_num_splits(k, split_k);
   return pulse::gemm_tile_n(m, n, (num_kb + splits - 1) / splits, splits, sms);
 }
 
-// output tile width (128 or 256) of the last GEMM launch issued from the host; 0 before the first
-extern "C" int pulse_gemm_last_tile_n(void) { return pulse::g_last_tile_n; }
+// the kernel the last GEMM launch issued from the host took: {epilogue mode, ring depth, tile width, tma_out, splits, grid}; zeros
+// before the first
+extern "C" int pulse_gemm_last_launch(int32_t* out) {
+  using namespace pulse;
+  PULSE_REQUIRE(out != nullptr, "pulse_gemm_last_launch: null argument");
+  memcpy(out, pulse::g_last_launch, sizeof(pulse::g_last_launch));
+  return PULSE_OK;
+}
+
+// output tile width (128 or 256) of the last GEMM launch issued from the host; 0 before the first (field 2 of pulse_gemm_last_launch)
+extern "C" int pulse_gemm_last_tile_n(void) { return pulse::g_last_launch[2]; }
 
 // flags: bit 0 = A is MN-major ([K, M] row-major in memory), bit 1 = B is MN-major ([K, N] row-major in memory)
 extern "C" int pulse_gemm_bf16(const void* a, int64_t lda, const void* b, int64_t ldb, int64_t m, int64_t n, int64_t k,

@@ -6,6 +6,8 @@ without."""
 import pytest
 import torch
 
+from pulse_b200 import _lib
+
 pytestmark = pytest.mark.gpu
 
 DEV = "cuda:0"
@@ -16,21 +18,16 @@ def _bf(g, r, c, scale=1.0):
     return (torch.randn(r, (c + 7) // 8 * 8, device=DEV, generator=g) * scale).bfloat16()[:, :c]
 
 
-def _last_tile_n():
-    from pulse_b200 import _lib
-    return _lib.load().pulse_gemm_last_tile_n()
-
-
 def _both(monkeypatch, run, wide):
     """run() (one GEMM launch) with the narrow tile forced, then with the shape rule; returns both results.  wide: the default launch
     must take the 128 x 256 tile (checked on 132 SMs, the count the shape expectations are written for)"""
     monkeypatch.setenv("PULSE_GEMM_BN", "128")
     ref = run()
-    assert _last_tile_n() == 128
+    assert _lib.gemm_last_launch()["tile_n"] == 128
     monkeypatch.delenv("PULSE_GEMM_BN")
     new = run()
     if torch.cuda.get_device_properties(DEV).multi_processor_count == 132:
-        assert _last_tile_n() == (256 if wide else 128)
+        assert _lib.gemm_last_launch()["tile_n"] == (256 if wide else 128)
     torch.cuda.synchronize()
     return ref, new
 

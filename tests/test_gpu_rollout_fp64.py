@@ -132,11 +132,6 @@ def test_imitation_act_into_links_fp64(monkeypatch, mode, M):
 
 
 # ------------------------------------------------------------------------------------------------------------------- latent-task policy
-def _last_tile_n():
-    from pulse_b200 import _lib
-    return _lib.load().pulse_gemm_last_tile_n()
-
-
 @pytest.mark.parametrize("M", SIZES)
 @pytest.mark.parametrize("mode", list(MODES))
 def test_latent_task_links_fp64(monkeypatch, mode, M):
@@ -186,7 +181,7 @@ def test_latent_task_links_fp64(monkeypatch, mode, M):
             prior_head, dec_in = vae.z_prior(obs)
             value = pol.heads_into(obs, mus=mus[:, t], side=torch.cuda.Stream(DEV) if t % 2 else None)
             pol.actor.forward(b["x"], out=mus[:, t])              # the head alone once more: the tile width of its launch
-            tile = _last_tile_n()
+            tile = _lib.gemm_last_launch()["tile_n"]
             eps = torch.zeros(M, E, device=DEV) if zero_noise else None
             a = _lib.LatentPostArgs(mu=mus[:, t].data_ptr(), ld_mu=mus.stride(0), logstd=pol.logstd.data_ptr(), seed=pol.rng_seed,
                                     rng_offset=pol.rng_offset.data_ptr(), rng_step=t, latent=E, actions=actions[:, t].data_ptr(),

@@ -151,14 +151,10 @@ def test_sept_update_links_fp64(monkeypatch, mode, case):
         print("\n" + rep.text() + note)
 
 
-def _last_tile_n():
-    from pulse_b200 import _lib
-    return _lib.load().pulse_gemm_last_tile_n()
-
-
 @pytest.mark.parametrize("M", [2051, 16384])
 @pytest.mark.parametrize("mode", ["default", "bn128"])
 def test_sept_eval_links_fp64(monkeypatch, mode, M):
+    from pulse_b200 import _lib
     for k, v in MODES[mode].items():
         monkeypatch.setenv(k, v)
     d = SEPT_FULL
@@ -190,7 +186,7 @@ def test_sept_eval_links_fp64(monkeypatch, mode, M):
         check_mlp_eval(rep, "critic (critic_values)", pol.critic, snap, P, M)
         pol.task.forward(T, out=P[:, :E])            # a lone task forward: its top layer is the last launch
         torch.cuda.synchronize()
-        tile = _last_tile_n()
+        tile = _lib.gemm_last_launch()["tile_n"]
         note = f"\n  task top layer (eval, N = {E}, into P[:, :{E}]): {tile}-wide output tile"
         if M == 16384:
             assert tile == (128 if mode == "bn128" else 256), f"task top layer at M={M} took the {tile}-wide tile"
